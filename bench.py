@@ -116,15 +116,16 @@ def peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s, not measured)"
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks during the timed region (NVML; B200_PROFILING.md "clocks line")
+# clocks during the timed region, and the card and power limit they were measured on (NVML)
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
     def __init__(self, index: int, period_s: float = 0.02):
         self.samples, self.reasons, self.max_mhz = [], set(), None
+        self.gpu, self.power_limit_w = None, None
         self._stop = threading.Event()
         self._thr = None
         try:
@@ -133,6 +134,9 @@ class ClockSampler:
             self.nv = pynvml
             self.h = pynvml.nvmlDeviceGetHandleByIndex(index)
             self.max_mhz = pynvml.nvmlDeviceGetMaxClockInfo(self.h, pynvml.NVML_CLOCK_SM)
+            name = pynvml.nvmlDeviceGetName(self.h)
+            self.gpu = name.decode() if isinstance(name, bytes) else name
+            self.power_limit_w = pynvml.nvmlDeviceGetEnforcedPowerLimit(self.h) / 1000.0
         except Exception:
             self.nv = None
         self.period = period_s
@@ -168,7 +172,7 @@ class ClockSampler:
             self._thr.join()
         s = sorted(self.samples)
         return {"sm_mhz": (s[len(s) // 2] if s else None), "sm_max_mhz": self.max_mhz,
-                "samples": len(s), "reasons": sorted(self.reasons)}
+                "samples": len(s), "reasons": sorted(self.reasons), "gpu": self.gpu, "power_limit_w": self.power_limit_w}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -249,7 +253,7 @@ def run_reference_arm(args):
 
 
 # ------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm (--impl b200: the name of the package's CUDA path)
 # ------------------------------------------------------------------------------------------------
 def run_b200_arm(args):
     import numpy as np
@@ -274,7 +278,7 @@ def run_b200_arm(args):
     man = manifest(wl)
     names = [n for n, _ in man]
     K, W = args.steps, max(args.warmup, 3)
-    R = rotation_for(N)                             # rotating state sets: defeats the 126 MB L2
+    R = rotation_for(N)                             # rotating state sets: defeats the L2
     gen = torch.Generator(device=dev); gen.manual_seed(19830610 + 1000 * rank)
 
     def lr_fn(s):
@@ -365,6 +369,9 @@ def run_b200_arm(args):
     torch.cuda.synchronize(dev)
     torch.cuda.profiler.stop()
     clocks = sampler.stop()
+    if args.dump_outputs:
+        op_l, params_l, _, _, dp_l = sets[(base + K - 1) % R]
+        dump_outputs(args.dump_outputs, op_l, params_l, dp_l, write=(rank == 0))
     if dist is not None:
         dist.barrier()
     total_ms = evs[0].elapsed_time(evs[K])
@@ -468,7 +475,7 @@ def run_b200_arm(args):
     a_ms, c_ms = mean(apply_ms), mean(acc_ms)
     achieved = ab / (a_ms * 1e-3) / 1e9 if apply_ms else float("nan")
     if world == 1:
-        kernel = ("apply_clip_kernel (a+=G, /N, global-norm clip, AdamWeightDecay, a=0; one cooperative launch: TMA-fed rings, ticketed tiles, Tensor-Memory stash, exact norm)"
+        kernel = ("apply_clip_kernel (a+=G, /N, global-norm clip, AdamWeightDecay, a=0; one cooperative launch: TMA-fed rings, ticketed tiles, shared-memory stash, exact norm)"
                   if hp.clip_norm > 0 else "apply_kernel (single pass: a+=G, /N, Adam, a=0; no clip)")
     else:
         kernel = "dp_apply_kernel (apply step at N>1: includes the NVLink exchange, so this is not an HBM roofline)"
@@ -488,7 +495,8 @@ def run_b200_arm(args):
                    "parallelism": f"dp{world}" + ("" if world == 1 else
                                                    " fused apply kernel: local a+=G + reduce-scatter + sharded update + all-gather over NVLink peer memory in one launch"
                                                    if args.dp == "fused" else " nccl all-reduce of the packed accum slab on apply steps"),
-                   "l2": f"rotating {R} independent state sets ({R * 5 * 4 * P / 1e6:.0f} MB of state+grads per rotation) > 126 MB L2",
+                   "l2": f"rotating {R} independent state sets ({R * 5 * 4 * P / 1e6:.0f} MB of state+grads per rotation), "
+                         f"L2 {torch.cuda.get_device_properties(dev).L2_cache_size / 1e6:.0f} MB",
                    "apply_launches": len(apply_ms), "accumulate_launches": len(acc_ms),
                    "window_exact": window_exact,
                    "window_exact_value": (world * N / (window_us * 1e-6)) if window_us else None,
@@ -529,6 +537,36 @@ def run_b200_arm(args):
     print(json.dumps(_finite(out)))
     if dist is not None:
         dist.destroy_process_group()
+
+
+DUMP_SAMPLE = 1 << 21     # elements per dumped array: 4 x 8 MB of state + a 16 MB index stay under 64 MB
+
+
+def dump_outputs(out_dir, op, params, dp, write=True):
+    """What the last timed micro-step left to its caller, for comparing two builds output for output: the parameters,
+    accumulators and Adam moments of the state set it used, packed in tensor order, each sampled at the same fixed,
+    seeded DUMP_SAMPLE positions (sample_index.npy), and its stats block [applied, lr, global_norm, clip_scale]."""
+    import numpy as np
+    import torch
+    sizes = [p.numel() for p in params]
+    full = dp.gather_state() if dp is not None else {"m": op.m, "v": op.v}      # fused data parallel: m, v are sharded
+
+    def packed(slab):
+        return torch.cat([slab[o:o + n] for o, n in zip(op.plan.offsets, sizes)])
+    arrays = {"params": torch.cat([p.detach().reshape(-1) for p in params]), "accum": packed(op.accum),
+              "adam_m": packed(full["m"]), "adam_v": packed(full["v"])}
+    st = op.stats()
+    if not write:
+        return
+    P = sum(sizes)
+    idx = np.sort(np.random.default_rng(19830610).choice(P, size=min(P, DUMP_SAMPLE), replace=False))
+    idx_t = torch.from_numpy(idx).to(arrays["params"].device)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "sample_index.npy"), idx.astype(np.float64))
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t[idx_t].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "stats.npy"),
+            np.array([float(st["applied"]), st["lr"], st["global_norm"], st["clip_scale"]], np.float32))
 
 
 def parity_check(args, wl, N, hp, variant_b, man, names, world, rank, dev, dist):
@@ -719,6 +757,8 @@ def main():
     ap.add_argument("--parity-steps", type=int, default=-1, help="micro-steps of the pre-timing parity self-check against the CPU oracle (-1: 2*min(N,4)+1, 0: skip)")
     ap.add_argument("--e2e-keep-affinity", action="store_true", help="experiment: keep the GPU-local CPU affinity for the whole e2e leg")
     ap.add_argument("--cpu-budget", type=float, default=12.0, help="seconds of CPU-oracle timing (0 disables)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step left to its caller as DIR/<name>.npy")
     args = ap.parse_args()
     args.cpu_budget_given = any(a.startswith("--cpu-budget") for a in sys.argv[1:])
     if args.impl == "reference":

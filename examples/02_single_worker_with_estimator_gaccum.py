@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""distributedExample/02_single_worker_with_estimator_gaccum.py on the B200 train_op, keeping the
+"""distributedExample/02_single_worker_with_estimator_gaccum.py on the H100 train_op, keeping the
 reference's structure: input_fn / model_fn(features, labels, mode, params) -> EstimatorSpec /
 RunConfig / Estimator / train_and_evaluate.  Synthetic MNIST-shaped data (the MNIST files are not
 shipped with the reference and there is no network here).

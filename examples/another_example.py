@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """The reference's another-example.py recipe (a custom-Estimator regressor whose ``_train_op_fn`` accumulates gradients,
-another-example.py:126-155) on the B200 train_op -- a thin launch script, not a re-implementation of tf.estimator.
+another-example.py:126-155) on the H100 train_op -- a thin launch script, not a re-implementation of tf.estimator.
 
   python examples/another_example.py --steps 600 --model-dir /tmp/housing           # fresh run (RESUME_TRAINING = False, :323-325)
   python examples/another_example.py --steps 600 --model-dir /tmp/housing --resume  # continue from model_dir (:326-327)

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """The reference's distributedExample/02 (single worker) and /04 (multi worker) recipes on the
-B200 train_op -- a thin launch script, not a re-implementation of tf.estimator.
+H100 train_op -- a thin launch script, not a re-implementation of tf.estimator.
 
   python examples/mnist_gaccum.py --steps 200                       # 02: 1 worker, batch 100, N=2
   torchrun --nproc-per-node 2 examples/mnist_gaccum.py --steps 200  # 04: 2 workers, batch 50 each

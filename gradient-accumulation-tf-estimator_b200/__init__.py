@@ -1,6 +1,6 @@
-"""gradient-accumulation-tf-estimator_b200 -- the B200-native accumulate-then-apply train_op.
+"""gradient-accumulation-tf-estimator_b200 -- the H100-native accumulate-then-apply train_op.
 
-One hot path of hpandana/gradient-accumulation-tf-estimator, rebuilt for sm_100a:
+One hot path of hpandana/gradient-accumulation-tf-estimator, rebuilt for sm_90a:
 ``create_optimizer``'s tf.cond train_op (reference optimization.py:25-104) with
 ``AdamWeightDecayOptimizer.apply_gradients`` (optimization.py:128-177) and the plain-Adam variant
 of the distributedExample scripts, as hand-written CUDA kernels behind a C ABI

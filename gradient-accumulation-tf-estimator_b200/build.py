@@ -1,4 +1,4 @@
-"""Builds csrc/libgaccum.so in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+"""Builds csrc/libgaccum.so in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -14,7 +14,7 @@ SOURCES = ["gaccum_abi.cu"]
 DEPS = SOURCES + sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + ["../../include/gaccum.h"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-shared",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-shared",
     "-Xcompiler", "-fPIC,-fvisibility=hidden,-ffp-contract=off,-O2",
     "-cudart", "static",
 ]

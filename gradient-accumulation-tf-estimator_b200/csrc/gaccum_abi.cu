@@ -64,7 +64,7 @@ struct gaccum_plan {
   unsigned long long* d_barrier = nullptr; // clip-apply kernel: monotonic arrival counter of the consumers' grid barrier
   LaunchCounters* d_counters = nullptr;    // ... two sets of per-launch counters (tickets, pool length, norm accumulator)
   bool p1_dynamic = false;                 // ... pass 1 hands out the non-parked tiles by atomic tickets (long passes) or by position (short ones)
-  int tmem_tiles = kTmemTiles;             // tiles of a' per consumer group parked in Tensor Memory (GACCUM_TMEM_TILES: A/B)
+  int stash_tiles = kStashTiles;           // tiles of a' per consumer group parked in shared memory (GACCUM_STASH_TILES: A/B)
 #ifdef GACCUM_EXPERIMENTS
   unsigned long long* d_debug = nullptr;   // per-CTA timestamps (tools/cta_timeline.py; experiments build only)
 #endif
@@ -157,7 +157,7 @@ static int grid_for(gaccum_plan* pl, const void* fn, int* out) {
 
 template <int CAP>
 static int launch_accumulate(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream_t st) {
-  // one tile per CTA: the hardware block scheduler balances better than a persistent loop (r01_tune_sweep.md)
+  // one tile per CTA: the hardware block scheduler balances better than a persistent loop
   const int grid = std::max(1, prm.num_tiles);
   accumulate_kernel<CAP><<<grid, kThreads, 0, st>>>(prm);
   CUDA_TRY(cudaGetLastError());
@@ -172,18 +172,18 @@ static int launch_apply_noclip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStre
   return GACCUM_OK;
 }
 
-// clip-apply: one cooperative launch, ONE 864-thread CTA per SM (it allocates all of Tensor Memory, so a second
-// CTA could never be co-resident -- the grid is clamped to the SM count, not derived from the occupancy API)
+// clip-apply: one cooperative launch, ONE 864-thread CTA per SM (ring + stash take nearly all of the SM's shared
+// memory, so a second CTA could never be co-resident -- the grid is clamped to the SM count)
 template <int VARIANT, bool HAS_G, int CAP>
 static int launch_apply_clip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream_t st) {
   const void* fn = (const void*)&apply_clip_kernel<VARIANT, HAS_G, CAP>;
   {
     std::lock_guard<std::mutex> lk(pl->mu);
     if (pl->grid_cache.find(fn) == pl->grid_cache.end()) {
-      CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kRingBytes));
+      CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kClipSmemBytes));
       int per_sm = 0;
-      CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kClipThreads, (size_t)kRingBytes));
-      if (per_sm < 1) return fail(GACCUM_ECUDA, "apply_clip_kernel does not fit on an SM (%d B dynamic shared memory)", kRingBytes);
+      CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kClipThreads, (size_t)kClipSmemBytes));
+      if (per_sm < 1) return fail(GACCUM_ECUDA, "apply_clip_kernel does not fit on an SM (%d B dynamic shared memory)", kClipSmemBytes);
       pl->grid_cache[fn] = pl->num_sms;
     }
   }
@@ -192,9 +192,9 @@ static int launch_apply_clip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream
   prm.barrier = pl->d_barrier;
   prm.counters = pl->d_counters;
   if (pl->p1_dynamic) prm.flags |= kFlagDynamicPass1;
-  prm.tmem_tiles = pl->tmem_tiles;
+  prm.stash_tiles = pl->stash_tiles;
   void* args[] = {(void*)&prm};
-  CUDA_TRY(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kClipThreads), args, (size_t)kRingBytes, st));
+  CUDA_TRY(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kClipThreads), args, (size_t)kClipSmemBytes, st));
   return GACCUM_OK;
 }
 
@@ -395,11 +395,11 @@ int gaccum_plan_create(gaccum_plan** out, int32_t T, const int64_t* numels, cons
   if (hp->variant == GACCUM_ADAM_WEIGHT_DECAY && decay) pl->decay.assign(decay, decay + T);
   if (int rc = build_layout(pl)) { delete pl; return rc; }
   pl->device = -1;
-  // GACCUM_TMEM_TILES: A/B measurement knob of the clip-apply kernel (how many a' tiles per group are parked in
-  // Tensor Memory); every value computes the same result.  Result-changing timing experiments do not exist in this build.
-  if (const char* t = getenv("GACCUM_TMEM_TILES")) pl->tmem_tiles = std::max(0, std::min(kTmemTiles, atoi(t)));
-  // measured on the same GPU (profiles/r02_tune_sweep.md): handing pass 1's non-parked tiles out by tickets is as fast as
-  // the static split at BERT-Small (176.5 vs 177.0 us) and 1.5-2 % faster at BERT-Base / -Large; GACCUM_P1_DYNAMIC=0 is the A/B knob
+  // GACCUM_STASH_TILES: A/B measurement knob of the clip-apply kernel (how many a' tiles per group are parked in
+  // shared memory); every value computes the same result.  Result-changing timing experiments do not exist in this build.
+  if (const char* t = getenv("GACCUM_STASH_TILES")) pl->stash_tiles = std::max(0, std::min(kStashTiles, atoi(t)));
+  // handing pass 1's non-parked tiles out by tickets keeps every SM busy to the end of the pass (SMs see unequal shares
+  // of HBM bandwidth); GACCUM_P1_DYNAMIC=0 is the A/B knob for the static split
   pl->p1_dynamic = true;
   if (const char* t = getenv("GACCUM_P1_DYNAMIC")) pl->p1_dynamic = atoi(t) != 0;
   if (device >= 0) {
@@ -674,7 +674,7 @@ struct gaccum_host_session {
 // One cudaMemcpyAsync per RUN of tensors whose host addresses are laid out like the device slab (same distance
 // between consecutive tensors on both sides, padding included): a caller that keeps its gradients / parameters
 // in one pinned arena with the plan's offsets gets a single copy per direction instead of one per tensor
-// (each costs ~6 us of copy-engine gap: 73 copies held the link at 44 GB/s, one copy reaches ~55).
+// (every copy costs a copy-engine gap: many small copies hold the link well below what one large copy reaches).
 extern "C++" {
 template <typename HostPtr, typename F>
 static int for_each_run(const gaccum_plan* pl, HostPtr const* host, F&& copy /* (t0, host_ptr, dev_offset, elements) -> cudaError_t */) {

@@ -6,7 +6,7 @@
 // happens once, inside the apply kernel.  Rank r OWNS the contiguous tile range
 // [bounds[r], bounds[r+1]) (equal element counts); m and v are only ever touched by their owner
 // (ZeRO-1 style).  The kernel is PUSH based -- remote STORES are fire-and-forget, remote loads would
-// have to cover ~2-3 us of NVLink latency with registers:
+// have to cover microseconds of NVLink latency with registers:
 //
 //   phase A   every tile of the model: x = a + G (the window's last local accumulate, folded in:
 //             optimization.py:81).  Owned tile: a <- x.  Foreign tile: x is STORED INTO THE OWNER'S
@@ -89,7 +89,7 @@ __device__ __forceinline__ void dp_phase_done(const DpParams<CAP>& prm, int phas
   __shared__ int s_last;
   // bar.sync orders every thread's stores before thread 0's fence, and a system-scope fence is cumulative: ONE
   // MEMBAR.SYS per block publishes the whole block's local and remote stores (one per thread -- 150 000 of them,
-  // all at the end of a phase -- cost 30 us per phase)
+  // all at the end of a phase -- serialise on the memory system)
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence_system();
@@ -117,7 +117,7 @@ __device__ __forceinline__ void dp_phase_done(const DpParams<CAP>& prm, int phas
   }
 }
 // Tiles of a phase are handed to the blocks by an atomic ticket counter (SMs see different shares of HBM and NVLink
-// bandwidth: with a static split the first block finished phase A 40 us before the last).  The block works on ticket i
+// bandwidth: with a static split the first blocks finish a phase long before the last).  The block works on ticket i
 // while every thread already holds ticket i+1 (so the caller can load that tile's descriptor) and thread 0 draws
 // ticket i+2: neither the atomic's round trip nor the descriptor load is on the critical path.
 struct TicketLoop {
@@ -356,7 +356,7 @@ dp_apply_kernel(const __grid_constant__ DpParams<CAP> prm) {
   TicketLoop tl;
   // ---- phase A: local accumulate + reduce-scatter by pushes.  Ticket q -> tile i = q / W of shard (R + 1 + q % W) % W:
   //      consecutive tickets go to W different owners (the last one is this rank itself), so pushes to every peer are
-  //      spread evenly over the whole phase instead of arriving in one burst that NVLink then needs 30 us to drain, and
+  //      spread evenly over the whole phase instead of arriving in one burst that NVLink then has to drain, and
   //      at any moment every owner receives from every source at the same rate ----
   {
     int max_shard = 0;
@@ -390,7 +390,7 @@ dp_apply_kernel(const __grid_constant__ DpParams<CAP> prm) {
   stamp(3);
 
   // ---- phase B: reduction of the owned shard in fixed rank order + norm partial.  Local traffic only and short: a static
-  //      split (block b takes owned tiles b, b + G, ...) beats tickets here (31 vs 48 us at W=2: per-tile barriers
+  //      split (block b takes owned tiles b, b + G, ...) beats tickets here (per-tile barriers
   //      cost more than the imbalance), and keeps the reduction order fixed: thread fp64 running sums -> block tree ->
   //      one partial per block -> the last block adds the partials in block order ---------------------------------
   {

@@ -1,4 +1,4 @@
-// gaccum_kernels.cuh -- sm_100a kernels of the gradient-accumulation train_op.
+// gaccum_kernels.cuh -- sm_90a kernels of the gradient-accumulation train_op.
 //
 // All kernels walk a static tile table (<= 2048 elements of one tensor per tile), so the work split --
 // and therefore every reduction -- is deterministic.
@@ -16,18 +16,16 @@
 //                                  prefetches of a run ahead), three 256-thread CONSUMER GROUPS load a,
 //                                  take G out of the slots, a' = a + G, reduce sum((a'/N)^2)
 //                                  (thread fp32 per tile -> fp64 running sum -> warp shuffle -> shared
-//                                  memory -> one fp64 partial per CTA); a' is PARKED ON CHIP: the first
-//                                  tiles in Tensor Memory (tcgen05.st), the last ones in the very slots
-//                                  their G landed in (the ring becomes the stash), the rest written back
-//                                  in place tagged L2::evict_last
+//                                  memory -> one fp64 partial per CTA); a' of the first tiles is PARKED
+//                                  ON CHIP in a shared-memory stash beside the ring, the rest written
+//                                  back in place tagged L2::evict_last
 //                          barrier every CTA adds the per-CTA partials in the same order
 //                                  (bit-identical gn and clip scale everywhere)
-//                          pass 2  L2-resident tiles youngest first, then the slots, then Tensor Memory:
+//                          pass 2  the stashed tiles, then the L2-resident tiles youngest first:
 //                                  clip, AdamWeightDecay/Adam, write p, m, v, a = 0
 // Arithmetic uses round-to-nearest intrinsics (__fmul_rn, __fadd_rn, __fdiv_rn, __fsqrt_rn) so nvcc
 // cannot contract mul+add into FMA: the reference graph is un-fused, one rounding per TF op, and we
 // reproduce it bit for bit (the kernels are HBM-bound, the extra flops are free).
-// Measurements and the experiments behind each choice: profiles/r01_tune_sweep.md, profiles/r02_*.md.
 #pragma once
 
 #include <cooperative_groups.h>
@@ -90,7 +88,7 @@ struct KernelParams {
   uint32_t flags;     // kFlag* bits (all of them produce correct results)
   unsigned long long* barrier;  // apply_clip_kernel: monotonic arrival counter of the consumers' grid barrier
   struct LaunchCounters* counters;  // apply_clip_kernel: two sets of per-launch counters (tickets, pool length, norm accumulator)
-  int32_t tmem_tiles;   // apply_clip_kernel: tiles of a' each consumer group parks in Tensor Memory (0..kTmemTiles)
+  int32_t stash_tiles;  // apply_clip_kernel: tiles of a' each consumer group parks in shared memory (0..kStashTiles)
 #ifdef GACCUM_EXPERIMENTS
   unsigned long long* debug;  // 16 words per CTA: 4 timestamps (ns) + wait-cycle counters (tools/cta_timeline.py)
 #endif
@@ -358,28 +356,27 @@ __device__ __forceinline__ double block_reduce_to_double(double x, double* smem 
 //
 // NO consumer ever issues a bulk load: every input stream of both passes is moved by TMA
 // (cp.async.bulk shared <- global, completing on an mbarrier by byte count) into a per-group ring in
-// shared memory, fed by the group's producer warp.  Why (measured, profiles/r02_tune_sweep.md):
+// shared memory, fed by the group's producer warp.  Why:
 //   * an LDG-fed pass can keep only as many bytes in flight as it has registers AND L1 lines to land them
-//     in; L1 and shared memory split 256 KB, so every KB of on-chip stash was paid for with bytes in
-//     flight (round 1: pass 1 at 4.6 TB/s with 192 KB of stash and 60 KB of L1);
+//     in; L1 and shared memory split 256 KB per SM, so every KB of on-chip stash is paid for with bytes in
+//     flight;
 //   * TMA loads need neither registers nor L1: bytes in flight = ring size, descriptors and addresses are
 //     computed by the producers ahead of the consumers, whose loop is wait -> LDS -> math -> store.
 // NO tile is bound to an SM before it is fetched: with the memory system saturated some SMs get a larger share
-// of it than others (with static tiles the first SM finished pass 2 forty microseconds before the last), so the
-// producers draw tiles from global atomic ticket counters -- every SM stays busy until the pass is over.
+// of it than others, so the producers draw tiles from global atomic ticket counters -- every SM stays busy until
+// the pass is over.
 //
 // pass 1   tickets over ALL tiles.  ring slot = [G tile | a tile] (16 KB, kP1Slots per group).  a' = a + G;
 //          sum((a'/N)^2): thread fp32 per tile -> warp shuffle in fp64 (fixed order) -> EXACT accumulation of the
 //          per-warp, per-tile sums in a 2176-bit fixed-point accumulator (integer atomics: associative, so the
 //          total does not depend on which SM reduced which tile -- the norm is bit-identical from run to run
-//          and across replicas although the schedule is dynamic).  a' of the first kTmemTiles tiles a group
-//          processes is parked in Tensor Memory (tcgen05.st: 256 KB per SM that a kernel without MMA leaves
-//          idle) and the tile is remembered in shared memory; every other a' goes back in place tagged
-//          L2::evict_last.  One flag per tile (plain store) says which of the two happened.
+//          and across replicas although the schedule is dynamic).  a' of the first kStashTiles tiles a group
+//          processes is parked in the group's shared-memory stash (the part of the SM's 227 KB the ring leaves
+//          free); every other a' goes back in place tagged L2::evict_last.
 // barrier  only the CONSUMERS rendezvous (named barrier + one atomic per CTA).  The producers do not: p, m, v do
-//          not depend on the clip scale, so they start streaming the group's own Tensor-Memory tiles into the
+//          not depend on the clip scale, so they start streaming the group's own stashed tiles into the
 //          ring as soon as pass 1 is drained -- HBM stays busy while the CTAs wait for each other.
-// pass 2   ring slot = [p | m | v | a'] (32 KB).  First the group's own Tensor-Memory tiles, then tickets over
+// pass 2   ring slot = [p | m | v | a'] (32 KB).  First the group's own stashed tiles, then tickets over
 //          all tiles, youngest first (a' still in L2), skipping the parked ones: clip, AdamWeightDecay/Adam,
 //          STG p, m, v, a = 0.
 // Tiles that bulk copies cannot move (gradient / parameter pointer not 16-byte aligned, or shorter than one
@@ -391,10 +388,6 @@ __device__ __forceinline__ double block_reduce_to_double(double x, double* smem 
 constexpr int kGroups = 3;                        // consumer groups per CTA
 constexpr int kConsumerThreads = kThreads * kGroups;        // 768
 constexpr int kClipThreads = kConsumerThreads + 32 * kGroups;   // + one producer warp per group = 864
-constexpr int kTmemCols = 512;                    // one CTA per SM: take all columns
-constexpr int kTmemColsPerWarp = 80;              // 6 warps share a lane quadrant: 6 x 80 = 480 <= 512
-constexpr int kTmemTiles = kTmemColsPerWarp / 8;  // 10 tiles per group
-constexpr uint32_t kNoTmem = 0xffffffffu;
 #ifndef GACCUM_P1_SLOTS
 #define GACCUM_P1_SLOTS 2
 #endif
@@ -402,16 +395,23 @@ constexpr int kP1Slots = GACCUM_P1_SLOTS;         // pass-1 ring slots per group
 constexpr int kP1SlotVecs = 2 * (kTile / 4);      // float4 per pass-1 slot: G | a
 constexpr int kP2SlotVecs = 4 * (kTile / 4);      // float4 per pass-2 slot: p | m | v | a'
 constexpr int kRingVecs = kP1Slots * kP1SlotVecs; // per group
-constexpr int kP2Slots = kRingVecs / kP2SlotVecs; // 2 x 16 KB = 32 KB -> 1 x 32 KB (deeper rings measured slower: r02_tune_sweep.md)
-constexpr int kRingBytes = kGroups * kRingVecs * 16;   // dynamic shared memory of the kernel (96 KB)
+constexpr int kP2Slots = kRingVecs / kP2SlotVecs; // 2 x 16 KB = 32 KB -> 1 x 32 KB
+constexpr int kRingBytes = kGroups * kRingVecs * 16;   // 96 KB
 static_assert(kP2Slots >= 1 && kP1Slots <= 8, "ring must hold at least one [p|m|v|a'] slot");
+// the stash: kStashTiles tiles of a' per group (8 KB each) in the shared memory the ring and the static arrays
+// (~16 KB) leave free of the 227 KB a block may have on sm_90
+constexpr int kStashTiles = 4;
+constexpr uint32_t kNoStash = 0xffffffffu;
+constexpr int kStashVecs = kStashTiles * (kTile / 4);          // float4 per group
+constexpr int kClipSmemBytes = kRingBytes + kGroups * kStashVecs * 16;   // dynamic shared memory of the kernel (192 KB)
+static_assert(kClipSmemBytes + 20 * 1024 <= 227 * 1024, "ring + stash + static shared memory must fit one sm_90 block");
 constexpr int kMaxSlots = 8;
 constexpr int kTicketBatch = 4;                   // pass-1 tickets a producer draws at once while plenty of tiles are left
 // what the producer tells the consumers about the tile it put into a slot
 struct __align__(16) SlotMeta {
   TileDesc d;          // len == 0: end of the pass
   uint32_t tile;       // index into the tile table
-  uint32_t tmem_slot;  // pass 2: a' is parked in this Tensor-Memory slot of the group (kNoTmem: it is in the slot's 4th quarter / in global memory)
+  uint32_t stash_slot; // pass 2: a' is parked in this stash slot of the group (kNoStash: it is in the slot's 4th quarter / in global memory)
   uint32_t pad[2];
 };
 // exact accumulation of non-negative doubles: 68 bins of 32 payload bits in 64-bit containers cover the whole
@@ -457,42 +457,12 @@ __device__ __forceinline__ unsigned long long ld_acquire_gpu_u64(const unsigned 
 }
 
 // ---------------------------------------------------------------------------------------------
-// Tensor Memory as a scratchpad.  TMEM (256 KB per SM, 512 columns x 128 lanes x 32 bit) normally
-// holds tcgen05.mma accumulators; this kernel has no MMA, so it is idle silicon -- 37 MB across the
-// chip.  The CTA allocates all 512 columns (one CTA per SM by construction); every consumer warp parks
-// a' values in the 32 lanes it may address (lane quadrant = warp % 4; the 6 warps sharing a quadrant
-// take 80 columns each): tcgen05.st 32x32b.x8 writes the thread's 8 words of a tile to 8 consecutive
-// columns of its own lane, tcgen05.ld reads them back in pass 2.  A thread only ever reads what it
-// wrote itself.
+// The stash: one CTA per SM by construction, so the shared memory the ring does not need holds a' of a
+// group's first tiles from pass 1 to pass 2.  A stash slot keeps the tile in its natural float4 order,
+// exactly like a ring slot, so thread t writes and later reads vectors t and t + kThreads of the tile:
+// a thread only ever reads what it wrote itself (no barrier), and a warp touches 512 consecutive
+// bytes per access (no bank conflicts).
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"((uint32_t)kTmemCols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"((uint32_t)kTmemCols) : "memory");
-}
-__device__ __forceinline__ void tmem_store8(uint32_t taddr, const float4& a, const float4& b) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-               ::"r"(taddr), "r"(__float_as_uint(a.x)), "r"(__float_as_uint(a.y)), "r"(__float_as_uint(a.z)),
-                 "r"(__float_as_uint(a.w)), "r"(__float_as_uint(b.x)), "r"(__float_as_uint(b.y)),
-                 "r"(__float_as_uint(b.z)), "r"(__float_as_uint(b.w)) : "memory");
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_load8(uint32_t taddr, float4& a, float4& b) {
-  uint32_t r0, r1, r2, r3, r4, r5, r6, r7;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3), "=r"(r4), "=r"(r5), "=r"(r6), "=r"(r7) : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-  a = make_float4(__uint_as_float(r0), __uint_as_float(r1), __uint_as_float(r2), __uint_as_float(r3));
-  b = make_float4(__uint_as_float(r4), __uint_as_float(r5), __uint_as_float(r6), __uint_as_float(r7));
-}
-// TMEM address of this warp's slot for stashed tile `slot` (0..kTmemTiles-1): lane quadrant = warp % 4,
-// column block = warp / 4 (0..5 across the three groups)
-__device__ __forceinline__ uint32_t tmem_slot_addr(uint32_t base, int slot) {
-  const uint32_t warp = threadIdx.x >> 5;
-  return base + (((warp & 3u) * 32u) << 16) + (warp >> 2) * kTmemColsPerWarp + (uint32_t)slot * 8u;
-}
 
 // Number of float4 vectors of this tile that pass 1 moves by bulk copy (0: scalar fallback).  The producer and
 // the consumers MUST agree on this.
@@ -504,9 +474,9 @@ __device__ __forceinline__ uint32_t bulk_vecs2(const TileDesc& d, const float* p
   return aligned16(p) ? (d.len >> 2) : 0u;
 }
 
-// a' of a tile may be parked in Tensor Memory only if BOTH passes take the vector path for it and it is a full tile
+// a' of a tile may be parked in the stash only if BOTH passes take the vector path for it and it is a full tile
 template <bool HAS_G, int CAP>
-__device__ __forceinline__ bool tmem_ok(const TileDesc& d, const KernelParams<CAP>& prm) {
+__device__ __forceinline__ bool stash_ok(const TileDesc& d, const KernelParams<CAP>& prm) {
   bool ok = d.len == (uint32_t)kTile && aligned16(param_ptr(prm.tab, d));
   if constexpr (HAS_G) { const float* g = grad_ptr(prm.tab, d); ok = ok && (g == nullptr || aligned16(g)); }
   return ok;
@@ -567,7 +537,7 @@ __device__ __forceinline__ double acc_value(const unsigned long long* bins /* kA
 // ---- pass 1, consumer side: one tile out of slot [G | a]; returns this THREAD's partial of sum((a'/N)^2) ----
 template <bool HAS_G, int CAP>
 __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float4* slot, uint64_t* empty,
-                                           const uint32_t tmem, const uint64_t pol) {
+                                           float4* const stash, const uint64_t pol) {
   const float* __restrict__ g = nullptr;
   if constexpr (HAS_G) g = grad_ptr(prm.tab, d);
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
@@ -592,14 +562,14 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
         if (g) {
           x[u].x = __fadd_rn(x[u].x, gg[u].x); x[u].y = __fadd_rn(x[u].y, gg[u].y);
           x[u].z = __fadd_rn(x[u].z, gg[u].z); x[u].w = __fadd_rn(x[u].w, gg[u].w);
-          if (tmem == kNoTmem) st_policy(a4 + i, x[u], pol);
+          if (stash == nullptr) st_policy(a4 + i, x[u], pol);
         }
+        if (stash != nullptr) stash[i] = x[u];
         const float nx = normalize(x[u].x, nf, inv_nf), ny = normalize(x[u].y, nf, inv_nf),
                     nz = normalize(x[u].z, nf, inv_nf), nw = normalize(x[u].w, nf, inv_nf);
         acc = fmaf(nx, nx, acc); acc = fmaf(ny, ny, acc); acc = fmaf(nz, nz, acc); acc = fmaf(nw, nw, acc);
       }
     }
-    if (tmem != kNoTmem) tmem_store8(tmem, x[0], x[1]);   // full tile: every lane of every warp carries data
     const uint32_t i = (nvec << 2) + tid;      // < 4 tail elements always travel through global memory
     if (i < len) {
       float xs = a[i];
@@ -621,11 +591,11 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
   return acc;
 }
 
-// ---- pass 2, consumer side: one tile out of slot [p | m | v | a']; a' from the slot or from Tensor Memory ----
+// ---- pass 2, consumer side: one tile out of slot [p | m | v | a']; a' from the slot or from the stash ----
 // The caller has waited on the slot's `full` barrier (it had to, to learn which tile this is).
 template <int VARIANT, int CAP>
 __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelParams<CAP>& prm, const float s, const float4* slot,
-                                             uint64_t* empty, const uint32_t tmem) {
+                                             uint64_t* empty, const float4* const stash) {
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
   float* __restrict__ m = prm.m + soff;
@@ -645,13 +615,12 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
     float4* v4 = reinterpret_cast<float4*>(v);
     float4* p4 = reinterpret_cast<float4*>(p);
     float4 va[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll];
-    if (tmem != kNoTmem) tmem_load8(tmem, va[0], va[1]);
 #pragma unroll
     for (int u = 0; u < kUnroll; ++u) {
       const uint32_t i = u * kThreads + tid;
       if (i < nvec) {
         vp[u] = slot[i]; vm[u] = slot[kTile / 4 + i]; vv[u] = slot[2 * (kTile / 4) + i];
-        if (tmem == kNoTmem) va[u] = slot[3 * (kTile / 4) + i];
+        va[u] = stash != nullptr ? stash[i] : slot[3 * (kTile / 4) + i];
       }
     }
     __syncwarp();
@@ -683,7 +652,11 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
   }
 }
 
-// Dynamic shared memory of apply_clip_kernel: 3 groups x kRingVecs float4 (192 KB).
+// Dynamic shared memory of apply_clip_kernel (kClipSmemBytes): 3 groups x kRingVecs float4 of ring, then
+// 3 groups x kStashVecs float4 of stash.
+// Registers: 864 threads in one CTA cap the kernel at 72 per thread.  The AdamWeightDecay instantiations (VARIANT 0)
+// fit without spilling; the plain-Adam ones with clipping (VARIANT 1, used only when tf_adam is combined with
+// clip_norm > 0) spill 8-20 bytes per thread to local memory (ptxas -v).  What that costs has not been measured.
 template <int VARIANT, bool HAS_G, int CAP>
 __global__ void __launch_bounds__(kClipThreads, 1)
 apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
@@ -691,7 +664,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   __shared__ unsigned long long s_bins[kConsumerThreads / 32][kAccBins];   // one exact accumulator per consumer warp (13 KB)
   __shared__ unsigned int s_nonfinite;
   __shared__ float s_bcast[2];
-  __shared__ uint32_t s_tmem_base, s_set;
+  __shared__ uint32_t s_set;
   __shared__ __align__(8) uint64_t s_full1[kGroups][kMaxSlots], s_empty1[kGroups][kMaxSlots];
   __shared__ __align__(8) uint64_t s_full2[kGroups][kMaxSlots], s_empty2[kGroups][kMaxSlots];
   __shared__ __align__(8) uint64_t s_go[kGroups];
@@ -703,9 +676,10 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   const int nt = prm.num_tiles, G = (int)gridDim.x * kGroups;
   const int b = (int)blockIdx.x * kGroups + grp;                   // virtual block id
   const int C = b < nt ? (nt - 1 - b) / G + 1 : 0;                 // tiles b, b + G, ... of this group's static share
-  const int n_tm = min(prm.tmem_tiles, C);                         // own tiles: a' parked in Tensor Memory
-  const int pool_lo = min(nt, prm.tmem_tiles * G);                 // tiles [pool_lo, nt): a' goes back to global memory
+  const int n_st = min(prm.stash_tiles, C);                        // own tiles: a' parked in the stash
+  const int pool_lo = min(nt, prm.stash_tiles * G);                // tiles [pool_lo, nt): a' goes back to global memory
   float4* const ring = reinterpret_cast<float4*>(smem_dyn) + (size_t)grp * kRingVecs;
+  float4* const stash = reinterpret_cast<float4*>(smem_dyn + kRingBytes) + (size_t)grp * kStashVecs;
   const uint64_t pol_last = policy_evict_last();
 
 #ifdef GACCUM_EXPERIMENTS
@@ -721,7 +695,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
 #endif
   stamp(0);
 
-  // ---- set-up: which counter set this launch uses, mbarriers, accumulator, Tensor Memory ---------------------
+  // ---- set-up: which counter set this launch uses, mbarriers, accumulator -----------------------------------
   if (threadIdx.x == 0) {
     // every CTA that has not yet arrived at this launch's barrier reads a value in [k*grid, (k+1)*grid)
     const unsigned long long k = ld_acquire_gpu_u64(prm.barrier) / gridDim.x;
@@ -737,11 +711,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   for (int i = threadIdx.x; i < (kConsumerThreads / 32) * kAccBins; i += kClipThreads) (&s_bins[0][0])[i] = 0ull;
-  if (prm.tmem_tiles > 0 && warp == 1) tmem_alloc(&s_tmem_base);
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = prm.tmem_tiles > 0 ? s_tmem_base : 0u;
   LaunchCounters* const ctr = prm.counters + s_set;
   if (blockIdx.x == 0 && threadIdx.x >= 64 && threadIdx.x < 64 + (int)(sizeof(LaunchCounters) / 8)) {
     // the other set was used by the previous launch on this plan, which is complete: clear it for the next one
@@ -756,7 +726,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     long long dbg_empty = 0;
     const long long dbg_p0 = clock64();
 #endif
-    // ---- pass 1.  First the group's OWN tiles b + j*G, j < tmem_tiles: their a' is parked in this SM's Tensor Memory, so
+    // ---- pass 1.  First the group's OWN tiles b + j*G, j < stash_tiles: their a' is parked in this SM's stash, so
     //      they are bound to it in both passes.  Then the rest of the model, tiles [pool_lo, nt): either this group's static
     //      share (b + j*G) or, with kFlagDynamicPass1, whatever the global ticket counter hands out -- kTicketBatch tickets at
     //      a time while plenty are left (one atomic per lane, the descriptor loads of a batch overlap), single tickets
@@ -796,7 +766,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         return dl;
       };
       const bool dynamic = (prm.flags & kFlagDynamicPass1) != 0;
-      const int n_static = dynamic ? n_tm : C;                                // tiles b + j*G, j < n_static, are this group's by position
+      const int n_static = dynamic ? n_st : C;                               // tiles b + j*G, j < n_static, are this group's by position
       for (int j0 = 0; j0 < n_static; j0 += 32) {                              // descriptors 32 at a time, one per lane
         TileDesc d{};
         if (j0 + lane < n_static) d = prm.tiles[b + (j0 + lane) * G];
@@ -846,7 +816,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
       prm.debug[blockIdx.x * 16 + 13 + grp] = (unsigned long long)(clock64() - dbg_p0);   // cycles until pass 1 was issued and drained
     }
 #endif
-    // ---- pass 2.  First the group's own Tensor-Memory tiles (their a' cannot move; their p, m, v do not depend on
+    // ---- pass 2.  First the group's own stashed tiles (their a' cannot move; their p, m, v do not depend on
     //      the clip scale, so these copies start BEFORE the grid barrier and HBM stays busy while the CTAs wait for
     //      each other).  Then tickets over the pool of L2-resident tiles, youngest first.  Pool tiles carry their a'
     //      in the slot's 4th quarter; they may only be fetched once every CTA has passed the barrier. ----
@@ -857,10 +827,10 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
       const unsigned long long pool_n = (unsigned long long)max(0, nt - pool_lo);
       while (true) {
         int tile;
-        uint32_t tmem_slot = kNoTmem;
-        if (jb < n_tm) {
+        uint32_t stash_slot = kNoStash;
+        if (jb < n_st) {
           tile = b + jb * G;
-          tmem_slot = (uint32_t)jb;
+          stash_slot = (uint32_t)jb;
           ++jb;
         } else {
           if (!past_barrier) {
@@ -875,8 +845,8 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         const TileDesc d = prm.tiles[tile];
         const float* p = param_ptr(prm.tab, d);
         const uint32_t nvec = bulk_vecs2(d, p);
-        const bool in_tmem = tmem_slot != kNoTmem && tmem_ok<HAS_G>(d, prm);
-        if (!in_tmem && !past_barrier) {                                        // an own tile whose a' had to go to global memory
+        const bool in_stash = stash_slot != kNoStash && stash_ok<HAS_G>(d, prm);
+        if (!in_stash && !past_barrier) {                                        // an own tile whose a' had to go to global memory
           mbar_wait(&s_go[grp], 0);
           asm volatile("fence.proxy.async;" ::: "memory");
           past_barrier = true;
@@ -885,15 +855,15 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         mbar_wait(&s_empty2[grp][rp.slot], rp.use & 1u);
         SlotMeta* meta = &s_meta2[grp][rp.slot];
         meta->d = d;
-        meta->tmem_slot = in_tmem ? tmem_slot : kNoTmem;
+        meta->stash_slot = in_stash ? stash_slot : kNoStash;
         if (nvec > 0) {
           const size_t soff = (size_t)d.soff32 * kSlabAlign;
           float4* dst = ring + (size_t)rp.slot * kP2SlotVecs;
-          mbar_arrive_expect_tx(full, nvec * 16u * (in_tmem ? 3u : 4u));
+          mbar_arrive_expect_tx(full, nvec * 16u * (in_stash ? 3u : 4u));
           bulk_g2s(dst, p, nvec * 16u, full, pol_first);
           bulk_g2s(dst + kTile / 4, prm.m + soff, nvec * 16u, full, pol_first);
           bulk_g2s(dst + 2 * (kTile / 4), prm.v + soff, nvec * 16u, full, pol_first);
-          if (!in_tmem) bulk_g2s(dst + 3 * (kTile / 4), prm.accum + soff, nvec * 16u, full, pol_first);
+          if (!in_stash) bulk_g2s(dst + 3 * (kTile / 4), prm.accum + soff, nvec * 16u, full, pol_first);
         } else {
           mbar_arrive(full);
         }
@@ -932,12 +902,12 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
 #endif
         const SlotMeta meta = s_meta1[grp][rp.slot];
         if (meta.d.len == 0) break;
-        // Tensor Memory takes the group's own tiles j < tmem_tiles (the first ones it is handed) when they are FULL,
-        // vector-path tiles (tcgen05.st/ld are warp-collective)
-        const bool own = n_seen < n_tm;
-        const bool park = own && tmem_ok<HAS_G>(meta.d, prm);
-        const uint32_t tm = park ? tmem_slot_addr(tmem_base, n_seen) : kNoTmem;
-        const float part = norm_tile<HAS_G>(meta.d, prm, ring + (size_t)rp.slot * kP1SlotVecs, &s_empty1[grp][rp.slot], tm, pol_last);
+        // the stash takes the group's own tiles j < stash_tiles (the first ones it is handed) when they are FULL,
+        // vector-path tiles (the same predicate the producer evaluates in pass 2)
+        const bool own = n_seen < n_st;
+        const bool park = own && stash_ok<HAS_G>(meta.d, prm);
+        float4* const st = park ? stash + (size_t)n_seen * (kTile / 4) : nullptr;
+        const float part = norm_tile<HAS_G>(meta.d, prm, ring + (size_t)rp.slot * kP1SlotVecs, &s_empty1[grp][rp.slot], st, pol_last);
         // warp total in fp64, fixed butterfly order; lane 0 adds it EXACTLY into its warp's accumulator
         double w = (double)part;
 #pragma unroll
@@ -994,8 +964,8 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         mbar_wait(&s_full2[grp][rp.slot], rp.use & 1u);
         const SlotMeta meta = s_meta2[grp][rp.slot];
         if (meta.d.len == 0) break;
-        const uint32_t tm = meta.tmem_slot != kNoTmem ? tmem_slot_addr(tmem_base, (int)meta.tmem_slot) : kNoTmem;
-        update_tile2<VARIANT>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], tm);
+        const float4* const st = meta.stash_slot != kNoStash ? stash + (size_t)meta.stash_slot * (kTile / 4) : nullptr;
+        update_tile2<VARIANT>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st);
         rp.advance(kP2Slots);
       }
     }
@@ -1005,7 +975,6 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   }
   __syncthreads();
   stamp(3);
-  if (prm.tmem_tiles > 0 && warp == 1) tmem_dealloc(tmem_base);
 }
 
 }  // namespace gaccum

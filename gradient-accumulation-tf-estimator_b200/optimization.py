@@ -6,7 +6,7 @@ keeps the reference signature (optimization.py:25).  Where the reference builds 
 ``assign_add`` / ``clip_by_global_norm`` / ``AdamWeightDecayOptimizer.apply_gradients`` and returns
 a ``tf.Operation``, this returns a :class:`TrainOp` whose ``run()`` is one ``session.run(train_op)``:
 forward + backward of ``loss`` (PyTorch autograd -- not our path) followed by exactly ONE launch of
-the sm_100a kernel behind ``include/gaccum.h``.  State (accumulators, adam_m, adam_v, global_step)
+the sm_90a kernel behind ``include/gaccum.h``.  State (accumulators, adam_m, adam_v, global_step)
 lives where the reference keeps it: in variables owned by the graph, here packed HBM slabs.
 
 ``loss`` is the symbolic loss of graph mode: a zero-argument callable that evaluates the loss on
@@ -220,7 +220,7 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
     """
     if use_tpu:
         # optimization.py:67-68 wraps the optimizer in tf.contrib.tpu.CrossShardOptimizer: TPU-only.
-        raise ValueError("use_tpu=True is not supported: this train_op targets B200 GPUs")
+        raise ValueError("use_tpu=True is not supported: this train_op targets H100 GPUs")
     global_step = graph.get_or_create_global_step()
     optimizer = AdamWeightDecayOptimizer(
         learning_rate=bert_learning_rate(init_lr, num_train_steps, num_warmup_steps),

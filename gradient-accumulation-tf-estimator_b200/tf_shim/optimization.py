@@ -114,7 +114,7 @@ def gaccum_train_op(loss, learning_rate, accum_n, variant=0, beta1=0.9, beta2=0.
 def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
     """Creates an optimizer training op (same signature as the reference, optimization.py:25)."""
     if use_tpu:
-        raise ValueError("use_tpu=True is not supported by the B200 train_op")
+        raise ValueError("use_tpu=True is not supported by the H100 train_op")
     global_step = tf.train.get_or_create_global_step()
     # optimization.py:29-54 verbatim semantics (this IS TensorFlow, so the schedule stays in-graph)
     learning_rate = tf.constant(value=init_lr, shape=[], dtype=tf.float32)

@@ -1,4 +1,4 @@
-/* gaccum.h -- C ABI of libgaccum.so: the B200 (sm_100a) gradient-accumulation train_op.
+/* gaccum.h -- C ABI of libgaccum.so: the H100 (sm_90a) gradient-accumulation train_op.
  *
  * This is the drop-in boundary for ONE path of hpandana/gradient-accumulation-tf-estimator:
  * the accumulate-then-apply train_op that `create_optimizer` builds

@@ -11,7 +11,7 @@
  * Structure mirrors the reference's UN-FUSED graph on purpose: one loop per TF op, every
  * intermediate materialised, because this file is also the stopwatch for "the reference's
  * CPU path" (all host cores via OpenMP, as TF's Eigen pool would use).
- * Citations are relative to /root/reference.
+ * Citations are relative to the reference repository's root.
  * Build: see oracle/Makefile (gcc -O2 -ffp-contract=off -fopenmp -shared -fPIC).
  */
 #include <math.h>

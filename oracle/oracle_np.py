@@ -4,12 +4,12 @@ TEST INFRASTRUCTURE ONLY.  Nothing in the shipped package imports this module:
 only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline`` /
 ``--impl reference`` legs may use it, and only as the checker / CPU stopwatch.
 
-PARITY STATUS: the reference (/root/reference, commit 74ae92b8) ships no tests, no
+PARITY STATUS: the reference (hpandana/gradient-accumulation-tf-estimator, commit 74ae92b8) ships no tests, no
 golden vectors and no fixtures, and its arithmetic executes inside TensorFlow 1.14/1.15,
 which is neither vendored nor installable here.  This restatement is therefore pinned in
 two ways only:
   (1) against fixtures produced by executing the reference's *own* ``optimization.py``
-      (imported unmodified from /root/reference) on top of ``oracle/tf_stub`` -- a
+      (imported unmodified from a reference checkout) on top of ``oracle/tf_stub`` -- a
       numpy-backed emulation of the ~40 TF1 graph primitives that file touches -- see
       ``tests/golden/make_golden.py``.  This pins op order, window logic, constants and
       the Python-side double->fp32 conversions of the reference's code; the semantics of
@@ -18,7 +18,7 @@ two ways only:
       **unpinned by a real TensorFlow run**  ("parity unpinned" at the TF-primitive level);
   (2) against hand-derived known-answer vectors (tests/test_oracle_kat.py).
 
-Every function cites the reference line(s) it follows, relative to /root/reference.
+Every function cites the reference line(s) it follows, relative to the reference repository's root.
 One numpy ufunc per TF op, temporaries materialised -- this mirrors the reference's
 un-fused graph and is what ``cpu_baseline`` times (kind="port").
 """

@@ -2,7 +2,7 @@
 ``optimization.py`` touches.  TEST INFRASTRUCTURE ONLY (see oracle/README.md).
 
 Purpose: TensorFlow cannot be installed in this image, so the reference cannot be executed as is.
-With this package first on ``sys.path`` the reference's OWN file (/root/reference/optimization.py,
+With this package first on ``sys.path`` the reference's OWN file (optimization.py of a reference checkout,
 imported unmodified) builds its graph against these primitives, and ``Session.run`` evaluates it in
 IEEE fp32 with one rounding per op.  That pins everything the reference's Python decides -- op
 order, window logic (pre-increment ``global_step % N``), constants, Python double -> fp32

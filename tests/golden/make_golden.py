@@ -1,15 +1,15 @@
 #!/usr/bin/env python
 """Generates tests/golden/ref_optimization_*.npz by EXECUTING THE REFERENCE'S OWN optimization.py.
 
-Runs only in the authoring container (it reads /root/reference, which does not exist on the GPU
-box).  TensorFlow is not installable here, so the reference file is imported unmodified with
+Needs a checkout of hpandana/gradient-accumulation-tf-estimator at commit 74ae92b8, which this
+repository does not contain.  The reference file is imported unmodified, without TensorFlow, with
 oracle/tf_stub first on sys.path (a numpy fp32 emulation of the TF1 primitives it calls; see that
 package's docstring for exactly what this does and does not pin).  For each case we build the
 reference graph with `optimization.create_optimizer(loss, init_lr, num_train_steps,
 num_warmup_steps, use_tpu=False)`, feed seeded gradients for 2*N+2 micro-steps (N = 8, hard-coded
 at optimization.py:76) and record every variable after every `session.run(train_op)`.
 
-    python tests/golden/make_golden.py          # rewrites the fixtures
+    python tests/golden/make_golden.py REFERENCE_CHECKOUT          # rewrites the fixtures
 """
 import importlib
 import json
@@ -20,7 +20,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REFERENCE = "/root/reference"
+REFERENCE = None          # the reference checkout (command-line argument)
 
 # mini-BERT: names drive the decay mask (LayerNorm / layer_norm / bias are excluded, :65)
 VARIABLES = [
@@ -101,8 +101,9 @@ def run_case(name, init_lr, num_train_steps, num_warmup_steps, sigma, seed):
 
 
 if __name__ == "__main__":
-    if not os.path.isdir(REFERENCE):
-        raise SystemExit("make_golden.py needs /root/reference (authoring container only)")
+    if len(sys.argv) != 2 or not os.path.isfile(os.path.join(sys.argv[1], "optimization.py")):
+        raise SystemExit("usage: make_golden.py REFERENCE_CHECKOUT (a checkout of the reference repository)")
+    REFERENCE = os.path.realpath(sys.argv[1])
     meta = {}
     for name, cfg in CASES.items():
         path, steps = run_case(name, *cfg)

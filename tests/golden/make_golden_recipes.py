@@ -1,9 +1,8 @@
 #!/usr/bin/env python
 """Generates tests/golden/ref_recipe_*.npz and the extra ref_optimization_* cases by EXECUTING THE
-REFERENCE'S OWN STATEMENTS, lifted by AST from the files under /root/reference.
-
-Runs only in the authoring container (it reads /root/reference).  TensorFlow is not installable, so the
-lifted statements run against oracle/tf_stub (numpy fp32 emulation; tests/golden/MANIFEST.json lists which
+REFERENCE'S OWN STATEMENTS, lifted by AST from the files of a checkout of the reference repository
+(hpandana/gradient-accumulation-tf-estimator at commit 74ae92b8, not contained in this repository).  The
+lifted statements run without TensorFlow, against oracle/tf_stub (numpy fp32 emulation; tests/golden/MANIFEST.json lists which
 stub primitives are restatements of TensorFlow rather than of the reference).
 
 What is lifted, verbatim (ast nodes selected by line number, compiled, exec'd -- never retyped):
@@ -22,7 +21,7 @@ N=3; nothing else changes.  A third calls the reference's AdamWeightDecayOptimiz
 with a (None, var) pair, the only way the reference's `if grad is None` branch (optimization.py:132-133) can
 execute (through create_optimizer a None gradient raises in assign_add, in TF and in the stub alike).
 
-    python tests/golden/make_golden_recipes.py          # rewrites the fixtures + MANIFEST entries
+    python tests/golden/make_golden_recipes.py REFERENCE_CHECKOUT          # rewrites the fixtures + MANIFEST entries
 """
 import ast
 import importlib
@@ -35,7 +34,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REFERENCE = "/root/reference"
+REFERENCE = None          # the reference checkout (command-line argument)
 SEED0 = 19830610
 
 MNIST = [("conv2d/kernel", (3, 3, 1, 32)), ("conv2d/bias", (32,)), ("dense/kernel", (5408, 64)), ("dense/bias", (64,)),
@@ -238,8 +237,18 @@ def run_optimization_case_full_size(case, N, init_lr, num_train_steps, num_warmu
            "N": N, "steps": steps, "init_lr": init_lr, "num_train_steps": num_train_steps, "num_warmup_steps": num_warmup_steps,
            "sigma": sigma, "seed": seed, "stride": BIG_STRIDE}
 
+    prev = {}
+
     def store(key, arr):
         arr = np.asarray(arr)
+        kind, s, name = key.split("/", 2)
+        # state a micro-step leaves unchanged (p, m, v on an accumulate step) is stored once: `key@same` names the step
+        # that holds it (keeps the fixture under 1 MB)
+        before = prev.get((kind, name))
+        if before is not None and np.array_equal(before[1], arr):
+            out[key + "@same"] = np.int64(before[0])
+            return
+        prev[(kind, name)] = (int(s), arr.copy())
         if arr.size > SUBSAMPLE_ABOVE:
             out[key + "@sub"] = arr.reshape(-1)[::BIG_STRIDE].copy()
             out[key + "@sum"] = np.float64(arr.astype(np.float64).sum())
@@ -299,8 +308,9 @@ def run_direct_apply_with_none(case, lr, sigma, seed, steps):
 
 
 if __name__ == "__main__":
-    if not os.path.isdir(REFERENCE):
-        raise SystemExit("make_golden_recipes.py needs /root/reference (authoring container only)")
+    if len(sys.argv) != 2 or not os.path.isfile(os.path.join(sys.argv[1], "optimization.py")):
+        raise SystemExit("usage: make_golden_recipes.py REFERENCE_CHECKOUT (a checkout of the reference repository)")
+    REFERENCE = os.path.realpath(sys.argv[1])
     meta = {}
     ex02 = "distributedExample/02_single_worker_with_estimator_gaccum.py"
     ex04 = "distributedExample/04_multi_worker_with_estimator_gaccum.py"
@@ -336,7 +346,8 @@ if __name__ == "__main__":
     path, edits = run_optimization_case_full_size("bert_small_n4", 4, 2e-5, 207900, 6, 1e-3, 41, 10)
     meta["fullsize_bert_small_n4"] = {"file": os.path.basename(path), "reference_file": "optimization.py",
                                       "edits": [f"line {ln}: literal {old} -> {new} (AST)" for ln, old, new in edits],
-                                      "shapes": "BERT-Small L4_H512 (T=73, P=28 764 674)", "stored": f"last two micro-steps, every {BIG_STRIDE}th element + fp64 sums",
+                                      "shapes": "BERT-Small L4_H512 (T=73, P=28 764 674)", "stored": f"last two micro-steps, every {BIG_STRIDE}th element + fp64 sums; "
+                                                "state a micro-step leaves unchanged is stored once (key@same names the step holding it)",
                                       "config": [2e-5, 207900, 6, 1e-3, 41, 10]}
     print("wrote", path)
     path = run_direct_apply_with_none("direct_apply_none_grad", 1e-3, 0.3, 33, 3)

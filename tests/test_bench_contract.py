@@ -77,3 +77,59 @@ def test_rotation_phases_give_one_apply_per_window(N):
         applies = (gs[r] % N) == 0
         gs[r] += 1
         assert applies == (i % N == N - 1), (N, R, i)
+
+
+def test_dump_outputs_writes_the_packed_state_sampled_at_fixed_positions(tmp_path, monkeypatch):
+    """dump_outputs on a stand-in op (CPU tensors): one float .npy per array, tensors packed without the slab padding,
+    every array sampled at the same seeded positions, and the whole dump within 64 MB at the real sample size."""
+    import numpy as np
+    import torch
+    sys.path.insert(0, ROOT)
+    import bench
+
+    class Plan:
+        offsets = [0, 32, 64]                       # slab offsets: tensors padded to 32 elements
+    sizes = [5, 20, 7]
+    slab = lambda k: torch.arange(96, dtype=torch.float32) + 1000 * k
+    op = type("Op", (), {"plan": Plan(), "accum": slab(1), "m": slab(2), "v": slab(3),
+                         "stats": lambda self: {"applied": True, "lr": 0.5, "global_norm": 2.0, "clip_scale": 0.25}})()
+    params = [torch.full((n,), float(i)) for i, n in enumerate(sizes)]
+    packed = lambda s: np.concatenate([s.numpy()[o:o + n] for o, n in zip(Plan.offsets, sizes)])
+    want = {"params": np.concatenate([p.numpy() for p in params]), "accum": packed(slab(1)),
+            "adam_m": packed(slab(2)), "adam_v": packed(slab(3))}
+
+    monkeypatch.setattr(bench, "DUMP_SAMPLE", 10)
+    bench.dump_outputs(str(tmp_path / "a"), op, params, None)
+    bench.dump_outputs(str(tmp_path / "b"), op, params, None)
+    files = sorted(os.listdir(tmp_path / "a"))
+    assert files == ["accum.npy", "adam_m.npy", "adam_v.npy", "params.npy", "sample_index.npy", "stats.npy"]
+    idx = np.load(tmp_path / "a" / "sample_index.npy")
+    assert idx.dtype == np.float64 and len(idx) == 10 and np.all(np.diff(idx) > 0) and idx.max() < sum(sizes)
+    for f in files:
+        a, b = np.load(tmp_path / "a" / f), np.load(tmp_path / "b" / f)
+        assert a.dtype in (np.float32, np.float64) and np.array_equal(a, b), f      # same inputs -> same dump
+    for name, full in want.items():
+        assert np.array_equal(np.load(tmp_path / "a" / f"{name}.npy"), full[idx.astype(np.int64)]), name
+    assert np.array_equal(np.load(tmp_path / "a" / "stats.npy"), np.array([1.0, 0.5, 2.0, 0.25], np.float32))
+
+    monkeypatch.setattr(bench, "DUMP_SAMPLE", 1000)                   # fewer elements than the sample: all of them
+    bench.dump_outputs(str(tmp_path / "c"), op, params, None)
+    assert np.array_equal(np.load(tmp_path / "c" / "sample_index.npy"), np.arange(sum(sizes), dtype=np.float64))
+    monkeypatch.undo()
+    assert 4 * 4 * bench.DUMP_SAMPLE + 8 * bench.DUMP_SAMPLE + 16 <= 64 << 20
+
+
+@pytest.mark.gpu
+def test_b200_arm_dumps_what_the_last_timed_step_computed(tmp_path):
+    """--dump-outputs writes the state set the last timed micro-step used: after an apply step its accumulators are
+    all zero (the other sets are mid-window), after an accumulate step they are not; the same arguments give the same dump."""
+    import numpy as np
+    lean = ["--workload", "mnist_cnn", "--warmup", "3", "--model-steps", "0", "--e2e-steps", "0", "--cpu-budget", "0",
+            "--parity-steps", "0"]
+    for K, tag in ((40, "a"), (40, "b"), (42, "c")):
+        _run(lean + ["--steps", str(K), "--dump-outputs", str(tmp_path / tag)])
+    load = lambda tag, name: np.load(tmp_path / tag / f"{name}.npy")
+    for name in ("params", "accum", "adam_m", "adam_v", "sample_index", "stats"):
+        assert np.array_equal(load("a", name), load("b", name)), name
+    assert load("a", "stats")[0] == 1.0 and not load("a", "accum").any()         # step 39 of N=4 applies
+    assert load("c", "stats")[0] == 0.0 and load("c", "accum").any()             # step 41 accumulates

@@ -26,11 +26,14 @@ for it in range(12):
         op.run_bound(b)
 torch.cuda.synchronize()
 op = sets[0][0]
-buf = (C.c_ulonglong * (16 * 148))()
-assert L.gaccum_debug_read(op.plan._h, buf, 16 * 148) == 0
-raw = np.array(buf, dtype=np.float64).reshape(148, 16)
+props = torch.cuda.get_device_properties(dev)
+nsm = props.multi_processor_count      # one clip-apply CTA per SM
+sm_mhz = props.clock_rate / 1000.0     # peak SM clock of the device the kernel ran on
+buf = (C.c_ulonglong * (16 * nsm))()
+assert L.gaccum_debug_read(op.plan._h, buf, 16 * nsm) == 0
+raw = np.array(buf, dtype=np.float64).reshape(nsm, 16)
 t = raw[:, :4].copy()
-cyc = raw[:, 4:16] / 1.965e3       # cycles -> us at 1965 MHz
+cyc = raw[:, 4:16] / sm_mhz        # cycles -> us at the maximum SM clock
 t0 = t[:, 0].min()
 t = (t - t0) / 1e3
 for name, col in (("start", 0), ("pass1 done", 1), ("barrier out", 2), ("pass2 done", 3)):

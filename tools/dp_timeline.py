@@ -29,7 +29,7 @@ for it in range(3 * N):
         dp.run_bound(b)
 torch.cuda.synchronize(); dist.barrier()
 dp = sets[0][0]
-nb = 16 * 148
+nb = 16 * torch.cuda.get_device_properties(dev).multi_processor_count      # the plan's largest grid
 buf = (C.c_ulonglong * (16 * nb))()
 assert L.gaccum_debug_read(dp.plan._h, buf, 16 * nb) == 0
 raw = np.array(buf, dtype=np.float64).reshape(nb, 16)

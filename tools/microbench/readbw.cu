@@ -1,5 +1,5 @@
-// Read-only vs copy HBM bandwidth on B200: what is the roofline of a pass that only READS?
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o readbw readbw.cu
+// Read-only vs copy HBM bandwidth: what is the roofline of a pass that only READS?
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o readbw readbw.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -23,9 +23,10 @@ int main(int argc, char** argv) {
   cudaMalloc(&a, n * 16); cudaMalloc(&b, n * 16); cudaMalloc(&c, n * 16 > ((size_t)512 << 20) ? n * 16 : ((size_t)512 << 20)); cudaMalloc(&out, 4);
   cudaMemset(a, 0, n * 16); cudaMemset(b, 0, n * 16);
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
+  int num_sms = 0; cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, 0);
   for (int mode = 0; mode < 2; ++mode)
     for (int per_sm : {3, 8}) {
-      int grid = 148 * per_sm;
+      int grid = num_sms * per_sm;
       float best = 1e9;
       for (int it = 0; it < 6; ++it) {
         if (n < ((size_t)16 << 20)) cudaMemsetAsync(c, 0, 512u << 20);   // evict a and b from L2 (c is >= 512 MB only when n is large: guard below)
