@@ -58,22 +58,18 @@ struct gaccum_plan {
   int64_t P = 0, padded = 0;
   // device side
   TileDesc* d_tiles = nullptr;
-  double* d_partials = nullptr;
+  double* d_partials = nullptr;            // data-parallel apply: one fp64 norm partial per block
   float* d_stats = nullptr;
   uint32_t* d_dp_sync = nullptr;           // data-parallel kernel: block-completion counters and tile tickets (zero between launches)
   unsigned long long* d_barrier = nullptr; // clip-apply kernel: monotonic arrival counter of the consumers' grid barrier
   LaunchCounters* d_counters = nullptr;    // ... two sets of per-launch counters (tickets, pool length, norm accumulator)
-  bool p1_dynamic = false;                 // ... pass 1 hands out the non-parked tiles by atomic tickets (long passes) or by position (short ones)
-  int stash_tiles = kStashTiles;           // tiles of a' per consumer group parked in shared memory (GACCUM_STASH_TILES: A/B)
 #ifdef GACCUM_EXPERIMENTS
   unsigned long long* d_debug = nullptr;   // per-CTA timestamps (tools/cta_timeline.py; experiments build only)
 #endif
   int num_sms = 0;
   int max_grid = 0;
-  uint32_t flags = 0;  // kFlag* bits; GACCUM_FLAGS selects A/B measurement variants (all compute the same result)
   std::mutex mu;
   std::map<const void*, int> grid_cache;   // kernel -> co-resident grid size
-  int smem_per_sm = 0, smem_optin = 0;
 };
 
 static int build_layout(gaccum_plan* pl) {
@@ -191,8 +187,6 @@ static int launch_apply_clip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream
   const int grid = std::max(1, std::min(pl->num_sms, ((int)pl->tiles.size() + kGroups - 1) / kGroups));
   prm.barrier = pl->d_barrier;
   prm.counters = pl->d_counters;
-  if (pl->p1_dynamic) prm.flags |= kFlagDynamicPass1;
-  prm.stash_tiles = pl->stash_tiles;
   void* args[] = {(void*)&prm};
   CUDA_TRY(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kClipThreads), args, (size_t)kClipSmemBytes, st));
   return GACCUM_OK;
@@ -234,12 +228,10 @@ static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, f
   prm.accum = accum;
   prm.m = m;
   prm.v = v;
-  prm.partials = pl->d_partials;
 #ifdef GACCUM_EXPERIMENTS
   prm.debug = pl->d_debug;
 #endif
   prm.stats = pl->d_stats;
-  prm.flags = pl->flags;
   prm.sc = sc;
 }
 
@@ -267,11 +259,10 @@ struct DeviceGuard {
 
 template <int CAP>
 static int do_accumulate_tab(gaccum_plan* pl, const float* const* grads, float* accum,
-                             const gaccum_step_args* a, cudaStream_t st, uint32_t extra_flags = 0) {
+                             const gaccum_step_args* a, cudaStream_t st) {
   KernelParams<CAP>* prm = new (std::nothrow) KernelParams<CAP>();
   if (!prm) return fail(GACCUM_ENOMEM, "out of host memory");
   fill_common(pl, *prm, accum, nullptr, nullptr, make_scalars(pl->hp, a));
-  prm->flags |= extra_flags;
   int rc = fill_table(pl, prm->tab, grads, nullptr);
   if (rc == GACCUM_OK) rc = launch_accumulate(pl, *prm, st);
   delete prm;
@@ -395,13 +386,6 @@ int gaccum_plan_create(gaccum_plan** out, int32_t T, const int64_t* numels, cons
   if (hp->variant == GACCUM_ADAM_WEIGHT_DECAY && decay) pl->decay.assign(decay, decay + T);
   if (int rc = build_layout(pl)) { delete pl; return rc; }
   pl->device = -1;
-  // GACCUM_STASH_TILES: A/B measurement knob of the clip-apply kernel (how many a' tiles per group are parked in
-  // shared memory); every value computes the same result.  Result-changing timing experiments do not exist in this build.
-  if (const char* t = getenv("GACCUM_STASH_TILES")) pl->stash_tiles = std::max(0, std::min(kStashTiles, atoi(t)));
-  // handing pass 1's non-parked tiles out by tickets keeps every SM busy to the end of the pass (SMs see unequal shares
-  // of HBM bandwidth); GACCUM_P1_DYNAMIC=0 is the A/B knob for the static split
-  pl->p1_dynamic = true;
-  if (const char* t = getenv("GACCUM_P1_DYNAMIC")) pl->p1_dynamic = atoi(t) != 0;
   if (device >= 0) {
     int n = gaccum_device_count();
     if (device >= n) { delete pl; return fail(GACCUM_ENODEVICE, "CUDA device %d requested but %d device(s) visible; libgaccum has no CPU fallback", device, n); }
@@ -411,13 +395,11 @@ int gaccum_plan_create(gaccum_plan** out, int32_t T, const int64_t* numels, cons
     if (e == cudaSuccess && !prop.cooperativeLaunch) e = cudaErrorNotSupported;
     const size_t tb = std::max<size_t>(1, pl->tiles.size()) * sizeof(TileDesc);
     pl->num_sms = prop.multiProcessorCount;
-    pl->smem_per_sm = (int)prop.sharedMemPerMultiprocessor;
-    pl->smem_optin = (int)prop.sharedMemPerBlockOptin;
     pl->max_grid = pl->num_sms * 16;
     if (e == cudaSuccess) e = cudaMalloc(&pl->d_tiles, tb);
     if (e == cudaSuccess && !pl->tiles.empty())
       e = cudaMemcpy(pl->d_tiles, pl->tiles.data(), pl->tiles.size() * sizeof(TileDesc), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&pl->d_partials, sizeof(double) * std::max<size_t>((size_t)pl->max_grid, pl->tiles.size()));   // per CTA (clip-apply) / per tile (data-parallel apply)
+    if (e == cudaSuccess) e = cudaMalloc(&pl->d_partials, sizeof(double) * (size_t)pl->max_grid);
     if (e == cudaSuccess) e = cudaMalloc(&pl->d_dp_sync, sizeof(uint32_t) * 8);
     if (e == cudaSuccess) e = cudaMemset(pl->d_dp_sync, 0, sizeof(uint32_t) * 8);
     if (e == cudaSuccess) e = cudaMalloc(&pl->d_barrier, sizeof(unsigned long long));
@@ -608,7 +590,6 @@ static int do_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float*
   int grid = 0;
   int rc = grid_for(pl, fn, &grid);
   if (rc == GACCUM_OK) {
-    if (const char* t = getenv("GACCUM_DP_BLOCKS_PER_SM")) grid = std::min(grid, std::max(1, atoi(t)) * pl->num_sms);   // A/B knob
     grid = std::max(1, std::min(grid, prm->num_tiles));
     void* args[] = {(void*)prm};
     cudaError_t e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kThreads), args, 0, st);

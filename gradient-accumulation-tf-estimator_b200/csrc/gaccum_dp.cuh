@@ -191,43 +191,24 @@ __device__ __forceinline__ void dp_push_tile(const TileDesc d, const int t, cons
     const int slot = prm.rank < owner ? prm.rank : prm.rank - 1;
     dst = prm.stage[owner] + (size_t)slot * prm.stage_span + (soff - (size_t)prm.shard_base32[owner] * kSlabAlign);
   }
-  const uint32_t len = d.len, tid = threadIdx.x;
   if (mine && g == nullptr) return;                       // nothing to add, nothing to send
-  if (g == nullptr || aligned16(g)) {
-    const uint32_t nvec = len >> 2;
-    const float4* g4 = reinterpret_cast<const float4*>(g);
-    float4* a4 = reinterpret_cast<float4*>(a);
-    float4* d4 = reinterpret_cast<float4*>(dst);
-    float4 va[kUnroll], vg[kUnroll];
-#pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const uint32_t i = u * kThreads + tid;
-      if (i < nvec) { va[u] = __ldcs(a4 + i); if (g) vg[u] = ld_stream(g4 + i); }
-    }
-#pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const uint32_t i = u * kThreads + tid;
-      if (i < nvec) {
-        if (g) {
-          va[u].x = __fadd_rn(va[u].x, vg[u].x); va[u].y = __fadd_rn(va[u].y, vg[u].y);
-          va[u].z = __fadd_rn(va[u].z, vg[u].z); va[u].w = __fadd_rn(va[u].w, vg[u].w);
-        }
-        if (mine) st_policy(a4 + i, va[u], pol);
-        else { d4[i] = va[u]; __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f)); }
-      }
-    }
-    const uint32_t i = (nvec << 2) + tid;
-    if (i < len) {
-      float x = a[i];
-      if (g) x = __fadd_rn(x, ld_stream(g + i));
-      if (mine) a[i] = x; else { dst[i] = x; a[i] = 0.f; }
-    }
-  } else {
-    for (uint32_t i = tid; i < len; i += kThreads) {
-      const float x = __fadd_rn(a[i], ld_stream(g + i));
-      if (mine) a[i] = x; else { dst[i] = x; a[i] = 0.f; }
-    }
-  }
+  const float4* g4 = reinterpret_cast<const float4*>(g);
+  float4* a4 = reinterpret_cast<float4*>(a);
+  float4* d4 = reinterpret_cast<float4*>(dst);
+  float4 va[kUnroll], vg[kUnroll];
+  walk_tile(d.len, (g == nullptr || aligned16(g)) ? d.len >> 2 : 0u, threadIdx.x,
+            [&](int u, uint32_t i) { va[u] = __ldcs(a4 + i); if (g) vg[u] = ld_stream(g4 + i); },
+            [] {},
+            [&](int u, uint32_t i) {
+              if (g) va[u] = add_rn(va[u], vg[u]);
+              if (mine) st_policy(a4 + i, va[u], pol);
+              else { d4[i] = va[u]; __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f)); }
+            },
+            [&](uint32_t i) {
+              float x = a[i];
+              if (g) x = __fadd_rn(x, ld_stream(g + i));
+              if (mine) a[i] = x; else { dst[i] = x; a[i] = 0.f; }
+            });
 }
 
 // ---- phase B: one owned tile.  a' = sum_w contribution_w in rank order; returns sum((a'/N)^2) ----
@@ -238,48 +219,41 @@ __device__ __forceinline__ float dp_reduce_tile(const TileDesc d, const DpParams
   float* __restrict__ a = prm.accum + soff;
   const float* __restrict__ stg = prm.stage[prm.rank] + rel;
   const int64_t span = prm.stage_span;
-  const uint32_t len = d.len, tid = threadIdx.x, nvec = len >> 2;
-  const float nf = prm.sc.nf, inv_nf = prm.sc.inv_nf;
   const int W = prm.world, R = prm.rank;
   float acc = 0.f;
   float4* a4 = reinterpret_cast<float4*>(a);
+  // one vector at a time, loads to store: the kernel is capped at 64 registers, and the rank loops of both vectors
+  // at once (or an unrolled tail) would spill more
+  walk_tile(d.len, d.len >> 2, threadIdx.x,
+            [](int, uint32_t) {},
+            [] {},
+            [&](int, uint32_t i) {
+              float4 part[kMaxRanks];
 #pragma unroll
-  for (int u = 0; u < kUnroll; ++u) {
-    const uint32_t i = u * kThreads + tid;
-    if (i < nvec) {
-      float4 part[kMaxRanks];
+              for (int w = 0; w < kMaxRanks; ++w) {
+                if (w < W) {
+                  // contributions arrived from other SMs / other GPUs during this kernel: read them at L2
+                  const float4* src = (w == R) ? (a4 + i) : reinterpret_cast<const float4*>(stg + (size_t)(w < R ? w : w - 1) * span) + i;
+                  part[w] = __ldcg(src);
+                }
+              }
+              float4 s = part[0];
 #pragma unroll
-      for (int w = 0; w < kMaxRanks; ++w) {
-        if (w < W) {
-          // contributions arrived from other SMs / other GPUs during this kernel: read them at L2
-          const float4* src = (w == R) ? (a4 + i) : reinterpret_cast<const float4*>(stg + (size_t)(w < R ? w : w - 1) * span) + i;
-          part[w] = __ldcg(src);
-        }
-      }
-      float4 s = part[0];
-#pragma unroll
-      for (int w = 1; w < kMaxRanks; ++w) {
-        if (w < W) {
-          s.x = __fadd_rn(s.x, part[w].x); s.y = __fadd_rn(s.y, part[w].y);
-          s.z = __fadd_rn(s.z, part[w].z); s.w = __fadd_rn(s.w, part[w].w);
-        }
-      }
-      st_policy(a4 + i, s, pol);
-      const float nx = normalize(s.x, nf, inv_nf), ny = normalize(s.y, nf, inv_nf), nz = normalize(s.z, nf, inv_nf), nw = normalize(s.w, nf, inv_nf);
-      acc = fmaf(nx, nx, acc); acc = fmaf(ny, ny, acc); acc = fmaf(nz, nz, acc); acc = fmaf(nw, nw, acc);
-    }
-  }
-  const uint32_t i = (nvec << 2) + tid;
-  if (i < len) {
-    float s = 0.f;
-    for (int w = 0; w < W; ++w) {
-      const float x = __ldcg((w == R) ? (a + i) : (stg + (size_t)(w < R ? w : w - 1) * span + i));
-      s = (w == 0) ? x : __fadd_rn(s, x);
-    }
-    a[i] = s;
-    const float n = normalize(s, nf, inv_nf);
-    acc = fmaf(n, n, acc);
-  }
+              for (int w = 1; w < kMaxRanks; ++w)
+                if (w < W) s = add_rn(s, part[w]);
+              st_policy(a4 + i, s, pol);
+              acc = add_sq(acc, s, prm.sc);
+            },
+            [&](uint32_t i) {
+              float x = 0.f;
+#pragma unroll 1
+              for (int w = 0; w < W; ++w) {
+                const float c = __ldcg((w == R) ? (a + i) : (stg + (size_t)(w < R ? w : w - 1) * span + i));
+                x = (w == 0) ? c : __fadd_rn(x, c);
+              }
+              a[i] = x;
+              acc = add_sq(acc, x, prm.sc);
+            });
   return acc;
 }
 
@@ -292,43 +266,48 @@ __device__ __forceinline__ void dp_update_tile(const TileDesc d, const DpParams<
   float* __restrict__ v = prm.v + soff;
   const float* __restrict__ p = prm.param[prm.rank] + soff;
   const bool decay = (d.tensor_flags >> 31) != 0;
-  const uint32_t len = d.len, tid = threadIdx.x, nvec = len >> 2;
   const Scalars& sc = prm.sc;
+  const bool scaled = sc.clip > 0.f;
   const int W = prm.world;
-  auto elem = [&](float ax, float& px, float& mx, float& vx) {
-    const float c = sc.clip > 0.f ? __fmul_rn(normalize(ax, sc.nf, sc.inv_nf), s) : normalize(ax, sc.nf, sc.inv_nf);
-    adam_elem<VARIANT>(c, px, mx, vx, decay, sc);
-  };
   float4* a4 = reinterpret_cast<float4*>(a);
   float4* m4 = reinterpret_cast<float4*>(m);
   float4* v4 = reinterpret_cast<float4*>(v);
   const float4* p4 = reinterpret_cast<const float4*>(p);
   float4 va[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll];
+  walk_tile(d.len, d.len >> 2, threadIdx.x,
+            [&](int u, uint32_t i) { va[u] = __ldcg(a4 + i); vp[u] = __ldcs(p4 + i); vm[u] = __ldcs(m4 + i); vv[u] = __ldcs(v4 + i); },
+            [] {},
+            [&](int u, uint32_t i) {
+              update_vec<VARIANT>(va[u], scaled, s, vp[u], vm[u], vv[u], decay, sc);
+              __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
+              __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));
 #pragma unroll
-  for (int u = 0; u < kUnroll; ++u) {
-    const uint32_t i = u * kThreads + tid;
-    if (i < nvec) { va[u] = __ldcg(a4 + i); vp[u] = __ldcs(p4 + i); vm[u] = __ldcs(m4 + i); vv[u] = __ldcs(v4 + i); }
-  }
+              for (int w = 0; w < kMaxRanks; ++w)      // all-gather: peer stores over NVLink (and the local copy)
+                if (w < W) *(reinterpret_cast<float4*>(prm.param[w] + soff) + i) = vp[u];
+            },
+            [&](uint32_t i) {
+              float px = p[i], mx = m[i], vx = v[i];
+              update_elem<VARIANT>(__ldcg(a + i), scaled, s, px, mx, vx, decay, sc);
+              m[i] = mx; v[i] = vx; a[i] = 0.f;
+              for (int w = 0; w < W; ++w) prm.param[w][soff + i] = px;
+            });
+}
+
+// Deterministic CTA reduction of one double per thread -> total in thread 0.  Threads add each
+// tile's 8-element fp32 partial into an fp64 running sum, so the norm of a 335 M-element model is
+// good to ~1e-7 relative even for adversarial (constant) data.
+__device__ __forceinline__ double block_reduce_to_double(double x, double* smem /* blockDim.x/32 */) {
 #pragma unroll
-  for (int u = 0; u < kUnroll; ++u) {
-    const uint32_t i = u * kThreads + tid;
-    if (i < nvec) {
-      elem(va[u].x, vp[u].x, vm[u].x, vv[u].x); elem(va[u].y, vp[u].y, vm[u].y, vv[u].y);
-      elem(va[u].z, vp[u].z, vm[u].z, vv[u].z); elem(va[u].w, vp[u].w, vm[u].w, vv[u].w);
-      __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
-      __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));
-#pragma unroll
-      for (int w = 0; w < kMaxRanks; ++w)      // all-gather: peer stores over NVLink (and the local copy)
-        if (w < W) *(reinterpret_cast<float4*>(prm.param[w] + soff) + i) = vp[u];
-    }
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) smem[warp] = x;
+  __syncthreads();
+  double tot = 0.0;
+  if (threadIdx.x == 0) {
+    const int nw = ((int)blockDim.x + 31) >> 5;
+    for (int w = 0; w < nw; ++w) tot += smem[w];
   }
-  const uint32_t i = (nvec << 2) + tid;
-  if (i < len) {
-    float px = p[i], mx = m[i], vx = v[i];
-    elem(__ldcg(a + i), px, mx, vx);
-    m[i] = mx; v[i] = vx; a[i] = 0.f;
-    for (int w = 0; w < W; ++w) prm.param[w][soff + i] = px;
-  }
+  return tot;
 }
 
 template <int VARIANT, int CAP>

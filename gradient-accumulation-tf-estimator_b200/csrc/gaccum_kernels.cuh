@@ -9,20 +9,8 @@
 //                        clip_norm <= 0): a' = a + G; n = a'/N; Adam; a = 0 in a single pass (36 B/elem).
 //   apply_clip_kernel    the apply branch WITH tf.clip_by_global_norm                  (36 B/elem)
 //                        optimization.py:80-88, 128-177.  The global norm of ALL tensors is needed before
-//                        ANY element can be updated, so it is one cooperative launch, one CTA per SM, with
-//                        two passes around a grid barrier:
-//                          pass 1  PRODUCER WARPS stream G into shared-memory tile slots with TMA bulk
-//                                  copies (cp.async.bulk + mbarrier complete_tx; descriptors and L2
-//                                  prefetches of a run ahead), three 256-thread CONSUMER GROUPS load a,
-//                                  take G out of the slots, a' = a + G, reduce sum((a'/N)^2)
-//                                  (thread fp32 per tile -> fp64 running sum -> warp shuffle -> shared
-//                                  memory -> one fp64 partial per CTA); a' of the first tiles is PARKED
-//                                  ON CHIP in a shared-memory stash beside the ring, the rest written
-//                                  back in place tagged L2::evict_last
-//                          barrier every CTA adds the per-CTA partials in the same order
-//                                  (bit-identical gn and clip scale everywhere)
-//                          pass 2  the stashed tiles, then the L2-resident tiles youngest first:
-//                                  clip, AdamWeightDecay/Adam, write p, m, v, a = 0
+//                        ANY element can be updated: one cooperative launch, two passes around a grid
+//                        barrier (described at the kernel).
 // Arithmetic uses round-to-nearest intrinsics (__fmul_rn, __fadd_rn, __fdiv_rn, __fsqrt_rn) so nvcc
 // cannot contract mul+add into FMA: the reference graph is un-fused, one rounding per TF op, and we
 // reproduce it bit for bit (the kernels are HBM-bound, the extra flops are free).
@@ -83,21 +71,15 @@ struct KernelParams {
   float* accum;
   float* m;
   float* v;
-  double* partials;   // one per CTA (apply with clip)
   float* stats;       // gaccum_stats
-  uint32_t flags;     // kFlag* bits (all of them produce correct results)
   unsigned long long* barrier;  // apply_clip_kernel: monotonic arrival counter of the consumers' grid barrier
   struct LaunchCounters* counters;  // apply_clip_kernel: two sets of per-launch counters (tickets, pool length, norm accumulator)
-  int32_t stash_tiles;  // apply_clip_kernel: tiles of a' each consumer group parks in shared memory (0..kStashTiles)
 #ifdef GACCUM_EXPERIMENTS
   unsigned long long* debug;  // 16 words per CTA: 4 timestamps (ns) + wait-cycle counters (tools/cta_timeline.py)
 #endif
   Scalars sc;
   PtrTable<CAP> tab;
 };
-
-constexpr uint32_t kFlagAssign = 1u;        // accumulate_kernel stores G instead of adding it
-constexpr uint32_t kFlagDynamicPass1 = 2u;  // apply_clip_kernel: pass 1 hands the non-parked tiles out by atomic tickets instead of by position
 
 // ---------------------------------------------------------------------------------------------
 // memory helpers: G is read exactly once -> streaming (evict-first) loads; zeroing the
@@ -178,6 +160,36 @@ __device__ __forceinline__ void adam_elem(float c, float& p, float& m, float& v,
   }
 }
 
+// optimization.py:83-85: c = a/N, times the clip scale s if `scaled` (never a multiply by 1: it could change a NaN's
+// payload), then one Adam step of p, m, v
+template <int VARIANT>
+__device__ __forceinline__ void update_elem(float a, bool scaled, float s, float& p, float& m, float& v, bool decay,
+                                            const Scalars& sc) {
+  float c = normalize(a, sc.nf, sc.inv_nf);
+  if (scaled) c = __fmul_rn(c, s);
+  adam_elem<VARIANT>(c, p, m, v, decay, sc);
+}
+template <int VARIANT>
+__device__ __forceinline__ void update_vec(const float4 a, bool scaled, float s, float4& p, float4& m, float4& v, bool decay,
+                                           const Scalars& sc) {
+  update_elem<VARIANT>(a.x, scaled, s, p.x, m.x, v.x, decay, sc);
+  update_elem<VARIANT>(a.y, scaled, s, p.y, m.y, v.y, decay, sc);
+  update_elem<VARIANT>(a.z, scaled, s, p.z, m.z, v.z, decay, sc);
+  update_elem<VARIANT>(a.w, scaled, s, p.w, m.w, v.w, decay, sc);
+}
+
+__device__ __forceinline__ float4 add_rn(const float4 a, const float4 b) {
+  return make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w));
+}
+// acc + (x/N)^2: one element of a thread's fp32 partial of the global norm
+__device__ __forceinline__ float add_sq(float acc, float x, const Scalars& sc) {
+  const float n = normalize(x, sc.nf, sc.inv_nf);
+  return fmaf(n, n, acc);
+}
+__device__ __forceinline__ float add_sq(float acc, const float4 x, const Scalars& sc) {
+  return add_sq(add_sq(add_sq(add_sq(acc, x.x, sc), x.y, sc), x.z, sc), x.w, sc);
+}
+
 // tf.clip_by_global_norm (TF 1.15): scale = clip * min(1/gn, 1/clip) + (gn - gn)
 __device__ __forceinline__ float clip_scale(float gn, float clip) {
   const float inv = __fdiv_rn(1.0f, gn);
@@ -188,6 +200,29 @@ __device__ __forceinline__ float clip_scale(float gn, float clip) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// One tile as every per-tile function walks it: thread `tid` owns the float4 vectors tid and tid + kThreads that are
+// below `nvec`, then at most one of the < 4 trailing elements.  nvec == 0 means the tile cannot take the vector path
+// (a view that is not 16-byte aligned, or fewer than 4 elements): `elem` then covers the whole tile, kThreads apart.
+// All of a thread's vector loads are issued before its first store; `loaded` runs between the two.
+// ---------------------------------------------------------------------------------------------
+template <typename Load, typename Loaded, typename Vec, typename Elem>
+__device__ __forceinline__ void walk_tile(const uint32_t len, const uint32_t nvec, const uint32_t tid, Load&& load,
+                                          Loaded&& loaded, Vec&& vec, Elem&& elem) {
+#pragma unroll
+  for (int u = 0; u < kUnroll; ++u) {
+    const uint32_t i = u * kThreads + tid;
+    if (i < nvec) load(u, i);
+  }
+  loaded();
+#pragma unroll
+  for (int u = 0; u < kUnroll; ++u) {
+    const uint32_t i = u * kThreads + tid;
+    if (i < nvec) vec(u, i);
+  }
+  for (uint32_t i = (nvec << 2) + tid; i < len; i += kThreads) elem(i);
+}
+
+// ---------------------------------------------------------------------------------------------
 // accumulate: a += G                                                   optimization.py:81,93
 // ---------------------------------------------------------------------------------------------
 template <int CAP>
@@ -195,54 +230,23 @@ __device__ __forceinline__ void accumulate_tile(const TileDesc d, const KernelPa
   const float* __restrict__ g = grad_ptr(prm.tab, d);
   if (g == nullptr) return;   // optimization.py:132 -- tensors without a gradient are skipped
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
-  const uint32_t len = d.len, tid = threadIdx.x;
-  if (prm.flags & kFlagAssign) {              // gather: a = G (G may live in pinned host memory)
-    for (uint32_t i = tid; i < len; i += kThreads) a[i] = ld_stream(g + i);
-    return;
-  }
-  if (aligned16(g)) {
-    const uint32_t nvec = len >> 2;
-    const float4* g4 = reinterpret_cast<const float4*>(g);
-    float4* a4 = reinterpret_cast<float4*>(a);
-    float4 vg[kUnroll], va[kUnroll];
-#pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const uint32_t i = u * kThreads + tid;
-      if (i < nvec) { vg[u] = ld_stream(g4 + i); va[u] = a4[i]; }
-    }
-#pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const uint32_t i = u * kThreads + tid;
-      if (i < nvec) {
-        va[u].x = __fadd_rn(va[u].x, vg[u].x); va[u].y = __fadd_rn(va[u].y, vg[u].y);
-        va[u].z = __fadd_rn(va[u].z, vg[u].z); va[u].w = __fadd_rn(va[u].w, vg[u].w);
-        a4[i] = va[u];
-      }
-    }
-    const uint32_t i = (nvec << 2) + tid;      // < 4 trailing elements
-    if (i < len) a[i] = __fadd_rn(a[i], ld_stream(g + i));
-  } else {
-    for (uint32_t i = tid; i < len; i += kThreads) a[i] = __fadd_rn(a[i], ld_stream(g + i));
-  }
+  const float4* g4 = reinterpret_cast<const float4*>(g);
+  float4* a4 = reinterpret_cast<float4*>(a);
+  float4 vg[kUnroll], va[kUnroll];
+  walk_tile(d.len, aligned16(g) ? d.len >> 2 : 0u, threadIdx.x,
+            [&](int u, uint32_t i) { vg[u] = ld_stream(g4 + i); va[u] = a4[i]; },
+            [] {},
+            [&](int u, uint32_t i) { a4[i] = add_rn(va[u], vg[u]); },
+            [&](uint32_t i) { a[i] = __fadd_rn(a[i], ld_stream(g + i)); });
 }
 
 template <int CAP>
 __global__ void __launch_bounds__(kThreads)
 accumulate_kernel(const __grid_constant__ KernelParams<CAP> prm) {
-  int t = blockIdx.x;
-  if (blockIdx.x == 0 && threadIdx.x == 0 && !(prm.flags & kFlagAssign)) {   // the gather pass is not a step
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
     prm.stats[0] = 0.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f;
   }
-  if (t >= prm.num_tiles) return;
-  TileDesc d = prm.tiles[t];
-  while (true) {
-    const int tn = t + gridDim.x;
-    TileDesc dn;
-    if (tn < prm.num_tiles) dn = prm.tiles[tn];   // prefetch the next descriptor
-    accumulate_tile(d, prm);
-    if (tn >= prm.num_tiles) break;
-    t = tn; d = dn;
-  }
+  if ((int)blockIdx.x < prm.num_tiles) accumulate_tile(prm.tiles[blockIdx.x], prm);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -258,96 +262,41 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
   float* __restrict__ v = prm.v + soff;
   float* __restrict__ p = param_ptr(prm.tab, d);
   const bool decay = (d.tensor_flags >> 31) != 0;
-  const uint32_t len = d.len, tid = threadIdx.x;
   const Scalars& sc = prm.sc;
-
-  // no gradient for this tile: a + 0 would turn -0 into +0 only; the add is skipped entirely
-  auto elem = [&](float ax, float gx, bool has_g, float& px, float& mx, float& vx) {
-    if (has_g) ax = __fadd_rn(ax, gx);                            // optimization.py:81
-    const float c = normalize(ax, sc.nf, sc.inv_nf);              // :83
-    adam_elem<VARIANT>(c, px, mx, vx, decay, sc);                 // :85
-  };
-
-  if (aligned16(p) && (g == nullptr || aligned16(g))) {
-    const uint32_t nvec = len >> 2;
-    const float4* g4 = reinterpret_cast<const float4*>(g);
-    float4* a4 = reinterpret_cast<float4*>(a);
-    float4* m4 = reinterpret_cast<float4*>(m);
-    float4* v4 = reinterpret_cast<float4*>(v);
-    float4* p4 = reinterpret_cast<float4*>(p);
-    float4 va[kUnroll], vg[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll];
-#pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const uint32_t i = u * kThreads + tid;
-      if (i < nvec) {
-        va[u] = __ldcs(a4 + i); vp[u] = __ldcs(p4 + i); vm[u] = __ldcs(m4 + i); vv[u] = __ldcs(v4 + i);
-        if (LOAD_G && g) vg[u] = ld_stream(g4 + i);
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const uint32_t i = u * kThreads + tid;
-      if (i < nvec) {
-        const bool hg = LOAD_G && g;
-        elem(va[u].x, vg[u].x, hg, vp[u].x, vm[u].x, vv[u].x); elem(va[u].y, vg[u].y, hg, vp[u].y, vm[u].y, vv[u].y);
-        elem(va[u].z, vg[u].z, hg, vp[u].z, vm[u].z, vv[u].z); elem(va[u].w, vg[u].w, hg, vp[u].w, vm[u].w, vv[u].w);
-        __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
-        __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
-      }
-    }
-    const uint32_t i = (nvec << 2) + tid;
-    if (i < len) {
-      float px = p[i], mx = m[i], vx = v[i];
-      const bool hg = LOAD_G && g;
-      elem(a[i], hg ? ld_stream(g + i) : 0.f, hg, px, mx, vx);
-      p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
-    }
-  } else {
-    for (uint32_t i = tid; i < len; i += kThreads) {
-      float px = p[i], mx = m[i], vx = v[i];
-      const bool hg = LOAD_G && g;
-      elem(a[i], hg ? ld_stream(g + i) : 0.f, hg, px, mx, vx);
-      p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
-    }
-  }
+  const float4* g4 = reinterpret_cast<const float4*>(g);
+  float4* a4 = reinterpret_cast<float4*>(a);
+  float4* m4 = reinterpret_cast<float4*>(m);
+  float4* v4 = reinterpret_cast<float4*>(v);
+  float4* p4 = reinterpret_cast<float4*>(p);
+  float4 va[kUnroll], vg[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll];
+  // no gradient for this tile: a + 0 would turn -0 into +0 only; the add is skipped entirely (optimization.py:81)
+  walk_tile(d.len, aligned16(p) && (g == nullptr || aligned16(g)) ? d.len >> 2 : 0u, threadIdx.x,
+            [&](int u, uint32_t i) {
+              va[u] = __ldcs(a4 + i); vp[u] = __ldcs(p4 + i); vm[u] = __ldcs(m4 + i); vv[u] = __ldcs(v4 + i);
+              if (LOAD_G && g) vg[u] = ld_stream(g4 + i);
+            },
+            [] {},
+            [&](int u, uint32_t i) {
+              if (LOAD_G && g) va[u] = add_rn(va[u], vg[u]);
+              update_vec<VARIANT>(va[u], false, 0.f, vp[u], vm[u], vv[u], decay, sc);
+              __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
+              __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
+            },
+            [&](uint32_t i) {
+              float ax = a[i], px = p[i], mx = m[i], vx = v[i];
+              if (LOAD_G && g) ax = __fadd_rn(ax, ld_stream(g + i));
+              update_elem<VARIANT>(ax, false, 0.f, px, mx, vx, decay, sc);
+              p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
+            });
 }
 
 template <int VARIANT, bool HAS_G, int CAP>
 __global__ void __launch_bounds__(kThreads)
 apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
-  const int nt = prm.num_tiles;
-  int t = blockIdx.x;
-  if (t < nt) {
-    TileDesc d = prm.tiles[t];
-    while (true) {
-      const int tn = t + gridDim.x;
-      TileDesc dn;
-      if (tn < nt) dn = prm.tiles[tn];
-      update_tile<VARIANT, HAS_G>(d, prm);
-      if (tn >= nt) break;
-      t = tn; d = dn;
-    }
-  }
+  if ((int)blockIdx.x < prm.num_tiles) update_tile<VARIANT, HAS_G>(prm.tiles[blockIdx.x], prm);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f;
   }
-}
-
-// Deterministic CTA reduction of one double per thread -> total in thread 0.  Threads add each
-// tile's 8-element fp32 partial into an fp64 running sum, so the norm of a 335 M-element model is
-// good to ~1e-7 relative even for adversarial (constant) data.
-__device__ __forceinline__ double block_reduce_to_double(double x, double* smem /* blockDim.x/32 */) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) smem[warp] = x;
-  __syncthreads();
-  double tot = 0.0;
-  if (threadIdx.x == 0) {
-    const int nw = ((int)blockDim.x + 31) >> 5;
-    for (int w = 0; w < nw; ++w) tot += smem[w];
-  }
-  return tot;
 }
 
 // =============================================================================================
@@ -366,18 +315,19 @@ __device__ __forceinline__ double block_reduce_to_double(double x, double* smem 
 // of it than others, so the producers draw tiles from global atomic ticket counters -- every SM stays busy until
 // the pass is over.
 //
-// pass 1   tickets over ALL tiles.  ring slot = [G tile | a tile] (16 KB, kP1Slots per group).  a' = a + G;
+// pass 1   the group's own tiles (the first kStashTiles of b, b + G, ... for group b of G) by position, then tickets
+//          over all other tiles.  ring slot = [G tile | a tile] (16 KB, kP1Slots per group).  a' = a + G;
 //          sum((a'/N)^2): thread fp32 per tile -> warp shuffle in fp64 (fixed order) -> EXACT accumulation of the
 //          per-warp, per-tile sums in a 2176-bit fixed-point accumulator (integer atomics: associative, so the
 //          total does not depend on which SM reduced which tile -- the norm is bit-identical from run to run
-//          and across replicas although the schedule is dynamic).  a' of the first kStashTiles tiles a group
-//          processes is parked in the group's shared-memory stash (the part of the SM's 227 KB the ring leaves
-//          free); every other a' goes back in place tagged L2::evict_last.
+//          and across replicas although the schedule is dynamic).  a' of the group's own tiles is parked in the
+//          group's shared-memory stash (the part of the SM's 227 KB the ring leaves free); every other a' goes
+//          back in place tagged L2::evict_last.
 // barrier  only the CONSUMERS rendezvous (named barrier + one atomic per CTA).  The producers do not: p, m, v do
 //          not depend on the clip scale, so they start streaming the group's own stashed tiles into the
 //          ring as soon as pass 1 is drained -- HBM stays busy while the CTAs wait for each other.
 // pass 2   ring slot = [p | m | v | a'] (32 KB).  First the group's own stashed tiles, then tickets over
-//          all tiles, youngest first (a' still in L2), skipping the parked ones: clip, AdamWeightDecay/Adam,
+//          all other tiles, youngest first (a' still in L2): clip, AdamWeightDecay/Adam,
 //          STG p, m, v, a = 0.
 // Tiles that bulk copies cannot move (gradient / parameter pointer not 16-byte aligned, or shorter than one
 // float4) go through the same full/empty protocol with nothing copied and are loaded by the consumers with
@@ -388,31 +338,26 @@ __device__ __forceinline__ double block_reduce_to_double(double x, double* smem 
 constexpr int kGroups = 3;                        // consumer groups per CTA
 constexpr int kConsumerThreads = kThreads * kGroups;        // 768
 constexpr int kClipThreads = kConsumerThreads + 32 * kGroups;   // + one producer warp per group = 864
-#ifndef GACCUM_P1_SLOTS
-#define GACCUM_P1_SLOTS 2
-#endif
-constexpr int kP1Slots = GACCUM_P1_SLOTS;         // pass-1 ring slots per group, 16 KB each
+constexpr int kP1Slots = 2;                       // pass-1 ring slots per group, 16 KB each
 constexpr int kP1SlotVecs = 2 * (kTile / 4);      // float4 per pass-1 slot: G | a
 constexpr int kP2SlotVecs = 4 * (kTile / 4);      // float4 per pass-2 slot: p | m | v | a'
 constexpr int kRingVecs = kP1Slots * kP1SlotVecs; // per group
 constexpr int kP2Slots = kRingVecs / kP2SlotVecs; // 2 x 16 KB = 32 KB -> 1 x 32 KB
 constexpr int kRingBytes = kGroups * kRingVecs * 16;   // 96 KB
-static_assert(kP2Slots >= 1 && kP1Slots <= 8, "ring must hold at least one [p|m|v|a'] slot");
+static_assert(kP2Slots >= 1, "ring must hold at least one [p|m|v|a'] slot");
 // the stash: kStashTiles tiles of a' per group (8 KB each) in the shared memory the ring and the static arrays
 // (~16 KB) leave free of the 227 KB a block may have on sm_90
 constexpr int kStashTiles = 4;
+static_assert(kStashTiles <= 32, "the producer loads the descriptors of a group's own tiles one per lane");
 constexpr uint32_t kNoStash = 0xffffffffu;
 constexpr int kStashVecs = kStashTiles * (kTile / 4);          // float4 per group
 constexpr int kClipSmemBytes = kRingBytes + kGroups * kStashVecs * 16;   // dynamic shared memory of the kernel (192 KB)
 static_assert(kClipSmemBytes + 20 * 1024 <= 227 * 1024, "ring + stash + static shared memory must fit one sm_90 block");
-constexpr int kMaxSlots = 8;
 constexpr int kTicketBatch = 4;                   // pass-1 tickets a producer draws at once while plenty of tiles are left
 // what the producer tells the consumers about the tile it put into a slot
 struct __align__(16) SlotMeta {
   TileDesc d;          // len == 0: end of the pass
-  uint32_t tile;       // index into the tile table
   uint32_t stash_slot; // pass 2: a' is parked in this stash slot of the group (kNoStash: it is in the slot's 4th quarter / in global memory)
-  uint32_t pad[2];
 };
 // exact accumulation of non-negative doubles: 68 bins of 32 payload bits in 64-bit containers cover the whole
 // binary64 range (2^-1074 .. 2^1024); a container overflows only after 2^31 additions
@@ -535,59 +480,32 @@ __device__ __forceinline__ double acc_value(const unsigned long long* bins /* kA
 }
 
 // ---- pass 1, consumer side: one tile out of slot [G | a]; returns this THREAD's partial of sum((a'/N)^2) ----
+// A tile the producer did not copy (nvec == 0), and the < 4 tail elements of any tile, travel through global memory.
 template <bool HAS_G, int CAP>
 __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float4* slot, uint64_t* empty,
                                            float4* const stash, const uint64_t pol) {
   const float* __restrict__ g = nullptr;
   if constexpr (HAS_G) g = grad_ptr(prm.tab, d);
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
-  const uint32_t len = d.len, tid = threadIdx.x & (kThreads - 1);
-  const float nf = prm.sc.nf, inv_nf = prm.sc.inv_nf;
-  const uint32_t nvec = bulk_vecs(d, g);
+  float4* a4 = reinterpret_cast<float4*>(a);
   float acc = 0.f;
-  if (nvec > 0) {
-    float4* a4 = reinterpret_cast<float4*>(a);
-    float4 x[kUnroll], gg[kUnroll];
-#pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const uint32_t i = u * kThreads + tid;
-      if (i < nvec) { x[u] = slot[kTile / 4 + i]; if (g) gg[u] = slot[i]; }
-    }
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(empty);        // this warp is done with the slot
-#pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const uint32_t i = u * kThreads + tid;
-      if (i < nvec) {
-        if (g) {
-          x[u].x = __fadd_rn(x[u].x, gg[u].x); x[u].y = __fadd_rn(x[u].y, gg[u].y);
-          x[u].z = __fadd_rn(x[u].z, gg[u].z); x[u].w = __fadd_rn(x[u].w, gg[u].w);
-          if (stash == nullptr) st_policy(a4 + i, x[u], pol);
-        }
-        if (stash != nullptr) stash[i] = x[u];
-        const float nx = normalize(x[u].x, nf, inv_nf), ny = normalize(x[u].y, nf, inv_nf),
-                    nz = normalize(x[u].z, nf, inv_nf), nw = normalize(x[u].w, nf, inv_nf);
-        acc = fmaf(nx, nx, acc); acc = fmaf(ny, ny, acc); acc = fmaf(nz, nz, acc); acc = fmaf(nw, nw, acc);
-      }
-    }
-    const uint32_t i = (nvec << 2) + tid;      // < 4 tail elements always travel through global memory
-    if (i < len) {
-      float xs = a[i];
-      if (g) { xs = __fadd_rn(xs, ld_stream(g + i)); a[i] = xs; }
-      const float n = normalize(xs, nf, inv_nf);
-      acc = fmaf(n, n, acc);
-    }
-  } else {
-    // unaligned gradient view, or a tile shorter than one float4: nothing was copied
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(empty);
-    for (uint32_t i = tid; i < len; i += kThreads) {
-      float xs = a[i];
-      if (g) { xs = __fadd_rn(xs, ld_stream(g + i)); a[i] = xs; }
-      const float n = normalize(xs, nf, inv_nf);
-      acc = fmaf(n, n, acc);
-    }
-  }
+  float4 x[kUnroll], gg[kUnroll];
+  walk_tile(d.len, bulk_vecs(d, g), threadIdx.x & (kThreads - 1),
+            [&](int u, uint32_t i) { x[u] = slot[kTile / 4 + i]; if (g) gg[u] = slot[i]; },
+            [&] { __syncwarp(); if ((threadIdx.x & 31) == 0) mbar_arrive(empty); },   // this warp is done with the slot
+            [&](int u, uint32_t i) {
+              if (g) {
+                x[u] = add_rn(x[u], gg[u]);
+                if (stash == nullptr) st_policy(a4 + i, x[u], pol);
+              }
+              if (stash != nullptr) stash[i] = x[u];
+              acc = add_sq(acc, x[u], prm.sc);
+            },
+            [&](uint32_t i) {
+              float xs = a[i];
+              if (g) { xs = __fadd_rn(xs, ld_stream(g + i)); a[i] = xs; }
+              acc = add_sq(acc, xs, prm.sc);
+            });
   return acc;
 }
 
@@ -602,54 +520,28 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
   float* __restrict__ v = prm.v + soff;
   float* __restrict__ p = param_ptr(prm.tab, d);
   const bool decay = (d.tensor_flags >> 31) != 0;
-  const uint32_t len = d.len, tid = threadIdx.x & (kThreads - 1);
   const Scalars& sc = prm.sc;
-  auto elem = [&](float ax, float& px, float& mx, float& vx) {
-    const float c = __fmul_rn(normalize(ax, sc.nf, sc.inv_nf), s);     // optimization.py:83-84
-    adam_elem<VARIANT>(c, px, mx, vx, decay, sc);           // :85
-  };
-  const uint32_t nvec = bulk_vecs2(d, p);
-  if (nvec > 0) {
-    float4* a4 = reinterpret_cast<float4*>(a);
-    float4* m4 = reinterpret_cast<float4*>(m);
-    float4* v4 = reinterpret_cast<float4*>(v);
-    float4* p4 = reinterpret_cast<float4*>(p);
-    float4 va[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll];
-#pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const uint32_t i = u * kThreads + tid;
-      if (i < nvec) {
-        vp[u] = slot[i]; vm[u] = slot[kTile / 4 + i]; vv[u] = slot[2 * (kTile / 4) + i];
-        va[u] = stash != nullptr ? stash[i] : slot[3 * (kTile / 4) + i];
-      }
-    }
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(empty);
-#pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const uint32_t i = u * kThreads + tid;
-      if (i < nvec) {
-        elem(va[u].x, vp[u].x, vm[u].x, vv[u].x); elem(va[u].y, vp[u].y, vm[u].y, vv[u].y);
-        elem(va[u].z, vp[u].z, vm[u].z, vv[u].z); elem(va[u].w, vp[u].w, vm[u].w, vv[u].w);
-        __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
-        __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
-      }
-    }
-    const uint32_t i = (nvec << 2) + tid;
-    if (i < len) {
-      float px = p[i], mx = m[i], vx = v[i];
-      elem(a[i], px, mx, vx);
-      p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
-    }
-  } else {
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(empty);
-    for (uint32_t i = tid; i < len; i += kThreads) {
-      float px = p[i], mx = m[i], vx = v[i];
-      elem(a[i], px, mx, vx);
-      p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
-    }
-  }
+  float4* a4 = reinterpret_cast<float4*>(a);
+  float4* m4 = reinterpret_cast<float4*>(m);
+  float4* v4 = reinterpret_cast<float4*>(v);
+  float4* p4 = reinterpret_cast<float4*>(p);
+  float4 va[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll];
+  walk_tile(d.len, bulk_vecs2(d, p), threadIdx.x & (kThreads - 1),
+            [&](int u, uint32_t i) {
+              vp[u] = slot[i]; vm[u] = slot[kTile / 4 + i]; vv[u] = slot[2 * (kTile / 4) + i];
+              va[u] = stash != nullptr ? stash[i] : slot[3 * (kTile / 4) + i];
+            },
+            [&] { __syncwarp(); if ((threadIdx.x & 31) == 0) mbar_arrive(empty); },
+            [&](int u, uint32_t i) {
+              update_vec<VARIANT>(va[u], true, s, vp[u], vm[u], vv[u], decay, sc);
+              __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
+              __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
+            },
+            [&](uint32_t i) {
+              float px = p[i], mx = m[i], vx = v[i];
+              update_elem<VARIANT>(a[i], true, s, px, mx, vx, decay, sc);
+              p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
+            });
 }
 
 // Dynamic shared memory of apply_clip_kernel (kClipSmemBytes): 3 groups x kRingVecs float4 of ring, then
@@ -665,19 +557,19 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   __shared__ unsigned int s_nonfinite;
   __shared__ float s_bcast[2];
   __shared__ uint32_t s_set;
-  __shared__ __align__(8) uint64_t s_full1[kGroups][kMaxSlots], s_empty1[kGroups][kMaxSlots];
-  __shared__ __align__(8) uint64_t s_full2[kGroups][kMaxSlots], s_empty2[kGroups][kMaxSlots];
+  __shared__ __align__(8) uint64_t s_full1[kGroups][kP1Slots], s_empty1[kGroups][kP1Slots];
+  __shared__ __align__(8) uint64_t s_full2[kGroups][kP2Slots], s_empty2[kGroups][kP2Slots];
   __shared__ __align__(8) uint64_t s_go[kGroups];
-  __shared__ SlotMeta s_meta1[kGroups][kMaxSlots], s_meta2[kGroups][kMaxSlots];
+  __shared__ SlotMeta s_meta1[kGroups][kP1Slots], s_meta2[kGroups][kP2Slots];
 
   const int warp = (int)threadIdx.x >> 5;
   const bool is_producer = warp >= kConsumerThreads / 32;
   const int grp = is_producer ? warp - kConsumerThreads / 32 : (int)threadIdx.x / kThreads;   // group served / group id
   const int nt = prm.num_tiles, G = (int)gridDim.x * kGroups;
   const int b = (int)blockIdx.x * kGroups + grp;                   // virtual block id
-  const int C = b < nt ? (nt - 1 - b) / G + 1 : 0;                 // tiles b, b + G, ... of this group's static share
-  const int n_st = min(prm.stash_tiles, C);                        // own tiles: a' parked in the stash
-  const int pool_lo = min(nt, prm.stash_tiles * G);                // tiles [pool_lo, nt): a' goes back to global memory
+  const int C = b < nt ? (nt - 1 - b) / G + 1 : 0;                 // tiles b, b + G, ... below nt
+  const int n_st = min(kStashTiles, C);                            // own tiles: a' parked in the stash
+  const int pool_lo = min(nt, kStashTiles * G);                    // tiles [pool_lo, nt): a' goes back to global memory
   float4* const ring = reinterpret_cast<float4*>(smem_dyn) + (size_t)grp * kRingVecs;
   float4* const stash = reinterpret_cast<float4*>(smem_dyn + kRingBytes) + (size_t)grp * kStashVecs;
   const uint64_t pol_last = policy_evict_last();
@@ -726,14 +618,13 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     long long dbg_empty = 0;
     const long long dbg_p0 = clock64();
 #endif
-    // ---- pass 1.  First the group's OWN tiles b + j*G, j < stash_tiles: their a' is parked in this SM's stash, so
-    //      they are bound to it in both passes.  Then the rest of the model, tiles [pool_lo, nt): either this group's static
-    //      share (b + j*G) or, with kFlagDynamicPass1, whatever the global ticket counter hands out -- kTicketBatch tickets at
-    //      a time while plenty are left (one atomic per lane, the descriptor loads of a batch overlap), single tickets
-    //      near the end so that no SM is left holding a batch ----
+    // ---- pass 1.  First the group's OWN tiles b + j*G, j < kStashTiles: their a' is parked in this SM's stash, so
+    //      they are bound to it in both passes.  Then the rest of the model, tiles [pool_lo, nt), as the global ticket
+    //      counter hands them out -- kTicketBatch tickets at a time while plenty are left (one atomic per lane, the
+    //      descriptor loads of a batch overlap), single tickets near the end so that no SM is left holding a batch ----
     {
       RingPos rp;
-      auto issue = [&](const TileDesc& dl, const uint32_t tile) {          // lane 0 only
+      auto issue = [&](const TileDesc& dl) {                               // lane 0 only
         const float* g = nullptr;
         if constexpr (HAS_G) g = grad_ptr(prm.tab, dl);
         const uint32_t nvec = bulk_vecs(dl, g);
@@ -747,7 +638,6 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
 #endif
         SlotMeta* meta = &s_meta1[grp][rp.slot];
         meta->d = dl;
-        meta->tile = tile;
         if (nvec > 0) {
           float4* dst = ring + (size_t)rp.slot * kP1SlotVecs;
           mbar_arrive_expect_tx(full, nvec * 16u * (g ? 2u : 1u));
@@ -765,19 +655,16 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         dl.soff32 = __shfl_sync(0xffffffffu, d.soff32, l);
         return dl;
       };
-      const bool dynamic = (prm.flags & kFlagDynamicPass1) != 0;
-      const int n_static = dynamic ? n_st : C;                               // tiles b + j*G, j < n_static, are this group's by position
-      for (int j0 = 0; j0 < n_static; j0 += 32) {                              // descriptors 32 at a time, one per lane
+      {
         TileDesc d{};
-        if (j0 + lane < n_static) d = prm.tiles[b + (j0 + lane) * G];
-        const int nb = min(32, n_static - j0);
-        for (int l = 0; l < nb; ++l) {
+        if (lane < n_st) d = prm.tiles[b + lane * G];                        // own tiles' descriptors, one per lane
+        for (int l = 0; l < n_st; ++l) {
           const TileDesc dl = shuffled(d, l);
-          if (lane == 0) issue(dl, (uint32_t)(b + (j0 + l) * G));
+          if (lane == 0) issue(dl);
           rp.advance(kP1Slots);
         }
       }
-      bool done = !dynamic;
+      bool done = false;
       long long last = pool_lo;
       while (!done) {
         const long long left = (long long)nt - last;
@@ -793,7 +680,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
           if (tl >= nt) { done = true; continue; }       // lanes get their tickets in no particular order: a valid one may follow
           last = tl;
           const TileDesc dl = shuffled(d, l);
-          if (lane == 0) issue(dl, (uint32_t)tl);
+          if (lane == 0) issue(dl);
           rp.advance(kP1Slots);
         }
       }
@@ -902,7 +789,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
 #endif
         const SlotMeta meta = s_meta1[grp][rp.slot];
         if (meta.d.len == 0) break;
-        // the stash takes the group's own tiles j < stash_tiles (the first ones it is handed) when they are FULL,
+        // the stash takes the group's own tiles j < kStashTiles (the first ones it is handed) when they are FULL,
         // vector-path tiles (the same predicate the producer evaluates in pass 2)
         const bool own = n_seen < n_st;
         const bool park = own && stash_ok<HAS_G>(meta.d, prm);
