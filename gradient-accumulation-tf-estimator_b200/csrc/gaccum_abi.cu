@@ -151,11 +151,13 @@ static int grid_for(gaccum_plan* pl, const void* fn, int* out) {
   return GACCUM_OK;
 }
 
+// from_zero: the accumulators hold +0.0 (first micro-step of a window), so the kernel does not read them
 template <int CAP>
-static int launch_accumulate(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream_t st) {
+static int launch_accumulate(gaccum_plan* pl, KernelParams<CAP>& prm, bool from_zero, cudaStream_t st) {
   // one tile per CTA: the hardware block scheduler balances better than a persistent loop
   const int grid = std::max(1, prm.num_tiles);
-  accumulate_kernel<CAP><<<grid, kThreads, 0, st>>>(prm);
+  if (from_zero) accumulate_kernel<CAP, true><<<grid, kThreads, 0, st>>>(prm);
+  else accumulate_kernel<CAP, false><<<grid, kThreads, 0, st>>>(prm);
   CUDA_TRY(cudaGetLastError());
   return GACCUM_OK;
 }
@@ -257,6 +259,16 @@ struct DeviceGuard {
   ~DeviceGuard() { if (prev >= 0 && ok) cudaSetDevice(prev); }
 };
 
+// An accumulate step is the first of its window when the previous micro-step took the apply branch, which left every
+// accumulator at +0.0 (optimization.py:86-87; they start as zeros, :78).  Both predicates take the reference's int32
+// cast of the step; subtracting after the cast cannot overflow and wraps like the reference's int32 step would.
+// False without step arguments (gaccum_accumulate), at global_step 0, and always for N = 1 (every step applies).
+static bool first_of_window(const gaccum_step_args* a) {
+  if (!a) return false;
+  const int64_t prev = (int64_t)(int32_t)a->global_step - 1;
+  return !gaccum_is_apply_step(a->global_step, a->accum_n) && gaccum_is_apply_step(prev, a->accum_n);
+}
+
 template <int CAP>
 static int do_accumulate_tab(gaccum_plan* pl, const float* const* grads, float* accum,
                              const gaccum_step_args* a, cudaStream_t st) {
@@ -264,7 +276,7 @@ static int do_accumulate_tab(gaccum_plan* pl, const float* const* grads, float* 
   if (!prm) return fail(GACCUM_ENOMEM, "out of host memory");
   fill_common(pl, *prm, accum, nullptr, nullptr, make_scalars(pl->hp, a));
   int rc = fill_table(pl, prm->tab, grads, nullptr);
-  if (rc == GACCUM_OK) rc = launch_accumulate(pl, *prm, st);
+  if (rc == GACCUM_OK) rc = launch_accumulate(pl, *prm, first_of_window(a), st);
   delete prm;
   return rc;
 }
@@ -447,6 +459,8 @@ int gaccum_offsets(const gaccum_plan* pl, int64_t* out) {
 int64_t gaccum_algorithmic_bytes(const gaccum_plan* pl, int32_t is_apply) {
   if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
   // accumulate: read G, read a, write a.  apply: read G,a,p,m,v + write p,m,v,a  (SURVEY.md 8(d))
+  // The first accumulate of a window does not read a (8 B x P), so a window of N >= 2 moves (8 + 12(N-2) + 36) B x P.
+  // The plan does not know N: the accumulate figure is the 12 B x P of the other accumulate steps.
   return pl->P * (is_apply ? 36 : 12);
 }
 
@@ -498,7 +512,8 @@ int gaccum_step_packed(gaccum_plan* pl, const float* grad_slab, float* param_sla
   prm.tab.p = param_slab;
   if (!apply) {
     if (!grad_slab) return fail(GACCUM_EINVAL, "grad_slab is NULL on an accumulate step");
-    return launch_accumulate(pl, prm, st);
+    // a forced branch says nothing about what the previous micro-step did: only the scheduled one may skip reading a
+    return launch_accumulate(pl, prm, force_branch < 0 && first_of_window(a), st);
   }
   if (!param_slab || !aligned16_host(param_slab)) return fail(GACCUM_EINVAL, "param_slab must be a 16-byte aligned device pointer");
   return launch_apply(pl, prm, grad_slab != nullptr, st);

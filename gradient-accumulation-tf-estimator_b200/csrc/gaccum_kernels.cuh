@@ -4,7 +4,8 @@
 // and therefore every reduction -- is deterministic.
 //
 //   accumulate_kernel    a += G                                  optimization.py:81,93    (12 B/elem)
-//                        one tile per CTA (hardware block scheduler)
+//                        one tile per CTA (hardware block scheduler); the first accumulate of a window
+//                        stores a = +0 + G without reading a                             (8 B/elem)
 //   apply_kernel         the apply branch WITHOUT clipping (plain Adam of the example scripts, or
 //                        clip_norm <= 0): a' = a + G; n = a'/N; Adam; a = 0 in a single pass (36 B/elem).
 //   apply_clip_kernel    the apply branch WITH tf.clip_by_global_norm                  (36 B/elem)
@@ -224,8 +225,11 @@ __device__ __forceinline__ void walk_tile(const uint32_t len, const uint32_t nve
 
 // ---------------------------------------------------------------------------------------------
 // accumulate: a += G                                                   optimization.py:81,93
+// FROM_ZERO: the first accumulate of a window.  The apply that ended the previous window left every accumulator at
+// +0.0 (optimization.py:78,86-87), so a is not loaded and a = +0 + G is stored (8 instead of 12 B/elem).  The add is
+// kept: it turns a gradient of -0.0 into +0.0, as assign_add onto a zero does, and a NaN comes out as a += G gives it.
 // ---------------------------------------------------------------------------------------------
-template <int CAP>
+template <bool FROM_ZERO, int CAP>
 __device__ __forceinline__ void accumulate_tile(const TileDesc d, const KernelParams<CAP>& prm) {
   const float* __restrict__ g = grad_ptr(prm.tab, d);
   if (g == nullptr) return;   // optimization.py:132 -- tensors without a gradient are skipped
@@ -234,19 +238,22 @@ __device__ __forceinline__ void accumulate_tile(const TileDesc d, const KernelPa
   float4* a4 = reinterpret_cast<float4*>(a);
   float4 vg[kUnroll], va[kUnroll];
   walk_tile(d.len, aligned16(g) ? d.len >> 2 : 0u, threadIdx.x,
-            [&](int u, uint32_t i) { vg[u] = ld_stream(g4 + i); va[u] = a4[i]; },
+            [&](int u, uint32_t i) {
+              vg[u] = ld_stream(g4 + i);
+              if constexpr (FROM_ZERO) va[u] = make_float4(0.f, 0.f, 0.f, 0.f); else va[u] = a4[i];
+            },
             [] {},
             [&](int u, uint32_t i) { a4[i] = add_rn(va[u], vg[u]); },
-            [&](uint32_t i) { a[i] = __fadd_rn(a[i], ld_stream(g + i)); });
+            [&](uint32_t i) { a[i] = __fadd_rn(FROM_ZERO ? 0.f : a[i], ld_stream(g + i)); });
 }
 
-template <int CAP>
+template <int CAP, bool FROM_ZERO>
 __global__ void __launch_bounds__(kThreads)
 accumulate_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     prm.stats[0] = 0.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f;
   }
-  if ((int)blockIdx.x < prm.num_tiles) accumulate_tile(prm.tiles[blockIdx.x], prm);
+  if ((int)blockIdx.x < prm.num_tiles) accumulate_tile<FROM_ZERO>(prm.tiles[blockIdx.x], prm);
 }
 
 // ---------------------------------------------------------------------------------------------

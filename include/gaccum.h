@@ -125,7 +125,10 @@ GACCUM_API int gaccum_offsets(const gaccum_plan* plan, int64_t* out);
 GACCUM_API int32_t gaccum_num_tensors(const gaccum_plan* plan);
 GACCUM_API int64_t gaccum_num_elements(const gaccum_plan* plan); /* P, real elements */
 GACCUM_API int32_t gaccum_num_tiles(const gaccum_plan* plan);
-/* Algorithmic bytes of one launch: accumulate = 12 B x P; apply = 36 B x P (SURVEY.md 8(d)). */
+/* Algorithmic bytes of one launch: accumulate = 12 B x P; apply = 36 B x P (SURVEY.md 8(d)).
+ * The first accumulate of a window does not read the accumulators (8 B x P; see gaccum_step), so
+ * a window of N >= 2 micro-steps moves (8 + 12 (N-2) + 36) B x P.  The plan does not know N: the
+ * accumulate figure stays 12 B x P. */
 GACCUM_API int64_t gaccum_algorithmic_bytes(const gaccum_plan* plan, int32_t is_apply);
 
 /* ---- the hot path --------------------------------------------------------------------- */
@@ -135,19 +138,31 @@ GACCUM_API int64_t gaccum_algorithmic_bytes(const gaccum_plan* plan, int32_t is_
  * any 4-byte alignment; 16-byte alignment takes the vector path).  grads[i] == NULL means
  * "no gradient for this tensor" (optimization.py:132 skips such pairs).
  * accum / m / v: device slabs of gaccum_padded_size() floats, 16-byte aligned.
- * The caller increments global_step afterwards (optimization.py:102-103). */
+ * The caller increments global_step afterwards (optimization.py:102-103).
+ * PRECONDITION, first micro-step of a window (global_step - 1 applies, global_step does not; never
+ * at global_step 0 or with accum_n = 1): `accum` is not read and must hold +0.0 in every tensor
+ * element; anything else there is overwritten, not added to.  That step stores accum = +0.0 + G
+ * (tensors without a gradient keep their +0.0), which is what the reference computes there: its
+ * accumulators start as zeros (optimization.py:78) and every apply zeroes them (:86-87).  A zero-
+ * initialised slab and the apply branch of this library leave exactly that; a caller that writes
+ * `accum` itself (e.g. restoring a checkpoint) must not leave non-zero values at a window start.
+ * The same holds for gaccum_step_packed with force_branch = -1, gaccum_step_dp and gaccum_step_host.
+ * gaccum_accumulate, and gaccum_step_packed with a forced branch, always compute accum += G. */
 GACCUM_API int gaccum_step(gaccum_plan* plan, const float* const* grads, float* const* params,
                            float* accum, float* m, float* v, const gaccum_step_args* args,
                            gaccum_stream_t stream);
 /* The two branches on their own (the data-parallel driver accumulates locally, all-reduces the
- * slab, then applies with grads == NULL).  gaccum_apply ignores args->global_step. */
+ * slab, then applies with grads == NULL).  gaccum_apply ignores args->global_step.
+ * gaccum_accumulate has no step arguments and always reads accum: accum += G for any accum. */
 GACCUM_API int gaccum_accumulate(gaccum_plan* plan, const float* const* grads, float* accum,
                                  gaccum_stream_t stream);
 GACCUM_API int gaccum_apply(gaccum_plan* plan, const float* const* grads, float* const* params,
                             float* accum, float* m, float* v, const gaccum_step_args* args,
                             gaccum_stream_t stream);
 /* Same step when gradients and parameters are themselves packed in slab layout (params as
- * views of one flat buffer): no pointer table.  grad_slab may be NULL on an apply step. */
+ * views of one flat buffer): no pointer table.  grad_slab may be NULL on an apply step.
+ * With force_branch = -1 the first micro-step of a window has gaccum_step's precondition; a forced
+ * accumulate (force_branch = 0) cannot know what the previous micro-step did and reads accum. */
 GACCUM_API int gaccum_step_packed(gaccum_plan* plan, const float* grad_slab, float* param_slab,
                                   float* accum, float* m, float* v, const gaccum_step_args* args,
                                   int32_t force_branch /* -1 = from global_step, 0 = accumulate, 1 = apply */,
@@ -188,6 +203,8 @@ GACCUM_API int64_t gaccum_dp_stage_elements(const gaccum_plan* plan, int32_t wor
  * NULL = none).  `epoch` must be non-zero, different from the previous apply's (e.g. an apply counter)
  * and the same on every rank.  m / v: local slabs; only the owned range is read or written.
  * All `world` ranks must call this for the same step; the call is asynchronous on `stream`.
+ * On the first micro-step of a window comm->accum is not read and must hold +0.0 (gaccum_step's
+ * precondition); the apply step leaves every rank's accumulators there.
  * If a peer never reaches the matching apply (crashed rank, mismatched epoch) the kernel traps after
  * 60 s of waiting and the failure surfaces as a CUDA error on the next runtime call. */
 GACCUM_API int gaccum_step_dp(gaccum_plan* plan, const gaccum_dp_comm* comm, const float* const* grads,
@@ -211,7 +228,10 @@ GACCUM_API int gaccum_host_session_destroy(gaccum_host_session* s);
 /* initial values of the trainable variables (optimization.py:70) -> HBM; synchronous */
 GACCUM_API int gaccum_host_session_set_params(gaccum_host_session* s, const float* const* host_params);
 /* host_grads[i] may be NULL (no gradient).  host_params_out (may be NULL) receives the updated
- * parameters on apply steps.  stats_out (may be NULL) receives the stats block every step. */
+ * parameters on apply steps.  stats_out (may be NULL) receives the stats block every step.
+ * The session's accumulators start zeroed and its apply steps zero them, so gaccum_step's
+ * precondition on the first micro-step of a window holds unless the caller writes them through
+ * gaccum_host_session_slabs. */
 GACCUM_API int gaccum_step_host(gaccum_host_session* s, const float* const* host_grads,
                                 float* const* host_params_out, const gaccum_step_args* args,
                                 gaccum_stats* stats_out);
