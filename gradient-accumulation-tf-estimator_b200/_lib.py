@@ -3,6 +3,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import re
 from typing import List, Optional, Sequence
 
 from . import build as _build
@@ -148,8 +149,11 @@ def learning_rate(init_lr: float, num_train_steps: int, num_warmup_steps: Option
 
 
 def is_apply_step(global_step: int, accum_n: int) -> bool:
-    """optimization.py:77,91."""
-    return bool(_load().gaccum_is_apply_step(int(global_step), int(accum_n)))
+    """optimization.py:77,91: the step is cast to int32 (two's-complement wraparound) before the modulo.  The same
+    decision as ``gaccum_is_apply_step`` without a foreign call, so every Python front end can take it per
+    micro-step.  Divisibility does not depend on whether ``%`` truncates (C) or floors (Python)."""
+    step32 = (int(global_step) + 0x80000000) % 0x100000000 - 0x80000000
+    return accum_n > 0 and step32 % accum_n == 0
 
 
 def _c_strs(strs: Sequence[str]):
@@ -158,25 +162,26 @@ def _c_strs(strs: Sequence[str]):
     return arr
 
 
+def _variable_name(name: str) -> str:
+    """optimization.py:189-194 (``_get_variable_name``): a trailing ``:<digits>`` is stripped."""
+    m = re.match("^(.*):\\d+$", name)
+    return name if m is None else m.group(1)
+
+
+def _use_weight_decay(name: str, weight_decay_rate: float, exclude: Optional[Sequence[str]]) -> bool:
+    """optimization.py:179-187 (``_do_use_weight_decay``)."""
+    if not weight_decay_rate:
+        return False
+    return not any(re.search(r, name) is not None for r in exclude or ())
+
+
 def decay_mask(names: Sequence[str], weight_decay_rate: float,
                exclude: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias")) -> List[bool]:
     """optimization.py:179-194, with the reference's own regular-expression engine: Python ``re.search`` on the
     name with a trailing ``:<digits>`` stripped.  (The C helper ``gaccum_decay_mask`` is for non-Python callers and
     speaks POSIX ERE: identical for the reference's plain substrings, different for Python-only syntax such as
     ``\\d`` or look-arounds -- both Python bindings therefore evaluate the patterns here.)"""
-    import re
-    out = []
-    for n in names:
-        m = re.match("^(.*):\\d+$", n)                      # _get_variable_name, optimization.py:189-194
-        if m is not None:
-            n = m.group(1)
-        use = bool(weight_decay_rate)                       # :181
-        if use and exclude:
-            for r in exclude:
-                if re.search(r, n) is not None:             # :183-186
-                    use = False
-        out.append(use)
-    return out
+    return [_use_weight_decay(_variable_name(n), weight_decay_rate, exclude) for n in names]
 
 
 def decay_mask_c(names: Sequence[str], weight_decay_rate: float,

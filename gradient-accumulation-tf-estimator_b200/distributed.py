@@ -21,6 +21,8 @@ from typing import Optional, Sequence
 import torch
 import torch.distributed as dist
 
+from . import _lib
+
 
 class DataParallelTrainOp:
     """Wraps an engine exposing accumulate_only / apply_only / run / accum / N / global_step."""
@@ -55,7 +57,7 @@ class DataParallelTrainOp:
         if self.world == 1:
             return e.run(grads)
         g = e.global_step
-        if (g % e.N) != 0:                       # optimization.py:91 predicate, accumulate branch
+        if not _lib.is_apply_step(g, e.N):       # optimization.py:91 predicate, accumulate branch
             return e.run(grads)
         e.accumulate_only(grads)                 # 04:58
         dist.all_reduce(e.accum, op=dist.ReduceOp.SUM, group=self.group)   # 04:55, once per window
@@ -86,7 +88,6 @@ class FusedDataParallelTrainOp:
                  process_group=None, exclude_from_weight_decay=("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0):
         import torch.distributed._symmetric_memory as symm
-        from . import _lib
         from .train_op import GaccumTrainOp
         if not dist.is_initialized():
             raise RuntimeError("torch.distributed must be initialised (backend nccl)")
@@ -145,18 +146,13 @@ class FusedDataParallelTrainOp:
     def run_bound(self, grad_table, stream: Optional[int] = None) -> bool:
         e = self.engine
         g = e.global_step
-        if (g % e.N) != 0:
+        if not _lib.is_apply_step(g, e.N):
             return e.run_bound(grad_table, stream)            # rank-local accumulate (04:58 without the all-reduce)
-        if stream is None:
-            stream = torch.cuda.current_stream(e.device).cuda_stream
-        from ._lib import StepArgs
         lr = e.lr_fn(g)
         self.epoch += 1
-        e.plan.apply_dp(self.comm, grad_table, e._m_ptr, e._v_ptr,
-                        StepArgs(g, e.N, 0, lr, e.beta1_power, e.beta2_power, 0.0), self.epoch, stream)
+        e.plan.apply_dp(self.comm, grad_table, e._m_ptr, e._v_ptr, e._step_args(g, lr), self.epoch, e._stream(stream))
         self.exchanges += 1
-        e._after(True, lr)
-        return True
+        return e._after(g, True, lr)
 
     # -- checkpoint compatibility under data parallelism (SURVEY.md 8(f) #3; reference 04:55 aggregation=SUM) --------
     def state_dict(self):

@@ -19,7 +19,6 @@ There is no CPU fallback: variables must be CUDA tensors.
 from __future__ import annotations
 
 import os
-import re
 from typing import Callable, Iterable, List, Optional, Sequence, Tuple, Union
 
 import torch
@@ -106,20 +105,11 @@ class AdamWeightDecayOptimizer(_OptimizerBase):
 
     def _do_use_weight_decay(self, param_name: str) -> bool:
         """optimization.py:179-187."""
-        if not self.weight_decay_rate:
-            return False
-        if self.exclude_from_weight_decay:
-            for r in self.exclude_from_weight_decay:
-                if re.search(r, param_name) is not None:
-                    return False
-        return True
+        return _lib._use_weight_decay(param_name, self.weight_decay_rate, self.exclude_from_weight_decay)
 
     def _get_variable_name(self, param_name: str) -> str:
         """optimization.py:189-194."""
-        m = re.match("^(.*):\\d+$", param_name)
-        if m is not None:
-            param_name = m.group(1)
-        return param_name
+        return _lib._variable_name(param_name)
 
 
 class AdamOptimizer(_OptimizerBase):

@@ -10,69 +10,85 @@ in csrc/.
 """
 from __future__ import annotations
 
-import ctypes as C
-import re
-from typing import Callable, Dict, List, Optional, Sequence
+from typing import Callable, Dict, Optional, Sequence
 
 import numpy as np
 import torch
 
 from . import _lib
-from ._lib import ADAM, HParams, Plan, StepArgs, Stats
+from ._lib import ADAM, HParams, Plan, StepArgs
 
 
 def _f32(x) -> float:
     return float(np.float32(x))
 
 
-class GaccumTrainOp:
+def _pinned_zeros(n: int) -> torch.Tensor:
+    """fp32 zeros in page-locked host memory (pageable where the CUDA runtime cannot pin)."""
+    t = torch.zeros(n, dtype=torch.float32)
+    try:
+        return t.pin_memory()
+    except Exception:
+        return t
+
+
+def _stats_dict(buf: torch.Tensor) -> Dict[str, float]:
+    """The 16-byte gaccum_stats block as ``stats()`` reports it."""
+    a, lr, gn, s = buf.tolist()
+    return {"applied": bool(a), "lr": lr, "global_norm": gn, "clip_scale": s}
+
+
+class _TrainOpCore:
+    """What every train op keeps besides its slabs: the plan, the hyper-parameters, ``global_step``
+    (optimization.py:27) and TF1's ``beta{1,2}_power`` non-slot variables, with the per-step scalars built from them."""
+
     def __init__(self, params: Sequence[torch.Tensor], names: Sequence[str], hp: HParams, accum_n: int,
-                 lr_fn: Callable[[int], float],
-                 exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
-                 global_step: int = 0, accum: Optional[torch.Tensor] = None):
+                 lr_fn: Callable[[int], float], exclude_from_weight_decay: Optional[Sequence[str]],
+                 global_step: int, device: int):
         if len(params) != len(names):
             raise ValueError("params and names differ in length")
-        if not params:
-            raise ValueError("no trainable variables")
-        dev = params[0].device
-        if dev.type != "cuda":
-            raise _lib.GaccumError(_lib.ENODEVICE, "parameters must live on a CUDA device: the train_op has no CPU fallback")
-        for p in params:
-            if p.dtype != torch.float32 or not p.is_contiguous() or p.device != dev:
-                raise ValueError("parameters must be contiguous fp32 tensors on one device")
-        self.device = dev
         self.params = list(params)
         # optimization.py:135-143 names slots after _get_variable_name(param.name): the ":0" tensor suffix is stripped
-        self.names = [re.sub(r":\d+$", "", n) for n in names]
-        self.hp = hp
-        self.N = int(accum_n)
-        self.lr_fn = lr_fn
-        self.global_step = int(global_step)
-        self.decay = _lib.decay_mask(self.names, hp.weight_decay_rate, exclude_from_weight_decay) \
+        self.names = [_lib._variable_name(n) for n in names]
+        self.hp, self.N, self.lr_fn, self.global_step = hp, int(accum_n), lr_fn, int(global_step)
+        self.decay = _lib.decay_mask(names, hp.weight_decay_rate, exclude_from_weight_decay) \
             if hp.variant == _lib.ADAM_WEIGHT_DECAY else [False] * len(params)
-        self.plan = Plan([p.numel() for p in params], self.decay, hp, device=dev.index or 0)
-        n = max(self.plan.padded_size, 32)
-        if accum is not None:          # caller-provided slab (e.g. NVLink peer-mapped symmetric memory)
-            if accum.numel() < n or accum.dtype != torch.float32 or accum.device != dev:
-                raise ValueError("accum must be an fp32 tensor of at least plan.padded_size elements on the params' device")
-            self.accum = accum
-        else:
-            self.accum = torch.zeros(n, dtype=torch.float32, device=dev)
-        self.m = torch.zeros(n, dtype=torch.float32, device=dev)
-        self.v = torch.zeros(n, dtype=torch.float32, device=dev)
+        self.plan = Plan([p.numel() for p in params], self.decay, hp, device=device)
         # TF1 AdamOptimizer._create_slots: beta powers start at beta
-        self.beta1_power = _f32(hp.beta1)
-        self.beta2_power = _f32(hp.beta2)
-        self._accum_ptr, self._m_ptr, self._v_ptr = self.accum.data_ptr(), self.m.data_ptr(), self.v.data_ptr()
-        self._param_ptrs = Plan.ptr_array([p.data_ptr() for p in self.params])
-        self._param_key = tuple(p.data_ptr() for p in self.params)
-        self._grad_key = None
-        self._grad_ptrs = None
-        self._stats_host = torch.zeros(4, dtype=torch.float32).pin_memory() if torch.cuda.is_available() else None
-        self.last_lr = 0.0
-        self.last_applied = False
+        self.beta1_power, self.beta2_power = _f32(hp.beta1), _f32(hp.beta2)
+        self._stats_host = _pinned_zeros(4)
 
-    # -- views under the reference's variable names -----------------------------------------
+    def _step_args(self, g: int, lr: float) -> StepArgs:
+        return StepArgs(g, self.N, 0, lr, self.beta1_power, self.beta2_power, 0.0)
+
+    def _advance_beta_powers(self) -> None:
+        """TF1 AdamOptimizer._finish: beta_power <- beta_power * beta (fp32) after the updates of an apply step."""
+        if self.hp.variant == ADAM:
+            self.beta1_power = _f32(np.float32(self.beta1_power) * np.float32(self.hp.beta1))
+            self.beta2_power = _f32(np.float32(self.beta2_power) * np.float32(self.hp.beta2))
+
+
+class _DeviceTrainOp(_TrainOpCore):
+    """A train op whose parameters live on one CUDA device and whose Adam moments are packed HBM slabs."""
+
+    def __init__(self, params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step):
+        if not params:
+            raise ValueError("no trainable variables")
+        self.device = params[0].device
+        if self.device.type != "cuda":
+            raise _lib.GaccumError(_lib.ENODEVICE, "parameters must live on a CUDA device: the train_op has no CPU fallback")
+        super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step,
+                         self.device.index or 0)
+        self.m = self._zeros_slab()
+        self.v = self._zeros_slab()
+
+    def _zeros_slab(self) -> torch.Tensor:
+        return torch.zeros(max(self.plan.padded_size, 32), dtype=torch.float32, device=self.device)
+
+    def _stream(self, stream: Optional[int] = None) -> int:
+        return torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
+
+    # -- views under the reference's variable names (read self.accum / m / v when called) -------------
     def _view(self, slab: torch.Tensor, i: int) -> torch.Tensor:
         o = self.plan.offsets[i]
         return slab[o:o + self.params[i].numel()].view(self.params[i].shape)
@@ -86,8 +102,36 @@ class GaccumTrainOp:
     def v_view(self, i: int) -> torch.Tensor:
         return self._view(self.v, i)
 
-    def _args(self, lr: float) -> StepArgs:
-        return StepArgs(self.global_step, self.N, 0, lr, self.beta1_power, self.beta2_power, 0.0)
+    def stats(self) -> Dict[str, float]:
+        """Synchronously read what the last step computed (applied, lr, global_norm, clip_scale)."""
+        stream = torch.cuda.current_stream(self.device)
+        self.plan.read_stats(self._stats_host.data_ptr(), stream.cuda_stream)
+        stream.synchronize()
+        return _stats_dict(self._stats_host)
+
+
+class GaccumTrainOp(_DeviceTrainOp):
+    def __init__(self, params: Sequence[torch.Tensor], names: Sequence[str], hp: HParams, accum_n: int,
+                 lr_fn: Callable[[int], float],
+                 exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
+                 global_step: int = 0, accum: Optional[torch.Tensor] = None):
+        super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step)
+        for p in self.params:
+            if p.dtype != torch.float32 or not p.is_contiguous() or p.device != self.device:
+                raise ValueError("parameters must be contiguous fp32 tensors on one device")
+        if accum is not None:          # caller-provided slab (e.g. NVLink peer-mapped symmetric memory)
+            if accum.numel() < self.m.numel() or accum.dtype != torch.float32 or accum.device != self.device:
+                raise ValueError("accum must be an fp32 tensor of at least plan.padded_size elements on the params' device")
+            self.accum = accum
+        else:
+            self.accum = self._zeros_slab()
+        self._accum_ptr, self._m_ptr, self._v_ptr = self.accum.data_ptr(), self.m.data_ptr(), self.v.data_ptr()
+        self._param_ptrs = Plan.ptr_array([p.data_ptr() for p in self.params])
+        self._param_key = tuple(p.data_ptr() for p in self.params)
+        self._grad_key = None
+        self._grad_ptrs = None
+        self.last_lr = 0.0
+        self.last_applied = False
 
     def _grad_table(self, grads: Sequence[Optional[torch.Tensor]]):
         key = tuple(0 if g is None else g.data_ptr() for g in grads)
@@ -130,35 +174,30 @@ class GaccumTrainOp:
         if stream is None:
             stream = torch.cuda.current_stream(self.device).cuda_stream
         self.plan.step(grad_table, self._param_ptrs, self._accum_ptr, self._m_ptr, self._v_ptr,
-                       StepArgs(g, self.N, 0, lr, self.beta1_power, self.beta2_power, 0.0), stream)
-        applied = (g % self.N) == 0 if 0 <= g < 2**31 else _lib.is_apply_step(g, self.N)
-        self._after(applied, lr)
-        return applied
+                       self._step_args(g, lr), stream)
+        return self._after(g, _lib.is_apply_step(g, self.N), lr)
 
     def accumulate_only(self, grads: Sequence[Optional[torch.Tensor]]) -> None:
         """The false branch alone (used by the data-parallel driver); does not touch global_step."""
-        stream = torch.cuda.current_stream(self.device).cuda_stream
-        self.plan.accumulate(self._grad_table(grads), self.accum.data_ptr(), stream)
+        self.plan.accumulate(self._grad_table(grads), self.accum.data_ptr(), self._stream())
 
     def apply_only(self, grads: Optional[Sequence[Optional[torch.Tensor]]] = None) -> None:
         """The true branch alone; ``grads=None`` applies the accumulators as they are."""
         lr = _f32(self.lr_fn(self.global_step))
-        stream = torch.cuda.current_stream(self.device).cuda_stream
         self._refresh_param_table()
         self.plan.apply(self._grad_table(grads) if grads is not None else None, self._param_ptrs,
-                        self.accum.data_ptr(), self.m.data_ptr(), self.v.data_ptr(), self._args(lr), stream)
+                        self.accum.data_ptr(), self.m.data_ptr(), self.v.data_ptr(),
+                        self._step_args(self.global_step, lr), self._stream())
         self.last_lr, self.last_applied = lr, True
-        if self.hp.variant == ADAM:
-            self.beta1_power = _f32(np.float32(self.beta1_power) * np.float32(self.hp.beta1))
-            self.beta2_power = _f32(np.float32(self.beta2_power) * np.float32(self.hp.beta2))
+        self._advance_beta_powers()
 
-    def _after(self, applied: bool, lr: float) -> None:
+    def _after(self, g: int, applied: bool, lr: float) -> bool:
+        """Bookkeeping once micro-step ``g`` is launched."""
         self.last_lr, self.last_applied = lr, applied
-        if applied and self.hp.variant == ADAM:
-            # TF1 AdamOptimizer._finish: beta_power <- beta_power * beta (fp32) after the updates
-            self.beta1_power = _f32(np.float32(self.beta1_power) * np.float32(self.hp.beta1))
-            self.beta2_power = _f32(np.float32(self.beta2_power) * np.float32(self.hp.beta2))
-        self.global_step += 1                                   # optimization.py:102-103
+        if applied:
+            self._advance_beta_powers()
+        self.global_step = g + 1                                # optimization.py:102-103
+        return applied
 
     __call__ = run
 
@@ -173,7 +212,7 @@ class GaccumTrainOp:
         self._h2d_done = [torch.cuda.Event() for _ in range(2)]
         self._k_done, self._d2h_done = torch.cuda.Event(), torch.cuda.Event()
         self._host_calls = 0
-        self._stats_ring = torch.zeros(4, dtype=torch.float32).pin_memory()
+        self._stats_ring = _pinned_zeros(4)
 
     def run_host(self, host_grads: Sequence[Optional[torch.Tensor]],
                  host_params_out: Optional[Sequence[torch.Tensor]] = None) -> bool:
@@ -210,14 +249,6 @@ class GaccumTrainOp:
             main.wait_event(self._d2h_done)
         return applied
 
-    def stats(self) -> Dict[str, float]:
-        """Synchronously read what the last step computed (applied, lr, global_norm, clip_scale)."""
-        stream = torch.cuda.current_stream(self.device)
-        self.plan.read_stats(self._stats_host.data_ptr(), stream.cuda_stream)
-        stream.synchronize()
-        a, lr, gn, s = self._stats_host.tolist()
-        return {"applied": bool(a), "lr": lr, "global_norm": gn, "clip_scale": s}
-
     # -- checkpoint compatibility: the reference's Saver sees per-variable tensors --------
     def state_dict(self) -> Dict[str, torch.Tensor]:
         """Per-tensor copies under the reference's names (optimization.py:78, 137-148)."""
@@ -248,7 +279,7 @@ class GaccumTrainOp:
             self.beta2_power = float(sd["beta2_power"])
 
 
-class PackedTrainOp:
+class PackedTrainOp(_DeviceTrainOp):
     """SURVEY.md 8(f) #2 -- gradient hand-off without the scatter.
 
     The reference keeps T parameters, T gradients and T ``accum_grads`` as separate tensors
@@ -268,40 +299,18 @@ class PackedTrainOp:
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0):
-        if not params:
-            raise ValueError("no trainable variables")
-        dev = params[0].device
-        if dev.type != "cuda":
-            raise _lib.GaccumError(_lib.ENODEVICE, "parameters must live on a CUDA device: the train_op has no CPU fallback")
-        self.device, self.params, self.names = dev, list(params), list(names)
-        self.hp, self.N, self.lr_fn, self.global_step = hp, int(accum_n), lr_fn, int(global_step)
-        self.decay = _lib.decay_mask(self.names, hp.weight_decay_rate, exclude_from_weight_decay) \
-            if hp.variant == _lib.ADAM_WEIGHT_DECAY else [False] * len(params)
-        self.plan = Plan([p.numel() for p in params], self.decay, hp, device=dev.index or 0)
-        n = max(self.plan.padded_size, 32)
-        self.param_slab = torch.zeros(n, dtype=torch.float32, device=dev)
-        self.accum = torch.zeros(n, dtype=torch.float32, device=dev)
-        self.m = torch.zeros(n, dtype=torch.float32, device=dev)
-        self.v = torch.zeros(n, dtype=torch.float32, device=dev)
+        super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step)
+        self.param_slab = self._zeros_slab()
+        self.accum = self._zeros_slab()
         with torch.no_grad():
-            for p, o in zip(self.params, self.plan.offsets):
+            for i, p in enumerate(self.params):
                 if p.dtype != torch.float32:
                     raise ValueError("parameters must be fp32")
-                view = self.param_slab[o:o + p.numel()].view(p.shape)
+                view = self._view(self.param_slab, i)
                 view.copy_(p)
-                p.data = view                                            # the caller's tensors now alias the slab
-                p.grad = self.accum[o:o + p.numel()].view(p.shape)      # autograd accumulates straight into accum_grads
-        self.beta1_power, self.beta2_power = _f32(hp.beta1), _f32(hp.beta2)
-        self._stats_host = torch.zeros(4, dtype=torch.float32).pin_memory()
+                p.data = view                          # the caller's tensors now alias the slab
+                p.grad = self.accum_view(i)            # autograd accumulates straight into accum_grads
         self.launches = 0
-
-    def _view(self, slab, i):
-        o = self.plan.offsets[i]
-        return slab[o:o + self.params[i].numel()].view(self.params[i].shape)
-
-    def accum_view(self, i): return self._view(self.accum, i)
-    def m_view(self, i): return self._view(self.m, i)
-    def v_view(self, i): return self._view(self.v, i)
 
     def step(self, stream: Optional[int] = None) -> bool:
         """One ``session.run(train_op)`` AFTER the backward pass has added this micro-batch's gradient into
@@ -313,26 +322,15 @@ class PackedTrainOp:
                 if p.grad is None or p.grad.data_ptr() != self.accum.data_ptr() + 4 * o:
                     raise RuntimeError("p.grad no longer aliases the packed accumulator (zero_grad(set_to_none=True)?)")
             lr = self.lr_fn(g)
-            if stream is None:
-                stream = torch.cuda.current_stream(self.device).cuda_stream
             self.plan.step_packed(0, self.param_slab.data_ptr(), self.accum.data_ptr(), self.m.data_ptr(), self.v.data_ptr(),
-                                  StepArgs(g, self.N, 0, lr, self.beta1_power, self.beta2_power, 0.0), 1, stream)
+                                  self._step_args(g, lr), 1, self._stream(stream))
             self.launches += 1
-            if self.hp.variant == ADAM:
-                self.beta1_power = _f32(np.float32(self.beta1_power) * np.float32(self.hp.beta1))
-                self.beta2_power = _f32(np.float32(self.beta2_power) * np.float32(self.hp.beta2))
+            self._advance_beta_powers()
         self.global_step = g + 1
         return applied
 
-    def stats(self) -> Dict[str, float]:
-        stream = torch.cuda.current_stream(self.device)
-        self.plan.read_stats(self._stats_host.data_ptr(), stream.cuda_stream)
-        stream.synchronize()
-        a, lr, gn, s = self._stats_host.tolist()
-        return {"applied": bool(a), "lr": lr, "global_norm": gn, "clip_scale": s}
 
-
-class HostTrainOp:
+class HostTrainOp(_TrainOpCore):
     """The train_op for a caller whose parameters and gradients live in HOST memory (the reference's
     CPU placement, distributedExample/02 "1 worker CPU").  A thin state holder over the C ABI's
     ``gaccum_host_session``: gradients go H2D every micro-step (double-buffered), the kernel runs,
@@ -346,11 +344,7 @@ class HostTrainOp:
         direction (gaccum_step_host coalesces tensors whose host spacing equals their slab spacing)."""
         numels = [int(np.prod(s)) for s in shapes]
         layout = Plan(numels, None, hp, device=-1)
-        flat = torch.zeros(max(layout.padded_size, 32), dtype=torch.float32)
-        try:
-            flat = flat.pin_memory()
-        except Exception:
-            pass
+        flat = _pinned_zeros(max(layout.padded_size, 32))
         views = [flat[o:o + n].view(tuple(s)) for o, n, s in zip(layout.offsets, numels, shapes)]
         return flat, views
 
@@ -377,24 +371,13 @@ class HostTrainOp:
         for p in host_params:
             if p.device.type != "cpu" or p.dtype != torch.float32 or not p.is_contiguous():
                 raise ValueError("host_params must be contiguous fp32 CPU tensors")
-        self.host_params = list(host_params)
-        self.names, self.hp, self.N, self.lr_fn = list(names), hp, int(accum_n), lr_fn
-        self.global_step = int(global_step)
-        self.decay = _lib.decay_mask(self.names, hp.weight_decay_rate, exclude_from_weight_decay) \
-            if hp.variant == _lib.ADAM_WEIGHT_DECAY else [False] * len(host_params)
-        self.plan = Plan([p.numel() for p in host_params], self.decay, hp, device=device)
+        super().__init__(host_params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, device)
         self.session = _lib.HostSession(self.plan)
-        self._param_ptrs = Plan.ptr_array([p.data_ptr() for p in self.host_params])
+        self._param_ptrs = Plan.ptr_array([p.data_ptr() for p in self.params])
         self.session.set_params(self._param_ptrs)
-        self.beta1_power, self.beta2_power = _f32(hp.beta1), _f32(hp.beta2)
-        self.stats_host = torch.zeros(4, dtype=torch.float32)
-        try:
-            self.stats_host = self.stats_host.pin_memory()
-        except Exception:
-            pass
 
     def bind(self, host_grads: Sequence[Optional[torch.Tensor]]):
-        for g, p in zip(host_grads, self.host_params):
+        for g, p in zip(host_grads, self.params):
             if g is not None and (g.device.type != "cpu" or g.dtype != torch.float32 or not g.is_contiguous() or g.numel() != p.numel()):
                 raise ValueError("host gradients must be contiguous fp32 CPU tensors shaped like their parameter")
         return Plan.ptr_array([0 if g is None else g.data_ptr() for g in host_grads])
@@ -405,12 +388,10 @@ class HostTrainOp:
     def run_bound(self, grad_ptrs) -> bool:
         g = self.global_step
         lr = self.lr_fn(g)
-        self.session.step(grad_ptrs, self._param_ptrs, StepArgs(g, self.N, 0, lr, self.beta1_power, self.beta2_power, 0.0),
-                          self.stats_host.data_ptr())
+        self.session.step(grad_ptrs, self._param_ptrs, self._step_args(g, lr), self._stats_host.data_ptr())
         applied = _lib.is_apply_step(g, self.N)
-        if applied and self.hp.variant == ADAM:
-            self.beta1_power = _f32(np.float32(self.beta1_power) * np.float32(self.hp.beta1))
-            self.beta2_power = _f32(np.float32(self.beta2_power) * np.float32(self.hp.beta2))
+        if applied:
+            self._advance_beta_powers()
         self.global_step = g + 1
         return applied
 
@@ -419,5 +400,4 @@ class HostTrainOp:
 
     def stats(self) -> Dict[str, float]:
         self.sync()
-        a, lr, gn, s = self.stats_host.tolist()
-        return {"applied": bool(a), "lr": lr, "global_norm": gn, "clip_scale": s}
+        return _stats_dict(self._stats_host)
