@@ -63,6 +63,24 @@ class Stats(C.Structure):
                 ("clip_scale", C.c_float)]
 
 
+class LossScaleConfig(C.Structure):
+    """gaccum_loss_scale_config: dynamic loss scaling as TF 2's ``DynamicLossScale`` does it, counted in windows
+    (defaults are TF 2's).  ``initial_scale`` and ``multiplier`` must be powers of two."""
+    _fields_ = [("initial_scale", C.c_double), ("multiplier", C.c_double), ("growth_interval", C.c_int32),
+                ("reserved", C.c_int32)]
+
+    def __init__(self, initial_scale: float = 2.0 ** 15, multiplier: float = 2.0, growth_interval: int = 2000,
+                 reserved: int = 0):
+        super().__init__(float(initial_scale), float(multiplier), int(growth_interval), int(reserved))
+
+
+class LossScaleState(C.Structure):
+    """gaccum_loss_scale_state: the 32-byte device block the apply launches update."""
+    _fields_ = [("scale", C.c_float), ("good_windows", C.c_int32), ("skipped_windows", C.c_uint32),
+                ("last_skipped", C.c_int32), ("beta1_power", C.c_float), ("beta2_power", C.c_float),
+                ("reserved", C.c_float * 2)]
+
+
 _lib = None
 
 
@@ -121,6 +139,8 @@ def _load():
         "gaccum_dp_stage_elements": (i64, [vp, i32]),
         "gaccum_apply_dp": (C.c_int, [vp, C.POINTER(DpComm), vp, vp, vp, C.POINTER(StepArgs), C.c_uint32, vp]),
         "gaccum_step_dp": (C.c_int, [vp, C.POINTER(DpComm), vp, vp, vp, C.POINTER(StepArgs), C.c_uint32, vp]),
+        "gaccum_plan_set_loss_scale": (C.c_int, [vp, C.POINTER(LossScaleConfig), vp]),
+        "gaccum_loss_scale_init": (C.c_int, [vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -257,6 +277,14 @@ class Plan:
 
     def read_stats(self, host_ptr: int, stream: int = 0) -> None:
         _check(_load().gaccum_read_stats(self._h, host_ptr, stream))
+
+    def set_loss_scale(self, cfg: LossScaleConfig, device_state: int) -> None:
+        """Turn dynamic loss scaling on (before the first compute call); ``device_state`` points to 32 bytes of
+        device memory that ``loss_scale_init`` fills."""
+        _check(_load().gaccum_plan_set_loss_scale(self._h, C.byref(cfg), device_state or None))
+
+    def loss_scale_init(self, device_state: int, stream: int = 0) -> None:
+        _check(_load().gaccum_loss_scale_init(self._h, device_state or None, stream))
 
     def close(self) -> None:
         if getattr(self, "_h", None):

@@ -68,6 +68,11 @@ struct gaccum_plan {
 #endif
   int num_sms = 0;
   int max_grid = 0;
+  // dynamic loss scaling (gaccum_plan_set_loss_scale); may be turned on only while `computed` is false
+  bool computed = false;
+  bool ls_on = false;
+  gaccum_loss_scale_config ls_cfg{};
+  gaccum_loss_scale_state* ls_state = nullptr;
   std::mutex mu;
   std::map<const void*, int> grid_cache;   // kernel -> co-resident grid size
 };
@@ -172,9 +177,9 @@ static int launch_apply_noclip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStre
 
 // clip-apply: one cooperative launch, ONE 864-thread CTA per SM (ring + stash take nearly all of the SM's shared
 // memory, so a second CTA could never be co-resident -- the grid is clamped to the SM count)
-template <int VARIANT, bool HAS_G, int CAP>
+template <int VARIANT, bool HAS_G, int CAP, int LS = kLsOff>
 static int launch_apply_clip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream_t st) {
-  const void* fn = (const void*)&apply_clip_kernel<VARIANT, HAS_G, CAP>;
+  const void* fn = (const void*)&apply_clip_kernel<VARIANT, HAS_G, CAP, LS>;
   {
     std::lock_guard<std::mutex> lk(pl->mu);
     if (pl->grid_cache.find(fn) == pl->grid_cache.end()) {
@@ -194,9 +199,27 @@ static int launch_apply_clip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream
   return GACCUM_OK;
 }
 
+// Loss scaling always takes the two-pass kernel: the single-pass apply_kernel stores p, m and v before it could know
+// whether the window overflowed.
+template <int CAP>
+static int launch_apply_loss_scaled(gaccum_plan* pl, KernelParams<CAP>& prm, bool has_g, bool clip, cudaStream_t st) {
+  const int key = (pl->hp.variant == GACCUM_ADAM ? 4 : 0) | (clip ? 2 : 0) | (has_g ? 1 : 0);
+  switch (key) {
+    case 0: return launch_apply_clip<0, false, CAP, kLsNoClip>(pl, prm, st);
+    case 1: return launch_apply_clip<0, true, CAP, kLsNoClip>(pl, prm, st);
+    case 2: return launch_apply_clip<0, false, CAP, kLsClip>(pl, prm, st);
+    case 3: return launch_apply_clip<0, true, CAP, kLsClip>(pl, prm, st);
+    case 4: return launch_apply_clip<1, false, CAP, kLsNoClip>(pl, prm, st);
+    case 5: return launch_apply_clip<1, true, CAP, kLsNoClip>(pl, prm, st);
+    case 6: return launch_apply_clip<1, false, CAP, kLsClip>(pl, prm, st);
+    default: return launch_apply_clip<1, true, CAP, kLsClip>(pl, prm, st);
+  }
+}
+
 template <int CAP>
 static int launch_apply(gaccum_plan* pl, KernelParams<CAP>& prm, bool has_g, cudaStream_t st) {
   const bool clip = pl->hp.clip_norm > 0.0;
+  if (pl->ls_on) return launch_apply_loss_scaled(pl, prm, has_g, clip, st);
   const int key = (pl->hp.variant == GACCUM_ADAM ? 4 : 0) | (clip ? 2 : 0) | (has_g ? 1 : 0);
   switch (key) {
     case 0: return launch_apply_noclip<0, false>(pl, prm, st);
@@ -214,6 +237,7 @@ static inline bool aligned16_host(const void* p) { return ((uintptr_t)p & 15u) =
 
 static int check_compute(gaccum_plan* pl, const float* accum, const float* m, const float* v, bool need_mv) {
   if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  pl->computed = true;   // from here on gaccum_plan_set_loss_scale is refused
   if (pl->device < 0)
     return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): libgaccum has no CPU fallback, a CUDA device is required");
   if (!accum || !aligned16_host(accum)) return fail(GACCUM_EINVAL, "accum must be a 16-byte aligned device pointer");
@@ -235,6 +259,11 @@ static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, f
 #endif
   prm.stats = pl->d_stats;
   prm.sc = sc;
+  if (pl->ls_on) {
+    prm.ls.state = reinterpret_cast<LossScaleState*>(pl->ls_state);
+    prm.ls.multiplier = (float)pl->ls_cfg.multiplier;
+    prm.ls.growth_interval = pl->ls_cfg.growth_interval;
+  }
 }
 
 template <int CAP>
@@ -464,6 +493,47 @@ int64_t gaccum_algorithmic_bytes(const gaccum_plan* pl, int32_t is_apply) {
   return pl->P * (is_apply ? 36 : 12);
 }
 
+// true iff x is 2^k for an integer k in [lo, hi]
+static bool pow2_in(double x, int lo, int hi) {
+  if (!(x > 0.0) || !std::isfinite(x)) return false;
+  int e = 0;
+  const double f = std::frexp(x, &e);   // x = f * 2^e, f in [0.5, 1)
+  return f == 0.5 && e - 1 >= lo && e - 1 <= hi;
+}
+
+int gaccum_plan_set_loss_scale(gaccum_plan* pl, const gaccum_loss_scale_config* cfg, gaccum_loss_scale_state* device_state) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (!cfg) return fail(GACCUM_EINVAL, "cfg is NULL");
+  if (!device_state || !aligned16_host(device_state))
+    return fail(GACCUM_EINVAL, "device_state must be a 16-byte aligned device pointer");
+  if (pl->computed) return fail(GACCUM_EINVAL, "loss scaling can only be set before the plan's first compute call");
+  if (!pow2_in(cfg->initial_scale, 0, 127))
+    return fail(GACCUM_EINVAL, "initial_scale must be a power of two in [1, 2^127] (got %g)", cfg->initial_scale);
+  if (!pow2_in(cfg->multiplier, 1, 127))
+    return fail(GACCUM_EINVAL, "multiplier must be a power of two in [2, 2^127] (got %g)", cfg->multiplier);
+  if (cfg->growth_interval < 1) return fail(GACCUM_EINVAL, "growth_interval must be >= 1 (got %d)", cfg->growth_interval);
+  if (cfg->reserved != 0) return fail(GACCUM_EINVAL, "reserved fields must be 0");
+  static_assert(sizeof(gaccum_loss_scale_state) == sizeof(LossScaleState), "header and kernel disagree");
+  pl->ls_cfg = *cfg;
+  pl->ls_state = device_state;
+  pl->ls_on = true;
+  return GACCUM_OK;
+}
+
+int gaccum_loss_scale_init(gaccum_plan* pl, gaccum_loss_scale_state* device_state, gaccum_stream_t stream) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (!pl->ls_on) return fail(GACCUM_EINVAL, "loss scaling is not set on this plan (gaccum_plan_set_loss_scale)");
+  if (!device_state || !aligned16_host(device_state))
+    return fail(GACCUM_EINVAL, "device_state must be a 16-byte aligned device pointer");
+  if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): a CUDA device is required");
+  DeviceGuard guard(pl->device);
+  loss_scale_init_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(reinterpret_cast<LossScaleState*>(device_state),
+                                                           (float)pl->ls_cfg.initial_scale, (float)pl->hp.beta1,
+                                                           (float)pl->hp.beta2);
+  CUDA_TRY(cudaGetLastError());
+  return GACCUM_OK;
+}
+
 static int accumulate_impl(gaccum_plan* pl, const float* const* grads, float* accum,
                            const gaccum_step_args* a, gaccum_stream_t stream) {
   if (int rc = check_compute(pl, accum, nullptr, nullptr, false)) return rc;
@@ -617,6 +687,7 @@ static int do_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float*
 
 int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* const* grads, float* m, float* v,
                     const gaccum_step_args* a, uint32_t epoch, gaccum_stream_t stream) {
+  if (pl && pl->ls_on) return fail(GACCUM_EINVAL, "the fused data-parallel apply does not support loss scaling");
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (comm->world < 2 || comm->world > GACCUM_MAX_RANKS || comm->rank < 0 || comm->rank >= comm->world)
     return fail(GACCUM_EINVAL, "world must be 2..%d and 0 <= rank < world", GACCUM_MAX_RANKS);
@@ -639,6 +710,7 @@ int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* co
 
 int gaccum_step_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* const* grads, float* m, float* v,
                    const gaccum_step_args* a, uint32_t epoch, gaccum_stream_t stream) {
+  if (pl && pl->ls_on) return fail(GACCUM_EINVAL, "the fused data-parallel step does not support loss scaling");
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (int rc = check_args(a)) return rc;
   if (!grads) return fail(GACCUM_EINVAL, "grads is NULL");
@@ -717,6 +789,8 @@ int gaccum_host_session_create(gaccum_host_session** out, gaccum_plan* pl) {
   if (!out) return fail(GACCUM_EINVAL, "out is NULL");
   *out = nullptr;
   if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  // host-resident models train in fp32 (no fp16 autocast on the CPU): nothing to loss-scale
+  if (pl->ls_on) return fail(GACCUM_EINVAL, "the host-buffer session does not support loss scaling");
   if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): libgaccum has no CPU fallback, a CUDA device is required");
   DeviceGuard guard(pl->device);
   gaccum_host_session* s = new (std::nothrow) gaccum_host_session();
@@ -824,6 +898,7 @@ int gaccum_step_host(gaccum_host_session* s, const float* const* host_grads, flo
   if (!s || !host_grads) return fail(GACCUM_EINVAL, "bad arguments to gaccum_step_host");
   if (int rc = check_args(a)) return rc;
   gaccum_plan* pl = s->plan;
+  if (pl->ls_on) return fail(GACCUM_EINVAL, "the host-buffer session does not support loss scaling");
   DeviceGuard guard(pl->device);
   const int b = (int)(s->calls & 1);
   ++s->calls;

@@ -11,7 +11,9 @@
 //   apply_clip_kernel    the apply branch WITH tf.clip_by_global_norm                  (36 B/elem)
 //                        optimization.py:80-88, 128-177.  The global norm of ALL tensors is needed before
 //                        ANY element can be updated: one cooperative launch, two passes around a grid
-//                        barrier (described at the kernel).
+//                        barrier (described at the kernel).  Its loss-scaled instantiations (LS != kLsOff) also
+//                        unscale by 1/S and skip the whole window when a' or the norm is not finite; with
+//                        clipping off they run the same two passes with the norm and the clip multiply compiled out.
 // Arithmetic uses round-to-nearest intrinsics (__fmul_rn, __fadd_rn, __fdiv_rn, __fsqrt_rn) so nvcc
 // cannot contract mul+add into FMA: the reference graph is un-fused, one rounding per TF op, and we
 // reproduce it bit for bit (the kernels are HBM-bound, the extra flops are free).
@@ -65,6 +67,28 @@ struct Scalars {
   float alpha;   // B only: lr*sqrt(1-b2^t)/(1-b1^t)          TF1 ApplyAdam
 };
 
+// gaccum_loss_scale_state (gaccum.h): caller-owned device memory, written only by the loss-scaled apply launch
+struct LossScaleState {
+  float scale;                // S, a power of two in [1, 2^127]
+  int32_t good_windows;       // applied windows since S last changed
+  uint32_t skipped_windows;   // overflowed windows since initialisation
+  int32_t last_skipped;       // 1 if the last apply launch skipped its window
+  float beta1_power, beta2_power;   // GACCUM_ADAM: TF1's beta powers, advanced on applied windows only
+  float reserved[2];
+};
+static_assert(sizeof(LossScaleState) == 32, "gaccum_loss_scale_state is 32 bytes");
+
+// Loss scaling of one apply launch.  Kept after the pointer table, at the end of KernelParams, so every other member
+// sits where it does without loss scaling.
+struct LossScaleParams {
+  LossScaleState* state;
+  float multiplier;           // a power of two >= 2
+  int32_t growth_interval;    // applied windows before S grows
+};
+constexpr int kLsOff = 0;       // no loss scaling
+constexpr int kLsClip = 1;      // loss scaling + tf.clip_by_global_norm
+constexpr int kLsNoClip = 2;    // loss scaling without clipping: pass 1 only looks for non-finite elements of a'
+
 template <int CAP>
 struct KernelParams {
   const TileDesc* tiles;
@@ -80,6 +104,7 @@ struct KernelParams {
 #endif
   Scalars sc;
   PtrTable<CAP> tab;
+  LossScaleParams ls;   // apply_clip_kernel with LS != kLsOff only
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -191,6 +216,51 @@ __device__ __forceinline__ float add_sq(float acc, const float4 x, const Scalars
   return add_sq(add_sq(add_sq(add_sq(acc, x.x, sc), x.y, sc), x.z, sc), x.w, sc);
 }
 
+// Loss scaling: the accumulators hold sums of S*g.  c = ((1.0*a')/N) * (1/S), two correctly rounded ops; S is a power of
+// two, so the multiply is exact wherever c is a normal number.  Pass 1 also notes any non-finite element of a'.
+__device__ __forceinline__ float unscale(float a, float inv_s, const Scalars& sc) {
+  return __fmul_rn(normalize(a, sc.nf, sc.inv_nf), inv_s);
+}
+template <int LS>
+__device__ __forceinline__ float ls_pass1(float acc, float x, float inv_s, bool& bad, const Scalars& sc) {
+  bad |= !(fabsf(x) <= 3.402823466e38f);
+  if constexpr (LS == kLsClip) {
+    const float c = unscale(x, inv_s, sc);
+    acc = fmaf(c, c, acc);
+  }
+  return acc;
+}
+template <int LS>
+__device__ __forceinline__ float ls_pass1(float acc, const float4 x, float inv_s, bool& bad, const Scalars& sc) {
+  return ls_pass1<LS>(ls_pass1<LS>(ls_pass1<LS>(ls_pass1<LS>(acc, x.x, inv_s, bad, sc), x.y, inv_s, bad, sc), x.z, inv_s, bad, sc),
+                      x.w, inv_s, bad, sc);
+}
+// pass 2 of the clip kernel on one element: c = a'/N (unscaled under loss scaling), times the clip scale s unless
+// clipping is off, then one Adam step
+template <int VARIANT, int LS>
+__device__ __forceinline__ void update_elem2(float a, float s, float inv_s, float& p, float& m, float& v, bool decay,
+                                             const Scalars& sc) {
+  if constexpr (LS == kLsOff) {
+    update_elem<VARIANT>(a, true, s, p, m, v, decay, sc);
+  } else {
+    float c = unscale(a, inv_s, sc);
+    if constexpr (LS == kLsClip) c = __fmul_rn(c, s);
+    adam_elem<VARIANT>(c, p, m, v, decay, sc);
+  }
+}
+template <int VARIANT, int LS>
+__device__ __forceinline__ void update_vec2(const float4 a, float s, float inv_s, float4& p, float4& m, float4& v, bool decay,
+                                            const Scalars& sc) {
+  if constexpr (LS == kLsOff) {
+    update_vec<VARIANT>(a, true, s, p, m, v, decay, sc);
+  } else {
+    update_elem2<VARIANT, LS>(a.x, s, inv_s, p.x, m.x, v.x, decay, sc);
+    update_elem2<VARIANT, LS>(a.y, s, inv_s, p.y, m.y, v.y, decay, sc);
+    update_elem2<VARIANT, LS>(a.z, s, inv_s, p.z, m.z, v.z, decay, sc);
+    update_elem2<VARIANT, LS>(a.w, s, inv_s, p.w, m.w, v.w, decay, sc);
+  }
+}
+
 // tf.clip_by_global_norm (TF 1.15): scale = clip * min(1/gn, 1/clip) + (gn - gn)
 __device__ __forceinline__ float clip_scale(float gn, float clip) {
   const float inv = __fdiv_rn(1.0f, gn);
@@ -254,6 +324,16 @@ accumulate_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     prm.stats[0] = 0.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f;
   }
   if ((int)blockIdx.x < prm.num_tiles) accumulate_tile<FROM_ZERO>(prm.tiles[blockIdx.x], prm);
+}
+
+// gaccum_loss_scale_init: one thread writes the initial loss-scaling state (a kernel, so the call stays asynchronous and
+// graph-capturable)
+__global__ void loss_scale_init_kernel(LossScaleState* st, float scale, float b1, float b2) {
+  LossScaleState s{};
+  s.scale = scale;
+  s.beta1_power = b1;
+  s.beta2_power = b2;
+  *st = s;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -369,9 +449,11 @@ struct __align__(16) SlotMeta {
 // exact accumulation of non-negative doubles: 68 bins of 32 payload bits in 64-bit containers cover the whole
 // binary64 range (2^-1074 .. 2^1024); a container overflows only after 2^31 additions
 constexpr int kAccBins = 68;
+constexpr unsigned int kElemNonfinite = 4u;
 struct LaunchCounters {
   unsigned long long p1_ticket, p2_ticket;
-  unsigned int nonfinite, pad;                  // nonfinite: bit 0 = +inf seen, bit 1 = NaN seen
+  unsigned int nonfinite, pad;                  // nonfinite: bit 0 = +inf seen, bit 1 = NaN seen (in the norm's sum),
+                                                // bit 2 = a non-finite element of a' (loss-scaled launches only)
   unsigned long long bins[kAccBins];
 };
 
@@ -488,9 +570,11 @@ __device__ __forceinline__ double acc_value(const unsigned long long* bins /* kA
 
 // ---- pass 1, consumer side: one tile out of slot [G | a]; returns this THREAD's partial of sum((a'/N)^2) ----
 // A tile the producer did not copy (nvec == 0), and the < 4 tail elements of any tile, travel through global memory.
-template <bool HAS_G, int CAP>
+// Loss-scaled (LS != kLsOff): the partial is of sum(((a'/N)(1/S))^2) (none without clipping), and `bad` is set when an
+// element of a' is not finite.
+template <bool HAS_G, int LS, int CAP>
 __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float4* slot, uint64_t* empty,
-                                           float4* const stash, const uint64_t pol) {
+                                           float4* const stash, const uint64_t pol, const float inv_s, bool& bad) {
   const float* __restrict__ g = nullptr;
   if constexpr (HAS_G) g = grad_ptr(prm.tab, d);
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
@@ -506,28 +590,33 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
                 if (stash == nullptr) st_policy(a4 + i, x[u], pol);
               }
               if (stash != nullptr) stash[i] = x[u];
-              acc = add_sq(acc, x[u], prm.sc);
+              if constexpr (LS == kLsOff) acc = add_sq(acc, x[u], prm.sc);
+              else acc = ls_pass1<LS>(acc, x[u], inv_s, bad, prm.sc);
             },
             [&](uint32_t i) {
               float xs = a[i];
               if (g) { xs = __fadd_rn(xs, ld_stream(g + i)); a[i] = xs; }
-              acc = add_sq(acc, xs, prm.sc);
+              if constexpr (LS == kLsOff) acc = add_sq(acc, xs, prm.sc);
+              else acc = ls_pass1<LS>(acc, xs, inv_s, bad, prm.sc);
             });
   return acc;
 }
 
 // ---- pass 2, consumer side: one tile out of slot [p | m | v | a']; a' from the slot or from the stash ----
 // The caller has waited on the slot's `full` barrier (it had to, to learn which tile this is).
-template <int VARIANT, int CAP>
+// Loss-scaled: `sc` carries the alpha computed from the device's beta powers, and a skipped window (`skip`) stores
+// a = 0 and nothing else.
+template <int VARIANT, int LS, int CAP>
 __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelParams<CAP>& prm, const float s, const float4* slot,
-                                             uint64_t* empty, const float4* const stash) {
+                                             uint64_t* empty, const float4* const stash, const Scalars& sc, const float inv_s,
+                                             const bool skip) {
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
   float* __restrict__ m = prm.m + soff;
   float* __restrict__ v = prm.v + soff;
   float* __restrict__ p = param_ptr(prm.tab, d);
   const bool decay = (d.tensor_flags >> 31) != 0;
-  const Scalars& sc = prm.sc;
+  const bool write = LS == kLsOff || !skip;
   float4* a4 = reinterpret_cast<float4*>(a);
   float4* m4 = reinterpret_cast<float4*>(m);
   float4* v4 = reinterpret_cast<float4*>(v);
@@ -540,14 +629,19 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
             },
             [&] { __syncwarp(); if ((threadIdx.x & 31) == 0) mbar_arrive(empty); },
             [&](int u, uint32_t i) {
-              update_vec<VARIANT>(va[u], true, s, vp[u], vm[u], vv[u], decay, sc);
-              __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
+              if (write) {
+                update_vec2<VARIANT, LS>(va[u], s, inv_s, vp[u], vm[u], vv[u], decay, sc);
+                __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
+              }
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
             },
             [&](uint32_t i) {
-              float px = p[i], mx = m[i], vx = v[i];
-              update_elem<VARIANT>(a[i], true, s, px, mx, vx, decay, sc);
-              p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
+              if (write) {
+                float px = p[i], mx = m[i], vx = v[i];
+                update_elem2<VARIANT, LS>(a[i], s, inv_s, px, mx, vx, decay, sc);
+                p[i] = px; m[i] = mx; v[i] = vx;
+              }
+              a[i] = 0.f;
             });
 }
 
@@ -556,13 +650,23 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
 // Registers: 864 threads in one CTA cap the kernel at 72 per thread.  The AdamWeightDecay instantiations (VARIANT 0)
 // fit without spilling; the plain-Adam ones with clipping (VARIANT 1, used only when tf_adam is combined with
 // clip_norm > 0) spill 8-20 bytes per thread to local memory (ptxas -v).  What that costs has not been measured.
-template <int VARIANT, bool HAS_G, int CAP>
+//
+// Loss scaling (LS != kLsOff, gaccum_plan_set_loss_scale).  Thread 0 of every CTA reads S, the counters and the beta
+// powers from prm.ls.state during set-up, i.e. before its CTA arrives at the grid barrier; pass 1 ORs kElemNonfinite
+// into the launch's counters when an element of a' is not finite.  After the barrier every CTA takes the same decision
+// from the same launch-wide flags: skip iff an element was non-finite or, with clipping, gn is.  A skipped window
+// stores a = 0 and leaves p, m and v alone.  Block 0's thread 0 writes the new state at the very end -- after the
+// barrier, so no CTA can see the new S or beta powers in this launch.
+template <int VARIANT, bool HAS_G, int CAP, int LS = kLsOff>
 __global__ void __launch_bounds__(kClipThreads, 1)
 apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   extern __shared__ __align__(128) unsigned char smem_dyn[];
   __shared__ unsigned long long s_bins[kConsumerThreads / 32][kAccBins];   // one exact accumulator per consumer warp (13 KB)
   __shared__ unsigned int s_nonfinite;
   __shared__ float s_bcast[2];
+  __shared__ LossScaleState s_ls;        // loss-scaled: the state as this launch found it
+  __shared__ Scalars s_sc;               // loss-scaled GACCUM_ADAM: prm.sc with alpha from the device's beta powers
+  __shared__ int s_skip;
   __shared__ uint32_t s_set;
   __shared__ __align__(8) uint64_t s_full1[kGroups][kP1Slots], s_empty1[kGroups][kP1Slots];
   __shared__ __align__(8) uint64_t s_full2[kGroups][kP2Slots], s_empty2[kGroups][kP2Slots];
@@ -608,6 +712,20 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    if constexpr (LS != kLsOff) {
+      const LossScaleState* st = prm.ls.state;
+      s_ls.scale = __ldcg(&st->scale);
+      s_ls.good_windows = __ldcg(&st->good_windows);
+      s_ls.skipped_windows = __ldcg(&st->skipped_windows);
+      s_ls.beta1_power = __ldcg(&st->beta1_power);
+      s_ls.beta2_power = __ldcg(&st->beta2_power);
+      if constexpr (VARIANT == 1) {
+        // make_scalars' op order: lr * sqrt(1 - b2^t) / (1 - b1^t), one rounding per op
+        s_sc = prm.sc;
+        s_sc.alpha = __fdiv_rn(__fmul_rn(prm.sc.lr, __fsqrt_rn(__fsub_rn(1.0f, s_ls.beta2_power))),
+                               __fsub_rn(1.0f, s_ls.beta1_power));
+      }
+    }
   }
   for (int i = threadIdx.x; i < (kConsumerThreads / 32) * kAccBins; i += kClipThreads) (&s_bins[0][0])[i] = 0ull;
   __syncthreads();
@@ -783,6 +901,8 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     }
     // ---- pass 1: whatever tiles the producer hands over, until its end marker ----
     unsigned int my_nonfinite = 0;
+    float inv_s = 1.0f;
+    if constexpr (LS != kLsOff) inv_s = __fdiv_rn(1.0f, s_ls.scale);   // exact: S is a power of two
     {
       RingPos rp;
       int n_seen = 0;
@@ -801,12 +921,17 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         const bool own = n_seen < n_st;
         const bool park = own && stash_ok<HAS_G>(meta.d, prm);
         float4* const st = park ? stash + (size_t)n_seen * (kTile / 4) : nullptr;
-        const float part = norm_tile<HAS_G>(meta.d, prm, ring + (size_t)rp.slot * kP1SlotVecs, &s_empty1[grp][rp.slot], st, pol_last);
-        // warp total in fp64, fixed butterfly order; lane 0 adds it EXACTLY into its warp's accumulator
-        double w = (double)part;
+        bool bad = false;
+        const float part = norm_tile<HAS_G, LS>(meta.d, prm, ring + (size_t)rp.slot * kP1SlotVecs, &s_empty1[grp][rp.slot], st,
+                                                pol_last, inv_s, bad);
+        if constexpr (LS != kLsOff) { if (bad) my_nonfinite |= kElemNonfinite; }
+        if constexpr (LS != kLsNoClip) {
+          // warp total in fp64, fixed butterfly order; lane 0 adds it EXACTLY into its warp's accumulator
+          double w = (double)part;
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) w += __shfl_xor_sync(0xffffffffu, w, o);
-        if ((threadIdx.x & 31) == 0) acc_add(s_bins[warp], my_nonfinite, w);
+          for (int o = 16; o > 0; o >>= 1) w += __shfl_xor_sync(0xffffffffu, w, o);
+          if ((threadIdx.x & 31) == 0) acc_add(s_bins[warp], my_nonfinite, w);
+        }
         ++n_seen;
         rp.advance(kP1Slots);
       }
@@ -841,16 +966,29 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     if (leader) mbar_arrive(&s_go[grp]);                     // this group's producer may now fetch pool tiles
     stamp(2);
     // ---- every CTA evaluates the same exact sum the same way: bit-identical gn and clip scale everywhere ----
-    if (threadIdx.x < kAccBins) s_bins[0][threadIdx.x] = __ldcg(&ctr->bins[threadIdx.x]);
-    named_bar_sync(1, kConsumerThreads);
-    if (threadIdx.x == 0) {
-      const double tot = acc_value(s_bins[0], __ldcg(&ctr->nonfinite));
-      const float g_norm = __fsqrt_rn((float)tot);          // tf.linalg.global_norm
-      s_bcast[0] = clip_scale(g_norm, prm.sc.clip);
-      s_bcast[1] = g_norm;
+    if constexpr (LS == kLsNoClip) {
+      if (threadIdx.x == 0) {
+        s_bcast[0] = 1.f;                                   // no clipping: stats as the un-clipped apply writes them
+        s_bcast[1] = 0.f;
+        s_skip = (__ldcg(&ctr->nonfinite) & kElemNonfinite) != 0;
+      }
+    } else {
+      if (threadIdx.x < kAccBins) s_bins[0][threadIdx.x] = __ldcg(&ctr->bins[threadIdx.x]);
+      named_bar_sync(1, kConsumerThreads);
+      if (threadIdx.x == 0) {
+        const unsigned int nonfinite = __ldcg(&ctr->nonfinite);
+        const double tot = acc_value(s_bins[0], nonfinite);
+        const float g_norm = __fsqrt_rn((float)tot);          // tf.linalg.global_norm
+        s_bcast[0] = clip_scale(g_norm, prm.sc.clip);
+        s_bcast[1] = g_norm;
+        if constexpr (LS != kLsOff) s_skip = (nonfinite & kElemNonfinite) != 0 || !(fabsf(g_norm) <= 3.402823466e38f);
+      }
     }
     named_bar_sync(1, kConsumerThreads);
     const float s = s_bcast[0];
+    bool skip = false;
+    if constexpr (LS != kLsOff) skip = s_skip != 0;
+    const Scalars& sc = (LS != kLsOff && VARIANT == 1) ? s_sc : prm.sc;
     // ---- pass 2: whatever tiles the producer hands over, until its end marker ----
     {
       RingPos rp;
@@ -859,12 +997,39 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         const SlotMeta meta = s_meta2[grp][rp.slot];
         if (meta.d.len == 0) break;
         const float4* const st = meta.stash_slot != kNoStash ? stash + (size_t)meta.stash_slot * (kTile / 4) : nullptr;
-        update_tile2<VARIANT>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st);
+        update_tile2<VARIANT, LS>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st, sc, inv_s,
+                                  skip);
         rp.advance(kP2Slots);
       }
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) {
       prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s;
+      if constexpr (LS != kLsOff) {
+        // TF 2 DynamicLossScale, counted in windows (gaccum.h, gaccum_loss_scale_config)
+        LossScaleState* out = prm.ls.state;
+        const float S = s_ls.scale;
+        if (skip) {
+          const float down = __fdiv_rn(S, prm.ls.multiplier);   // exact: both are powers of two
+          out->scale = down < 1.0f ? 1.0f : down;
+          out->good_windows = 0;
+          out->skipped_windows = s_ls.skipped_windows + 1u;
+          out->last_skipped = 1;
+        } else {
+          const int32_t good = s_ls.good_windows + 1;
+          if (good >= prm.ls.growth_interval) {
+            const float up = __fmul_rn(S, prm.ls.multiplier);
+            if (fabsf(up) <= 3.402823466e38f) out->scale = up;
+            out->good_windows = 0;
+          } else {
+            out->good_windows = good;
+          }
+          out->last_skipped = 0;
+          if constexpr (VARIANT == 1) {                         // TF1 AdamOptimizer._finish, applied windows only
+            out->beta1_power = __fmul_rn(s_ls.beta1_power, prm.sc.b1);
+            out->beta2_power = __fmul_rn(s_ls.beta2_power, prm.sc.b2);
+          }
+        }
+      }
     }
   }
   __syncthreads();

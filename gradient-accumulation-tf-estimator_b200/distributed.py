@@ -9,7 +9,8 @@ packed accumulator slab is exchanged ONCE per window, on the apply step, over NC
     apply step       : a += G (local)  ->  all-reduce(a)  ->  apply kernel without a gradient
 
 Every rank then runs the identical deterministic apply on identical inputs, so replicas stay
-bit-identical without an extra norm exchange.  The producer keeps 04's convention of dividing the
+bit-identical without an extra norm exchange.  Under loss scaling the same holds for the skip decision: it is
+taken from the all-reduced accumulators, so an overflow on one rank makes every rank skip.  The producer keeps 04's convention of dividing the
 loss by ``num_workers``.  (04's second reduction inside ``apply_gradients`` -- SURVEY.md 5.8 -- is
 not reproduced.)
 """
@@ -86,9 +87,11 @@ class FusedDataParallelTrainOp:
 
     def __init__(self, params: Sequence[torch.Tensor], names: Sequence[str], hp, accum_n: int, lr_fn,
                  process_group=None, exclude_from_weight_decay=("LayerNorm", "layer_norm", "bias"),
-                 global_step: int = 0):
+                 global_step: int = 0, loss_scale=None):
         import torch.distributed._symmetric_memory as symm
         from .train_op import GaccumTrainOp
+        if loss_scale is not None:
+            raise ValueError("the fused data-parallel train op does not support loss scaling; use dp_mode='allreduce'")
         if not dist.is_initialized():
             raise RuntimeError("torch.distributed must be initialised (backend nccl)")
         self.group = process_group if process_group is not None else dist.group.WORLD

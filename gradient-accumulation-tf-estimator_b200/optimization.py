@@ -24,13 +24,15 @@ from typing import Callable, Iterable, List, Optional, Sequence, Tuple, Union
 import torch
 
 from . import _lib, graph
-from ._lib import ADAM, ADAM_WEIGHT_DECAY, HParams
+from ._lib import ADAM, ADAM_WEIGHT_DECAY, HParams, LossScaleConfig
 from .train_op import GaccumTrainOp
 
 # optimization.py:76 hard-codes 8 (README.md:17,34 says 4).  The signature has no argument for
 # it, so it is a module attribute (and GACCUM_MULTIPLIER in the environment) -- default as shipped.
 gradient_accumulation_multiplier = int(os.environ.get("GACCUM_MULTIPLIER", "8"))
 clip_norm = 1.0   # optimization.py:84
+# Dynamic loss scaling for fp16 mixed precision (a LossScaleConfig), off by default; create_optimizer reads it.
+loss_scale: Optional[LossScaleConfig] = None
 
 LossLike = Union[torch.Tensor, Callable[[], torch.Tensor]]
 LrLike = Union[float, Callable[[int], float]]
@@ -130,7 +132,7 @@ class TrainOp:
 
     def __init__(self, loss: LossLike, tvars: Sequence[graph.Variable], optimizer: _OptimizerBase,
                  accum_n: int, clip: Optional[float], global_step: graph.GlobalStep, process_group=None,
-                 dp_mode: str = "fused"):
+                 dp_mode: str = "fused", loss_scale: Optional[LossScaleConfig] = None):
         self.loss = loss
         self.tvars = list(tvars)
         self.optimizer = optimizer
@@ -146,13 +148,16 @@ class TrainOp:
             from .distributed import DataParallelTrainOp, FusedDataParallelTrainOp
             pg = None if process_group is True else process_group
             if dp_mode == "fused":
-                self.dp = FusedDataParallelTrainOp(tensors, names, hp, accum_n, lr_fn, pg, exclude, int(global_step))
+                self.dp = FusedDataParallelTrainOp(tensors, names, hp, accum_n, lr_fn, pg, exclude, int(global_step),
+                                                   loss_scale=loss_scale)
                 self.engine = self.dp.engine
             else:
-                self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step))
+                self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step),
+                                            loss_scale=loss_scale)
                 self.dp = DataParallelTrainOp(self.engine, pg)
         else:
-            self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step))
+            self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step),
+                                        loss_scale=loss_scale)
         self.last_loss: Optional[torch.Tensor] = None
 
     @property
@@ -169,9 +174,12 @@ class TrainOp:
         self.global_step.assign(int(sd["global_step"]))
 
     def gradients(self) -> List[Optional[torch.Tensor]]:
-        """``tf.gradients(loss, tvars)`` (optimization.py:71): evaluated every micro-step."""
+        """``tf.gradients(loss, tvars)`` (optimization.py:71): evaluated every micro-step.  Under loss scaling these
+        are the gradients of ``loss * S``, S read on the device; ``last_loss`` stays unscaled."""
         loss = self.loss() if callable(self.loss) else self.loss
         self.last_loss = loss.detach()
+        if self.engine.loss_scale is not None:
+            loss = loss * self.engine.loss_scale
         grads = torch.autograd.grad(loss, [v.tensor for v in self.tvars], allow_unused=True)
         return [None if g is None else g.contiguous() for g in grads]
 
@@ -191,14 +199,16 @@ class TrainOp:
 def gradient_accumulation_train_op(loss: LossLike, optimizer: _OptimizerBase, gradient_accumulation_multiplier: int,
                                    clip_norm: Optional[float] = None, global_step: Optional[graph.GlobalStep] = None,
                                    tvars: Optional[Sequence[graph.Variable]] = None, process_group=None,
-                                   dp_mode: str = "fused") -> TrainOp:
+                                   dp_mode: str = "fused", loss_scale: Optional[LossScaleConfig] = None) -> TrainOp:
     """The recipe the example scripts inline (02:47-73, 04:48-74, another-example.py:126-155):
-    N from ``params``, optimizer given, no clipping unless asked."""
+    N from ``params``, optimizer given, no clipping unless asked.  ``loss_scale`` turns on dynamic loss scaling for
+    fp16 mixed precision: gradients are taken of ``loss * S`` and a window that overflows is skipped on the device."""
     gs = global_step or graph.get_or_create_global_step()
     tv = list(tvars) if tvars is not None else graph.trainable_variables()
     if not tv:
         raise ValueError("no trainable variables registered (graph.add_variable / graph.register_module)")
-    return TrainOp(loss, tv, optimizer, int(gradient_accumulation_multiplier), clip_norm, gs, process_group, dp_mode)
+    return TrainOp(loss, tv, optimizer, int(gradient_accumulation_multiplier), clip_norm, gs, process_group, dp_mode,
+                   loss_scale)
 
 
 def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
@@ -217,4 +227,4 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
         weight_decay_rate=0.01, beta_1=0.9, beta_2=0.999, epsilon=1e-6,
         exclude_from_weight_decay=["LayerNorm", "layer_norm", "bias"])
     return gradient_accumulation_train_op(loss, optimizer, gradient_accumulation_multiplier,
-                                          clip_norm=clip_norm, global_step=global_step)
+                                          clip_norm=clip_norm, global_step=global_step, loss_scale=loss_scale)

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import ADAM, HParams, Plan, StepArgs
+from ._lib import ADAM, HParams, LossScaleConfig, Plan, StepArgs
 
 
 def _f32(x) -> float:
@@ -57,13 +57,17 @@ class _TrainOpCore:
         # TF1 AdamOptimizer._create_slots: beta powers start at beta
         self.beta1_power, self.beta2_power = _f32(hp.beta1), _f32(hp.beta2)
         self._stats_host = _pinned_zeros(4)
+        self._ls_state: Optional[torch.Tensor] = None    # the loss-scaling block, when loss scaling is on
+        self.loss_scale: Optional[torch.Tensor] = None
 
     def _step_args(self, g: int, lr: float) -> StepArgs:
         return StepArgs(g, self.N, 0, lr, self.beta1_power, self.beta2_power, 0.0)
 
     def _advance_beta_powers(self) -> None:
-        """TF1 AdamOptimizer._finish: beta_power <- beta_power * beta (fp32) after the updates of an apply step."""
-        if self.hp.variant == ADAM:
+        """TF1 AdamOptimizer._finish: beta_power <- beta_power * beta (fp32) after the updates of an apply step.
+        Under loss scaling the beta powers live in the device block and the apply kernel advances them, on applied
+        windows only."""
+        if self.hp.variant == ADAM and self._ls_state is None:
             self.beta1_power = _f32(np.float32(self.beta1_power) * np.float32(self.hp.beta1))
             self.beta2_power = _f32(np.float32(self.beta2_power) * np.float32(self.hp.beta2))
 
@@ -71,7 +75,8 @@ class _TrainOpCore:
 class _DeviceTrainOp(_TrainOpCore):
     """A train op whose parameters live on one CUDA device and whose Adam moments are packed HBM slabs."""
 
-    def __init__(self, params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step):
+    def __init__(self, params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step,
+                 loss_scale: Optional[LossScaleConfig] = None):
         if not params:
             raise ValueError("no trainable variables")
         self.device = params[0].device
@@ -81,6 +86,13 @@ class _DeviceTrainOp(_TrainOpCore):
                          self.device.index or 0)
         self.m = self._zeros_slab()
         self.v = self._zeros_slab()
+        if loss_scale is not None:
+            # gaccum_loss_scale_state: 8 x 4 bytes; `loss_scale` views its first word, S, so a producer can write
+            # (loss * op.loss_scale).backward() without reading S back to the host
+            self._ls_state = torch.zeros(8, dtype=torch.float32, device=self.device)
+            self.plan.set_loss_scale(loss_scale, self._ls_state.data_ptr())
+            self.plan.loss_scale_init(self._ls_state.data_ptr(), self._stream())
+            self.loss_scale = self._ls_state[0]
 
     def _zeros_slab(self) -> torch.Tensor:
         return torch.zeros(max(self.plan.padded_size, 32), dtype=torch.float32, device=self.device)
@@ -109,13 +121,47 @@ class _DeviceTrainOp(_TrainOpCore):
         stream.synchronize()
         return _stats_dict(self._stats_host)
 
+    def loss_scale_state(self) -> Dict[str, float]:
+        """Synchronously read the loss-scaling block (for logging): scale, good_windows, skipped_windows and
+        last_skipped (True if the last apply step skipped its window)."""
+        if self._ls_state is None:
+            raise ValueError("loss scaling is off for this train op")
+        words = self._ls_state.cpu()
+        ints = words.view(torch.int32)
+        return {"scale": float(words[0]), "good_windows": int(ints[1]),
+                "skipped_windows": int(ints[2]) & 0xFFFFFFFF, "last_skipped": bool(ints[3])}
+
+    def _loss_scale_state_dict(self, out: Dict[str, torch.Tensor]) -> None:
+        """TF 2 LossScaleOptimizer's variable names; the beta powers come from the device block."""
+        words = self._ls_state.cpu()
+        out["loss_scale/current_loss_scale"] = words[0].clone()
+        out["loss_scale/good_steps"] = torch.tensor(int(words.view(torch.int32)[1]), dtype=torch.int64)
+        if self.hp.variant == ADAM:
+            out["beta1_power"] = words[4].clone()
+            out["beta2_power"] = words[5].clone()
+
+    def _load_loss_scale_state(self, sd: Dict[str, torch.Tensor]) -> None:
+        words = self._ls_state.cpu()
+        if "loss_scale/current_loss_scale" in sd:
+            s = float(sd["loss_scale/current_loss_scale"])
+            m, e = np.frexp(s)
+            if not (m == 0.5 and 1 <= e <= 128):
+                raise ValueError(f"loss_scale/current_loss_scale must be a power of two in [1, 2^127], got {s!r}")
+            words[0] = s
+            words.view(torch.int32)[1] = int(sd["loss_scale/good_steps"])
+        if self.hp.variant == ADAM and "beta1_power" in sd:
+            words[4] = float(sd["beta1_power"])
+            words[5] = float(sd["beta2_power"])
+        self._ls_state.copy_(words)
+
 
 class GaccumTrainOp(_DeviceTrainOp):
     def __init__(self, params: Sequence[torch.Tensor], names: Sequence[str], hp: HParams, accum_n: int,
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
-                 global_step: int = 0, accum: Optional[torch.Tensor] = None):
-        super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step)
+                 global_step: int = 0, accum: Optional[torch.Tensor] = None,
+                 loss_scale: Optional[LossScaleConfig] = None):
+        super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale)
         for p in self.params:
             if p.dtype != torch.float32 or not p.is_contiguous() or p.device != self.device:
                 raise ValueError("parameters must be contiguous fp32 tensors on one device")
@@ -261,6 +307,8 @@ class GaccumTrainOp(_DeviceTrainOp):
         if self.hp.variant == ADAM:
             out["beta1_power"] = torch.tensor(self.beta1_power, dtype=torch.float32)
             out["beta2_power"] = torch.tensor(self.beta2_power, dtype=torch.float32)
+        if self._ls_state is not None:
+            self._loss_scale_state_dict(out)
         return out
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True) -> None:
@@ -274,7 +322,9 @@ class GaccumTrainOp(_DeviceTrainOp):
                         view(i).copy_(sd[n + suffix])
                     elif strict:
                         raise KeyError(n + suffix)
-        if self.hp.variant == ADAM and "beta1_power" in sd:
+        if self._ls_state is not None:
+            self._load_loss_scale_state(sd)
+        elif self.hp.variant == ADAM and "beta1_power" in sd:
             self.beta1_power = float(sd["beta1_power"])
             self.beta2_power = float(sd["beta2_power"])
 
@@ -298,8 +348,8 @@ class PackedTrainOp(_DeviceTrainOp):
     def __init__(self, params: Sequence[torch.Tensor], names: Sequence[str], hp: HParams, accum_n: int,
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
-                 global_step: int = 0):
-        super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step)
+                 global_step: int = 0, loss_scale: Optional[LossScaleConfig] = None):
+        super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale)
         self.param_slab = self._zeros_slab()
         self.accum = self._zeros_slab()
         with torch.no_grad():
@@ -366,7 +416,9 @@ class HostTrainOp(_TrainOpCore):
     def __init__(self, host_params: Sequence[torch.Tensor], names: Sequence[str], hp: HParams, accum_n: int,
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
-                 global_step: int = 0, device: int = 0):
+                 global_step: int = 0, device: int = 0, loss_scale: Optional[LossScaleConfig] = None):
+        if loss_scale is not None:   # host-resident models have no fp16 autocast: nothing to loss-scale
+            raise ValueError("HostTrainOp does not support loss scaling")
         self.world = 1
         for p in host_params:
             if p.device.type != "cpu" or p.dtype != torch.float32 or not p.is_contiguous():

@@ -85,6 +85,34 @@ typedef struct gaccum_stats {
   float clip_scale;  /* the scalar tf.clip_by_global_norm multiplies by (1 when not clipping) */
 } gaccum_stats;
 
+/* Dynamic loss scaling for fp16 mixed precision (TF 2's DynamicLossScale, counted in windows).  The producer computes
+ * gradients of loss * S, so the accumulators hold sums of S * g.  The apply step unscales, c = ((1.0 * a') / N) * (1/S),
+ * and skips the window -- a = +0.0 everywhere, p, m, v (and GACCUM_ADAM's beta powers) unchanged bit for bit -- when an
+ * element of a' is not finite or, with clipping on, the global norm is not.  Then, on a skipped window,
+ * S = max(1, S / multiplier) and good_windows = 0; on an applied one, if good_windows + 1 >= growth_interval,
+ * S = S * multiplier (only if that is finite) and good_windows = 0, else good_windows += 1.  S is always a power of two,
+ * so the unscale is exact and a run whose scaled values stay normal fp32 numbers is bit-identical to the same run
+ * without loss scaling fed unscaled gradients.  Accumulate steps are unchanged. */
+typedef struct gaccum_loss_scale_config {
+  double initial_scale;    /* a power of two in [1, 2^127] */
+  double multiplier;       /* a power of two in [2, 2^127] (TF 2: 2) */
+  int32_t growth_interval; /* >= 1: applied windows before S grows (TF 2: 2000) */
+  int32_t reserved;        /* must be 0 */
+} gaccum_loss_scale_config;
+
+/* The loss-scaling state: 32 bytes of caller-owned DEVICE memory (16-byte aligned), written by
+ * gaccum_loss_scale_init and afterwards only by the apply launches, so no step needs the host.  A producer may read
+ * `scale` on the device (e.g. multiply its loss by it) between steps. */
+typedef struct gaccum_loss_scale_state {
+  float scale;              /* S */
+  int32_t good_windows;     /* applied windows since S last changed */
+  uint32_t skipped_windows; /* overflowed windows since gaccum_loss_scale_init */
+  int32_t last_skipped;     /* 1 if the last apply step skipped its window, else 0 */
+  float beta1_power;        /* GACCUM_ADAM: TF1's beta1^t, used instead of gaccum_step_args.beta1_power and */
+  float beta2_power;        /*   advanced (one fp32 multiply each) on applied windows only */
+  float reserved[2];
+} gaccum_loss_scale_state;
+
 /* ---- library -------------------------------------------------------------------------- */
 GACCUM_API int gaccum_version(void);
 GACCUM_API const char* gaccum_last_error(void);
@@ -130,6 +158,19 @@ GACCUM_API int32_t gaccum_num_tiles(const gaccum_plan* plan);
  * a window of N >= 2 micro-steps moves (8 + 12 (N-2) + 36) B x P.  The plan does not know N: the
  * accumulate figure stays 12 B x P. */
 GACCUM_API int64_t gaccum_algorithmic_bytes(const gaccum_plan* plan, int32_t is_apply);
+
+/* Turns dynamic loss scaling on for this plan (see gaccum_loss_scale_config).  Host-only: validates `cfg` and keeps
+ * `device_state` (non-NULL, 16-byte aligned; not dereferenced here).  Allowed only before the first call of a compute
+ * entry point on the plan (gaccum_step, _accumulate, _apply, _step_packed, _step_dp, _apply_dp), returns
+ * GACCUM_EINVAL afterwards.  gaccum_step, gaccum_apply and gaccum_step_packed then apply with loss scaling, whatever
+ * clip_norm is: their apply step is the two-pass clip-apply kernel (with clip_norm <= 0 it does not clip, but still
+ * checks every element before it writes).  gaccum_accumulate is unchanged.  gaccum_step_dp, gaccum_apply_dp,
+ * gaccum_host_session_create and gaccum_step_host refuse a loss-scaled plan with GACCUM_EINVAL. */
+GACCUM_API int gaccum_plan_set_loss_scale(gaccum_plan* plan, const gaccum_loss_scale_config* cfg,
+                                          gaccum_loss_scale_state* device_state);
+/* Writes the initial state into `device_state` asynchronously on `stream`: scale = initial_scale, the three counters 0,
+ * beta powers fp32(beta1) and fp32(beta2) (TF1's initial values).  The plan must have loss scaling on. */
+GACCUM_API int gaccum_loss_scale_init(gaccum_plan* plan, gaccum_loss_scale_state* device_state, gaccum_stream_t stream);
 
 /* ---- the hot path --------------------------------------------------------------------- */
 /* One micro-step of the train_op (optimization.py:91-94): if gaccum_is_apply_step() the apply
