@@ -13,6 +13,8 @@ ADAM = 1                # tf.train.AdamOptimizer (02:41, 04:42, another-example.
 
 OK, EINVAL, ENODEVICE, ECUDA, ENCCL, ENOMEM = 0, -1, -2, -3, -4, -5
 
+DTYPE_F32, DTYPE_BF16, DTYPE_F16 = 0, 1, 2   # element type of the model's weights and gradients
+
 
 class GaccumError(RuntimeError):
     def __init__(self, code: int, msg: str):
@@ -141,6 +143,7 @@ def _load():
         "gaccum_step_dp": (C.c_int, [vp, C.POINTER(DpComm), vp, vp, vp, C.POINTER(StepArgs), C.c_uint32, vp]),
         "gaccum_plan_set_loss_scale": (C.c_int, [vp, C.POINTER(LossScaleConfig), vp]),
         "gaccum_loss_scale_init": (C.c_int, [vp, vp, vp]),
+        "gaccum_plan_set_param_dtype": (C.c_int, [vp, i32, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -285,6 +288,12 @@ class Plan:
 
     def loss_scale_init(self, device_state: int, stream: int = 0) -> None:
         _check(_load().gaccum_loss_scale_init(self._h, device_state or None, stream))
+
+    def set_param_dtype(self, dtype: int, master_slab: int) -> None:
+        """Train a bf16 / fp16 model (DTYPE_BF16 / DTYPE_F16) with fp32 master weights (before the first compute
+        call); ``master_slab`` points to ``padded_size`` floats of device memory in the plan's layout, 16-byte
+        aligned.  The step calls then take 16-bit gradient and parameter pointers."""
+        _check(_load().gaccum_plan_set_param_dtype(self._h, int(dtype), master_slab or None))
 
     def close(self) -> None:
         if getattr(self, "_h", None):

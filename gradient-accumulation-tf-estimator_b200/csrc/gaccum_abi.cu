@@ -73,6 +73,9 @@ struct gaccum_plan {
   bool ls_on = false;
   gaccum_loss_scale_config ls_cfg{};
   gaccum_loss_scale_state* ls_state = nullptr;
+  // 16-bit model (gaccum_plan_set_param_dtype); set only while `computed` is false
+  int32_t param_dtype = GACCUM_DTYPE_F32;
+  float* master = nullptr;
   std::mutex mu;
   std::map<const void*, int> grid_cache;   // kernel -> co-resident grid size
 };
@@ -157,29 +160,30 @@ static int grid_for(gaccum_plan* pl, const void* fn, int* out) {
 }
 
 // from_zero: the accumulators hold +0.0 (first micro-step of a window), so the kernel does not read them
-template <int CAP>
+// H: a 16-bit model (gaccum_plan_set_param_dtype), scattered pointer tables only
+template <int CAP, bool H = false>
 static int launch_accumulate(gaccum_plan* pl, KernelParams<CAP>& prm, bool from_zero, cudaStream_t st) {
   // one tile per CTA: the hardware block scheduler balances better than a persistent loop
   const int grid = std::max(1, prm.num_tiles);
-  if (from_zero) accumulate_kernel<CAP, true><<<grid, kThreads, 0, st>>>(prm);
-  else accumulate_kernel<CAP, false><<<grid, kThreads, 0, st>>>(prm);
+  if (from_zero) accumulate_kernel<CAP, true, H><<<grid, kThreads, 0, st>>>(prm);
+  else accumulate_kernel<CAP, false, H><<<grid, kThreads, 0, st>>>(prm);
   CUDA_TRY(cudaGetLastError());
   return GACCUM_OK;
 }
 
-template <int VARIANT, bool HAS_G, int CAP>
+template <int VARIANT, bool HAS_G, int CAP, bool H>
 static int launch_apply_noclip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream_t st) {
   const int grid = std::max(1, prm.num_tiles);
-  apply_kernel<VARIANT, HAS_G, CAP><<<grid, kThreads, 0, st>>>(prm);
+  apply_kernel<VARIANT, HAS_G, CAP, H><<<grid, kThreads, 0, st>>>(prm);
   CUDA_TRY(cudaGetLastError());
   return GACCUM_OK;
 }
 
 // clip-apply: one cooperative launch, ONE 864-thread CTA per SM (ring + stash take nearly all of the SM's shared
 // memory, so a second CTA could never be co-resident -- the grid is clamped to the SM count)
-template <int VARIANT, bool HAS_G, int CAP, int LS = kLsOff>
+template <int VARIANT, bool HAS_G, int CAP, int LS, bool H>
 static int launch_apply_clip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream_t st) {
-  const void* fn = (const void*)&apply_clip_kernel<VARIANT, HAS_G, CAP, LS>;
+  const void* fn = (const void*)&apply_clip_kernel<VARIANT, HAS_G, CAP, LS, H>;
   {
     std::lock_guard<std::mutex> lk(pl->mu);
     if (pl->grid_cache.find(fn) == pl->grid_cache.end()) {
@@ -201,35 +205,35 @@ static int launch_apply_clip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream
 
 // Loss scaling always takes the two-pass kernel: the single-pass apply_kernel stores p, m and v before it could know
 // whether the window overflowed.
-template <int CAP>
+template <int CAP, bool H>
 static int launch_apply_loss_scaled(gaccum_plan* pl, KernelParams<CAP>& prm, bool has_g, bool clip, cudaStream_t st) {
   const int key = (pl->hp.variant == GACCUM_ADAM ? 4 : 0) | (clip ? 2 : 0) | (has_g ? 1 : 0);
   switch (key) {
-    case 0: return launch_apply_clip<0, false, CAP, kLsNoClip>(pl, prm, st);
-    case 1: return launch_apply_clip<0, true, CAP, kLsNoClip>(pl, prm, st);
-    case 2: return launch_apply_clip<0, false, CAP, kLsClip>(pl, prm, st);
-    case 3: return launch_apply_clip<0, true, CAP, kLsClip>(pl, prm, st);
-    case 4: return launch_apply_clip<1, false, CAP, kLsNoClip>(pl, prm, st);
-    case 5: return launch_apply_clip<1, true, CAP, kLsNoClip>(pl, prm, st);
-    case 6: return launch_apply_clip<1, false, CAP, kLsClip>(pl, prm, st);
-    default: return launch_apply_clip<1, true, CAP, kLsClip>(pl, prm, st);
+    case 0: return launch_apply_clip<0, false, CAP, kLsNoClip, H>(pl, prm, st);
+    case 1: return launch_apply_clip<0, true, CAP, kLsNoClip, H>(pl, prm, st);
+    case 2: return launch_apply_clip<0, false, CAP, kLsClip, H>(pl, prm, st);
+    case 3: return launch_apply_clip<0, true, CAP, kLsClip, H>(pl, prm, st);
+    case 4: return launch_apply_clip<1, false, CAP, kLsNoClip, H>(pl, prm, st);
+    case 5: return launch_apply_clip<1, true, CAP, kLsNoClip, H>(pl, prm, st);
+    case 6: return launch_apply_clip<1, false, CAP, kLsClip, H>(pl, prm, st);
+    default: return launch_apply_clip<1, true, CAP, kLsClip, H>(pl, prm, st);
   }
 }
 
-template <int CAP>
+template <int CAP, bool H = false>
 static int launch_apply(gaccum_plan* pl, KernelParams<CAP>& prm, bool has_g, cudaStream_t st) {
   const bool clip = pl->hp.clip_norm > 0.0;
-  if (pl->ls_on) return launch_apply_loss_scaled(pl, prm, has_g, clip, st);
+  if (pl->ls_on) return launch_apply_loss_scaled<CAP, H>(pl, prm, has_g, clip, st);
   const int key = (pl->hp.variant == GACCUM_ADAM ? 4 : 0) | (clip ? 2 : 0) | (has_g ? 1 : 0);
   switch (key) {
-    case 0: return launch_apply_noclip<0, false>(pl, prm, st);
-    case 1: return launch_apply_noclip<0, true>(pl, prm, st);
-    case 2: return launch_apply_clip<0, false>(pl, prm, st);
-    case 3: return launch_apply_clip<0, true>(pl, prm, st);
-    case 4: return launch_apply_noclip<1, false>(pl, prm, st);
-    case 5: return launch_apply_noclip<1, true>(pl, prm, st);
-    case 6: return launch_apply_clip<1, false>(pl, prm, st);
-    default: return launch_apply_clip<1, true>(pl, prm, st);
+    case 0: return launch_apply_noclip<0, false, CAP, H>(pl, prm, st);
+    case 1: return launch_apply_noclip<0, true, CAP, H>(pl, prm, st);
+    case 2: return launch_apply_clip<0, false, CAP, kLsOff, H>(pl, prm, st);
+    case 3: return launch_apply_clip<0, true, CAP, kLsOff, H>(pl, prm, st);
+    case 4: return launch_apply_noclip<1, false, CAP, H>(pl, prm, st);
+    case 5: return launch_apply_noclip<1, true, CAP, H>(pl, prm, st);
+    case 6: return launch_apply_clip<1, false, CAP, kLsOff, H>(pl, prm, st);
+    default: return launch_apply_clip<1, true, CAP, kLsOff, H>(pl, prm, st);
   }
 }
 
@@ -264,6 +268,8 @@ static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, f
     prm.ls.multiplier = (float)pl->ls_cfg.multiplier;
     prm.ls.growth_interval = pl->ls_cfg.growth_interval;
   }
+  prm.half.master = pl->master;
+  prm.half.bf16 = pl->param_dtype == GACCUM_DTYPE_BF16;
 }
 
 template <int CAP>
@@ -305,7 +311,10 @@ static int do_accumulate_tab(gaccum_plan* pl, const float* const* grads, float* 
   if (!prm) return fail(GACCUM_ENOMEM, "out of host memory");
   fill_common(pl, *prm, accum, nullptr, nullptr, make_scalars(pl->hp, a));
   int rc = fill_table(pl, prm->tab, grads, nullptr);
-  if (rc == GACCUM_OK) rc = launch_accumulate(pl, *prm, first_of_window(a), st);
+  if (rc == GACCUM_OK) {
+    rc = pl->master ? launch_accumulate<CAP, true>(pl, *prm, first_of_window(a), st)
+                    : launch_accumulate<CAP, false>(pl, *prm, first_of_window(a), st);
+  }
   delete prm;
   return rc;
 }
@@ -317,7 +326,10 @@ static int do_apply_tab(gaccum_plan* pl, const float* const* grads, float* const
   if (!prm) return fail(GACCUM_ENOMEM, "out of host memory");
   fill_common(pl, *prm, accum, m, v, make_scalars(pl->hp, a));
   int rc = fill_table(pl, prm->tab, grads, params);
-  if (rc == GACCUM_OK) rc = launch_apply(pl, *prm, grads != nullptr, st);
+  if (rc == GACCUM_OK) {
+    rc = pl->master ? launch_apply<CAP, true>(pl, *prm, grads != nullptr, st)
+                    : launch_apply<CAP, false>(pl, *prm, grads != nullptr, st);
+  }
   delete prm;
   return rc;
 }
@@ -490,6 +502,9 @@ int64_t gaccum_algorithmic_bytes(const gaccum_plan* pl, int32_t is_apply) {
   // accumulate: read G, read a, write a.  apply: read G,a,p,m,v + write p,m,v,a  (SURVEY.md 8(d))
   // The first accumulate of a window does not read a (8 B x P), so a window of N >= 2 moves (8 + 12(N-2) + 36) B x P.
   // The plan does not know N: the accumulate figure is the 12 B x P of the other accumulate steps.
+  // 16-bit model: G is 2 bytes (accumulate 10 B x P); the apply reads G 2 + a, p, m, v 16 and writes p, m, v, a 16 +
+  // the 2-byte model copy (36 B x P).
+  if (pl->master) return pl->P * (is_apply ? 36 : 10);
   return pl->P * (is_apply ? 36 : 12);
 }
 
@@ -518,6 +533,23 @@ int gaccum_plan_set_loss_scale(gaccum_plan* pl, const gaccum_loss_scale_config* 
   pl->ls_state = device_state;
   pl->ls_on = true;
   return GACCUM_OK;
+}
+
+int gaccum_plan_set_param_dtype(gaccum_plan* pl, int32_t dtype, float* master_slab) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (dtype != GACCUM_DTYPE_BF16 && dtype != GACCUM_DTYPE_F16)
+    return fail(GACCUM_EINVAL, "dtype must be GACCUM_DTYPE_BF16 or GACCUM_DTYPE_F16 (got %d)", dtype);
+  if (!master_slab || !aligned16_host(master_slab))
+    return fail(GACCUM_EINVAL, "master_slab must be a 16-byte aligned device pointer");
+  if (pl->computed) return fail(GACCUM_EINVAL, "the parameter dtype can only be set before the plan's first compute call");
+  pl->param_dtype = dtype;
+  pl->master = master_slab;
+  return GACCUM_OK;
+}
+
+static int refuse_half(const gaccum_plan* pl, const char* what) {
+  return pl && pl->master ? fail(GACCUM_EINVAL, "%s does not support 16-bit parameters (gaccum_plan_set_param_dtype)", what)
+                          : GACCUM_OK;
 }
 
 int gaccum_loss_scale_init(gaccum_plan* pl, gaccum_loss_scale_state* device_state, gaccum_stream_t stream) {
@@ -570,6 +602,7 @@ int gaccum_step(gaccum_plan* pl, const float* const* grads, float* const* params
 int gaccum_step_packed(gaccum_plan* pl, const float* grad_slab, float* param_slab, float* accum,
                        float* m, float* v, const gaccum_step_args* a, int32_t force_branch,
                        gaccum_stream_t stream) {
+  if (int rc = refuse_half(pl, "gaccum_step_packed")) return rc;
   if (int rc = check_args(a)) return rc;
   const bool apply = force_branch < 0 ? gaccum_is_apply_step(a->global_step, a->accum_n) != 0 : force_branch != 0;
   if (int rc = check_compute(pl, accum, m, v, apply)) return rc;
@@ -688,6 +721,7 @@ static int do_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float*
 int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* const* grads, float* m, float* v,
                     const gaccum_step_args* a, uint32_t epoch, gaccum_stream_t stream) {
   if (pl && pl->ls_on) return fail(GACCUM_EINVAL, "the fused data-parallel apply does not support loss scaling");
+  if (int rc = refuse_half(pl, "the fused data-parallel apply")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (comm->world < 2 || comm->world > GACCUM_MAX_RANKS || comm->rank < 0 || comm->rank >= comm->world)
     return fail(GACCUM_EINVAL, "world must be 2..%d and 0 <= rank < world", GACCUM_MAX_RANKS);
@@ -711,6 +745,7 @@ int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* co
 int gaccum_step_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* const* grads, float* m, float* v,
                    const gaccum_step_args* a, uint32_t epoch, gaccum_stream_t stream) {
   if (pl && pl->ls_on) return fail(GACCUM_EINVAL, "the fused data-parallel step does not support loss scaling");
+  if (int rc = refuse_half(pl, "the fused data-parallel step")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (int rc = check_args(a)) return rc;
   if (!grads) return fail(GACCUM_EINVAL, "grads is NULL");
@@ -791,6 +826,7 @@ int gaccum_host_session_create(gaccum_host_session** out, gaccum_plan* pl) {
   if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
   // host-resident models train in fp32 (no fp16 autocast on the CPU): nothing to loss-scale
   if (pl->ls_on) return fail(GACCUM_EINVAL, "the host-buffer session does not support loss scaling");
+  if (int rc = refuse_half(pl, "the host-buffer session")) return rc;
   if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): libgaccum has no CPU fallback, a CUDA device is required");
   DeviceGuard guard(pl->device);
   gaccum_host_session* s = new (std::nothrow) gaccum_host_session();
@@ -899,6 +935,7 @@ int gaccum_step_host(gaccum_host_session* s, const float* const* host_grads, flo
   if (int rc = check_args(a)) return rc;
   gaccum_plan* pl = s->plan;
   if (pl->ls_on) return fail(GACCUM_EINVAL, "the host-buffer session does not support loss scaling");
+  if (int rc = refuse_half(pl, "the host-buffer session")) return rc;
   DeviceGuard guard(pl->device);
   const int b = (int)(s->calls & 1);
   ++s->calls;

@@ -17,9 +17,16 @@
 // Arithmetic uses round-to-nearest intrinsics (__fmul_rn, __fadd_rn, __fdiv_rn, __fsqrt_rn) so nvcc
 // cannot contract mul+add into FMA: the reference graph is un-fused, one rounding per TF op, and we
 // reproduce it bit for bit (the kernels are HBM-bound, the extra flops are free).
+//
+// 16-bit models (template flag H, scattered pointer tables only): G and the model's weights are bf16 or fp16 (one
+// launch-uniform flag, prm.half.bf16), the fp32 master weights are a slab in the plan's layout.  G is widened exactly
+// on load, so every fp32 operation is the one the fp32 kernels perform on the upcast gradient; the apply stores the
+// master weights and, rounded to nearest-even, the model copy.  accumulate 10 B/elem (first of a window 6), apply 36.
 #pragma once
 
 #include <cooperative_groups.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -89,6 +96,13 @@ constexpr int kLsOff = 0;       // no loss scaling
 constexpr int kLsClip = 1;      // loss scaling + tf.clip_by_global_norm
 constexpr int kLsNoClip = 2;    // loss scaling without clipping: pass 1 only looks for non-finite elements of a'
 
+// A 16-bit model (gaccum_plan_set_param_dtype): the pointer table's g[] and p[] point at bf16 or fp16 tensors.  Kept
+// after LossScaleParams, so every member of the fp32 instantiations sits where it does without it.
+struct HalfParams {
+  float* master;      // fp32 master weights, a slab in the plan's layout (16-byte aligned)
+  int32_t bf16;       // 1: bf16, 0: fp16
+};
+
 template <int CAP>
 struct KernelParams {
   const TileDesc* tiles;
@@ -105,6 +119,7 @@ struct KernelParams {
   Scalars sc;
   PtrTable<CAP> tab;
   LossScaleParams ls;   // apply_clip_kernel with LS != kLsOff only
+  HalfParams half;      // kernels with H = true only
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -153,6 +168,71 @@ __device__ __forceinline__ float* param_ptr(const PtrTable<CAP>& tab, const Tile
   }
 }
 __device__ __forceinline__ bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
+__device__ __forceinline__ bool aligned8(const void* p) { return ((uintptr_t)p & 7u) == 0; }
+
+// ---- 16-bit models: widening is exact; narrowing rounds to nearest-even (cvt.rn), as torch's .to(dtype) does ----
+__device__ __forceinline__ float h2f(uint16_t x, bool bf16) {
+  return bf16 ? __uint_as_float((uint32_t)x << 16) : __half2float(__ushort_as_half(x));
+}
+__device__ __forceinline__ uint32_t f2h(float x, bool bf16) {
+  return bf16 ? (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(x)) : (uint32_t)__half_as_ushort(__float2half_rn(x));
+}
+__device__ __forceinline__ float4 h2f4(const uint2 r, bool bf16) {   // 4 elements, the first in the low half of r.x
+  return make_float4(h2f((uint16_t)r.x, bf16), h2f((uint16_t)(r.x >> 16), bf16), h2f((uint16_t)r.y, bf16),
+                     h2f((uint16_t)(r.y >> 16), bf16));
+}
+// the model copy of 4 master weights at elements 4i..4i+3: one 8-byte store if the tensor is 8-byte aligned
+__device__ __forceinline__ void store_model4(uint16_t* q, uint32_t i, const float4 p, bool bf16) {
+  if (aligned8(q)) {
+    __stcs(reinterpret_cast<uint2*>(q) + i, make_uint2(f2h(p.x, bf16) | (f2h(p.y, bf16) << 16), f2h(p.z, bf16) | (f2h(p.w, bf16) << 16)));
+  } else {
+    q[4 * i] = (uint16_t)f2h(p.x, bf16); q[4 * i + 1] = (uint16_t)f2h(p.y, bf16);
+    q[4 * i + 2] = (uint16_t)f2h(p.z, bf16); q[4 * i + 3] = (uint16_t)f2h(p.w, bf16);
+  }
+}
+
+// The gradient stream of one tile, widened to fp32 on load.  H: bf16 / fp16, the vector path reads 4 x 16 bit (8 B).
+// A default-constructed Grad is "no gradient" (g == nullptr).
+template <bool H> struct Grad;
+template <>
+struct Grad<false> {
+  const float* g = nullptr;
+  __device__ __forceinline__ Grad() {}
+  template <int CAP>
+  __device__ __forceinline__ Grad(const KernelParams<CAP>& prm, const TileDesc& d) : g(grad_ptr(prm.tab, d)) {}
+  __device__ __forceinline__ bool vec_ok() const { return aligned16(g); }
+  __device__ __forceinline__ float4 vec(uint32_t i) const { return ld_stream(reinterpret_cast<const float4*>(g) + i); }
+  __device__ __forceinline__ float elem(uint32_t i) const { return ld_stream(g + i); }
+  // the G half of a pass-1 ring slot
+  __device__ __forceinline__ float4 slot(const float4* s, uint32_t i) const { return s[i]; }
+};
+template <>
+struct Grad<true> {
+  const uint16_t* g = nullptr;
+  bool bf16 = false;
+  __device__ __forceinline__ Grad() {}
+  template <int CAP>
+  __device__ __forceinline__ Grad(const KernelParams<CAP>& prm, const TileDesc& d) : bf16(prm.half.bf16 != 0) {
+    const uint16_t* b = reinterpret_cast<const uint16_t*>(prm.tab.g[d.tensor_flags & 0x7fffffffu]);
+    g = b ? b + d.toff : nullptr;
+  }
+  __device__ __forceinline__ bool vec_ok() const { return aligned8(g); }
+  __device__ __forceinline__ float4 vec(uint32_t i) const { return h2f4(__ldcs(reinterpret_cast<const uint2*>(g) + i), bf16); }
+  __device__ __forceinline__ float elem(uint32_t i) const { return h2f(__ldcs(g + i), bf16); }
+  __device__ __forceinline__ float4 slot(const float4* s, uint32_t i) const { return h2f4(reinterpret_cast<const uint2*>(s)[i], bf16); }
+};
+
+// The fp32 weights the update reads and writes: the parameters themselves, or (H) the master slab
+template <bool H, int CAP>
+__device__ __forceinline__ float* update_ptr(const KernelParams<CAP>& prm, const TileDesc& d) {
+  if constexpr (H) return prm.half.master + (size_t)d.soff32 * kSlabAlign;
+  else return param_ptr(prm.tab, d);
+}
+// H: the model copy of the tile (16-bit)
+template <int CAP>
+__device__ __forceinline__ uint16_t* model_ptr(const KernelParams<CAP>& prm, const TileDesc& d) {
+  return reinterpret_cast<uint16_t*>(prm.tab.p[d.tensor_flags & 0x7fffffffu]) + d.toff;
+}
 
 // ---------------------------------------------------------------------------------------------
 // per-element math, one rounding per reference op
@@ -299,31 +379,30 @@ __device__ __forceinline__ void walk_tile(const uint32_t len, const uint32_t nve
 // +0.0 (optimization.py:78,86-87), so a is not loaded and a = +0 + G is stored (8 instead of 12 B/elem).  The add is
 // kept: it turns a gradient of -0.0 into +0.0, as assign_add onto a zero does, and a NaN comes out as a += G gives it.
 // ---------------------------------------------------------------------------------------------
-template <bool FROM_ZERO, int CAP>
+template <bool FROM_ZERO, bool H, int CAP>
 __device__ __forceinline__ void accumulate_tile(const TileDesc d, const KernelParams<CAP>& prm) {
-  const float* __restrict__ g = grad_ptr(prm.tab, d);
-  if (g == nullptr) return;   // optimization.py:132 -- tensors without a gradient are skipped
+  const Grad<H> g(prm, d);
+  if (g.g == nullptr) return;   // optimization.py:132 -- tensors without a gradient are skipped
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
-  const float4* g4 = reinterpret_cast<const float4*>(g);
   float4* a4 = reinterpret_cast<float4*>(a);
   float4 vg[kUnroll], va[kUnroll];
-  walk_tile(d.len, aligned16(g) ? d.len >> 2 : 0u, threadIdx.x,
+  walk_tile(d.len, g.vec_ok() ? d.len >> 2 : 0u, threadIdx.x,
             [&](int u, uint32_t i) {
-              vg[u] = ld_stream(g4 + i);
+              vg[u] = g.vec(i);
               if constexpr (FROM_ZERO) va[u] = make_float4(0.f, 0.f, 0.f, 0.f); else va[u] = a4[i];
             },
             [] {},
             [&](int u, uint32_t i) { a4[i] = add_rn(va[u], vg[u]); },
-            [&](uint32_t i) { a[i] = __fadd_rn(FROM_ZERO ? 0.f : a[i], ld_stream(g + i)); });
+            [&](uint32_t i) { a[i] = __fadd_rn(FROM_ZERO ? 0.f : a[i], g.elem(i)); });
 }
 
-template <int CAP, bool FROM_ZERO>
+template <int CAP, bool FROM_ZERO, bool H = false>
 __global__ void __launch_bounds__(kThreads)
 accumulate_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     prm.stats[0] = 0.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f;
   }
-  if ((int)blockIdx.x < prm.num_tiles) accumulate_tile<FROM_ZERO>(prm.tiles[blockIdx.x], prm);
+  if ((int)blockIdx.x < prm.num_tiles) accumulate_tile<FROM_ZERO, H>(prm.tiles[blockIdx.x], prm);
 }
 
 // gaccum_loss_scale_init: one thread writes the initial loss-scaling state (a kernel, so the call stays asynchronous and
@@ -339,48 +418,53 @@ __global__ void loss_scale_init_kernel(LossScaleState* st, float scale, float b1
 // ---------------------------------------------------------------------------------------------
 // apply without clipping: one pass.  HAS_G = false applies the accumulators as they are.
 // ---------------------------------------------------------------------------------------------
-template <int VARIANT, bool LOAD_G, int CAP>
+// H: p is the master slab (always 16-byte aligned); the model copy is stored after it.
+template <int VARIANT, bool LOAD_G, bool H, int CAP>
 __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams<CAP>& prm) {
-  const float* __restrict__ g = nullptr;
-  if constexpr (LOAD_G) g = grad_ptr(prm.tab, d);
+  Grad<H> g;
+  if constexpr (LOAD_G) g = Grad<H>(prm, d);
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
   float* __restrict__ m = prm.m + soff;
   float* __restrict__ v = prm.v + soff;
-  float* __restrict__ p = param_ptr(prm.tab, d);
+  float* __restrict__ p = update_ptr<H>(prm, d);
+  uint16_t* q = nullptr;
+  bool bf16 = false;
+  if constexpr (H) { q = model_ptr(prm, d); bf16 = prm.half.bf16 != 0; }
   const bool decay = (d.tensor_flags >> 31) != 0;
   const Scalars& sc = prm.sc;
-  const float4* g4 = reinterpret_cast<const float4*>(g);
   float4* a4 = reinterpret_cast<float4*>(a);
   float4* m4 = reinterpret_cast<float4*>(m);
   float4* v4 = reinterpret_cast<float4*>(v);
   float4* p4 = reinterpret_cast<float4*>(p);
   float4 va[kUnroll], vg[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll];
   // no gradient for this tile: a + 0 would turn -0 into +0 only; the add is skipped entirely (optimization.py:81)
-  walk_tile(d.len, aligned16(p) && (g == nullptr || aligned16(g)) ? d.len >> 2 : 0u, threadIdx.x,
+  walk_tile(d.len, (H || aligned16(p)) && (g.g == nullptr || g.vec_ok()) ? d.len >> 2 : 0u, threadIdx.x,
             [&](int u, uint32_t i) {
               va[u] = __ldcs(a4 + i); vp[u] = __ldcs(p4 + i); vm[u] = __ldcs(m4 + i); vv[u] = __ldcs(v4 + i);
-              if (LOAD_G && g) vg[u] = ld_stream(g4 + i);
+              if (LOAD_G && g.g) vg[u] = g.vec(i);
             },
             [] {},
             [&](int u, uint32_t i) {
-              if (LOAD_G && g) va[u] = add_rn(va[u], vg[u]);
+              if (LOAD_G && g.g) va[u] = add_rn(va[u], vg[u]);
               update_vec<VARIANT>(va[u], false, 0.f, vp[u], vm[u], vv[u], decay, sc);
               __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
+              if constexpr (H) store_model4(q, i, vp[u], bf16);
             },
             [&](uint32_t i) {
               float ax = a[i], px = p[i], mx = m[i], vx = v[i];
-              if (LOAD_G && g) ax = __fadd_rn(ax, ld_stream(g + i));
+              if (LOAD_G && g.g) ax = __fadd_rn(ax, g.elem(i));
               update_elem<VARIANT>(ax, false, 0.f, px, mx, vx, decay, sc);
               p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
+              if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
             });
 }
 
-template <int VARIANT, bool HAS_G, int CAP>
+template <int VARIANT, bool HAS_G, int CAP, bool H = false>
 __global__ void __launch_bounds__(kThreads)
 apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
-  if ((int)blockIdx.x < prm.num_tiles) update_tile<VARIANT, HAS_G>(prm.tiles[blockIdx.x], prm);
+  if ((int)blockIdx.x < prm.num_tiles) update_tile<VARIANT, HAS_G, H>(prm.tiles[blockIdx.x], prm);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f;
   }
@@ -500,19 +584,23 @@ __device__ __forceinline__ unsigned long long ld_acquire_gpu_u64(const unsigned 
 
 // Number of float4 vectors of this tile that pass 1 moves by bulk copy (0: scalar fallback).  The producer and
 // the consumers MUST agree on this.
-__device__ __forceinline__ uint32_t bulk_vecs(const TileDesc& d, const float* g) {
-  return (g == nullptr || aligned16(g)) ? (d.len >> 2) : 0u;
+// A 16-bit G (H) moves in 16-byte granules of 8 elements, i.e. an even number of vectors: the G half of the slot holds
+// nvec x 8 bytes of it.
+template <bool H>
+__device__ __forceinline__ uint32_t bulk_vecs(const TileDesc& d, const Grad<H>& g) {
+  if constexpr (H) return g.g == nullptr ? (d.len >> 2) : aligned16(g.g) ? (d.len >> 3) << 1 : 0u;
+  else return (g.g == nullptr || aligned16(g.g)) ? (d.len >> 2) : 0u;
 }
-// ... and that pass 2 moves by bulk copy
+// ... and that pass 2 moves by bulk copy (p: the parameters, or the master slab of a 16-bit model)
 __device__ __forceinline__ uint32_t bulk_vecs2(const TileDesc& d, const float* p) {
   return aligned16(p) ? (d.len >> 2) : 0u;
 }
 
 // a' of a tile may be parked in the stash only if BOTH passes take the vector path for it and it is a full tile
-template <bool HAS_G, int CAP>
+template <bool HAS_G, bool H, int CAP>
 __device__ __forceinline__ bool stash_ok(const TileDesc& d, const KernelParams<CAP>& prm) {
-  bool ok = d.len == (uint32_t)kTile && aligned16(param_ptr(prm.tab, d));
-  if constexpr (HAS_G) { const float* g = grad_ptr(prm.tab, d); ok = ok && (g == nullptr || aligned16(g)); }
+  bool ok = d.len == (uint32_t)kTile && aligned16(update_ptr<H>(prm, d));
+  if constexpr (HAS_G) { const Grad<H> g(prm, d); ok = ok && (g.g == nullptr || aligned16(g.g)); }
   return ok;
 }
 
@@ -572,20 +660,20 @@ __device__ __forceinline__ double acc_value(const unsigned long long* bins /* kA
 // A tile the producer did not copy (nvec == 0), and the < 4 tail elements of any tile, travel through global memory.
 // Loss-scaled (LS != kLsOff): the partial is of sum(((a'/N)(1/S))^2) (none without clipping), and `bad` is set when an
 // element of a' is not finite.
-template <bool HAS_G, int LS, int CAP>
+template <bool HAS_G, int LS, bool H, int CAP>
 __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float4* slot, uint64_t* empty,
                                            float4* const stash, const uint64_t pol, const float inv_s, bool& bad) {
-  const float* __restrict__ g = nullptr;
-  if constexpr (HAS_G) g = grad_ptr(prm.tab, d);
+  Grad<H> g;
+  if constexpr (HAS_G) g = Grad<H>(prm, d);
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
   float4* a4 = reinterpret_cast<float4*>(a);
   float acc = 0.f;
   float4 x[kUnroll], gg[kUnroll];
   walk_tile(d.len, bulk_vecs(d, g), threadIdx.x & (kThreads - 1),
-            [&](int u, uint32_t i) { x[u] = slot[kTile / 4 + i]; if (g) gg[u] = slot[i]; },
+            [&](int u, uint32_t i) { x[u] = slot[kTile / 4 + i]; if (g.g) gg[u] = g.slot(slot, i); },
             [&] { __syncwarp(); if ((threadIdx.x & 31) == 0) mbar_arrive(empty); },   // this warp is done with the slot
             [&](int u, uint32_t i) {
-              if (g) {
+              if (g.g) {
                 x[u] = add_rn(x[u], gg[u]);
                 if (stash == nullptr) st_policy(a4 + i, x[u], pol);
               }
@@ -595,7 +683,7 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
             },
             [&](uint32_t i) {
               float xs = a[i];
-              if (g) { xs = __fadd_rn(xs, ld_stream(g + i)); a[i] = xs; }
+              if (g.g) { xs = __fadd_rn(xs, g.elem(i)); a[i] = xs; }
               if constexpr (LS == kLsOff) acc = add_sq(acc, xs, prm.sc);
               else acc = ls_pass1<LS>(acc, xs, inv_s, bad, prm.sc);
             });
@@ -605,8 +693,8 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
 // ---- pass 2, consumer side: one tile out of slot [p | m | v | a']; a' from the slot or from the stash ----
 // The caller has waited on the slot's `full` barrier (it had to, to learn which tile this is).
 // Loss-scaled: `sc` carries the alpha computed from the device's beta powers, and a skipped window (`skip`) stores
-// a = 0 and nothing else.
-template <int VARIANT, int LS, int CAP>
+// a = 0 and nothing else.  H: p is the master slab, and the model copy is stored after it (not on a skipped window).
+template <int VARIANT, int LS, bool H, int CAP>
 __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelParams<CAP>& prm, const float s, const float4* slot,
                                              uint64_t* empty, const float4* const stash, const Scalars& sc, const float inv_s,
                                              const bool skip) {
@@ -614,7 +702,10 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
   float* __restrict__ a = prm.accum + soff;
   float* __restrict__ m = prm.m + soff;
   float* __restrict__ v = prm.v + soff;
-  float* __restrict__ p = param_ptr(prm.tab, d);
+  float* __restrict__ p = update_ptr<H>(prm, d);
+  uint16_t* q = nullptr;
+  bool bf16 = false;
+  if constexpr (H) { q = model_ptr(prm, d); bf16 = prm.half.bf16 != 0; }
   const bool decay = (d.tensor_flags >> 31) != 0;
   const bool write = LS == kLsOff || !skip;
   float4* a4 = reinterpret_cast<float4*>(a);
@@ -632,6 +723,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
               if (write) {
                 update_vec2<VARIANT, LS>(va[u], s, inv_s, vp[u], vm[u], vv[u], decay, sc);
                 __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
+                if constexpr (H) store_model4(q, i, vp[u], bf16);
               }
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
             },
@@ -640,6 +732,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
                 float px = p[i], mx = m[i], vx = v[i];
                 update_elem2<VARIANT, LS>(a[i], s, inv_s, px, mx, vx, decay, sc);
                 p[i] = px; m[i] = mx; v[i] = vx;
+                if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
               }
               a[i] = 0.f;
             });
@@ -657,7 +750,10 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
 // from the same launch-wide flags: skip iff an element was non-finite or, with clipping, gn is.  A skipped window
 // stores a = 0 and leaves p, m and v alone.  Block 0's thread 0 writes the new state at the very end -- after the
 // barrier, so no CTA can see the new S or beta powers in this launch.
-template <int VARIANT, bool HAS_G, int CAP, int LS = kLsOff>
+//
+// 16-bit models (H): pass 1 moves the 16-bit G tile into the G half of the [G | a] slot (bulk_vecs), pass 2 moves the
+// master weights, and every store of p is followed by the model copy.  Ring and stash are the same.
+template <int VARIANT, bool HAS_G, int CAP, int LS = kLsOff, bool H = false>
 __global__ void __launch_bounds__(kClipThreads, 1)
 apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   extern __shared__ __align__(128) unsigned char smem_dyn[];
@@ -750,8 +846,8 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     {
       RingPos rp;
       auto issue = [&](const TileDesc& dl) {                               // lane 0 only
-        const float* g = nullptr;
-        if constexpr (HAS_G) g = grad_ptr(prm.tab, dl);
+        Grad<H> g;
+        if constexpr (HAS_G) g = Grad<H>(prm, dl);
         const uint32_t nvec = bulk_vecs(dl, g);
         uint64_t* full = &s_full1[grp][rp.slot];
 #ifdef GACCUM_EXPERIMENTS
@@ -765,8 +861,13 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         meta->d = dl;
         if (nvec > 0) {
           float4* dst = ring + (size_t)rp.slot * kP1SlotVecs;
-          mbar_arrive_expect_tx(full, nvec * 16u * (g ? 2u : 1u));
-          if (g) bulk_g2s(dst, g, nvec * 16u, full, pol_first);
+          if constexpr (H) {
+            mbar_arrive_expect_tx(full, nvec * 16u + (g.g ? nvec * 8u : 0u));
+            if (g.g) bulk_g2s(dst, g.g, nvec * 8u, full, pol_first);
+          } else {
+            mbar_arrive_expect_tx(full, nvec * 16u * (g.g ? 2u : 1u));
+            if (g.g) bulk_g2s(dst, g.g, nvec * 16u, full, pol_first);
+          }
           bulk_g2s(dst + kTile / 4, prm.accum + (size_t)dl.soff32 * kSlabAlign, nvec * 16u, full, pol_first);
         } else {
           mbar_arrive(full);                                                 // nothing to copy: complete the phase
@@ -855,9 +956,9 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
           tile = nt - 1 - (int)tk;                                              // youngest a' lines first
         }
         const TileDesc d = prm.tiles[tile];
-        const float* p = param_ptr(prm.tab, d);
+        const float* p = update_ptr<H>(prm, d);
         const uint32_t nvec = bulk_vecs2(d, p);
-        const bool in_stash = stash_slot != kNoStash && stash_ok<HAS_G>(d, prm);
+        const bool in_stash = stash_slot != kNoStash && stash_ok<HAS_G, H>(d, prm);
         if (!in_stash && !past_barrier) {                                        // an own tile whose a' had to go to global memory
           mbar_wait(&s_go[grp], 0);
           asm volatile("fence.proxy.async;" ::: "memory");
@@ -919,10 +1020,10 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         // the stash takes the group's own tiles j < kStashTiles (the first ones it is handed) when they are FULL,
         // vector-path tiles (the same predicate the producer evaluates in pass 2)
         const bool own = n_seen < n_st;
-        const bool park = own && stash_ok<HAS_G>(meta.d, prm);
+        const bool park = own && stash_ok<HAS_G, H>(meta.d, prm);
         float4* const st = park ? stash + (size_t)n_seen * (kTile / 4) : nullptr;
         bool bad = false;
-        const float part = norm_tile<HAS_G, LS>(meta.d, prm, ring + (size_t)rp.slot * kP1SlotVecs, &s_empty1[grp][rp.slot], st,
+        const float part = norm_tile<HAS_G, LS, H>(meta.d, prm, ring + (size_t)rp.slot * kP1SlotVecs, &s_empty1[grp][rp.slot], st,
                                                 pol_last, inv_s, bad);
         if constexpr (LS != kLsOff) { if (bad) my_nonfinite |= kElemNonfinite; }
         if constexpr (LS != kLsNoClip) {
@@ -997,7 +1098,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         const SlotMeta meta = s_meta2[grp][rp.slot];
         if (meta.d.len == 0) break;
         const float4* const st = meta.stash_slot != kNoStash ? stash + (size_t)meta.stash_slot * (kTile / 4) : nullptr;
-        update_tile2<VARIANT, LS>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st, sc, inv_s,
+        update_tile2<VARIANT, LS, H>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st, sc, inv_s,
                                   skip);
         rp.advance(kP2Slots);
       }

@@ -30,6 +30,8 @@ class DataParallelTrainOp:
     launches_per_apply = 2      # local accumulate + apply (the all-reduce between them is NCCL's kernel)
 
     def __init__(self, engine, process_group=None):
+        if getattr(engine, "master", None) is not None:
+            raise ValueError("multi-GPU training of bf16 / fp16 parameters is not supported yet")
         self.engine = engine
         self.group = process_group if process_group is not None and process_group is not True else None
         self.world = dist.get_world_size(self.group) if dist.is_initialized() else 1
@@ -92,6 +94,8 @@ class FusedDataParallelTrainOp:
         from .train_op import GaccumTrainOp
         if loss_scale is not None:
             raise ValueError("the fused data-parallel train op does not support loss scaling; use dp_mode='allreduce'")
+        if any(p.dtype in (torch.bfloat16, torch.float16) for p in params):
+            raise ValueError("multi-GPU training of bf16 / fp16 parameters is not supported yet")
         if not dist.is_initialized():
             raise RuntimeError("torch.distributed must be initialised (backend nccl)")
         self.group = process_group if process_group is not None else dist.group.WORLD

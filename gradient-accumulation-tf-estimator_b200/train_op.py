@@ -23,6 +23,15 @@ def _f32(x) -> float:
     return float(np.float32(x))
 
 
+# 16-bit models GaccumTrainOp trains with fp32 master weights (gaccum_plan_set_param_dtype)
+_HALF_DTYPES = {torch.bfloat16: _lib.DTYPE_BF16, torch.float16: _lib.DTYPE_F16}
+
+
+def _refuse_half(params: Sequence[torch.Tensor], what: str) -> None:
+    if any(p.dtype in _HALF_DTYPES for p in params):
+        raise ValueError(f"{what} does not support bf16 / fp16 parameters; use GaccumTrainOp")
+
+
 def _pinned_zeros(n: int) -> torch.Tensor:
     """fp32 zeros in page-locked host memory (pageable where the CUDA runtime cannot pin)."""
     t = torch.zeros(n, dtype=torch.float32)
@@ -156,15 +165,38 @@ class _DeviceTrainOp(_TrainOpCore):
 
 
 class GaccumTrainOp(_DeviceTrainOp):
+    """The train op over scattered parameter and gradient tensors.
+
+    A bf16 or fp16 model (every parameter of one of these dtypes) is trained with fp32 master weights: gradients of
+    the parameters' dtype are accumulated in fp32, the apply updates the master weights (``master_view``) exactly as
+    an fp32 model's parameters, then rewrites the model's tensors with them rounded to nearest-even.  The master
+    weights are the truth: an edit of the model's tensors between applies is overwritten by the next apply (write
+    checkpoints through ``load_state_dict``, which refreshes both)."""
+
     def __init__(self, params: Sequence[torch.Tensor], names: Sequence[str], hp: HParams, accum_n: int,
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, accum: Optional[torch.Tensor] = None,
                  loss_scale: Optional[LossScaleConfig] = None):
+        dtypes = {p.dtype for p in params}
+        if len(dtypes) > 1 and dtypes & set(_HALF_DTYPES):
+            raise ValueError(f"parameters of mixed dtypes ({', '.join(sorted(str(d) for d in dtypes))}): "
+                             "a 16-bit model must be all bf16 or all fp16")
+        self.param_dtype = params[0].dtype if len(dtypes) == 1 and params[0].dtype in _HALF_DTYPES else torch.float32
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale)
         for p in self.params:
-            if p.dtype != torch.float32 or not p.is_contiguous() or p.device != self.device:
+            if p.dtype != self.param_dtype or not p.is_contiguous() or p.device != self.device:
+                if self.param_dtype != torch.float32:
+                    raise ValueError("parameters must be contiguous tensors of one dtype on one device")
                 raise ValueError("parameters must be contiguous fp32 tensors on one device")
+        self.master: Optional[torch.Tensor] = None
+        if self.param_dtype != torch.float32:
+            # the fp32 master weights: a slab in the plan's layout, starting at the exact upcast of the model
+            self.master = self._zeros_slab()
+            with torch.no_grad():
+                for i, p in enumerate(self.params):
+                    self.master_view(i).copy_(p)
+            self.plan.set_param_dtype(_HALF_DTYPES[self.param_dtype], self.master.data_ptr())
         if accum is not None:          # caller-provided slab (e.g. NVLink peer-mapped symmetric memory)
             if accum.numel() < self.m.numel() or accum.dtype != torch.float32 or accum.device != self.device:
                 raise ValueError("accum must be an fp32 tensor of at least plan.padded_size elements on the params' device")
@@ -185,7 +217,9 @@ class GaccumTrainOp(_DeviceTrainOp):
             for g, p in zip(grads, self.params):
                 if g is None:
                     continue
-                if g.dtype != torch.float32 or not g.is_contiguous() or g.numel() != p.numel() or g.device != self.device:
+                if self.param_dtype != torch.float32 and g.dtype != self.param_dtype:
+                    raise ValueError(f"gradients of a {self.param_dtype} model must be {self.param_dtype} (got {g.dtype})")
+                if g.dtype != self.param_dtype or not g.is_contiguous() or g.numel() != p.numel() or g.device != self.device:
                     raise ValueError("gradients must be contiguous fp32 tensors shaped like their parameter")
             self._grad_ptrs = Plan.ptr_array(list(key))
             self._grad_key = key
@@ -269,6 +303,8 @@ class GaccumTrainOp(_DeviceTrainOp):
         the updated parameters into ``host_params_out``.  Everything is stream-ordered; the caller's
         current stream observes completion.  Returns True if the step applied.
         """
+        if self.master is not None:
+            raise ValueError("run_host stages fp32 gradients: it does not support bf16 / fp16 parameters")
         if not hasattr(self, "_stage"):
             self._host_init()
         main = torch.cuda.current_stream(self.device)
@@ -295,12 +331,26 @@ class GaccumTrainOp(_DeviceTrainOp):
             main.wait_event(self._d2h_done)
         return applied
 
+    def master_view(self, i: int) -> torch.Tensor:
+        """The fp32 master weights of parameter i (16-bit models only)."""
+        if self.master is None:
+            raise ValueError("fp32 parameters have no master copy")
+        return self._view(self.master, i)
+
+    def _refresh_model(self) -> None:
+        """The model's 16-bit tensors = the master weights rounded to nearest-even, as the apply leaves them."""
+        with torch.no_grad():
+            for i, p in enumerate(self.params):
+                p.copy_(self.master_view(i))
+
     # -- checkpoint compatibility: the reference's Saver sees per-variable tensors --------
     def state_dict(self) -> Dict[str, torch.Tensor]:
-        """Per-tensor copies under the reference's names (optimization.py:78, 137-148)."""
+        """Per-tensor copies under the reference's names (optimization.py:78, 137-148).  A 16-bit model stores its
+        fp32 master weights under the variables' names, as TF mixed precision saves its fp32 variables, so fp32 and
+        16-bit checkpoints load into each other."""
         out: Dict[str, torch.Tensor] = {"global_step": torch.tensor(self.global_step, dtype=torch.int64)}
         for i, n in enumerate(self.names):
-            out[n] = self.params[i].detach().clone()
+            out[n] = self.params[i].detach().clone() if self.master is None else self.master_view(i).clone()
             out[n + "/adam_m"] = self.m_view(i).clone()
             out[n + "/adam_v"] = self.v_view(i).clone()
             out[n + "/accum_grad"] = self.accum_view(i).clone()
@@ -316,7 +366,7 @@ class GaccumTrainOp(_DeviceTrainOp):
         for i, n in enumerate(self.names):
             with torch.no_grad():
                 if n in sd:
-                    self.params[i].copy_(sd[n])
+                    (self.params[i] if self.master is None else self.master_view(i)).copy_(sd[n])
                 for suffix, view in (("/adam_m", self.m_view), ("/adam_v", self.v_view), ("/accum_grad", self.accum_view)):
                     if n + suffix in sd:
                         view(i).copy_(sd[n + suffix])
@@ -327,6 +377,8 @@ class GaccumTrainOp(_DeviceTrainOp):
         elif self.hp.variant == ADAM and "beta1_power" in sd:
             self.beta1_power = float(sd["beta1_power"])
             self.beta2_power = float(sd["beta2_power"])
+        if self.master is not None:
+            self._refresh_model()
 
 
 class PackedTrainOp(_DeviceTrainOp):
@@ -349,6 +401,8 @@ class PackedTrainOp(_DeviceTrainOp):
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, loss_scale: Optional[LossScaleConfig] = None):
+        # autograd accumulates a 16-bit parameter's gradient in its own dtype: it cannot add into an fp32 slab
+        _refuse_half(params, "PackedTrainOp")
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale)
         self.param_slab = self._zeros_slab()
         self.accum = self._zeros_slab()
@@ -419,6 +473,7 @@ class HostTrainOp(_TrainOpCore):
                  global_step: int = 0, device: int = 0, loss_scale: Optional[LossScaleConfig] = None):
         if loss_scale is not None:   # host-resident models have no fp16 autocast: nothing to loss-scale
             raise ValueError("HostTrainOp does not support loss scaling")
+        _refuse_half(host_params, "HostTrainOp")
         self.world = 1
         for p in host_params:
             if p.device.type != "cpu" or p.dtype != torch.float32 or not p.is_contiguous():

@@ -50,6 +50,11 @@ extern "C" {
 #define GACCUM_ADAM_WEIGHT_DECAY 0 /* optimization.py:107-194 (BERT path; "variant A") */
 #define GACCUM_ADAM 1              /* tf.train.AdamOptimizer, TF1 ApplyAdam (02:41,61; 04:42,62) */
 
+/* element types of the model's weights and gradients (gaccum_plan_set_param_dtype) */
+#define GACCUM_DTYPE_F32 0  /* the default: no call needed */
+#define GACCUM_DTYPE_BF16 1
+#define GACCUM_DTYPE_F16 2
+
 typedef struct gaccum_plan gaccum_plan;
 typedef void* gaccum_stream_t; /* a cudaStream_t */
 
@@ -156,8 +161,23 @@ GACCUM_API int32_t gaccum_num_tiles(const gaccum_plan* plan);
 /* Algorithmic bytes of one launch: accumulate = 12 B x P; apply = 36 B x P (SURVEY.md 8(d)).
  * The first accumulate of a window does not read the accumulators (8 B x P; see gaccum_step), so
  * a window of N >= 2 micro-steps moves (8 + 12 (N-2) + 36) B x P.  The plan does not know N: the
- * accumulate figure stays 12 B x P. */
+ * accumulate figure stays 12 B x P.  A 16-bit plan (gaccum_plan_set_param_dtype) reads 2-byte gradients:
+ * accumulate = 10 B x P (first of a window 6 B x P); apply = 36 B x P (the 2 bytes saved on G are spent on
+ * the model copy). */
 GACCUM_API int64_t gaccum_algorithmic_bytes(const gaccum_plan* plan, int32_t is_apply);
+
+/* Trains a bf16 or fp16 model (dtype GACCUM_DTYPE_BF16 / GACCUM_DTYPE_F16) with fp32 master weights.  Host-only:
+ * validates its arguments and keeps `master_slab`, which must be a 16-byte aligned device slab of
+ * gaccum_padded_size() floats in the plan's layout (gaccum_offsets), holding the fp32 weights (e.g. the exact upcast
+ * of the model's).  Allowed only before the first compute call on the plan, like gaccum_plan_set_loss_scale; the two
+ * combine in either order.  From then on gaccum_step, gaccum_accumulate and gaccum_apply read grads[i] and params[i]
+ * as pointers to 16-bit tensors (any 2-byte alignment; 8-byte alignment takes the vector path).  The gradients are
+ * widened exactly and accumulated in fp32; the apply updates the master weights exactly as an fp32 plan updates its
+ * parameters, then stores params[i] = the master weights rounded to nearest-even (also after tensors without a
+ * gradient; never on a window that loss scaling skips).  The master weights are the truth: params[i] is an output.
+ * gaccum_step_packed, gaccum_step_dp, gaccum_apply_dp, gaccum_host_session_create and gaccum_step_host refuse such a
+ * plan with GACCUM_EINVAL. */
+GACCUM_API int gaccum_plan_set_param_dtype(gaccum_plan* plan, int32_t dtype, float* master_slab);
 
 /* Turns dynamic loss scaling on for this plan (see gaccum_loss_scale_config).  Host-only: validates `cfg` and keeps
  * `device_state` (non-NULL, 16-byte aligned; not dereferenced here).  Allowed only before the first call of a compute
@@ -177,7 +197,8 @@ GACCUM_API int gaccum_loss_scale_init(gaccum_plan* plan, gaccum_loss_scale_state
  * branch (assign_add -> /N -> clip_by_global_norm -> apply_gradients -> zero; :80-88), else
  * the accumulate branch (:93).  grads[i] / params[i]: device pointers to tensor i (scattered,
  * any 4-byte alignment; 16-byte alignment takes the vector path).  grads[i] == NULL means
- * "no gradient for this tensor" (optimization.py:132 skips such pairs).
+ * "no gradient for this tensor" (optimization.py:132 skips such pairs).  On a 16-bit plan
+ * (gaccum_plan_set_param_dtype) grads[i] and params[i] point at bf16 / fp16 tensors, cast to float*.
  * accum / m / v: device slabs of gaccum_padded_size() floats, 16-byte aligned.
  * The caller increments global_step afterwards (optimization.py:102-103).
  * PRECONDITION, first micro-step of a window (global_step - 1 applies, global_step does not; never
@@ -194,7 +215,8 @@ GACCUM_API int gaccum_step(gaccum_plan* plan, const float* const* grads, float* 
                            gaccum_stream_t stream);
 /* The two branches on their own (the data-parallel driver accumulates locally, all-reduces the
  * slab, then applies with grads == NULL).  gaccum_apply ignores args->global_step.
- * gaccum_accumulate has no step arguments and always reads accum: accum += G for any accum. */
+ * gaccum_accumulate has no step arguments and always reads accum: accum += G for any accum.
+ * On a 16-bit plan both take 16-bit grads[i] / params[i], as gaccum_step does. */
 GACCUM_API int gaccum_accumulate(gaccum_plan* plan, const float* const* grads, float* accum,
                                  gaccum_stream_t stream);
 GACCUM_API int gaccum_apply(gaccum_plan* plan, const float* const* grads, float* const* params,
