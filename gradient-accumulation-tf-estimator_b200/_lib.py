@@ -10,6 +10,7 @@ from . import build as _build
 
 ADAM_WEIGHT_DECAY = 0   # reference optimization.py:107-194
 ADAM = 1                # tf.train.AdamOptimizer (02:41, 04:42, another-example.py:135)
+LAMB = 2                # LAMB (You et al. 2019), TF-Addons' form with AdamWeightDecay's op order (gaccum.h)
 
 OK, EINVAL, ENODEVICE, ECUDA, ENCCL, ENOMEM = 0, -1, -2, -3, -4, -5
 
@@ -31,6 +32,10 @@ class HParams(C.Structure):
     @classmethod
     def bert(cls) -> "HParams":
         return cls(ADAM_WEIGHT_DECAY, 0, 0.9, 0.999, 1e-6, 0.01, 1.0)
+
+    @classmethod
+    def lamb(cls, beta1=0.9, beta2=0.999, epsilon=1e-6, weight_decay_rate=0.01, clip_norm=1.0) -> "HParams":
+        return cls(LAMB, 0, beta1, beta2, epsilon, weight_decay_rate, clip_norm)
 
     @classmethod
     def tf_adam(cls, beta1=0.9, beta2=0.999, epsilon=1e-8) -> "HParams":
@@ -144,6 +149,8 @@ def _load():
         "gaccum_plan_set_loss_scale": (C.c_int, [vp, C.POINTER(LossScaleConfig), vp]),
         "gaccum_loss_scale_init": (C.c_int, [vp, vp, vp]),
         "gaccum_plan_set_param_dtype": (C.c_int, [vp, i32, vp]),
+        "gaccum_plan_set_layer_adaptation": (C.c_int, [vp, vp]),
+        "gaccum_read_trust_ratios": (C.c_int, [vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -205,6 +212,13 @@ def decay_mask(names: Sequence[str], weight_decay_rate: float,
     speaks POSIX ERE: identical for the reference's plain substrings, different for Python-only syntax such as
     ``\\d`` or look-arounds -- both Python bindings therefore evaluate the patterns here.)"""
     return [_use_weight_decay(_variable_name(n), weight_decay_rate, exclude) for n in names]
+
+
+def adaptation_mask(names: Sequence[str], exclude: Optional[Sequence[str]]) -> List[bool]:
+    """LAMB's layer-adaptation mask (TF-Addons ``_do_layer_adaptation``): tensor i adapts unless a pattern of ``exclude``
+    is found (Python ``re.search``) in its name with a trailing ``:<digits>`` stripped.  Unlike the decay mask it does not
+    depend on the weight-decay rate."""
+    return [not any(re.search(r, _variable_name(n)) is not None for r in exclude or ()) for n in names]
 
 
 def decay_mask_c(names: Sequence[str], weight_decay_rate: float,
@@ -294,6 +308,17 @@ class Plan:
         call); ``master_slab`` points to ``padded_size`` floats of device memory in the plan's layout, 16-byte
         aligned.  The step calls then take 16-bit gradient and parameter pointers."""
         _check(_load().gaccum_plan_set_param_dtype(self._h, int(dtype), master_slab or None))
+
+    def set_layer_adaptation(self, adapt: Sequence[bool]) -> None:
+        """LAMB: which tensors are scaled by their trust ratio (before the first compute call; default all)."""
+        if len(adapt) != self.T:
+            raise ValueError(f"the adaptation mask has {len(adapt)} entries, the plan {self.T} tensors")
+        arr = (C.c_uint8 * max(self.T, 1))(*[1 if a else 0 for a in adapt])
+        _check(_load().gaccum_plan_set_layer_adaptation(self._h, C.cast(arr, C.c_void_p)))
+
+    def read_trust_ratios(self, host_ptr: int, stream: int = 0) -> None:
+        """LAMB: copy the last applied window's T trust ratios (fp32) to ``host_ptr``, asynchronously on ``stream``."""
+        _check(_load().gaccum_read_trust_ratios(self._h, host_ptr or None, stream))
 
     def close(self) -> None:
         if getattr(self, "_h", None):

@@ -18,6 +18,7 @@
 #include "../../include/gaccum.h"
 #include "gaccum_kernels.cuh"
 #include "gaccum_dp.cuh"
+#include "gaccum_lamb.cuh"
 
 using namespace gaccum;
 
@@ -76,6 +77,12 @@ struct gaccum_plan {
   // 16-bit model (gaccum_plan_set_param_dtype); set only while `computed` is false
   int32_t param_dtype = GACCUM_DTYPE_F32;
   float* master = nullptr;
+  // GACCUM_LAMB: per-tensor layer-adaptation flags (gaccum_plan_set_layer_adaptation), the exact per-tensor norm
+  // accumulators (two sets) and the trust ratios of the last applied window
+  std::vector<uint8_t> adapt;
+  uint8_t* d_adapt = nullptr;
+  LambTensorAcc* d_lamb_acc = nullptr;
+  float* d_ratios = nullptr;
   std::mutex mu;
   std::map<const void*, int> grid_cache;   // kernel -> co-resident grid size
 };
@@ -124,8 +131,8 @@ static Scalars make_scalars(const gaccum_hparams& hp, const gaccum_step_args* a)
   s.eps = (float)hp.epsilon;
   s.wd = (float)hp.weight_decay_rate;
   s.clip = (float)hp.clip_norm;
-  if (hp.variant == GACCUM_ADAM_WEIGHT_DECAY) {
-    s.omb1 = (float)(1.0 - hp.beta1);   // optimization.py:152 -- Python double, then fp32
+  if (hp.variant != GACCUM_ADAM) {
+    s.omb1 = (float)(1.0 - hp.beta1);   // optimization.py:152 -- Python double, then fp32 (GACCUM_LAMB the same)
     s.omb2 = (float)(1.0 - hp.beta2);   // optimization.py:154
   } else {
     volatile float o1 = 1.0f - s.b1, o2 = 1.0f - s.b2;   // ApplyAdam: T(1) - beta1()
@@ -220,8 +227,61 @@ static int launch_apply_loss_scaled(gaccum_plan* pl, KernelParams<CAP>& prm, boo
   }
 }
 
+// GACCUM_LAMB: one cooperative launch of kLambBlocksPerSm CTAs per SM (gaccum_lamb.cuh).  The grid depends on the plan
+// only -- the barrier counter advances by gridDim.x per barrier -- so every instantiation must fit kLambBlocksPerSm
+// CTAs on an SM; one that does not is an error, never a smaller grid.
+template <bool HAS_G, int CAP, int MODE, bool H>
+static int launch_lamb_kernel(gaccum_plan* pl, LambKernelParams<CAP>& lp, cudaStream_t st) {
+  const void* fn = (const void*)&lamb_apply_kernel<HAS_G, CAP, MODE, H>;
+  {
+    std::lock_guard<std::mutex> lk(pl->mu);
+    if (pl->grid_cache.find(fn) == pl->grid_cache.end()) {
+      int per_sm = 0;
+      CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kThreads, 0));
+      if (per_sm < kLambBlocksPerSm)
+        return fail(GACCUM_ECUDA, "lamb_apply_kernel fits %d CTAs per SM, it needs %d", per_sm, kLambBlocksPerSm);
+      pl->grid_cache[fn] = kLambBlocksPerSm;
+    }
+  }
+  const int grid = std::max(1, std::min(pl->num_sms * kLambBlocksPerSm, (int)pl->tiles.size()));
+  void* args[] = {(void*)&lp};
+  CUDA_TRY(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kThreads), args, 0, st));
+  return GACCUM_OK;
+}
+
+template <int CAP, bool H>
+static int launch_lamb(gaccum_plan* pl, const KernelParams<CAP>& prm, bool has_g, const gaccum_step_args* a, cudaStream_t st) {
+  LambKernelParams<CAP>* lp = new (std::nothrow) LambKernelParams<CAP>();
+  if (!lp) return fail(GACCUM_ENOMEM, "out of host memory");
+  lp->k = prm;
+  lp->k.barrier = pl->d_barrier;
+  lp->k.counters = pl->d_counters;
+  lp->lamb.acc = pl->d_lamb_acc;
+  lp->lamb.ratios = pl->d_ratios;
+  lp->lamb.adapt = pl->d_adapt;
+  lp->lamb.num_tensors = pl->T;
+  lp->lamb.beta1_power = a ? a->beta1_power : 0.0f;
+  lp->lamb.beta2_power = a ? a->beta2_power : 0.0f;
+  const bool clip = pl->hp.clip_norm > 0.0;
+  const int mode = pl->ls_on ? (clip ? kLambLsClip : kLambLsNoClip) : (clip ? kLambClip : kLambNoClip);
+  int rc;
+  switch (mode * 2 + (has_g ? 1 : 0)) {
+    case 0: rc = launch_lamb_kernel<false, CAP, kLambNoClip, H>(pl, *lp, st); break;
+    case 1: rc = launch_lamb_kernel<true, CAP, kLambNoClip, H>(pl, *lp, st); break;
+    case 2: rc = launch_lamb_kernel<false, CAP, kLambClip, H>(pl, *lp, st); break;
+    case 3: rc = launch_lamb_kernel<true, CAP, kLambClip, H>(pl, *lp, st); break;
+    case 4: rc = launch_lamb_kernel<false, CAP, kLambLsClip, H>(pl, *lp, st); break;
+    case 5: rc = launch_lamb_kernel<true, CAP, kLambLsClip, H>(pl, *lp, st); break;
+    case 6: rc = launch_lamb_kernel<false, CAP, kLambLsNoClip, H>(pl, *lp, st); break;
+    default: rc = launch_lamb_kernel<true, CAP, kLambLsNoClip, H>(pl, *lp, st); break;
+  }
+  delete lp;
+  return rc;
+}
+
 template <int CAP, bool H = false>
-static int launch_apply(gaccum_plan* pl, KernelParams<CAP>& prm, bool has_g, cudaStream_t st) {
+static int launch_apply(gaccum_plan* pl, KernelParams<CAP>& prm, bool has_g, const gaccum_step_args* a, cudaStream_t st) {
+  if (pl->hp.variant == GACCUM_LAMB) return launch_lamb<CAP, H>(pl, prm, has_g, a, st);
   const bool clip = pl->hp.clip_norm > 0.0;
   if (pl->ls_on) return launch_apply_loss_scaled<CAP, H>(pl, prm, has_g, clip, st);
   const int key = (pl->hp.variant == GACCUM_ADAM ? 4 : 0) | (clip ? 2 : 0) | (has_g ? 1 : 0);
@@ -327,8 +387,8 @@ static int do_apply_tab(gaccum_plan* pl, const float* const* grads, float* const
   fill_common(pl, *prm, accum, m, v, make_scalars(pl->hp, a));
   int rc = fill_table(pl, prm->tab, grads, params);
   if (rc == GACCUM_OK) {
-    rc = pl->master ? launch_apply<CAP, true>(pl, *prm, grads != nullptr, st)
-                    : launch_apply<CAP, false>(pl, *prm, grads != nullptr, st);
+    rc = pl->master ? launch_apply<CAP, true>(pl, *prm, grads != nullptr, a, st)
+                    : launch_apply<CAP, false>(pl, *prm, grads != nullptr, a, st);
   }
   delete prm;
   return rc;
@@ -343,6 +403,7 @@ static int check_args(const gaccum_step_args* a) {
 
 static void free_plan_device(gaccum_plan* pl) {
   cudaFree(pl->d_tiles); cudaFree(pl->d_partials); cudaFree(pl->d_stats); cudaFree(pl->d_dp_sync); cudaFree(pl->d_barrier); cudaFree(pl->d_counters);
+  cudaFree(pl->d_adapt); cudaFree(pl->d_lamb_acc); cudaFree(pl->d_ratios);
 #ifdef GACCUM_EXPERIMENTS
   cudaFree(pl->d_debug);
 #endif
@@ -425,7 +486,7 @@ int gaccum_plan_create(gaccum_plan** out, int32_t T, const int64_t* numels, cons
   *out = nullptr;
   if (T < 0 || (T > 0 && !numels)) return fail(GACCUM_EINVAL, "bad tensor list");
   if (!hp) return fail(GACCUM_EINVAL, "hp is NULL");
-  if (hp->variant != GACCUM_ADAM_WEIGHT_DECAY && hp->variant != GACCUM_ADAM)
+  if (hp->variant != GACCUM_ADAM_WEIGHT_DECAY && hp->variant != GACCUM_ADAM && hp->variant != GACCUM_LAMB)
     return fail(GACCUM_EINVAL, "unknown optimizer variant %d", hp->variant);
   if (hp->reserved != 0) return fail(GACCUM_EINVAL, "reserved fields must be 0");
   if (T > kCapLarge)
@@ -436,7 +497,8 @@ int gaccum_plan_create(gaccum_plan** out, int32_t T, const int64_t* numels, cons
   pl->hp = *hp;
   pl->numel.assign(numels, numels + T);
   pl->decay.assign((size_t)T, 0);
-  if (hp->variant == GACCUM_ADAM_WEIGHT_DECAY && decay) pl->decay.assign(decay, decay + T);
+  if (hp->variant != GACCUM_ADAM && decay) pl->decay.assign(decay, decay + T);
+  if (hp->variant == GACCUM_LAMB) pl->adapt.assign((size_t)T, 1);   // every tensor adapts unless told otherwise
   if (int rc = build_layout(pl)) { delete pl; return rc; }
   pl->device = -1;
   if (device >= 0) {
@@ -465,6 +527,16 @@ int gaccum_plan_create(gaccum_plan** out, int32_t T, const int64_t* numels, cons
 #endif
     if (e == cudaSuccess) e = cudaMalloc(&pl->d_stats, sizeof(gaccum_stats));
     if (e == cudaSuccess) e = cudaMemset(pl->d_stats, 0, sizeof(gaccum_stats));
+    if (hp->variant == GACCUM_LAMB) {
+      const size_t nt = (size_t)std::max(1, T);
+      const std::vector<float> ones(nt, 1.0f);
+      if (e == cudaSuccess) e = cudaMalloc(&pl->d_adapt, nt);
+      if (e == cudaSuccess && T > 0) e = cudaMemcpy(pl->d_adapt, pl->adapt.data(), (size_t)T, cudaMemcpyHostToDevice);
+      if (e == cudaSuccess) e = cudaMalloc(&pl->d_lamb_acc, 2 * nt * sizeof(LambTensorAcc));
+      if (e == cudaSuccess) e = cudaMemset(pl->d_lamb_acc, 0, 2 * nt * sizeof(LambTensorAcc));
+      if (e == cudaSuccess) e = cudaMalloc(&pl->d_ratios, nt * sizeof(float));
+      if (e == cudaSuccess) e = cudaMemcpy(pl->d_ratios, ones.data(), nt * sizeof(float), cudaMemcpyHostToDevice);
+    }
     if (e != cudaSuccess) {
       free_plan_device(pl);
       delete pl;
@@ -504,8 +576,11 @@ int64_t gaccum_algorithmic_bytes(const gaccum_plan* pl, int32_t is_apply) {
   // The plan does not know N: the accumulate figure is the 12 B x P of the other accumulate steps.
   // 16-bit model: G is 2 bytes (accumulate 10 B x P); the apply reads G 2 + a, p, m, v 16 and writes p, m, v, a 16 +
   // the 2-byte model copy (36 B x P).
-  if (pl->master) return pl->P * (is_apply ? 36 : 10);
-  return pl->P * (is_apply ? 36 : 12);
+  // GACCUM_LAMB apply: those 36 B, plus p read a second time (phase 3) and u written and read back: 48 B x P (a 16-bit
+  // plan the same).  Phase 1's a' round trip is not counted, as the clip-apply's is not.
+  const int64_t apply_bytes = pl->hp.variant == GACCUM_LAMB ? 48 : 36;
+  if (pl->master) return pl->P * (is_apply ? apply_bytes : 10);
+  return pl->P * (is_apply ? apply_bytes : 12);
 }
 
 // true iff x is 2^k for an integer k in [lo, hi]
@@ -544,6 +619,33 @@ int gaccum_plan_set_param_dtype(gaccum_plan* pl, int32_t dtype, float* master_sl
   if (pl->computed) return fail(GACCUM_EINVAL, "the parameter dtype can only be set before the plan's first compute call");
   pl->param_dtype = dtype;
   pl->master = master_slab;
+  return GACCUM_OK;
+}
+
+static int refuse_lamb(const gaccum_plan* pl, const char* what) {
+  return pl && pl->hp.variant == GACCUM_LAMB ? fail(GACCUM_EINVAL, "%s does not support GACCUM_LAMB", what) : GACCUM_OK;
+}
+
+int gaccum_plan_set_layer_adaptation(gaccum_plan* pl, const uint8_t* adapt) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (pl->hp.variant != GACCUM_LAMB) return fail(GACCUM_EINVAL, "layer adaptation is a GACCUM_LAMB setting (plan variant %d)", pl->hp.variant);
+  if (!adapt && pl->T > 0) return fail(GACCUM_EINVAL, "adapt is NULL");
+  if (pl->computed) return fail(GACCUM_EINVAL, "layer adaptation can only be set before the plan's first compute call");
+  for (int32_t t = 0; t < pl->T; ++t) pl->adapt[t] = adapt[t] ? 1 : 0;
+  if (pl->device >= 0 && pl->T > 0) {
+    DeviceGuard guard(pl->device);
+    CUDA_TRY(cudaMemcpy(pl->d_adapt, pl->adapt.data(), (size_t)pl->T, cudaMemcpyHostToDevice));
+  }
+  return GACCUM_OK;
+}
+
+int gaccum_read_trust_ratios(gaccum_plan* pl, float* host_out, gaccum_stream_t stream) {
+  if (!pl || !host_out) return fail(GACCUM_EINVAL, "bad arguments to gaccum_read_trust_ratios");
+  if (pl->hp.variant != GACCUM_LAMB) return fail(GACCUM_EINVAL, "trust ratios exist on GACCUM_LAMB plans only (plan variant %d)", pl->hp.variant);
+  if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan has no trust ratios");
+  if (pl->T == 0) return GACCUM_OK;
+  DeviceGuard guard(pl->device);
+  CUDA_TRY(cudaMemcpyAsync(host_out, pl->d_ratios, sizeof(float) * (size_t)pl->T, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   return GACCUM_OK;
 }
 
@@ -619,7 +721,7 @@ int gaccum_step_packed(gaccum_plan* pl, const float* grad_slab, float* param_sla
     return launch_accumulate(pl, prm, force_branch < 0 && first_of_window(a), st);
   }
   if (!param_slab || !aligned16_host(param_slab)) return fail(GACCUM_EINVAL, "param_slab must be a 16-byte aligned device pointer");
-  return launch_apply(pl, prm, grad_slab != nullptr, st);
+  return launch_apply(pl, prm, grad_slab != nullptr, a, st);
 }
 
 // contiguous tile ranges with (nearly) equal element counts: boundary r = first tile whose cumulative
@@ -721,6 +823,7 @@ static int do_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float*
 int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* const* grads, float* m, float* v,
                     const gaccum_step_args* a, uint32_t epoch, gaccum_stream_t stream) {
   if (pl && pl->ls_on) return fail(GACCUM_EINVAL, "the fused data-parallel apply does not support loss scaling");
+  if (int rc = refuse_lamb(pl, "the fused data-parallel apply")) return rc;
   if (int rc = refuse_half(pl, "the fused data-parallel apply")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (comm->world < 2 || comm->world > GACCUM_MAX_RANKS || comm->rank < 0 || comm->rank >= comm->world)
@@ -745,6 +848,7 @@ int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* co
 int gaccum_step_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* const* grads, float* m, float* v,
                    const gaccum_step_args* a, uint32_t epoch, gaccum_stream_t stream) {
   if (pl && pl->ls_on) return fail(GACCUM_EINVAL, "the fused data-parallel step does not support loss scaling");
+  if (int rc = refuse_lamb(pl, "the fused data-parallel step")) return rc;
   if (int rc = refuse_half(pl, "the fused data-parallel step")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (int rc = check_args(a)) return rc;
@@ -827,6 +931,7 @@ int gaccum_host_session_create(gaccum_host_session** out, gaccum_plan* pl) {
   // host-resident models train in fp32 (no fp16 autocast on the CPU): nothing to loss-scale
   if (pl->ls_on) return fail(GACCUM_EINVAL, "the host-buffer session does not support loss scaling");
   if (int rc = refuse_half(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse_lamb(pl, "the host-buffer session")) return rc;
   if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): libgaccum has no CPU fallback, a CUDA device is required");
   DeviceGuard guard(pl->device);
   gaccum_host_session* s = new (std::nothrow) gaccum_host_session();
@@ -936,6 +1041,7 @@ int gaccum_step_host(gaccum_host_session* s, const float* const* host_grads, flo
   gaccum_plan* pl = s->plan;
   if (pl->ls_on) return fail(GACCUM_EINVAL, "the host-buffer session does not support loss scaling");
   if (int rc = refuse_half(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse_lamb(pl, "the host-buffer session")) return rc;
   DeviceGuard guard(pl->device);
   const int b = (int)(s->calls & 1);
   ++s->calls;

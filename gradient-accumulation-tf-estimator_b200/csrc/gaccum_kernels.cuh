@@ -656,6 +656,79 @@ __device__ __forceinline__ double acc_value(const unsigned long long* bins /* kA
   return scalbn(m, 32 * (top - 2) - 1074);
 }
 
+// ---- pieces the cooperative apply kernels share (apply_clip_kernel, lamb_apply_kernel in gaccum_lamb.cuh) ----------
+// block 0: the other counter set was used by the previous launch on this plan, which is complete: clear it for the next
+// one (threads 64 .. 64 + sizeof(LaunchCounters) / 8)
+__device__ __forceinline__ void clear_other_counters(LaunchCounters* counters, const uint32_t set) {
+  if (blockIdx.x == 0 && threadIdx.x >= 64 && threadIdx.x < 64 + (int)(sizeof(LaunchCounters) / 8)) {
+    reinterpret_cast<unsigned long long*>(counters + (set ^ 1u))[threadIdx.x - 64] = 0ull;
+  }
+}
+// grid barrier, executed by ONE thread per CTA: one atomic on a monotonic counter (every launch on a plan uses the same
+// grid, so the counter advances by gridDim.x per barrier); cooperative launch guarantees that all CTAs are co-resident
+__device__ __forceinline__ void grid_barrier(unsigned long long* barrier) {
+  __threadfence();
+  const unsigned long long old = atomicAdd(barrier, 1ull);
+  const unsigned long long target = (old / gridDim.x + 1ull) * gridDim.x;
+  while (ld_acquire_gpu_u64(barrier) < target) { __nanosleep(20); }
+}
+// loss scaling: the state as this launch finds it (thread 0, before its CTA arrives at the first grid barrier)
+__device__ __forceinline__ void ls_load(const LossScaleState* st, LossScaleState& s) {
+  s.scale = __ldcg(&st->scale);
+  s.good_windows = __ldcg(&st->good_windows);
+  s.skipped_windows = __ldcg(&st->skipped_windows);
+  s.beta1_power = __ldcg(&st->beta1_power);
+  s.beta2_power = __ldcg(&st->beta2_power);
+}
+// thread 0 after the barrier, from the launch-wide counters (`bins`: their accumulator, copied where the thread reads
+// it): the clip scale s and the global norm gn (1 and 0 without clipping) and, loss-scaled, whether the window is
+// skipped -- an element of a' or, with clipping, gn is not finite.  Every CTA computes the same values.
+template <int LS>
+__device__ __forceinline__ void window_decision(const LaunchCounters* ctr, const unsigned long long* bins, const float clip,
+                                                float& s, float& gn, int& skip) {
+  if constexpr (LS == kLsNoClip) {
+    s = 1.f;                                              // no clipping: stats as the un-clipped apply writes them
+    gn = 0.f;
+    skip = (__ldcg(&ctr->nonfinite) & kElemNonfinite) != 0;
+  } else {
+    const unsigned int nonfinite = __ldcg(&ctr->nonfinite);
+    const double tot = acc_value(bins, nonfinite);
+    const float g_norm = __fsqrt_rn((float)tot);          // tf.linalg.global_norm
+    s = clip_scale(g_norm, clip);
+    gn = g_norm;
+    if constexpr (LS != kLsOff) skip = (nonfinite & kElemNonfinite) != 0 || !(fabsf(g_norm) <= 3.402823466e38f);
+  }
+}
+// block 0's thread 0 at the very end of a loss-scaled launch: TF 2 DynamicLossScale, counted in windows (gaccum.h,
+// gaccum_loss_scale_config); BETAS: the optimizer keeps TF1's beta powers, advanced on applied windows only
+template <bool BETAS>
+__device__ __forceinline__ void ls_finish(const LossScaleParams& ls, const LossScaleState& s_ls, const bool skip,
+                                          const float b1, const float b2) {
+  LossScaleState* out = ls.state;
+  const float S = s_ls.scale;
+  if (skip) {
+    const float down = __fdiv_rn(S, ls.multiplier);   // exact: both are powers of two
+    out->scale = down < 1.0f ? 1.0f : down;
+    out->good_windows = 0;
+    out->skipped_windows = s_ls.skipped_windows + 1u;
+    out->last_skipped = 1;
+  } else {
+    const int32_t good = s_ls.good_windows + 1;
+    if (good >= ls.growth_interval) {
+      const float up = __fmul_rn(S, ls.multiplier);
+      if (fabsf(up) <= 3.402823466e38f) out->scale = up;
+      out->good_windows = 0;
+    } else {
+      out->good_windows = good;
+    }
+    out->last_skipped = 0;
+    if constexpr (BETAS) {                            // TF1 AdamOptimizer._finish, applied windows only
+      out->beta1_power = __fmul_rn(s_ls.beta1_power, b1);
+      out->beta2_power = __fmul_rn(s_ls.beta2_power, b2);
+    }
+  }
+}
+
 // ---- pass 1, consumer side: one tile out of slot [G | a]; returns this THREAD's partial of sum((a'/N)^2) ----
 // A tile the producer did not copy (nvec == 0), and the < 4 tail elements of any tile, travel through global memory.
 // Loss-scaled (LS != kLsOff): the partial is of sum(((a'/N)(1/S))^2) (none without clipping), and `bad` is set when an
@@ -809,12 +882,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     if constexpr (LS != kLsOff) {
-      const LossScaleState* st = prm.ls.state;
-      s_ls.scale = __ldcg(&st->scale);
-      s_ls.good_windows = __ldcg(&st->good_windows);
-      s_ls.skipped_windows = __ldcg(&st->skipped_windows);
-      s_ls.beta1_power = __ldcg(&st->beta1_power);
-      s_ls.beta2_power = __ldcg(&st->beta2_power);
+      ls_load(prm.ls.state, s_ls);
       if constexpr (VARIANT == 1) {
         // make_scalars' op order: lr * sqrt(1 - b2^t) / (1 - b1^t), one rounding per op
         s_sc = prm.sc;
@@ -826,10 +894,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   for (int i = threadIdx.x; i < (kConsumerThreads / 32) * kAccBins; i += kClipThreads) (&s_bins[0][0])[i] = 0ull;
   __syncthreads();
   LaunchCounters* const ctr = prm.counters + s_set;
-  if (blockIdx.x == 0 && threadIdx.x >= 64 && threadIdx.x < 64 + (int)(sizeof(LaunchCounters) / 8)) {
-    // the other set was used by the previous launch on this plan, which is complete: clear it for the next one
-    reinterpret_cast<unsigned long long*>(prm.counters + (s_set ^ 1u))[threadIdx.x - 64] = 0ull;
-  }
+  clear_other_counters(prm.counters, s_set);
 
   if (is_producer) {
     // =========================== producer warp of group `grp` ===========================
@@ -1054,37 +1119,17 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     named_bar_sync(1, kConsumerThreads);
     if (threadIdx.x == 0 && s_nonfinite) atomicOr(&ctr->nonfinite, s_nonfinite);
     stamp(1);
-    // ---- grid barrier of the consumers: one atomic per CTA on a monotonic counter (every launch of this plan
-    //      uses the same grid, so the counter advances by gridDim.x per launch); cooperative launch guarantees
-    //      that all CTAs are co-resident ----
-    if (threadIdx.x == 0) {
-      __threadfence();
-      const unsigned long long old = atomicAdd(prm.barrier, 1ull);
-      const unsigned long long target = (old / gridDim.x + 1ull) * gridDim.x;
-      while (ld_acquire_gpu_u64(prm.barrier) < target) { __nanosleep(20); }
-    }
+    // ---- grid barrier of the consumers (grid_barrier: one atomic per CTA on the plan's monotonic counter) ----
+    if (threadIdx.x == 0) grid_barrier(prm.barrier);
     named_bar_sync(1, kConsumerThreads);
     if (leader) mbar_arrive(&s_go[grp]);                     // this group's producer may now fetch pool tiles
     stamp(2);
     // ---- every CTA evaluates the same exact sum the same way: bit-identical gn and clip scale everywhere ----
-    if constexpr (LS == kLsNoClip) {
-      if (threadIdx.x == 0) {
-        s_bcast[0] = 1.f;                                   // no clipping: stats as the un-clipped apply writes them
-        s_bcast[1] = 0.f;
-        s_skip = (__ldcg(&ctr->nonfinite) & kElemNonfinite) != 0;
-      }
-    } else {
+    if constexpr (LS != kLsNoClip) {
       if (threadIdx.x < kAccBins) s_bins[0][threadIdx.x] = __ldcg(&ctr->bins[threadIdx.x]);
       named_bar_sync(1, kConsumerThreads);
-      if (threadIdx.x == 0) {
-        const unsigned int nonfinite = __ldcg(&ctr->nonfinite);
-        const double tot = acc_value(s_bins[0], nonfinite);
-        const float g_norm = __fsqrt_rn((float)tot);          // tf.linalg.global_norm
-        s_bcast[0] = clip_scale(g_norm, prm.sc.clip);
-        s_bcast[1] = g_norm;
-        if constexpr (LS != kLsOff) s_skip = (nonfinite & kElemNonfinite) != 0 || !(fabsf(g_norm) <= 3.402823466e38f);
-      }
     }
+    if (threadIdx.x == 0) window_decision<LS>(ctr, s_bins[0], prm.sc.clip, s_bcast[0], s_bcast[1], s_skip);
     named_bar_sync(1, kConsumerThreads);
     const float s = s_bcast[0];
     bool skip = false;
@@ -1105,32 +1150,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) {
       prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s;
-      if constexpr (LS != kLsOff) {
-        // TF 2 DynamicLossScale, counted in windows (gaccum.h, gaccum_loss_scale_config)
-        LossScaleState* out = prm.ls.state;
-        const float S = s_ls.scale;
-        if (skip) {
-          const float down = __fdiv_rn(S, prm.ls.multiplier);   // exact: both are powers of two
-          out->scale = down < 1.0f ? 1.0f : down;
-          out->good_windows = 0;
-          out->skipped_windows = s_ls.skipped_windows + 1u;
-          out->last_skipped = 1;
-        } else {
-          const int32_t good = s_ls.good_windows + 1;
-          if (good >= prm.ls.growth_interval) {
-            const float up = __fmul_rn(S, prm.ls.multiplier);
-            if (fabsf(up) <= 3.402823466e38f) out->scale = up;
-            out->good_windows = 0;
-          } else {
-            out->good_windows = good;
-          }
-          out->last_skipped = 0;
-          if constexpr (VARIANT == 1) {                         // TF1 AdamOptimizer._finish, applied windows only
-            out->beta1_power = __fmul_rn(s_ls.beta1_power, prm.sc.b1);
-            out->beta2_power = __fmul_rn(s_ls.beta2_power, prm.sc.b2);
-          }
-        }
-      }
+      if constexpr (LS != kLsOff) ls_finish<VARIANT == 1>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
     }
   }
   __syncthreads();

@@ -94,6 +94,8 @@ class FusedDataParallelTrainOp:
         from .train_op import GaccumTrainOp
         if loss_scale is not None:
             raise ValueError("the fused data-parallel train op does not support loss scaling; use dp_mode='allreduce'")
+        if hp.variant == _lib.LAMB:
+            raise ValueError("the fused data-parallel train op does not support LAMB; use dp_mode='allreduce'")
         if any(p.dtype in (torch.bfloat16, torch.float16) for p in params):
             raise ValueError("multi-GPU training of bf16 / fp16 parameters is not supported yet")
         if not dist.is_initialized():

@@ -24,7 +24,7 @@ from typing import Callable, Iterable, List, Optional, Sequence, Tuple, Union
 import torch
 
 from . import _lib, graph
-from ._lib import ADAM, ADAM_WEIGHT_DECAY, HParams, LossScaleConfig
+from ._lib import ADAM, ADAM_WEIGHT_DECAY, LAMB, HParams, LossScaleConfig
 from .train_op import GaccumTrainOp
 
 # optimization.py:76 hard-codes 8 (README.md:17,34 says 4).  The signature has no argument for
@@ -33,6 +33,9 @@ gradient_accumulation_multiplier = int(os.environ.get("GACCUM_MULTIPLIER", "8"))
 clip_norm = 1.0   # optimization.py:84
 # Dynamic loss scaling for fp16 mixed precision (a LossScaleConfig), off by default; create_optimizer reads it.
 loss_scale: Optional[LossScaleConfig] = None
+# The optimizer create_optimizer builds: "adam" (the reference's AdamWeightDecayOptimizer) or "lamb" (LAMBOptimizer with
+# the same hyper-parameters and exclusions, for large effective batches).
+optimizer_type = "adam"
 
 LossLike = Union[torch.Tensor, Callable[[], torch.Tensor]]
 LrLike = Union[float, Callable[[int], float]]
@@ -74,7 +77,8 @@ class _OptimizerBase:
         if self._direct_op is None or self._direct_key != key:
             self._direct_op = GaccumTrainOp([v.tensor for v in vars_], [v.name for v in vars_],
                                             self._hparams(0.0), 1, _lr_callable(self.learning_rate),
-                                            exclude_from_weight_decay=getattr(self, "exclude_from_weight_decay", None))
+                                            exclude_from_weight_decay=getattr(self, "exclude_from_weight_decay", None),
+                                            exclude_from_layer_adaptation=getattr(self, "exclude_from_layer_adaptation", None))
             self._direct_key = key
         op = self._direct_op
         gs = graph.get_global_step()
@@ -114,6 +118,40 @@ class AdamWeightDecayOptimizer(_OptimizerBase):
         return _lib._variable_name(param_name)
 
 
+class LAMBOptimizer(_OptimizerBase):
+    """LAMB (You et al. 2019, "Large Batch Optimization for Deep Learning") in TF-Addons' form: bias-corrected Adam
+    moments, decoupled weight decay, and each tensor's update scaled by its trust ratio ||p|| / ||u||.
+    ``exclude_from_layer_adaptation`` defaults to ``exclude_from_weight_decay``, as in TF-Addons."""
+    variant = LAMB
+
+    def __init__(self, learning_rate: LrLike, weight_decay_rate=0.01, beta_1=0.9, beta_2=0.999, epsilon=1e-6,
+                 exclude_from_weight_decay: Optional[Sequence[str]] = None,
+                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None, name="LAMBOptimizer"):
+        super().__init__()
+        self.learning_rate = learning_rate
+        self.weight_decay_rate = weight_decay_rate
+        self.beta_1 = beta_1
+        self.beta_2 = beta_2
+        self.epsilon = epsilon
+        self.exclude_from_weight_decay = exclude_from_weight_decay
+        self.exclude_from_layer_adaptation = exclude_from_layer_adaptation if exclude_from_layer_adaptation is not None \
+            else exclude_from_weight_decay
+        self.name = name
+
+    def _hparams(self, clip: float) -> HParams:
+        return HParams(LAMB, 0, self.beta_1, self.beta_2, self.epsilon, self.weight_decay_rate, clip)
+
+    def _do_use_weight_decay(self, param_name: str) -> bool:
+        return _lib._use_weight_decay(param_name, self.weight_decay_rate, self.exclude_from_weight_decay)
+
+    def _do_layer_adaptation(self, param_name: str) -> bool:
+        """TF-Addons LAMB._do_layer_adaptation: by name only, whatever the weight-decay rate."""
+        return _lib.adaptation_mask([param_name], self.exclude_from_layer_adaptation)[0]
+
+    def _get_variable_name(self, param_name: str) -> str:
+        return _lib._variable_name(param_name)
+
+
 class AdamOptimizer(_OptimizerBase):
     """``tf.train.AdamOptimizer`` as the example scripts use it (02:41, 04:42, another-example.py:135)."""
     variant = ADAM
@@ -141,6 +179,8 @@ class TrainOp:
         hp = optimizer._hparams(clip or 0.0)
         lr_fn = _lr_callable(optimizer.learning_rate)
         exclude = getattr(optimizer, "exclude_from_weight_decay", None)
+        adapt_kw = {"exclude_from_layer_adaptation": getattr(optimizer, "exclude_from_layer_adaptation", None)} \
+            if hp.variant == LAMB else {}
         self.dp = None
         if process_group is not None:
             # reference 04: MultiWorkerMirroredStrategy.  "fused": the exchange happens inside the apply
@@ -153,11 +193,11 @@ class TrainOp:
                 self.engine = self.dp.engine
             else:
                 self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step),
-                                            loss_scale=loss_scale)
+                                            loss_scale=loss_scale, **adapt_kw)
                 self.dp = DataParallelTrainOp(self.engine, pg)
         else:
             self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step),
-                                        loss_scale=loss_scale)
+                                        loss_scale=loss_scale, **adapt_kw)
         self.last_loss: Optional[torch.Tensor] = None
 
     @property
@@ -217,12 +257,17 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
     Schedule :29-54; AdamWeightDecayOptimizer(0.01, 0.9, 0.999, 1e-6, exclude LayerNorm/layer_norm/
     bias) :59-65; window ``gradient_accumulation_multiplier`` :76; apply branch (/N, clip 1.0,
     apply_gradients, zero) :80-88; ``tf.cond`` on the pre-increment step :91-94; step++ :102-103.
+    With the module attribute ``optimizer_type = "lamb"`` the optimizer is a LAMBOptimizer with the same
+    hyper-parameters and exclusions (layer adaptation excludes what weight decay excludes).
     """
     if use_tpu:
         # optimization.py:67-68 wraps the optimizer in tf.contrib.tpu.CrossShardOptimizer: TPU-only.
         raise ValueError("use_tpu=True is not supported: this train_op targets H100 GPUs")
     global_step = graph.get_or_create_global_step()
-    optimizer = AdamWeightDecayOptimizer(
+    if optimizer_type not in ("adam", "lamb"):
+        raise ValueError(f"optimizer_type must be 'adam' or 'lamb' (got {optimizer_type!r})")
+    cls = LAMBOptimizer if optimizer_type == "lamb" else AdamWeightDecayOptimizer
+    optimizer = cls(
         learning_rate=bert_learning_rate(init_lr, num_train_steps, num_warmup_steps),
         weight_decay_rate=0.01, beta_1=0.9, beta_2=0.999, epsilon=1e-6,
         exclude_from_weight_decay=["LayerNorm", "layer_norm", "bias"])

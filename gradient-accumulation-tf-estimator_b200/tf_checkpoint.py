@@ -5,7 +5,8 @@ the parameters, ``global_step``, one UNNAMED ``tf.Variable`` per trainable varia
 (optimization.py:78, 02:54, another-example.py:133 -- TensorFlow names them ``Variable``, ``Variable_1``, ... in creation =
 ``tf.trainable_variables()`` order), and the optimizer's slots: ``<name>/adam_m``, ``<name>/adam_v`` for
 ``AdamWeightDecayOptimizer`` (optimization.py:137-148), ``<name>/Adam``, ``<name>/Adam_1``, ``beta1_power``,
-``beta2_power`` for ``tf.train.AdamOptimizer`` (02:41, another-example.py:135).  A run that was checkpointed by the reference
+``beta2_power`` for ``tf.train.AdamOptimizer`` (02:41, another-example.py:135), ``<name>/lamb_m``, ``<name>/lamb_v`` and
+the beta powers for LAMB.  A run that was checkpointed by the reference
 mid-window can therefore be continued by this train_op, and the other way round, if those files can be read and written.
 
 File format (restated from TensorFlow's published sources, tensorflow/core/util/tensor_bundle/ and core/lib/io/table*):
@@ -380,8 +381,10 @@ def latest_checkpoint(model_dir: str) -> Optional[str]:
 # ---------------------------------------------------------------------------------------------------------------------
 # the reference's variable names  <->  this train_op's state_dict()
 # ---------------------------------------------------------------------------------------------------------------------
-ADAM_WEIGHT_DECAY, ADAM = 0, 1
-_SLOTS = {ADAM_WEIGHT_DECAY: ("/adam_m", "/adam_v"), ADAM: ("/Adam", "/Adam_1")}      # optimization.py:137-148 / TF1 AdamOptimizer slots
+ADAM_WEIGHT_DECAY, ADAM, LAMB = 0, 1, 2
+# optimization.py:137-148 / TF1 AdamOptimizer slots / LAMB's slots, named like AdamWeightDecay's (NVIDIA's TF BERT)
+_SLOTS = {ADAM_WEIGHT_DECAY: ("/adam_m", "/adam_v"), ADAM: ("/Adam", "/Adam_1"), LAMB: ("/lamb_m", "/lamb_v")}
+_BETA_POWERS = (ADAM, LAMB)      # variants that keep TF1's beta1_power / beta2_power
 
 
 def _accum_name(i: int) -> str:
@@ -400,7 +403,7 @@ def to_reference_names(state: Dict[str, object], names: Sequence[str], variant: 
         out[n + m_s] = arr(state[n + "/adam_m"])
         out[n + v_s] = arr(state[n + "/adam_v"])
         out[_accum_name(i)] = arr(state[n + "/accum_grad"])
-    if variant == ADAM:
+    if variant in _BETA_POWERS:
         out["beta1_power"] = arr(state["beta1_power"], np.float32)
         out["beta2_power"] = arr(state["beta2_power"], np.float32)
     return out
@@ -417,7 +420,7 @@ def from_reference_names(tensors: Dict[str, np.ndarray], names: Sequence[str], v
                 out[dst] = tensors[src]
             elif strict:
                 raise KeyError(f"checkpoint has no tensor {src!r}")
-    if variant == ADAM:
+    if variant in _BETA_POWERS:
         for k in ("beta1_power", "beta2_power"):
             if k in tensors:
                 out[k] = tensors[k]
@@ -455,7 +458,7 @@ def to_shim_names(ref: Dict[str, np.ndarray], names: Sequence[str], variant: int
                 buf[offs[i]:offs[i] + sizes[i]] = np.asarray(ref[src], np.float32).reshape(-1)
         out[slab] = buf
     out["gaccum/beta_powers"] = np.asarray([ref.get("beta1_power", betas[0]), ref.get("beta2_power", betas[1])], np.float32) \
-        if variant == ADAM else np.asarray(betas, np.float32)
+        if variant in _BETA_POWERS else np.asarray(betas, np.float32)
     return out
 
 
@@ -472,7 +475,7 @@ def from_shim_names(shim: Dict[str, np.ndarray], names: Sequence[str], variant: 
             raise ValueError(f"{slab} holds {buf.size} elements, the variables need {total}")
         for i, n in enumerate(names):
             out[_accum_name(i) if key is None else n + key] = buf[offs[i]:offs[i] + sizes[i]].reshape(np.asarray(shim[n]).shape).copy()
-    if variant == ADAM:
+    if variant in _BETA_POWERS:
         bp = np.asarray(shim["gaccum/beta_powers"], np.float32).reshape(-1)
         out["beta1_power"], out["beta2_power"] = np.float32(bp[0]), np.float32(bp[1])
     return out
@@ -526,7 +529,7 @@ def restore(prefix_or_dir: str, train_op, names: Optional[Sequence[str]] = None,
 
 def _main(argv: Optional[Sequence[str]] = None) -> int:
     """python -m gaccum_b200.tf_checkpoint list <prefix|model_dir>
-       python -m gaccum_b200.tf_checkpoint convert {to-shim|to-reference} <in prefix> <out prefix> --names FILE [--variant 0|1]
+       python -m gaccum_b200.tf_checkpoint convert {to-shim|to-reference} <in prefix> <out prefix> --names FILE [--variant 0|1|2]
     (FILE: one trainable-variable name per line, in tf.trainable_variables() order -- the order is not in a checkpoint)"""
     import argparse
     ap = argparse.ArgumentParser(prog="gaccum_b200.tf_checkpoint", description=_main.__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
@@ -538,7 +541,7 @@ def _main(argv: Optional[Sequence[str]] = None) -> int:
     cv.add_argument("src")
     cv.add_argument("dst")
     cv.add_argument("--names", required=True)
-    cv.add_argument("--variant", type=int, default=0, choices=[0, 1])
+    cv.add_argument("--variant", type=int, default=0, choices=[0, 1, 2])
     a = ap.parse_args(argv)
     if a.cmd == "list":
         prefix = latest_checkpoint(a.prefix) if os.path.isdir(a.prefix) else a.prefix

@@ -85,6 +85,9 @@ class GaccumStepOpT : public tf::OpKernel {
     OP_REQUIRES_OK(c, c->GetAttr("N", &n_));
     OP_REQUIRES_OK(c, c->GetAttr("accum_n", &accum_n_));
     OP_REQUIRES_OK(c, c->GetAttr("variant", &hp_.variant));
+    // the graph op carries no trust-ratio state or adaptation mask: LAMB (variant 2) is a Python train_op feature
+    OP_REQUIRES(c, hp_.variant == GACCUM_ADAM_WEIGHT_DECAY || hp_.variant == GACCUM_ADAM,
+                tf::errors::InvalidArgument("variant must be 0 (AdamWeightDecay) or 1 (Adam), got ", hp_.variant));
     OP_REQUIRES_OK(c, c->GetAttr("beta1", &b1));
     OP_REQUIRES_OK(c, c->GetAttr("beta2", &b2));
     OP_REQUIRES_OK(c, c->GetAttr("epsilon", &eps));

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import ADAM, HParams, LossScaleConfig, Plan, StepArgs
+from ._lib import ADAM, ADAM_WEIGHT_DECAY, LAMB, HParams, LossScaleConfig, Plan, StepArgs
 
 
 def _f32(x) -> float:
@@ -53,7 +53,7 @@ class _TrainOpCore:
 
     def __init__(self, params: Sequence[torch.Tensor], names: Sequence[str], hp: HParams, accum_n: int,
                  lr_fn: Callable[[int], float], exclude_from_weight_decay: Optional[Sequence[str]],
-                 global_step: int, device: int):
+                 global_step: int, device: int, exclude_from_layer_adaptation: Optional[Sequence[str]] = None):
         if len(params) != len(names):
             raise ValueError("params and names differ in length")
         self.params = list(params)
@@ -61,8 +61,15 @@ class _TrainOpCore:
         self.names = [_lib._variable_name(n) for n in names]
         self.hp, self.N, self.lr_fn, self.global_step = hp, int(accum_n), lr_fn, int(global_step)
         self.decay = _lib.decay_mask(names, hp.weight_decay_rate, exclude_from_weight_decay) \
-            if hp.variant == _lib.ADAM_WEIGHT_DECAY else [False] * len(params)
+            if hp.variant in (ADAM_WEIGHT_DECAY, LAMB) else [False] * len(params)
         self.plan = Plan([p.numel() for p in params], self.decay, hp, device=device)
+        # LAMB: the layer-adaptation mask; as in TF-Addons, its exclusions default to the weight-decay ones, and it is
+        # evaluated by name whatever the weight-decay rate
+        self.adapt: Optional[list] = None
+        if hp.variant == LAMB:
+            excl = exclude_from_layer_adaptation if exclude_from_layer_adaptation is not None else exclude_from_weight_decay
+            self.adapt = _lib.adaptation_mask(names, excl)
+            self.plan.set_layer_adaptation(self.adapt)
         # TF1 AdamOptimizer._create_slots: beta powers start at beta
         self.beta1_power, self.beta2_power = _f32(hp.beta1), _f32(hp.beta2)
         self._stats_host = _pinned_zeros(4)
@@ -76,7 +83,7 @@ class _TrainOpCore:
         """TF1 AdamOptimizer._finish: beta_power <- beta_power * beta (fp32) after the updates of an apply step.
         Under loss scaling the beta powers live in the device block and the apply kernel advances them, on applied
         windows only."""
-        if self.hp.variant == ADAM and self._ls_state is None:
+        if self.hp.variant in (ADAM, LAMB) and self._ls_state is None:
             self.beta1_power = _f32(np.float32(self.beta1_power) * np.float32(self.hp.beta1))
             self.beta2_power = _f32(np.float32(self.beta2_power) * np.float32(self.hp.beta2))
 
@@ -85,14 +92,14 @@ class _DeviceTrainOp(_TrainOpCore):
     """A train op whose parameters live on one CUDA device and whose Adam moments are packed HBM slabs."""
 
     def __init__(self, params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step,
-                 loss_scale: Optional[LossScaleConfig] = None):
+                 loss_scale: Optional[LossScaleConfig] = None, exclude_from_layer_adaptation=None):
         if not params:
             raise ValueError("no trainable variables")
         self.device = params[0].device
         if self.device.type != "cuda":
             raise _lib.GaccumError(_lib.ENODEVICE, "parameters must live on a CUDA device: the train_op has no CPU fallback")
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step,
-                         self.device.index or 0)
+                         self.device.index or 0, exclude_from_layer_adaptation)
         self.m = self._zeros_slab()
         self.v = self._zeros_slab()
         if loss_scale is not None:
@@ -130,6 +137,17 @@ class _DeviceTrainOp(_TrainOpCore):
         stream.synchronize()
         return _stats_dict(self._stats_host)
 
+    def trust_ratios(self) -> np.ndarray:
+        """LAMB: synchronously read the per-tensor trust ratios r of the last applied window (1 for tensors without
+        layer adaptation, and before the first apply) -- what LAMB users log per layer."""
+        if self.hp.variant != LAMB:
+            raise ValueError("trust ratios exist for LAMB train ops only")
+        out = _pinned_zeros(len(self.params))
+        stream = torch.cuda.current_stream(self.device)
+        self.plan.read_trust_ratios(out.data_ptr(), stream.cuda_stream)
+        stream.synchronize()
+        return out.numpy().copy()
+
     def loss_scale_state(self) -> Dict[str, float]:
         """Synchronously read the loss-scaling block (for logging): scale, good_windows, skipped_windows and
         last_skipped (True if the last apply step skipped its window)."""
@@ -145,7 +163,7 @@ class _DeviceTrainOp(_TrainOpCore):
         words = self._ls_state.cpu()
         out["loss_scale/current_loss_scale"] = words[0].clone()
         out["loss_scale/good_steps"] = torch.tensor(int(words.view(torch.int32)[1]), dtype=torch.int64)
-        if self.hp.variant == ADAM:
+        if self.hp.variant in (ADAM, LAMB):
             out["beta1_power"] = words[4].clone()
             out["beta2_power"] = words[5].clone()
 
@@ -158,7 +176,7 @@ class _DeviceTrainOp(_TrainOpCore):
                 raise ValueError(f"loss_scale/current_loss_scale must be a power of two in [1, 2^127], got {s!r}")
             words[0] = s
             words.view(torch.int32)[1] = int(sd["loss_scale/good_steps"])
-        if self.hp.variant == ADAM and "beta1_power" in sd:
+        if self.hp.variant in (ADAM, LAMB) and "beta1_power" in sd:
             words[4] = float(sd["beta1_power"])
             words[5] = float(sd["beta2_power"])
         self._ls_state.copy_(words)
@@ -177,13 +195,15 @@ class GaccumTrainOp(_DeviceTrainOp):
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, accum: Optional[torch.Tensor] = None,
-                 loss_scale: Optional[LossScaleConfig] = None):
+                 loss_scale: Optional[LossScaleConfig] = None,
+                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None):
         dtypes = {p.dtype for p in params}
         if len(dtypes) > 1 and dtypes & set(_HALF_DTYPES):
             raise ValueError(f"parameters of mixed dtypes ({', '.join(sorted(str(d) for d in dtypes))}): "
                              "a 16-bit model must be all bf16 or all fp16")
         self.param_dtype = params[0].dtype if len(dtypes) == 1 and params[0].dtype in _HALF_DTYPES else torch.float32
-        super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale)
+        super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale,
+                         exclude_from_layer_adaptation)
         for p in self.params:
             if p.dtype != self.param_dtype or not p.is_contiguous() or p.device != self.device:
                 if self.param_dtype != torch.float32:
@@ -354,7 +374,7 @@ class GaccumTrainOp(_DeviceTrainOp):
             out[n + "/adam_m"] = self.m_view(i).clone()
             out[n + "/adam_v"] = self.v_view(i).clone()
             out[n + "/accum_grad"] = self.accum_view(i).clone()
-        if self.hp.variant == ADAM:
+        if self.hp.variant in (ADAM, LAMB):
             out["beta1_power"] = torch.tensor(self.beta1_power, dtype=torch.float32)
             out["beta2_power"] = torch.tensor(self.beta2_power, dtype=torch.float32)
         if self._ls_state is not None:
@@ -374,7 +394,7 @@ class GaccumTrainOp(_DeviceTrainOp):
                         raise KeyError(n + suffix)
         if self._ls_state is not None:
             self._load_loss_scale_state(sd)
-        elif self.hp.variant == ADAM and "beta1_power" in sd:
+        elif self.hp.variant in (ADAM, LAMB) and "beta1_power" in sd:
             self.beta1_power = float(sd["beta1_power"])
             self.beta2_power = float(sd["beta2_power"])
         if self.master is not None:
@@ -400,10 +420,12 @@ class PackedTrainOp(_DeviceTrainOp):
     def __init__(self, params: Sequence[torch.Tensor], names: Sequence[str], hp: HParams, accum_n: int,
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
-                 global_step: int = 0, loss_scale: Optional[LossScaleConfig] = None):
+                 global_step: int = 0, loss_scale: Optional[LossScaleConfig] = None,
+                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None):
         # autograd accumulates a 16-bit parameter's gradient in its own dtype: it cannot add into an fp32 slab
         _refuse_half(params, "PackedTrainOp")
-        super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale)
+        super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale,
+                         exclude_from_layer_adaptation)
         self.param_slab = self._zeros_slab()
         self.accum = self._zeros_slab()
         with torch.no_grad():
@@ -473,6 +495,8 @@ class HostTrainOp(_TrainOpCore):
                  global_step: int = 0, device: int = 0, loss_scale: Optional[LossScaleConfig] = None):
         if loss_scale is not None:   # host-resident models have no fp16 autocast: nothing to loss-scale
             raise ValueError("HostTrainOp does not support loss scaling")
+        if hp.variant == LAMB:
+            raise ValueError("HostTrainOp does not support LAMB; use GaccumTrainOp")
         _refuse_half(host_params, "HostTrainOp")
         self.world = 1
         for p in host_params:

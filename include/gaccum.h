@@ -49,6 +49,29 @@ extern "C" {
 /* optimizer variants */
 #define GACCUM_ADAM_WEIGHT_DECAY 0 /* optimization.py:107-194 (BERT path; "variant A") */
 #define GACCUM_ADAM 1              /* tf.train.AdamOptimizer, TF1 ApplyAdam (02:41,61; 04:42,62) */
+#define GACCUM_LAMB 2              /* LAMB (You et al. 2019, "Large Batch Optimization for Deep Learning"), see below */
+
+/* GACCUM_LAMB, in the form of TF-Addons' LAMB with the fp32 op order of GACCUM_ADAM_WEIGHT_DECAY (one correctly rounded
+ * op per TF op, no FMA contraction).  It uses the same hyper-parameters as AdamWeightDecay.  The apply step's prelude is
+ * unchanged: c = (1.0 * a') / N, times 1/S under loss scaling, times the clip scale.  Then, per tensor:
+ *     m  = b1*m + omb1*c            v  = b2*v + omb2*(c*c)      omb = fp32(1.0 - beta) from double, as variant A
+ *     mh = m / (1 - beta1_power)    vh = v / (1 - beta2_power)  fp32 ops
+ *     u  = mh / (sqrt(vh) + eps)
+ *     if decay[i]:  u = u + wd*p
+ *     r  = 1
+ *     if adapt[i]:  wn = ||p||, un = ||u||   (p before the update; ||x|| = sqrtf(fp32(sum x^2)))
+ *                   r  = (wn > 0 && un > 0) ? wn / un : 1
+ *     p  = p - (r*lr)*u              the scalar product first, as `ratio * lr * update` evaluates
+ * The beta powers are TF1 Adam's running fp32 products (beta_power *= beta after every APPLIED window, starting at
+ * fp32(beta)), not pow(beta, t): gaccum_step_args.beta{1,2}_power, or under loss scaling the device block's, which the
+ * apply advances on windows it does not skip.  decay[] is gaccum_plan_create's mask; adapt[] is set with
+ * gaccum_plan_set_layer_adaptation (default: every tensor adapts).  The sums of squares are exact (fixed-point
+ * accumulation of fp64 partials, independent of the work split) and rounded to fp32 once, so r is deterministic from run
+ * to run; it can differ in the last bit from a plain fp64 sum.  Everything else -- the pre-increment predicate, the
+ * first-accumulate precondition, tensors without a gradient, stats, the loss-scaling skip (a = +0 only; p, m, v, the
+ * master weights, the model copy and the beta powers unchanged bit for bit) -- is as for AdamWeightDecay.
+ * gaccum_step_dp, gaccum_apply_dp, gaccum_host_session_create and gaccum_step_host refuse a LAMB plan with
+ * GACCUM_EINVAL. */
 
 /* element types of the model's weights and gradients (gaccum_plan_set_param_dtype) */
 #define GACCUM_DTYPE_F32 0  /* the default: no call needed */
@@ -62,7 +85,7 @@ typedef void* gaccum_stream_t; /* a cudaStream_t */
  * floats and converts to fp32 at specific points (e.g. `1.0 - self.beta_1` is evaluated in
  * double first, optimization.py:152). */
 typedef struct gaccum_hparams {
-  int32_t variant;          /* GACCUM_ADAM_WEIGHT_DECAY | GACCUM_ADAM */
+  int32_t variant;          /* GACCUM_ADAM_WEIGHT_DECAY | GACCUM_ADAM | GACCUM_LAMB */
   int32_t reserved;         /* must be 0 */
   double beta1;             /* optimization.py:62  (0.9)  */
   double beta2;             /* optimization.py:63  (0.999) */
@@ -77,8 +100,8 @@ typedef struct gaccum_step_args {
   int32_t accum_n;     /* gradient_accumulation_multiplier, optimization.py:76 */
   int32_t reserved;    /* must be 0 */
   float lr;            /* learning rate of this micro-step (gaccum_learning_rate) */
-  float beta1_power;   /* GACCUM_ADAM only: TF1 Adam non-slot variable, beta1^t, t = #applies+1 */
-  float beta2_power;   /* GACCUM_ADAM only */
+  float beta1_power;   /* GACCUM_ADAM, GACCUM_LAMB: TF1 Adam non-slot variable, beta1^t, t = #applies+1 */
+  float beta2_power;   /* GACCUM_ADAM, GACCUM_LAMB */
   float reserved2;     /* must be 0 */
 } gaccum_step_args;
 
@@ -113,7 +136,7 @@ typedef struct gaccum_loss_scale_state {
   int32_t good_windows;     /* applied windows since S last changed */
   uint32_t skipped_windows; /* overflowed windows since gaccum_loss_scale_init */
   int32_t last_skipped;     /* 1 if the last apply step skipped its window, else 0 */
-  float beta1_power;        /* GACCUM_ADAM: TF1's beta1^t, used instead of gaccum_step_args.beta1_power and */
+  float beta1_power;        /* GACCUM_ADAM, GACCUM_LAMB: TF1's beta1^t, used instead of gaccum_step_args.beta1_power and */
   float beta2_power;        /*   advanced (one fp32 multiply each) on applied windows only */
   float reserved[2];
 } gaccum_loss_scale_state;
@@ -163,7 +186,8 @@ GACCUM_API int32_t gaccum_num_tiles(const gaccum_plan* plan);
  * a window of N >= 2 micro-steps moves (8 + 12 (N-2) + 36) B x P.  The plan does not know N: the
  * accumulate figure stays 12 B x P.  A 16-bit plan (gaccum_plan_set_param_dtype) reads 2-byte gradients:
  * accumulate = 10 B x P (first of a window 6 B x P); apply = 36 B x P (the 2 bytes saved on G are spent on
- * the model copy). */
+ * the model copy).  A GACCUM_LAMB apply moves 48 B x P (fp32 or 16-bit): those 36, plus p read a second time and the
+ * update u written and read back (the a' round trip of a clipped or loss-scaled apply is not counted, as above). */
 GACCUM_API int64_t gaccum_algorithmic_bytes(const gaccum_plan* plan, int32_t is_apply);
 
 /* Trains a bf16 or fp16 model (dtype GACCUM_DTYPE_BF16 / GACCUM_DTYPE_F16) with fp32 master weights.  Host-only:
@@ -188,6 +212,12 @@ GACCUM_API int gaccum_plan_set_param_dtype(gaccum_plan* plan, int32_t dtype, flo
  * gaccum_host_session_create and gaccum_step_host refuse a loss-scaled plan with GACCUM_EINVAL. */
 GACCUM_API int gaccum_plan_set_loss_scale(gaccum_plan* plan, const gaccum_loss_scale_config* cfg,
                                           gaccum_loss_scale_state* device_state);
+/* GACCUM_LAMB: which tensors get layer adaptation (adapt[i] != 0: the update is scaled by the trust ratio; 0: r = 1).
+ * Without a call every tensor adapts.  Allowed on LAMB plans only, and only before the first compute call on the plan,
+ * like gaccum_plan_set_loss_scale; adapt[] (num_tensors bytes, host memory) is copied, synchronously into the plan's
+ * device memory on a device plan. */
+GACCUM_API int gaccum_plan_set_layer_adaptation(gaccum_plan* plan, const uint8_t* adapt);
+
 /* Writes the initial state into `device_state` asynchronously on `stream`: scale = initial_scale, the three counters 0,
  * beta powers fp32(beta1) and fp32(beta2) (TF1's initial values).  The plan must have loss scaling on. */
 GACCUM_API int gaccum_loss_scale_init(gaccum_plan* plan, gaccum_loss_scale_state* device_state, gaccum_stream_t stream);
@@ -326,6 +356,10 @@ GACCUM_API int gaccum_host_session_slabs(gaccum_host_session* s, float** out);
 
 /* Asynchronously copy the stats block of the last step to host memory (pinned for true async). */
 GACCUM_API int gaccum_read_stats(gaccum_plan* plan, gaccum_stats* host_out, gaccum_stream_t stream);
+/* GACCUM_LAMB: asynchronously copy the trust ratios r of the last applied window (num_tensors floats; 1 for tensors
+ * without layer adaptation, and everywhere before the first applied window) to host memory, like gaccum_read_stats.  A
+ * window that loss scaling skips leaves them.  GACCUM_EINVAL on other variants, GACCUM_ENODEVICE on a layout-only plan. */
+GACCUM_API int gaccum_read_trust_ratios(gaccum_plan* plan, float* host_out, gaccum_stream_t stream);
 
 #ifdef __cplusplus
 }
