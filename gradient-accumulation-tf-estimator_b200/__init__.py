@@ -9,8 +9,8 @@ of the distributedExample scripts, as hand-written CUDA kernels behind a C ABI
 There is no CPU fallback anywhere in this package: importing works without a GPU (layout and
 scalar host logic are usable), every compute call raises ``GaccumError`` without one.
 """
-from ._lib import (ADAM, ADAM_WEIGHT_DECAY, LAMB, GaccumError, HParams, LossScaleConfig, Plan, StepArgs, decay_mask,
-                   device_count, is_apply_step, learning_rate, lib_path, version)
+from ._lib import (ADAM, ADAM_WEIGHT_DECAY, LAMB, EmaConfig, GaccumError, HParams, LossScaleConfig, Plan, StepArgs,
+                   decay_mask, device_count, is_apply_step, learning_rate, lib_path, version)
 
-__all__ = ["ADAM", "ADAM_WEIGHT_DECAY", "LAMB", "GaccumError", "HParams", "LossScaleConfig", "Plan", "StepArgs", "decay_mask",
-           "device_count", "is_apply_step", "learning_rate", "lib_path", "version"]
+__all__ = ["ADAM", "ADAM_WEIGHT_DECAY", "LAMB", "EmaConfig", "GaccumError", "HParams", "LossScaleConfig", "Plan", "StepArgs",
+           "decay_mask", "device_count", "is_apply_step", "learning_rate", "lib_path", "version"]

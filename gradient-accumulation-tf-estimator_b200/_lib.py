@@ -88,6 +88,16 @@ class LossScaleState(C.Structure):
                 ("reserved", C.c_float * 2)]
 
 
+class EmaConfig(C.Structure):
+    """gaccum_ema_config: an exponential moving average of the weights, updated by the apply step once per applied
+    window (TF1 ``ExponentialMovingAverage(decay, num_updates=...)``, ``zero_debias=False``).  ``num_updates=True``
+    turns on TF's warm-up ``d = min(decay, (1 + n) / (10 + n))``, n counting the windows averaged so far."""
+    _fields_ = [("decay", C.c_double), ("num_updates", C.c_int32), ("reserved", C.c_int32)]
+
+    def __init__(self, decay: float = 0.9999, num_updates: bool = False, reserved: int = 0):
+        super().__init__(float(decay), int(num_updates), int(reserved))
+
+
 _lib = None
 
 
@@ -151,6 +161,8 @@ def _load():
         "gaccum_plan_set_param_dtype": (C.c_int, [vp, i32, vp]),
         "gaccum_plan_set_layer_adaptation": (C.c_int, [vp, vp]),
         "gaccum_read_trust_ratios": (C.c_int, [vp, vp, vp]),
+        "gaccum_plan_set_ema": (C.c_int, [vp, C.POINTER(EmaConfig), vp, vp]),
+        "gaccum_ema_init": (C.c_int, [vp, vp, i64, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -319,6 +331,15 @@ class Plan:
     def read_trust_ratios(self, host_ptr: int, stream: int = 0) -> None:
         """LAMB: copy the last applied window's T trust ratios (fp32) to ``host_ptr``, asynchronously on ``stream``."""
         _check(_load().gaccum_read_trust_ratios(self._h, host_ptr or None, stream))
+
+    def set_ema(self, cfg: EmaConfig, ema_slab: int, device_state: int) -> None:
+        """Keep an exponential moving average of the weights (before the first compute call): ``ema_slab`` points to
+        ``padded_size`` floats of device memory in the plan's layout holding the initial averages, ``device_state`` to
+        16 bytes of device memory that ``ema_init`` fills."""
+        _check(_load().gaccum_plan_set_ema(self._h, C.byref(cfg), ema_slab or None, device_state or None))
+
+    def ema_init(self, device_state: int, num_updates: int = 0, stream: int = 0) -> None:
+        _check(_load().gaccum_ema_init(self._h, device_state or None, int(num_updates), stream))
 
     def close(self) -> None:
         if getattr(self, "_h", None):

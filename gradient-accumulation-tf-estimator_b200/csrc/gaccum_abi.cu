@@ -83,6 +83,12 @@ struct gaccum_plan {
   uint8_t* d_adapt = nullptr;
   LambTensorAcc* d_lamb_acc = nullptr;
   float* d_ratios = nullptr;
+  // exponential moving average of the weights (gaccum_plan_set_ema); set only while `computed` is false
+  bool ema_on = false;
+  gaccum_ema_config ema_cfg{};
+  float* ema_slab = nullptr;
+  gaccum_ema_state* ema_state = nullptr;
+  unsigned int* d_ema_done = nullptr;      // apply_kernel: CTAs of the launch that are through (zero between launches)
   std::mutex mu;
   std::map<const void*, int> grid_cache;   // kernel -> co-resident grid size
 };
@@ -178,19 +184,26 @@ static int launch_accumulate(gaccum_plan* pl, KernelParams<CAP>& prm, bool from_
   return GACCUM_OK;
 }
 
-template <int VARIANT, bool HAS_G, int CAP, bool H>
-static int launch_apply_noclip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream_t st) {
-  const int grid = std::max(1, prm.num_tiles);
-  apply_kernel<VARIANT, HAS_G, CAP, H><<<grid, kThreads, 0, st>>>(prm);
+// the KernelParams inside an apply kernel's parameter block
+template <int CAP>
+static KernelParams<CAP>& base_params(KernelParams<CAP>& p) { return p; }
+template <int CAP>
+static KernelParams<CAP>& base_params(EmaKernelParams<CAP>& p) { return p.k; }
+
+template <int VARIANT, bool HAS_G, int CAP, bool H, bool EMA>
+static int launch_apply_noclip(gaccum_plan* pl, ApplyParams<CAP, EMA>& ap, cudaStream_t st) {
+  const int grid = std::max(1, base_params(ap).num_tiles);
+  apply_kernel<VARIANT, HAS_G, CAP, H, EMA><<<grid, kThreads, 0, st>>>(ap);
   CUDA_TRY(cudaGetLastError());
   return GACCUM_OK;
 }
 
 // clip-apply: one cooperative launch, ONE 864-thread CTA per SM (ring + stash take nearly all of the SM's shared
 // memory, so a second CTA could never be co-resident -- the grid is clamped to the SM count)
-template <int VARIANT, bool HAS_G, int CAP, int LS, bool H>
-static int launch_apply_clip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream_t st) {
-  const void* fn = (const void*)&apply_clip_kernel<VARIANT, HAS_G, CAP, LS, H>;
+template <int VARIANT, bool HAS_G, int CAP, int LS, bool H, bool EMA>
+static int launch_apply_clip(gaccum_plan* pl, ApplyParams<CAP, EMA>& ap, cudaStream_t st) {
+  const void* fn = (const void*)&apply_clip_kernel<VARIANT, HAS_G, CAP, LS, H, EMA>;
+  KernelParams<CAP>& prm = base_params(ap);
   {
     std::lock_guard<std::mutex> lk(pl->mu);
     if (pl->grid_cache.find(fn) == pl->grid_cache.end()) {
@@ -205,34 +218,34 @@ static int launch_apply_clip(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream
   const int grid = std::max(1, std::min(pl->num_sms, ((int)pl->tiles.size() + kGroups - 1) / kGroups));
   prm.barrier = pl->d_barrier;
   prm.counters = pl->d_counters;
-  void* args[] = {(void*)&prm};
+  void* args[] = {(void*)&ap};
   CUDA_TRY(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kClipThreads), args, (size_t)kClipSmemBytes, st));
   return GACCUM_OK;
 }
 
 // Loss scaling always takes the two-pass kernel: the single-pass apply_kernel stores p, m and v before it could know
 // whether the window overflowed.
-template <int CAP, bool H>
-static int launch_apply_loss_scaled(gaccum_plan* pl, KernelParams<CAP>& prm, bool has_g, bool clip, cudaStream_t st) {
+template <int CAP, bool H, bool EMA>
+static int launch_apply_loss_scaled(gaccum_plan* pl, ApplyParams<CAP, EMA>& ap, bool has_g, bool clip, cudaStream_t st) {
   const int key = (pl->hp.variant == GACCUM_ADAM ? 4 : 0) | (clip ? 2 : 0) | (has_g ? 1 : 0);
   switch (key) {
-    case 0: return launch_apply_clip<0, false, CAP, kLsNoClip, H>(pl, prm, st);
-    case 1: return launch_apply_clip<0, true, CAP, kLsNoClip, H>(pl, prm, st);
-    case 2: return launch_apply_clip<0, false, CAP, kLsClip, H>(pl, prm, st);
-    case 3: return launch_apply_clip<0, true, CAP, kLsClip, H>(pl, prm, st);
-    case 4: return launch_apply_clip<1, false, CAP, kLsNoClip, H>(pl, prm, st);
-    case 5: return launch_apply_clip<1, true, CAP, kLsNoClip, H>(pl, prm, st);
-    case 6: return launch_apply_clip<1, false, CAP, kLsClip, H>(pl, prm, st);
-    default: return launch_apply_clip<1, true, CAP, kLsClip, H>(pl, prm, st);
+    case 0: return launch_apply_clip<0, false, CAP, kLsNoClip, H, EMA>(pl, ap, st);
+    case 1: return launch_apply_clip<0, true, CAP, kLsNoClip, H, EMA>(pl, ap, st);
+    case 2: return launch_apply_clip<0, false, CAP, kLsClip, H, EMA>(pl, ap, st);
+    case 3: return launch_apply_clip<0, true, CAP, kLsClip, H, EMA>(pl, ap, st);
+    case 4: return launch_apply_clip<1, false, CAP, kLsNoClip, H, EMA>(pl, ap, st);
+    case 5: return launch_apply_clip<1, true, CAP, kLsNoClip, H, EMA>(pl, ap, st);
+    case 6: return launch_apply_clip<1, false, CAP, kLsClip, H, EMA>(pl, ap, st);
+    default: return launch_apply_clip<1, true, CAP, kLsClip, H, EMA>(pl, ap, st);
   }
 }
 
 // GACCUM_LAMB: one cooperative launch of kLambBlocksPerSm CTAs per SM (gaccum_lamb.cuh).  The grid depends on the plan
 // only -- the barrier counter advances by gridDim.x per barrier -- so every instantiation must fit kLambBlocksPerSm
 // CTAs on an SM; one that does not is an error, never a smaller grid.
-template <bool HAS_G, int CAP, int MODE, bool H>
-static int launch_lamb_kernel(gaccum_plan* pl, LambKernelParams<CAP>& lp, cudaStream_t st) {
-  const void* fn = (const void*)&lamb_apply_kernel<HAS_G, CAP, MODE, H>;
+template <bool HAS_G, int CAP, int MODE, bool H, bool EMA>
+static int launch_lamb_kernel(gaccum_plan* pl, LambApplyParams<CAP, EMA>& lp, cudaStream_t st) {
+  const void* fn = (const void*)&lamb_apply_kernel<HAS_G, CAP, MODE, H, EMA>;
   {
     std::lock_guard<std::mutex> lk(pl->mu);
     if (pl->grid_cache.find(fn) == pl->grid_cache.end()) {
@@ -249,11 +262,13 @@ static int launch_lamb_kernel(gaccum_plan* pl, LambKernelParams<CAP>& lp, cudaSt
   return GACCUM_OK;
 }
 
-template <int CAP, bool H>
-static int launch_lamb(gaccum_plan* pl, const KernelParams<CAP>& prm, bool has_g, const gaccum_step_args* a, cudaStream_t st) {
-  LambKernelParams<CAP>* lp = new (std::nothrow) LambKernelParams<CAP>();
+template <int CAP, bool H, bool EMA>
+static int launch_lamb(gaccum_plan* pl, const KernelParams<CAP>& prm, const EmaParams& ema, bool has_g, const gaccum_step_args* a,
+                       cudaStream_t st) {
+  LambApplyParams<CAP, EMA>* lp = new (std::nothrow) LambApplyParams<CAP, EMA>();
   if (!lp) return fail(GACCUM_ENOMEM, "out of host memory");
   lp->k = prm;
+  if constexpr (EMA) lp->ema = ema;
   lp->k.barrier = pl->d_barrier;
   lp->k.counters = pl->d_counters;
   lp->lamb.acc = pl->d_lamb_acc;
@@ -266,35 +281,60 @@ static int launch_lamb(gaccum_plan* pl, const KernelParams<CAP>& prm, bool has_g
   const int mode = pl->ls_on ? (clip ? kLambLsClip : kLambLsNoClip) : (clip ? kLambClip : kLambNoClip);
   int rc;
   switch (mode * 2 + (has_g ? 1 : 0)) {
-    case 0: rc = launch_lamb_kernel<false, CAP, kLambNoClip, H>(pl, *lp, st); break;
-    case 1: rc = launch_lamb_kernel<true, CAP, kLambNoClip, H>(pl, *lp, st); break;
-    case 2: rc = launch_lamb_kernel<false, CAP, kLambClip, H>(pl, *lp, st); break;
-    case 3: rc = launch_lamb_kernel<true, CAP, kLambClip, H>(pl, *lp, st); break;
-    case 4: rc = launch_lamb_kernel<false, CAP, kLambLsClip, H>(pl, *lp, st); break;
-    case 5: rc = launch_lamb_kernel<true, CAP, kLambLsClip, H>(pl, *lp, st); break;
-    case 6: rc = launch_lamb_kernel<false, CAP, kLambLsNoClip, H>(pl, *lp, st); break;
-    default: rc = launch_lamb_kernel<true, CAP, kLambLsNoClip, H>(pl, *lp, st); break;
+    case 0: rc = launch_lamb_kernel<false, CAP, kLambNoClip, H, EMA>(pl, *lp, st); break;
+    case 1: rc = launch_lamb_kernel<true, CAP, kLambNoClip, H, EMA>(pl, *lp, st); break;
+    case 2: rc = launch_lamb_kernel<false, CAP, kLambClip, H, EMA>(pl, *lp, st); break;
+    case 3: rc = launch_lamb_kernel<true, CAP, kLambClip, H, EMA>(pl, *lp, st); break;
+    case 4: rc = launch_lamb_kernel<false, CAP, kLambLsClip, H, EMA>(pl, *lp, st); break;
+    case 5: rc = launch_lamb_kernel<true, CAP, kLambLsClip, H, EMA>(pl, *lp, st); break;
+    case 6: rc = launch_lamb_kernel<false, CAP, kLambLsNoClip, H, EMA>(pl, *lp, st); break;
+    default: rc = launch_lamb_kernel<true, CAP, kLambLsNoClip, H, EMA>(pl, *lp, st); break;
   }
   delete lp;
   return rc;
 }
 
-template <int CAP, bool H = false>
-static int launch_apply(gaccum_plan* pl, KernelParams<CAP>& prm, bool has_g, const gaccum_step_args* a, cudaStream_t st) {
-  if (pl->hp.variant == GACCUM_LAMB) return launch_lamb<CAP, H>(pl, prm, has_g, a, st);
+template <int CAP, bool H, bool EMA>
+static int launch_apply_params(gaccum_plan* pl, ApplyParams<CAP, EMA>& ap, bool has_g, cudaStream_t st) {
   const bool clip = pl->hp.clip_norm > 0.0;
-  if (pl->ls_on) return launch_apply_loss_scaled<CAP, H>(pl, prm, has_g, clip, st);
+  if (pl->ls_on) return launch_apply_loss_scaled<CAP, H, EMA>(pl, ap, has_g, clip, st);
   const int key = (pl->hp.variant == GACCUM_ADAM ? 4 : 0) | (clip ? 2 : 0) | (has_g ? 1 : 0);
   switch (key) {
-    case 0: return launch_apply_noclip<0, false, CAP, H>(pl, prm, st);
-    case 1: return launch_apply_noclip<0, true, CAP, H>(pl, prm, st);
-    case 2: return launch_apply_clip<0, false, CAP, kLsOff, H>(pl, prm, st);
-    case 3: return launch_apply_clip<0, true, CAP, kLsOff, H>(pl, prm, st);
-    case 4: return launch_apply_noclip<1, false, CAP, H>(pl, prm, st);
-    case 5: return launch_apply_noclip<1, true, CAP, H>(pl, prm, st);
-    case 6: return launch_apply_clip<1, false, CAP, kLsOff, H>(pl, prm, st);
-    default: return launch_apply_clip<1, true, CAP, kLsOff, H>(pl, prm, st);
+    case 0: return launch_apply_noclip<0, false, CAP, H, EMA>(pl, ap, st);
+    case 1: return launch_apply_noclip<0, true, CAP, H, EMA>(pl, ap, st);
+    case 2: return launch_apply_clip<0, false, CAP, kLsOff, H, EMA>(pl, ap, st);
+    case 3: return launch_apply_clip<0, true, CAP, kLsOff, H, EMA>(pl, ap, st);
+    case 4: return launch_apply_noclip<1, false, CAP, H, EMA>(pl, ap, st);
+    case 5: return launch_apply_noclip<1, true, CAP, H, EMA>(pl, ap, st);
+    case 6: return launch_apply_clip<1, false, CAP, kLsOff, H, EMA>(pl, ap, st);
+    default: return launch_apply_clip<1, true, CAP, kLsOff, H, EMA>(pl, ap, st);
   }
+}
+
+static EmaParams ema_params_of(const gaccum_plan* pl) {
+  EmaParams e{};
+  e.slab = pl->ema_slab;
+  e.state = reinterpret_cast<EmaState*>(pl->ema_state);
+  e.done = pl->d_ema_done;
+  e.decay = (float)pl->ema_cfg.decay;
+  e.num_updates = pl->ema_cfg.num_updates;
+  return e;
+}
+
+template <int CAP, bool H = false>
+static int launch_apply(gaccum_plan* pl, KernelParams<CAP>& prm, bool has_g, const gaccum_step_args* a, cudaStream_t st) {
+  if (!pl->ema_on) {
+    if (pl->hp.variant == GACCUM_LAMB) return launch_lamb<CAP, H, false>(pl, prm, EmaParams{}, has_g, a, st);
+    return launch_apply_params<CAP, H, false>(pl, prm, has_g, st);
+  }
+  if (pl->hp.variant == GACCUM_LAMB) return launch_lamb<CAP, H, true>(pl, prm, ema_params_of(pl), has_g, a, st);
+  EmaKernelParams<CAP>* ep = new (std::nothrow) EmaKernelParams<CAP>();
+  if (!ep) return fail(GACCUM_ENOMEM, "out of host memory");
+  ep->k = prm;
+  ep->ema = ema_params_of(pl);
+  const int rc = launch_apply_params<CAP, H, true>(pl, *ep, has_g, st);
+  delete ep;
+  return rc;
 }
 
 static inline bool aligned16_host(const void* p) { return ((uintptr_t)p & 15u) == 0; }
@@ -403,7 +443,7 @@ static int check_args(const gaccum_step_args* a) {
 
 static void free_plan_device(gaccum_plan* pl) {
   cudaFree(pl->d_tiles); cudaFree(pl->d_partials); cudaFree(pl->d_stats); cudaFree(pl->d_dp_sync); cudaFree(pl->d_barrier); cudaFree(pl->d_counters);
-  cudaFree(pl->d_adapt); cudaFree(pl->d_lamb_acc); cudaFree(pl->d_ratios);
+  cudaFree(pl->d_adapt); cudaFree(pl->d_lamb_acc); cudaFree(pl->d_ratios); cudaFree(pl->d_ema_done);
 #ifdef GACCUM_EXPERIMENTS
   cudaFree(pl->d_debug);
 #endif
@@ -527,6 +567,8 @@ int gaccum_plan_create(gaccum_plan** out, int32_t T, const int64_t* numels, cons
 #endif
     if (e == cudaSuccess) e = cudaMalloc(&pl->d_stats, sizeof(gaccum_stats));
     if (e == cudaSuccess) e = cudaMemset(pl->d_stats, 0, sizeof(gaccum_stats));
+    if (e == cudaSuccess) e = cudaMalloc(&pl->d_ema_done, sizeof(unsigned int));
+    if (e == cudaSuccess) e = cudaMemset(pl->d_ema_done, 0, sizeof(unsigned int));
     if (hp->variant == GACCUM_LAMB) {
       const size_t nt = (size_t)std::max(1, T);
       const std::vector<float> ones(nt, 1.0f);
@@ -578,7 +620,8 @@ int64_t gaccum_algorithmic_bytes(const gaccum_plan* pl, int32_t is_apply) {
   // the 2-byte model copy (36 B x P).
   // GACCUM_LAMB apply: those 36 B, plus p read a second time (phase 3) and u written and read back: 48 B x P (a 16-bit
   // plan the same).  Phase 1's a' round trip is not counted, as the clip-apply's is not.
-  const int64_t apply_bytes = pl->hp.variant == GACCUM_LAMB ? 48 : 36;
+  // An EMA plan also reads and writes the average on every apply: + 8 B x P.
+  const int64_t apply_bytes = (pl->hp.variant == GACCUM_LAMB ? 48 : 36) + (pl->ema_on ? 8 : 0);
   if (pl->master) return pl->P * (is_apply ? apply_bytes : 10);
   return pl->P * (is_apply ? apply_bytes : 12);
 }
@@ -647,6 +690,41 @@ int gaccum_read_trust_ratios(gaccum_plan* pl, float* host_out, gaccum_stream_t s
   DeviceGuard guard(pl->device);
   CUDA_TRY(cudaMemcpyAsync(host_out, pl->d_ratios, sizeof(float) * (size_t)pl->T, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   return GACCUM_OK;
+}
+
+int gaccum_plan_set_ema(gaccum_plan* pl, const gaccum_ema_config* cfg, float* ema_slab, gaccum_ema_state* device_state) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (!cfg) return fail(GACCUM_EINVAL, "cfg is NULL");
+  if (!ema_slab || !aligned16_host(ema_slab)) return fail(GACCUM_EINVAL, "ema_slab must be a 16-byte aligned device pointer");
+  if (!device_state || !aligned16_host(device_state))
+    return fail(GACCUM_EINVAL, "device_state must be a 16-byte aligned device pointer");
+  if (pl->computed) return fail(GACCUM_EINVAL, "the moving average can only be set before the plan's first compute call");
+  if (!(cfg->decay >= 0.0 && cfg->decay <= 1.0)) return fail(GACCUM_EINVAL, "decay must be in [0, 1] (got %g)", cfg->decay);
+  if (cfg->num_updates != 0 && cfg->num_updates != 1) return fail(GACCUM_EINVAL, "num_updates must be 0 or 1 (got %d)", cfg->num_updates);
+  if (cfg->reserved != 0) return fail(GACCUM_EINVAL, "reserved fields must be 0");
+  static_assert(sizeof(gaccum_ema_state) == sizeof(EmaState), "header and kernel disagree");
+  pl->ema_cfg = *cfg;
+  pl->ema_slab = ema_slab;
+  pl->ema_state = device_state;
+  pl->ema_on = true;
+  return GACCUM_OK;
+}
+
+int gaccum_ema_init(gaccum_plan* pl, gaccum_ema_state* device_state, int64_t num_updates, gaccum_stream_t stream) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (!pl->ema_on) return fail(GACCUM_EINVAL, "this plan keeps no moving average (gaccum_plan_set_ema)");
+  if (device_state != pl->ema_state)
+    return fail(GACCUM_EINVAL, "device_state is not the state block given to gaccum_plan_set_ema, which the apply reads");
+  if (num_updates < 0) return fail(GACCUM_EINVAL, "num_updates must be >= 0 (got %lld)", (long long)num_updates);
+  if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): a CUDA device is required");
+  DeviceGuard guard(pl->device);
+  ema_init_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(reinterpret_cast<EmaState*>(device_state), (long long)num_updates);
+  CUDA_TRY(cudaGetLastError());
+  return GACCUM_OK;
+}
+
+static int refuse_ema(const gaccum_plan* pl, const char* what) {
+  return pl && pl->ema_on ? fail(GACCUM_EINVAL, "%s does not support a moving average (gaccum_plan_set_ema)", what) : GACCUM_OK;
 }
 
 static int refuse_half(const gaccum_plan* pl, const char* what) {
@@ -825,6 +903,7 @@ int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* co
   if (pl && pl->ls_on) return fail(GACCUM_EINVAL, "the fused data-parallel apply does not support loss scaling");
   if (int rc = refuse_lamb(pl, "the fused data-parallel apply")) return rc;
   if (int rc = refuse_half(pl, "the fused data-parallel apply")) return rc;
+  if (int rc = refuse_ema(pl, "the fused data-parallel apply")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (comm->world < 2 || comm->world > GACCUM_MAX_RANKS || comm->rank < 0 || comm->rank >= comm->world)
     return fail(GACCUM_EINVAL, "world must be 2..%d and 0 <= rank < world", GACCUM_MAX_RANKS);
@@ -850,6 +929,7 @@ int gaccum_step_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* con
   if (pl && pl->ls_on) return fail(GACCUM_EINVAL, "the fused data-parallel step does not support loss scaling");
   if (int rc = refuse_lamb(pl, "the fused data-parallel step")) return rc;
   if (int rc = refuse_half(pl, "the fused data-parallel step")) return rc;
+  if (int rc = refuse_ema(pl, "the fused data-parallel step")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (int rc = check_args(a)) return rc;
   if (!grads) return fail(GACCUM_EINVAL, "grads is NULL");
@@ -932,6 +1012,7 @@ int gaccum_host_session_create(gaccum_host_session** out, gaccum_plan* pl) {
   if (pl->ls_on) return fail(GACCUM_EINVAL, "the host-buffer session does not support loss scaling");
   if (int rc = refuse_half(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_lamb(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse_ema(pl, "the host-buffer session")) return rc;
   if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): libgaccum has no CPU fallback, a CUDA device is required");
   DeviceGuard guard(pl->device);
   gaccum_host_session* s = new (std::nothrow) gaccum_host_session();
@@ -1042,6 +1123,7 @@ int gaccum_step_host(gaccum_host_session* s, const float* const* host_grads, flo
   if (pl->ls_on) return fail(GACCUM_EINVAL, "the host-buffer session does not support loss scaling");
   if (int rc = refuse_half(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_lamb(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse_ema(pl, "the host-buffer session")) return rc;
   DeviceGuard guard(pl->device);
   const int b = (int)(s->calls & 1);
   ++s->calls;

@@ -22,6 +22,9 @@
 // launch-uniform flag, prm.half.bf16), the fp32 master weights are a slab in the plan's layout.  G is widened exactly
 // on load, so every fp32 operation is the one the fp32 kernels perform on the upcast gradient; the apply stores the
 // master weights and, rounded to nearest-even, the model copy.  accumulate 10 B/elem (first of a window 6), apply 36.
+//
+// Exponential moving average of the weights (template flag EMA, gaccum_plan_set_ema): every apply kernel also reads the
+// average e and stores e - (e - p) * c after p, on applied windows only (+8 B/elem); see EmaParams.
 #pragma once
 
 #include <cooperative_groups.h>
@@ -29,6 +32,8 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 namespace gaccum {
 namespace cg = cooperative_groups;
@@ -121,6 +126,74 @@ struct KernelParams {
   LossScaleParams ls;   // apply_clip_kernel with LS != kLsOff only
   HalfParams half;      // kernels with H = true only
 };
+
+// gaccum_ema_state (gaccum.h): caller-owned device memory, written by gaccum_ema_init and afterwards only by the apply
+// launches of an EMA plan
+struct EmaState {
+  long long num_updates;   // n: windows averaged so far
+  float decay;             // d of the last averaged window
+  float reserved;
+};
+static_assert(sizeof(EmaState) == 16, "gaccum_ema_state is 16 bytes");
+
+// The exponential moving average of the weights (gaccum_plan_set_ema).  The apply kernels of an EMA plan take
+// EmaKernelParams: KernelParams as every other kernel sees it, then these, so no existing parameter block moves.
+struct EmaParams {
+  float* slab;             // the averages, a slab in the plan's layout (16-byte aligned)
+  EmaState* state;
+  unsigned int* done;      // apply_kernel: CTAs of the launch that are through (0 between launches)
+  float decay;             // fp32(decay)
+  int32_t num_updates;     // 1: d = min(decay, (1 + n) / (10 + n))
+};
+template <int CAP>
+struct EmaKernelParams {
+  KernelParams<CAP> k;
+  EmaParams ema;
+};
+// the parameter block of an apply kernel with (EMA) or without an EMA
+template <int CAP, bool EMA>
+using ApplyParams = typename std::conditional<EMA, EmaKernelParams<CAP>, KernelParams<CAP>>::type;
+template <int CAP>
+__device__ __forceinline__ const KernelParams<CAP>& kparams(const KernelParams<CAP>& p) { return p; }
+template <int CAP>
+__device__ __forceinline__ const KernelParams<CAP>& kparams(const EmaKernelParams<CAP>& p) { return p.k; }
+template <int CAP>
+__device__ __forceinline__ const EmaParams* ema_params(const KernelParams<CAP>&) { return nullptr; }
+template <int CAP>
+__device__ __forceinline__ const EmaParams* ema_params(const EmaKernelParams<CAP>& p) { return &p.ema; }
+
+// What every CTA of an EMA launch derives from the state as the launch finds it (TF1 ExponentialMovingAverage, one
+// correctly rounded fp32 op per TF op): d = fp32(decay), in num_updates mode d = min(d, (1 + fp32(n)) / (10 + fp32(n)));
+// c = 1 - d (assign_moving_average's `1.0 - decay`)
+struct EmaLaunch {
+  long long n;
+  float d, c;
+};
+__device__ __forceinline__ void ema_load(const EmaParams& ep, EmaLaunch& el) {
+  const long long n = __ldcg(&ep.state->num_updates);
+  float d = ep.decay;
+  if (ep.num_updates) {
+    const float nf = (float)n;                                         // round to nearest, as TF's cast
+    const float w = __fdiv_rn(__fadd_rn(1.0f, nf), __fadd_rn(10.0f, nf));
+    d = w < d ? w : d;
+  }
+  el.n = n;
+  el.d = d;
+  el.c = __fsub_rn(1.0f, d);
+}
+// one averaged window: n + 1 windows averaged, the last with decay d
+__device__ __forceinline__ void ema_finish(const EmaParams& ep, const EmaLaunch& el) {
+  EmaState s;
+  s.num_updates = el.n + 1;
+  s.decay = el.d;
+  s.reserved = 0.f;
+  *ep.state = s;
+}
+// e = e - (e - p) * c: assign_sub of the update delta; p is the value the apply just stored
+__device__ __forceinline__ float ema_elem(float e, float p, float c) { return __fsub_rn(e, __fmul_rn(__fsub_rn(e, p), c)); }
+__device__ __forceinline__ float4 ema_vec(const float4 e, const float4 p, float c) {
+  return make_float4(ema_elem(e.x, p.x, c), ema_elem(e.y, p.y, c), ema_elem(e.z, p.z, c), ema_elem(e.w, p.w, c));
+}
 
 // ---------------------------------------------------------------------------------------------
 // memory helpers: G is read exactly once -> streaming (evict-first) loads; zeroing the
@@ -415,12 +488,21 @@ __global__ void loss_scale_init_kernel(LossScaleState* st, float scale, float b1
   *st = s;
 }
 
+// gaccum_ema_init: n and d = 0, by one thread (asynchronous and graph-capturable, as loss_scale_init_kernel)
+__global__ void ema_init_kernel(EmaState* st, long long num_updates) {
+  EmaState s{};
+  s.num_updates = num_updates;
+  *st = s;
+}
+
 // ---------------------------------------------------------------------------------------------
 // apply without clipping: one pass.  HAS_G = false applies the accumulators as they are.
 // ---------------------------------------------------------------------------------------------
 // H: p is the master slab (always 16-byte aligned); the model copy is stored after it.
-template <int VARIANT, bool LOAD_G, bool H, int CAP>
-__device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams<CAP>& prm) {
+// EMA: the average e (slab `ema`, always 16-byte aligned) is read with p and stored after it: e - (e - p) * c.
+template <int VARIANT, bool LOAD_G, bool H, int CAP, bool EMA = false>
+__device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams<CAP>& prm, float* ema = nullptr,
+                                            const float ema_c = 0.f) {
   Grad<H> g;
   if constexpr (LOAD_G) g = Grad<H>(prm, d);
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
@@ -428,6 +510,7 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
   float* __restrict__ m = prm.m + soff;
   float* __restrict__ v = prm.v + soff;
   float* __restrict__ p = update_ptr<H>(prm, d);
+  float* __restrict__ e = EMA ? ema + soff : nullptr;
   uint16_t* q = nullptr;
   bool bf16 = false;
   if constexpr (H) { q = model_ptr(prm, d); bf16 = prm.half.bf16 != 0; }
@@ -437,12 +520,14 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
   float4* m4 = reinterpret_cast<float4*>(m);
   float4* v4 = reinterpret_cast<float4*>(v);
   float4* p4 = reinterpret_cast<float4*>(p);
-  float4 va[kUnroll], vg[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll];
+  float4* e4 = reinterpret_cast<float4*>(e);
+  float4 va[kUnroll], vg[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll], ve[kUnroll];
   // no gradient for this tile: a + 0 would turn -0 into +0 only; the add is skipped entirely (optimization.py:81)
   walk_tile(d.len, (H || aligned16(p)) && (g.g == nullptr || g.vec_ok()) ? d.len >> 2 : 0u, threadIdx.x,
             [&](int u, uint32_t i) {
               va[u] = __ldcs(a4 + i); vp[u] = __ldcs(p4 + i); vm[u] = __ldcs(m4 + i); vv[u] = __ldcs(v4 + i);
               if (LOAD_G && g.g) vg[u] = g.vec(i);
+              if constexpr (EMA) ve[u] = __ldcs(e4 + i);
             },
             [] {},
             [&](int u, uint32_t i) {
@@ -451,6 +536,7 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
               __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
               if constexpr (H) store_model4(q, i, vp[u], bf16);
+              if constexpr (EMA) __stcs(e4 + i, ema_vec(ve[u], vp[u], ema_c));
             },
             [&](uint32_t i) {
               float ax = a[i], px = p[i], mx = m[i], vx = v[i];
@@ -458,13 +544,32 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
               update_elem<VARIANT>(ax, false, 0.f, px, mx, vx, decay, sc);
               p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
               if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
+              if constexpr (EMA) e[i] = ema_elem(e[i], px, ema_c);
             });
 }
 
-template <int VARIANT, bool HAS_G, int CAP, bool H = false>
+// EMA: every CTA reads n (thread 0, before its tile); the CTA that finishes last -- a counter of finished CTAs, so
+// every other CTA of the launch has read n by then -- writes n + 1 and d, and resets the counter for the next launch.
+template <int VARIANT, bool HAS_G, int CAP, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads)
-apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
-  if ((int)blockIdx.x < prm.num_tiles) update_tile<VARIANT, HAS_G, H>(prm.tiles[blockIdx.x], prm);
+apply_kernel(const __grid_constant__ ApplyParams<CAP, EMA> ap) {
+  const KernelParams<CAP>& prm = kparams(ap);
+  if constexpr (!EMA) {
+    if ((int)blockIdx.x < prm.num_tiles) update_tile<VARIANT, HAS_G, H>(prm.tiles[blockIdx.x], prm);
+  } else {
+    const EmaParams& ep = *ema_params(ap);
+    __shared__ EmaLaunch s_ema;
+    if (threadIdx.x == 0) ema_load(ep, s_ema);
+    __syncthreads();
+    if ((int)blockIdx.x < prm.num_tiles) update_tile<VARIANT, HAS_G, H, CAP, true>(prm.tiles[blockIdx.x], prm, ep.slab, s_ema.c);
+    if (threadIdx.x == 0) {
+      __threadfence();
+      if (atomicAdd(ep.done, 1u) == gridDim.x - 1u) {
+        ema_finish(ep, s_ema);
+        *ep.done = 0u;
+      }
+    }
+  }
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f;
   }
@@ -524,6 +629,23 @@ constexpr uint32_t kNoStash = 0xffffffffu;
 constexpr int kStashVecs = kStashTiles * (kTile / 4);          // float4 per group
 constexpr int kClipSmemBytes = kRingBytes + kGroups * kStashVecs * 16;   // dynamic shared memory of the kernel (192 KB)
 static_assert(kClipSmemBytes + 20 * 1024 <= 227 * 1024, "ring + stash + static shared memory must fit one sm_90 block");
+// The same shared memory laid out for either kind of launch.  An EMA launch moves a fifth stream, e, into its pass-2
+// slot [p | m | v | a' | e] (40 KB): the ring grows to one such slot per group (pass 1 keeps its two 16 KB slots), and
+// the stash shrinks to the tiles that then fit -- 3 per group instead of 4 -- so that no consumer issues a bulk load.
+template <bool EMA>
+struct ClipLayout {
+  static constexpr int kP2SlotVecs = (EMA ? 5 : 4) * (kTile / 4);
+  static constexpr int kRingVecs = kP1Slots * kP1SlotVecs > kP2SlotVecs ? kP1Slots * kP1SlotVecs : kP2SlotVecs;
+  static constexpr int kP2Slots = kRingVecs / kP2SlotVecs;
+  static constexpr int kRingBytes = kGroups * kRingVecs * 16;
+  static constexpr int kStashTiles = (kClipSmemBytes - kRingBytes) / (kGroups * kTile * 4);
+  static constexpr int kStashVecs = kStashTiles * (kTile / 4);
+};
+static_assert(ClipLayout<false>::kRingVecs == kRingVecs && ClipLayout<false>::kP2Slots == kP2Slots &&
+              ClipLayout<false>::kStashTiles == kStashTiles, "the layout without an EMA is the one above");
+static_assert(ClipLayout<true>::kP2Slots >= 1 && ClipLayout<true>::kStashTiles >= 1 &&
+              ClipLayout<true>::kRingBytes + kGroups * ClipLayout<true>::kStashVecs * 16 <= kClipSmemBytes,
+              "the EMA layout fits the same dynamic shared memory");
 constexpr int kTicketBatch = 4;                   // pass-1 tickets a producer draws at once while plenty of tiles are left
 // what the producer tells the consumers about the tile it put into a slot
 struct __align__(16) SlotMeta {
@@ -767,15 +889,17 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
 // The caller has waited on the slot's `full` barrier (it had to, to learn which tile this is).
 // Loss-scaled: `sc` carries the alpha computed from the device's beta powers, and a skipped window (`skip`) stores
 // a = 0 and nothing else.  H: p is the master slab, and the model copy is stored after it (not on a skipped window).
-template <int VARIANT, int LS, bool H, int CAP>
+// EMA: the slot is [p | m | v | a' | e], and e - (e - p) * c is stored after p (not on a skipped window).
+template <int VARIANT, int LS, bool H, int CAP, bool EMA = false>
 __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelParams<CAP>& prm, const float s, const float4* slot,
                                              uint64_t* empty, const float4* const stash, const Scalars& sc, const float inv_s,
-                                             const bool skip) {
+                                             const bool skip, float* ema = nullptr, const float ema_c = 0.f) {
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
   float* __restrict__ m = prm.m + soff;
   float* __restrict__ v = prm.v + soff;
   float* __restrict__ p = update_ptr<H>(prm, d);
+  float* __restrict__ e = EMA ? ema + soff : nullptr;
   uint16_t* q = nullptr;
   bool bf16 = false;
   if constexpr (H) { q = model_ptr(prm, d); bf16 = prm.half.bf16 != 0; }
@@ -785,11 +909,13 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
   float4* m4 = reinterpret_cast<float4*>(m);
   float4* v4 = reinterpret_cast<float4*>(v);
   float4* p4 = reinterpret_cast<float4*>(p);
-  float4 va[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll];
+  float4* e4 = reinterpret_cast<float4*>(e);
+  float4 va[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll], ve[kUnroll];
   walk_tile(d.len, bulk_vecs2(d, p), threadIdx.x & (kThreads - 1),
             [&](int u, uint32_t i) {
               vp[u] = slot[i]; vm[u] = slot[kTile / 4 + i]; vv[u] = slot[2 * (kTile / 4) + i];
               va[u] = stash != nullptr ? stash[i] : slot[3 * (kTile / 4) + i];
+              if constexpr (EMA) ve[u] = slot[4 * (kTile / 4) + i];
             },
             [&] { __syncwarp(); if ((threadIdx.x & 31) == 0) mbar_arrive(empty); },
             [&](int u, uint32_t i) {
@@ -797,6 +923,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
                 update_vec2<VARIANT, LS>(va[u], s, inv_s, vp[u], vm[u], vv[u], decay, sc);
                 __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
                 if constexpr (H) store_model4(q, i, vp[u], bf16);
+                if constexpr (EMA) __stcs(e4 + i, ema_vec(ve[u], vp[u], ema_c));
               }
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
             },
@@ -806,6 +933,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
                 update_elem2<VARIANT, LS>(a[i], s, inv_s, px, mx, vx, decay, sc);
                 p[i] = px; m[i] = mx; v[i] = vx;
                 if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
+                if constexpr (EMA) e[i] = ema_elem(e[i], px, ema_c);
               }
               a[i] = 0.f;
             });
@@ -826,9 +954,23 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
 //
 // 16-bit models (H): pass 1 moves the 16-bit G tile into the G half of the [G | a] slot (bulk_vecs), pass 2 moves the
 // master weights, and every store of p is followed by the model copy.  Ring and stash are the same.
-template <int VARIANT, bool HAS_G, int CAP, int LS = kLsOff, bool H = false>
+//
+// EMA: ClipLayout<true> -- pass 2's producer moves e by bulk copy as the fifth stream of the slot.  Thread 0 of every
+// CTA reads n during set-up, before its CTA arrives at the grid barrier; block 0's thread 0 writes n + 1 and d at the
+// very end, on an applied window only, as it writes the loss-scaling state.
+template <int VARIANT, bool HAS_G, int CAP, int LS = kLsOff, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kClipThreads, 1)
-apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
+apply_clip_kernel(const __grid_constant__ ApplyParams<CAP, EMA> ap) {
+  using L = ClipLayout<EMA>;
+  constexpr int kRingVecs = L::kRingVecs, kP2SlotVecs = L::kP2SlotVecs, kP2Slots = L::kP2Slots, kRingBytes = L::kRingBytes;
+  constexpr int kStashTiles = L::kStashTiles, kStashVecs = L::kStashVecs;
+  const KernelParams<CAP>& prm = kparams(ap);
+  const EmaParams* const ema = ema_params(ap);
+  EmaLaunch* s_ema = nullptr;            // EMA: n, d and c as this launch found them
+  if constexpr (EMA) {
+    __shared__ EmaLaunch s_ema_launch;
+    s_ema = &s_ema_launch;
+  }
   extern __shared__ __align__(128) unsigned char smem_dyn[];
   __shared__ unsigned long long s_bins[kConsumerThreads / 32][kAccBins];   // one exact accumulator per consumer warp (13 KB)
   __shared__ unsigned int s_nonfinite;
@@ -890,6 +1032,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
                                __fsub_rn(1.0f, s_ls.beta1_power));
       }
     }
+    if constexpr (EMA) ema_load(*ema, *s_ema);
   }
   for (int i = threadIdx.x; i < (kConsumerThreads / 32) * kAccBins; i += kClipThreads) (&s_bins[0][0])[i] = 0ull;
   __syncthreads();
@@ -1037,11 +1180,13 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         if (nvec > 0) {
           const size_t soff = (size_t)d.soff32 * kSlabAlign;
           float4* dst = ring + (size_t)rp.slot * kP2SlotVecs;
-          mbar_arrive_expect_tx(full, nvec * 16u * (in_stash ? 3u : 4u));
+          if constexpr (EMA) mbar_arrive_expect_tx(full, nvec * 16u * (in_stash ? 4u : 5u));
+          else mbar_arrive_expect_tx(full, nvec * 16u * (in_stash ? 3u : 4u));
           bulk_g2s(dst, p, nvec * 16u, full, pol_first);
           bulk_g2s(dst + kTile / 4, prm.m + soff, nvec * 16u, full, pol_first);
           bulk_g2s(dst + 2 * (kTile / 4), prm.v + soff, nvec * 16u, full, pol_first);
           if (!in_stash) bulk_g2s(dst + 3 * (kTile / 4), prm.accum + soff, nvec * 16u, full, pol_first);
+          if constexpr (EMA) bulk_g2s(dst + 4 * (kTile / 4), ema->slab + soff, nvec * 16u, full, pol_first);
         } else {
           mbar_arrive(full);
         }
@@ -1143,14 +1288,20 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         const SlotMeta meta = s_meta2[grp][rp.slot];
         if (meta.d.len == 0) break;
         const float4* const st = meta.stash_slot != kNoStash ? stash + (size_t)meta.stash_slot * (kTile / 4) : nullptr;
-        update_tile2<VARIANT, LS, H>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st, sc, inv_s,
-                                  skip);
+        if constexpr (EMA) {
+          update_tile2<VARIANT, LS, H, CAP, true>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot],
+                                                  st, sc, inv_s, skip, ema->slab, s_ema->c);
+        } else {
+          update_tile2<VARIANT, LS, H>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st, sc, inv_s,
+                                    skip);
+        }
         rp.advance(kP2Slots);
       }
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) {
       prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s;
       if constexpr (LS != kLsOff) ls_finish<VARIANT == 1>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
+      if constexpr (EMA) { if (!skip) ema_finish(*ema, *s_ema); }
     }
   }
   __syncthreads();

@@ -58,6 +58,20 @@ struct LambKernelParams {
   LambParams lamb;
 };
 static_assert(sizeof(LambKernelParams<1920>) <= 32764, "kernel parameters must fit the 32 KB limit");
+// ... and with an EMA (gaccum_plan_set_ema), the EMA's after LAMB's
+template <int CAP>
+struct LambEmaKernelParams {
+  KernelParams<CAP> k;
+  LambParams lamb;
+  EmaParams ema;
+};
+static_assert(sizeof(LambEmaKernelParams<1920>) <= 32764, "kernel parameters must fit the 32 KB limit");
+template <int CAP, bool EMA>
+using LambApplyParams = typename std::conditional<EMA, LambEmaKernelParams<CAP>, LambKernelParams<CAP>>::type;
+template <int CAP>
+__device__ __forceinline__ const EmaParams* ema_params(const LambEmaKernelParams<CAP>& p) { return &p.ema; }
+template <int CAP>
+__device__ __forceinline__ const EmaParams* ema_params(const LambKernelParams<CAP>&) { return nullptr; }
 
 // what phase 2 needs besides Scalars: the clip scale, 1/S, and the bias corrections 1 - beta^t
 struct LambCoef {
@@ -159,19 +173,28 @@ __device__ __forceinline__ void lamb_update_tile(const TileDesc& d, const Kernel
 }
 
 // ---- phase 3: p = p - (r*lr)*u and a = +0 (a = +0 only on a skipped window) ----
-template <bool H, int CAP>
-__device__ __forceinline__ void lamb_write_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float rlr, const bool write) {
+// EMA: e is read with p and u, and e - (e - p) * c stored after p.
+template <bool H, int CAP, bool EMA = false>
+__device__ __forceinline__ void lamb_write_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float rlr, const bool write,
+                                                float* ema = nullptr, const float ema_c = 0.f) {
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
   float* __restrict__ p = update_ptr<H>(prm, d);
+  float* __restrict__ e = EMA ? ema + soff : nullptr;
   uint16_t* q = nullptr;
   bool bf16 = false;
   if constexpr (H) { q = model_ptr(prm, d); bf16 = prm.half.bf16 != 0; }
   float4* a4 = reinterpret_cast<float4*>(a);
   float4* p4 = reinterpret_cast<float4*>(p);
-  float4 vu[kUnroll], vp[kUnroll];
+  float4* e4 = reinterpret_cast<float4*>(e);
+  float4 vu[kUnroll], vp[kUnroll], ve[kUnroll];
   walk_tile(d.len, H || aligned16(p) ? d.len >> 2 : 0u, threadIdx.x,
-            [&](int u, uint32_t i) { if (write) { vu[u] = __ldcs(a4 + i); vp[u] = __ldcs(p4 + i); } },
+            [&](int u, uint32_t i) {
+              if (write) {
+                vu[u] = __ldcs(a4 + i); vp[u] = __ldcs(p4 + i);
+                if constexpr (EMA) ve[u] = __ldcs(e4 + i);
+              }
+            },
             [] {},
             [&](int u, uint32_t i) {
               if (write) {
@@ -181,6 +204,7 @@ __device__ __forceinline__ void lamb_write_tile(const TileDesc& d, const KernelP
                 vp[u].w = __fsub_rn(vp[u].w, __fmul_rn(rlr, vu[u].w));
                 __stcs(p4 + i, vp[u]);
                 if constexpr (H) store_model4(q, i, vp[u], bf16);
+                if constexpr (EMA) __stcs(e4 + i, ema_vec(ve[u], vp[u], ema_c));
               }
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
             },
@@ -189,6 +213,7 @@ __device__ __forceinline__ void lamb_write_tile(const TileDesc& d, const KernelP
                 const float px = __fsub_rn(p[i], __fmul_rn(rlr, a[i]));
                 p[i] = px;
                 if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
+                if constexpr (EMA) e[i] = ema_elem(e[i], px, ema_c);
               }
               a[i] = 0.f;
             });
@@ -201,15 +226,23 @@ __device__ __forceinline__ double warp_sum(double w) {
   return w;
 }
 
-template <bool HAS_G, int CAP, int MODE, bool H = false>
+// EMA: thread 0 of every CTA reads n during set-up; block 0's thread 0 writes n + 1 and d at the very end, past the
+// grid barriers, on an applied window only.
+template <bool HAS_G, int CAP, int MODE, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads, kLambBlocksPerSm)
-lamb_apply_kernel(const __grid_constant__ LambKernelParams<CAP> lp) {
+lamb_apply_kernel(const __grid_constant__ LambApplyParams<CAP, EMA> lp) {
   constexpr int LS = MODE == kLambLsClip ? kLsClip : MODE == kLambLsNoClip ? kLsNoClip : kLsOff;
   constexpr bool kPhase1 = MODE != kLambNoClip;
   constexpr unsigned long long kBarriers = kPhase1 ? 3 : 2;
   constexpr int kWarps = kThreads / 32;
   const KernelParams<CAP>& prm = lp.k;
   const LambParams& lb = lp.lamb;
+  const EmaParams* const ema = ema_params(lp);
+  EmaLaunch* s_ema = nullptr;            // EMA: n, d and c as this launch found them
+  if constexpr (EMA) {
+    __shared__ EmaLaunch s_ema_launch;
+    s_ema = &s_ema_launch;
+  }
   __shared__ unsigned long long s_bins[kWarps][2][kAccBins];   // one pair of exact accumulators per warp (8.5 KB)
   __shared__ unsigned int s_nonfinite[2];
   __shared__ LossScaleState s_ls;
@@ -231,6 +264,7 @@ lamb_apply_kernel(const __grid_constant__ LambKernelParams<CAP> lp) {
     s_bcast[1] = 0.f;
     s_skip = 0;
     if constexpr (LS != kLsOff) ls_load(prm.ls.state, s_ls);
+    if constexpr (EMA) ema_load(*ema, *s_ema);
   }
   for (int i = threadIdx.x; i < kWarps * 2 * kAccBins; i += kThreads) (&s_bins[0][0][0])[i] = 0ull;
   __syncthreads();
@@ -361,12 +395,14 @@ lamb_apply_kernel(const __grid_constant__ LambKernelParams<CAP> lp) {
   for (int t = t_lo; t < t_hi; ++t) {
     const TileDesc d = prm.tiles[t];
     const float rlr = skip ? 0.f : __fmul_rn(__ldcg(&lb.ratios[d.tensor_flags & 0x7fffffffu]), prm.sc.lr);   // ratio * lr first
-    lamb_write_tile<H>(d, prm, rlr, !skip);
+    if constexpr (EMA) lamb_write_tile<H, CAP, true>(d, prm, rlr, !skip, ema->slab, s_ema->c);
+    else lamb_write_tile<H>(d, prm, rlr, !skip);
   }
 
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s_bcast[0];
     if constexpr (LS != kLsOff) ls_finish<true>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
+    if constexpr (EMA) { if (!skip) ema_finish(*ema, *s_ema); }
   }
 }
 

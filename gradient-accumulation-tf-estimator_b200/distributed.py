@@ -89,9 +89,12 @@ class FusedDataParallelTrainOp:
 
     def __init__(self, params: Sequence[torch.Tensor], names: Sequence[str], hp, accum_n: int, lr_fn,
                  process_group=None, exclude_from_weight_decay=("LayerNorm", "layer_norm", "bias"),
-                 global_step: int = 0, loss_scale=None):
+                 global_step: int = 0, loss_scale=None, ema=None):
         import torch.distributed._symmetric_memory as symm
         from .train_op import GaccumTrainOp
+        if ema is not None:
+            raise ValueError("the fused data-parallel train op does not keep a moving average of the weights; "
+                             "use dp_mode='allreduce'")
         if loss_scale is not None:
             raise ValueError("the fused data-parallel train op does not support loss scaling; use dp_mode='allreduce'")
         if hp.variant == _lib.LAMB:

@@ -24,7 +24,7 @@ from typing import Callable, Iterable, List, Optional, Sequence, Tuple, Union
 import torch
 
 from . import _lib, graph
-from ._lib import ADAM, ADAM_WEIGHT_DECAY, LAMB, HParams, LossScaleConfig
+from ._lib import ADAM, ADAM_WEIGHT_DECAY, LAMB, EmaConfig, HParams, LossScaleConfig
 from .train_op import GaccumTrainOp
 
 # optimization.py:76 hard-codes 8 (README.md:17,34 says 4).  The signature has no argument for
@@ -36,6 +36,9 @@ loss_scale: Optional[LossScaleConfig] = None
 # The optimizer create_optimizer builds: "adam" (the reference's AdamWeightDecayOptimizer) or "lamb" (LAMBOptimizer with
 # the same hyper-parameters and exclusions, for large effective batches).
 optimizer_type = "adam"
+# The decay of an exponential moving average of the weights (ExponentialMovingAverage), off by default; create_optimizer
+# reads it.
+moving_average_decay: Optional[float] = None
 
 LossLike = Union[torch.Tensor, Callable[[], torch.Tensor]]
 LrLike = Union[float, Callable[[int], float]]
@@ -165,12 +168,46 @@ class AdamOptimizer(_OptimizerBase):
         return HParams(ADAM, 0, self.beta1, self.beta2, self.epsilon, 0.0, clip)
 
 
+class ExponentialMovingAverage:
+    """``tf.train.ExponentialMovingAverage(decay, num_updates=...)`` (``zero_debias=False``) for the train op: pass it as
+    ``gradient_accumulation_train_op(..., ema=)``.  The TF idiom ``with tf.control_dependencies([train_op]):
+    ema.apply(tvars)`` would average on every micro-step; here the apply step averages every trainable variable once per
+    applied window, on the device, after the update (the fp32 master weights of a bf16 / fp16 model).  With
+    ``num_updates=True`` the decay is TF's ``min(decay, (1 + n) / (10 + n))``, n counting the windows averaged so far."""
+
+    def __init__(self, decay: float, num_updates: bool = False, name: str = "ExponentialMovingAverage"):
+        self.decay, self.num_updates, self.name = float(decay), bool(num_updates), name
+        self._train_op: Optional["TrainOp"] = None
+
+    def config(self) -> EmaConfig:
+        return EmaConfig(self.decay, self.num_updates)
+
+    def average_name(self, var: graph.Variable) -> str:
+        return _lib._variable_name(var.name) + "/" + self.name
+
+    def average(self, var: graph.Variable) -> torch.Tensor:
+        """The moving average of ``var`` (a view of the train op's device slab)."""
+        if self._train_op is None:
+            raise ValueError("this ExponentialMovingAverage is not attached to a train op")
+        ids = [id(v) for v in self._train_op.tvars]
+        if id(var) not in ids:
+            raise KeyError(f"{var.name} is not averaged")
+        return self._train_op.engine.ema_view(ids.index(id(var)))
+
+    def variables_to_restore(self):
+        """{shadow-variable name: variable}: what a Saver restoring the averages into the variables maps (TF's
+        evaluation idiom); ``TrainOp.engine.averaged_weights()`` does the same swap in place."""
+        tv = self._train_op.tvars if self._train_op is not None else graph.trainable_variables()
+        return {self.average_name(v): v for v in tv}
+
+
 class TrainOp:
     """The object ``create_optimizer`` returns; ``run()`` == ``session.run(train_op)``."""
 
     def __init__(self, loss: LossLike, tvars: Sequence[graph.Variable], optimizer: _OptimizerBase,
                  accum_n: int, clip: Optional[float], global_step: graph.GlobalStep, process_group=None,
-                 dp_mode: str = "fused", loss_scale: Optional[LossScaleConfig] = None):
+                 dp_mode: str = "fused", loss_scale: Optional[LossScaleConfig] = None,
+                 ema: Optional[ExponentialMovingAverage] = None):
         self.loss = loss
         self.tvars = list(tvars)
         self.optimizer = optimizer
@@ -181,6 +218,8 @@ class TrainOp:
         exclude = getattr(optimizer, "exclude_from_weight_decay", None)
         adapt_kw = {"exclude_from_layer_adaptation": getattr(optimizer, "exclude_from_layer_adaptation", None)} \
             if hp.variant == LAMB else {}
+        self.ema = ema
+        ema_cfg = ema.config() if ema is not None else None
         self.dp = None
         if process_group is not None:
             # reference 04: MultiWorkerMirroredStrategy.  "fused": the exchange happens inside the apply
@@ -189,15 +228,17 @@ class TrainOp:
             pg = None if process_group is True else process_group
             if dp_mode == "fused":
                 self.dp = FusedDataParallelTrainOp(tensors, names, hp, accum_n, lr_fn, pg, exclude, int(global_step),
-                                                   loss_scale=loss_scale)
+                                                   loss_scale=loss_scale, ema=ema_cfg)
                 self.engine = self.dp.engine
             else:
                 self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step),
-                                            loss_scale=loss_scale, **adapt_kw)
+                                            loss_scale=loss_scale, ema=ema_cfg, **adapt_kw)
                 self.dp = DataParallelTrainOp(self.engine, pg)
         else:
             self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step),
-                                        loss_scale=loss_scale, **adapt_kw)
+                                        loss_scale=loss_scale, ema=ema_cfg, **adapt_kw)
+        if ema is not None:
+            ema._train_op = self
         self.last_loss: Optional[torch.Tensor] = None
 
     @property
@@ -239,16 +280,18 @@ class TrainOp:
 def gradient_accumulation_train_op(loss: LossLike, optimizer: _OptimizerBase, gradient_accumulation_multiplier: int,
                                    clip_norm: Optional[float] = None, global_step: Optional[graph.GlobalStep] = None,
                                    tvars: Optional[Sequence[graph.Variable]] = None, process_group=None,
-                                   dp_mode: str = "fused", loss_scale: Optional[LossScaleConfig] = None) -> TrainOp:
+                                   dp_mode: str = "fused", loss_scale: Optional[LossScaleConfig] = None,
+                                   ema: Optional[ExponentialMovingAverage] = None) -> TrainOp:
     """The recipe the example scripts inline (02:47-73, 04:48-74, another-example.py:126-155):
     N from ``params``, optimizer given, no clipping unless asked.  ``loss_scale`` turns on dynamic loss scaling for
-    fp16 mixed precision: gradients are taken of ``loss * S`` and a window that overflows is skipped on the device."""
+    fp16 mixed precision: gradients are taken of ``loss * S`` and a window that overflows is skipped on the device.
+    ``ema`` keeps an exponential moving average of the trainable variables, updated by the apply step."""
     gs = global_step or graph.get_or_create_global_step()
     tv = list(tvars) if tvars is not None else graph.trainable_variables()
     if not tv:
         raise ValueError("no trainable variables registered (graph.add_variable / graph.register_module)")
     return TrainOp(loss, tv, optimizer, int(gradient_accumulation_multiplier), clip_norm, gs, process_group, dp_mode,
-                   loss_scale)
+                   loss_scale, ema)
 
 
 def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
@@ -258,7 +301,8 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
     bias) :59-65; window ``gradient_accumulation_multiplier`` :76; apply branch (/N, clip 1.0,
     apply_gradients, zero) :80-88; ``tf.cond`` on the pre-increment step :91-94; step++ :102-103.
     With the module attribute ``optimizer_type = "lamb"`` the optimizer is a LAMBOptimizer with the same
-    hyper-parameters and exclusions (layer adaptation excludes what weight decay excludes).
+    hyper-parameters and exclusions (layer adaptation excludes what weight decay excludes).  With the module attribute
+    ``moving_average_decay`` set, the train op keeps an ExponentialMovingAverage of the variables (``train_op.ema``).
     """
     if use_tpu:
         # optimization.py:67-68 wraps the optimizer in tf.contrib.tpu.CrossShardOptimizer: TPU-only.
@@ -271,5 +315,6 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
         learning_rate=bert_learning_rate(init_lr, num_train_steps, num_warmup_steps),
         weight_decay_rate=0.01, beta_1=0.9, beta_2=0.999, epsilon=1e-6,
         exclude_from_weight_decay=["LayerNorm", "layer_norm", "bias"])
+    ema = ExponentialMovingAverage(moving_average_decay) if moving_average_decay is not None else None
     return gradient_accumulation_train_op(loss, optimizer, gradient_accumulation_multiplier,
-                                          clip_norm=clip_norm, global_step=global_step, loss_scale=loss_scale)
+                                          clip_norm=clip_norm, global_step=global_step, loss_scale=loss_scale, ema=ema)

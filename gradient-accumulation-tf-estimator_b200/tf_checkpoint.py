@@ -387,6 +387,9 @@ _SLOTS = {ADAM_WEIGHT_DECAY: ("/adam_m", "/adam_v"), ADAM: ("/Adam", "/Adam_1"),
 _BETA_POWERS = (ADAM, LAMB)      # variants that keep TF1's beta1_power / beta2_power
 
 
+_EMA, _EMA_STEP = "/ExponentialMovingAverage", "ExponentialMovingAverage/num_updates"
+
+
 def _accum_name(i: int) -> str:
     return "Variable" if i == 0 else f"Variable_{i}"             # unnamed tf.Variable, uniquified by the graph (optimization.py:78)
 
@@ -406,12 +409,19 @@ def to_reference_names(state: Dict[str, object], names: Sequence[str], variant: 
     if variant in _BETA_POWERS:
         out["beta1_power"] = arr(state["beta1_power"], np.float32)
         out["beta2_power"] = arr(state["beta2_power"], np.float32)
+    if _EMA_STEP in state:                                        # tf.train.ExponentialMovingAverage's shadow variables
+        for n in names:
+            out[n + _EMA] = arr(state[n + _EMA])
+        out[_EMA_STEP] = arr(state[_EMA_STEP], np.int64)
     return out
 
 
-def from_reference_names(tensors: Dict[str, np.ndarray], names: Sequence[str], variant: int, strict: bool = True) -> Dict[str, np.ndarray]:
+def from_reference_names(tensors: Dict[str, np.ndarray], names: Sequence[str], variant: int, strict: bool = True,
+                         ema: bool = False) -> Dict[str, np.ndarray]:
     """{reference Saver key: array} -> the dictionary train_op.load_state_dict() takes.  A checkpoint written before the
-    optimizer existed (a pre-trained BERT: parameters only) loads with strict=False: moments and accumulators stay zero."""
+    optimizer existed (a pre-trained BERT: parameters only) loads with strict=False: moments and accumulators stay zero.
+    The moving averages (``<var>/ExponentialMovingAverage``, ``ExponentialMovingAverage/num_updates``) are taken when
+    present, and required in strict mode when ``ema`` is True (a train op that keeps them)."""
     m_s, v_s = _SLOTS[variant]
     out: Dict[str, np.ndarray] = {"global_step": np.asarray(tensors.get("global_step", 0), dtype=np.int64)}
     for i, n in enumerate(names):
@@ -426,6 +436,11 @@ def from_reference_names(tensors: Dict[str, np.ndarray], names: Sequence[str], v
                 out[k] = tensors[k]
             elif strict:
                 raise KeyError(f"checkpoint has no tensor {k!r}")
+    for k in [n + _EMA for n in names] + [_EMA_STEP]:
+        if k in tensors:
+            out[k] = tensors[k]
+        elif strict and ema:
+            raise KeyError(f"checkpoint has no tensor {k!r}")
     return out
 
 
@@ -522,7 +537,7 @@ def restore(prefix_or_dir: str, train_op, names: Optional[Sequence[str]] = None,
         raise FileNotFoundError(f"no checkpoint state in {prefix_or_dir}")
     eng = _engine_of(train_op)
     names = list(names if names is not None else eng.names)
-    sd = from_reference_names(read_bundle(prefix), names, int(eng.hp.variant), strict)
+    sd = from_reference_names(read_bundle(prefix), names, int(eng.hp.variant), strict, getattr(eng, "ema", None) is not None)
     train_op.load_state_dict({k: torch.from_numpy(np.array(v, order="C")) for k, v in sd.items()}, strict)
     return prefix
 

@@ -10,13 +10,14 @@ in csrc/.
 """
 from __future__ import annotations
 
+import contextlib
 from typing import Callable, Dict, Optional, Sequence
 
 import numpy as np
 import torch
 
 from . import _lib
-from ._lib import ADAM, ADAM_WEIGHT_DECAY, LAMB, HParams, LossScaleConfig, Plan, StepArgs
+from ._lib import ADAM, ADAM_WEIGHT_DECAY, LAMB, EmaConfig, HParams, LossScaleConfig, Plan, StepArgs
 
 
 def _f32(x) -> float:
@@ -93,6 +94,8 @@ class _DeviceTrainOp(_TrainOpCore):
 
     def __init__(self, params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step,
                  loss_scale: Optional[LossScaleConfig] = None, exclude_from_layer_adaptation=None):
+        self.ema: Optional[torch.Tensor] = None          # the moving average of the weights, when one is kept
+        self._ema_state: Optional[torch.Tensor] = None
         if not params:
             raise ValueError("no trainable variables")
         self.device = params[0].device
@@ -109,6 +112,17 @@ class _DeviceTrainOp(_TrainOpCore):
             self.plan.set_loss_scale(loss_scale, self._ls_state.data_ptr())
             self.plan.loss_scale_init(self._ls_state.data_ptr(), self._stream())
             self.loss_scale = self._ls_state[0]
+
+    def _init_ema(self, cfg: EmaConfig, weights: Callable[[int], torch.Tensor]) -> None:
+        """Keep an exponential moving average of ``weights(i)`` (the fp32 weights the apply updates).  TF initialises
+        a shadow variable to its variable's value: the average starts at the weights, and n at 0."""
+        self.ema = self._zeros_slab()
+        with torch.no_grad():
+            for i in range(len(self.params)):
+                self.ema_view(i).copy_(weights(i))
+        self._ema_state = torch.zeros(2, dtype=torch.int64, device=self.device)    # gaccum_ema_state: 16 bytes
+        self.plan.set_ema(cfg, self.ema.data_ptr(), self._ema_state.data_ptr())
+        self.plan.ema_init(self._ema_state.data_ptr(), 0, self._stream())
 
     def _zeros_slab(self) -> torch.Tensor:
         return torch.zeros(max(self.plan.padded_size, 32), dtype=torch.float32, device=self.device)
@@ -129,6 +143,39 @@ class _DeviceTrainOp(_TrainOpCore):
 
     def v_view(self, i: int) -> torch.Tensor:
         return self._view(self.v, i)
+
+    def ema_view(self, i: int) -> torch.Tensor:
+        """The moving average of parameter i (fp32; of the master weights on a 16-bit model)."""
+        if self.ema is None:
+            raise ValueError("this train op keeps no moving average (ema=None)")
+        return self._view(self.ema, i)
+
+    def ema_state(self) -> Dict[str, float]:
+        """Synchronously read the moving average's state: num_updates (windows averaged so far) and decay (the d of
+        the last averaged window, 0 before the first)."""
+        if self._ema_state is None:
+            raise ValueError("this train op keeps no moving average (ema=None)")
+        words = self._ema_state.cpu()
+        return {"num_updates": int(words[0]), "decay": float(words.view(torch.float32)[2])}
+
+    @contextlib.contextmanager
+    def averaged_weights(self):
+        """Evaluate with the averaged weights: inside the block the parameters hold the moving averages (a 16-bit
+        model: rounded to nearest-even); on leaving it they are restored bit for bit (a 16-bit model: from the master
+        weights, as the apply leaves them).  Do not train inside the block."""
+        if self.ema is None:
+            raise ValueError("this train op keeps no moving average (ema=None)")
+        master = getattr(self, "master", None)
+        with torch.no_grad():
+            saved = [p.detach().clone() for p in self.params] if master is None else None
+            for i, p in enumerate(self.params):
+                p.copy_(self.ema_view(i))
+        try:
+            yield self
+        finally:
+            with torch.no_grad():
+                for i, p in enumerate(self.params):
+                    p.copy_(saved[i] if master is None else self._view(master, i))
 
     def stats(self) -> Dict[str, float]:
         """Synchronously read what the last step computed (applied, lr, global_norm, clip_scale)."""
@@ -196,7 +243,7 @@ class GaccumTrainOp(_DeviceTrainOp):
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, accum: Optional[torch.Tensor] = None,
                  loss_scale: Optional[LossScaleConfig] = None,
-                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None):
+                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None):
         dtypes = {p.dtype for p in params}
         if len(dtypes) > 1 and dtypes & set(_HALF_DTYPES):
             raise ValueError(f"parameters of mixed dtypes ({', '.join(sorted(str(d) for d in dtypes))}): "
@@ -217,6 +264,8 @@ class GaccumTrainOp(_DeviceTrainOp):
                 for i, p in enumerate(self.params):
                     self.master_view(i).copy_(p)
             self.plan.set_param_dtype(_HALF_DTYPES[self.param_dtype], self.master.data_ptr())
+        if ema is not None:
+            self._init_ema(ema, self._weights)
         if accum is not None:          # caller-provided slab (e.g. NVLink peer-mapped symmetric memory)
             if accum.numel() < self.m.numel() or accum.dtype != torch.float32 or accum.device != self.device:
                 raise ValueError("accum must be an fp32 tensor of at least plan.padded_size elements on the params' device")
@@ -357,6 +406,10 @@ class GaccumTrainOp(_DeviceTrainOp):
             raise ValueError("fp32 parameters have no master copy")
         return self._view(self.master, i)
 
+    def _weights(self, i: int) -> torch.Tensor:
+        """The fp32 weights the apply updates: parameter i, or its master weights on a 16-bit model."""
+        return self.params[i] if self.master is None else self.master_view(i)
+
     def _refresh_model(self) -> None:
         """The model's 16-bit tensors = the master weights rounded to nearest-even, as the apply leaves them."""
         with torch.no_grad():
@@ -379,6 +432,11 @@ class GaccumTrainOp(_DeviceTrainOp):
             out["beta2_power"] = torch.tensor(self.beta2_power, dtype=torch.float32)
         if self._ls_state is not None:
             self._loss_scale_state_dict(out)
+        if self.ema is not None:
+            # tf.train.ExponentialMovingAverage's shadow-variable names
+            for i, n in enumerate(self.names):
+                out[n + "/ExponentialMovingAverage"] = self.ema_view(i).clone()
+            out["ExponentialMovingAverage/num_updates"] = torch.tensor(self.ema_state()["num_updates"], dtype=torch.int64)
         return out
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True) -> None:
@@ -397,8 +455,36 @@ class GaccumTrainOp(_DeviceTrainOp):
         elif self.hp.variant in (ADAM, LAMB) and "beta1_power" in sd:
             self.beta1_power = float(sd["beta1_power"])
             self.beta2_power = float(sd["beta2_power"])
+        if self.ema is not None:
+            self._load_ema_state(sd, strict)
         if self.master is not None:
             self._refresh_model()
+
+    def _load_ema_state(self, sd: Dict[str, torch.Tensor], strict: bool) -> None:
+        """The averages and n from a checkpoint.  Non-strict, a checkpoint without them (a pre-trained model, or a run
+        without an EMA) starts the average afresh, as TF creates a shadow variable from its variable's restored value:
+        each tensor whose weights were loaded but whose average was not averages from the loaded fp32 weights (the
+        master weights of a 16-bit model), and without a stored n the count restarts at 0."""
+        for i, n in enumerate(self.names):
+            key = n + "/ExponentialMovingAverage"
+            if key in sd:
+                with torch.no_grad():
+                    self.ema_view(i).copy_(sd[key])
+            elif strict:
+                raise KeyError(key)
+            elif n in sd:
+                with torch.no_grad():
+                    self.ema_view(i).copy_(self._weights(i))
+        key = "ExponentialMovingAverage/num_updates"
+        if key in sd:
+            n = int(sd[key])
+            if n < 0:
+                raise ValueError(f"{key} must be >= 0, got {n}")
+        elif strict:
+            raise KeyError(key)
+        else:
+            n = 0
+        self.plan.ema_init(self._ema_state.data_ptr(), n, self._stream())
 
 
 class PackedTrainOp(_DeviceTrainOp):
@@ -421,7 +507,7 @@ class PackedTrainOp(_DeviceTrainOp):
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, loss_scale: Optional[LossScaleConfig] = None,
-                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None):
+                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None):
         # autograd accumulates a 16-bit parameter's gradient in its own dtype: it cannot add into an fp32 slab
         _refuse_half(params, "PackedTrainOp")
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale,
@@ -436,6 +522,8 @@ class PackedTrainOp(_DeviceTrainOp):
                 view.copy_(p)
                 p.data = view                          # the caller's tensors now alias the slab
                 p.grad = self.accum_view(i)            # autograd accumulates straight into accum_grads
+        if ema is not None:
+            self._init_ema(ema, lambda i: self._view(self.param_slab, i))
         self.launches = 0
 
     def step(self, stream: Optional[int] = None) -> bool:
@@ -492,7 +580,10 @@ class HostTrainOp(_TrainOpCore):
     def __init__(self, host_params: Sequence[torch.Tensor], names: Sequence[str], hp: HParams, accum_n: int,
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
-                 global_step: int = 0, device: int = 0, loss_scale: Optional[LossScaleConfig] = None):
+                 global_step: int = 0, device: int = 0, loss_scale: Optional[LossScaleConfig] = None,
+                 ema: Optional[EmaConfig] = None):
+        if ema is not None:
+            raise ValueError("HostTrainOp does not keep a moving average of the weights; use GaccumTrainOp")
         if loss_scale is not None:   # host-resident models have no fp16 autocast: nothing to loss-scale
             raise ValueError("HostTrainOp does not support loss scaling")
         if hp.variant == LAMB:

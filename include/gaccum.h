@@ -141,6 +141,34 @@ typedef struct gaccum_loss_scale_state {
   float reserved[2];
 } gaccum_loss_scale_state;
 
+/* An exponential moving average of the weights, kept by the apply step (TF1 tf.train.ExponentialMovingAverage with
+ * zero_debias=False, applied once per APPLIED window -- `with tf.control_dependencies([train_op]): ema.apply(tvars)`
+ * without its pull toward unchanged weights on every micro-step).  Every step is one correctly rounded fp32 op, no FMA:
+ *     d = fp32(decay)
+ *     num_updates mode:  nf = fp32(n);  d = min(d, (1 + nf) / (10 + nf))      (fp32 add, add, div, min)
+ *     c = 1 - d                                                                (fp32 subtract)
+ *     e = e - (e - p) * c                                                      (fp32 sub, mul, sub)
+ * p is the value the apply just stored: the parameter, or the fp32 master weight of a 16-bit plan.  Every tensor is
+ * averaged, tensors without a gradient in the window included; accumulate steps do not touch the average.  n is the
+ * number of windows averaged before this one: it lives in the device state and the apply advances it, so a captured
+ * graph replayed k times advances it k times.  A window that loss scaling skips leaves the average and the state
+ * unchanged bit for bit.  Nothing the training computes (p, m, v, accumulators, stats, trust ratios, the loss-scaling
+ * state, the model copy) depends on whether an average is kept.  The caller initialises the average, as TF initialises
+ * a shadow variable to its variable's value. */
+typedef struct gaccum_ema_config {
+  double decay;          /* in [0, 1] (TF: e.g. 0.9999) */
+  int32_t num_updates;   /* 0, or 1: TF's num_updates warm-up d = min(decay, (1 + n) / (10 + n)) */
+  int32_t reserved;      /* must be 0 */
+} gaccum_ema_config;
+
+/* The EMA state: 16 bytes of caller-owned DEVICE memory (16-byte aligned), written by gaccum_ema_init and afterwards only
+ * by the apply launches. */
+typedef struct gaccum_ema_state {
+  int64_t num_updates; /* n: windows averaged so far */
+  float decay;         /* d of the last averaged window (0 before the first) */
+  float reserved;
+} gaccum_ema_state;
+
 /* ---- library -------------------------------------------------------------------------- */
 GACCUM_API int gaccum_version(void);
 GACCUM_API const char* gaccum_last_error(void);
@@ -187,7 +215,9 @@ GACCUM_API int32_t gaccum_num_tiles(const gaccum_plan* plan);
  * accumulate figure stays 12 B x P.  A 16-bit plan (gaccum_plan_set_param_dtype) reads 2-byte gradients:
  * accumulate = 10 B x P (first of a window 6 B x P); apply = 36 B x P (the 2 bytes saved on G are spent on
  * the model copy).  A GACCUM_LAMB apply moves 48 B x P (fp32 or 16-bit): those 36, plus p read a second time and the
- * update u written and read back (the a' round trip of a clipped or loss-scaled apply is not counted, as above). */
+ * update u written and read back (the a' round trip of a clipped or loss-scaled apply is not counted, as above).
+ * A plan that keeps an EMA (gaccum_plan_set_ema) reads and writes the average on every apply: 8 B x P more (44, or
+ * 56 for GACCUM_LAMB). */
 GACCUM_API int64_t gaccum_algorithmic_bytes(const gaccum_plan* plan, int32_t is_apply);
 
 /* Trains a bf16 or fp16 model (dtype GACCUM_DTYPE_BF16 / GACCUM_DTYPE_F16) with fp32 master weights.  Host-only:
@@ -221,6 +251,20 @@ GACCUM_API int gaccum_plan_set_layer_adaptation(gaccum_plan* plan, const uint8_t
 /* Writes the initial state into `device_state` asynchronously on `stream`: scale = initial_scale, the three counters 0,
  * beta powers fp32(beta1) and fp32(beta2) (TF1's initial values).  The plan must have loss scaling on. */
 GACCUM_API int gaccum_loss_scale_init(gaccum_plan* plan, gaccum_loss_scale_state* device_state, gaccum_stream_t stream);
+
+/* Keeps an exponential moving average of the weights (see gaccum_ema_config).  Host-only: validates `cfg` and keeps
+ * `ema_slab` (a 16-byte aligned device slab of gaccum_padded_size() floats in the plan's layout, holding the initial
+ * averages) and `device_state` (16-byte aligned; not dereferenced here).  Allowed only before the first compute call on
+ * the plan, like gaccum_plan_set_loss_scale; combines with gaccum_plan_set_param_dtype, gaccum_plan_set_loss_scale and
+ * gaccum_plan_set_layer_adaptation in any order.  gaccum_step, gaccum_apply and gaccum_step_packed then update the
+ * average in their apply step; gaccum_step_dp, gaccum_apply_dp, gaccum_host_session_create and gaccum_step_host refuse
+ * such a plan with GACCUM_EINVAL. */
+GACCUM_API int gaccum_plan_set_ema(gaccum_plan* plan, const gaccum_ema_config* cfg, float* ema_slab,
+                                   gaccum_ema_state* device_state);
+/* Writes num_updates = `num_updates` (>= 0; e.g. from a checkpoint) and decay = 0 into `device_state` asynchronously on
+ * `stream`.  The plan must keep an EMA, and `device_state` must be the block given to gaccum_plan_set_ema (GACCUM_EINVAL
+ * otherwise: the apply reads that one). */
+GACCUM_API int gaccum_ema_init(gaccum_plan* plan, gaccum_ema_state* device_state, int64_t num_updates, gaccum_stream_t stream);
 
 /* ---- the hot path --------------------------------------------------------------------- */
 /* One micro-step of the train_op (optimization.py:91-94): if gaccum_is_apply_step() the apply
