@@ -533,7 +533,8 @@ class PackedTrainOp(_DeviceTrainOp):
         applied = _lib.is_apply_step(g, self.N)
         if applied:
             for p, o in zip(self.params, self.plan.offsets):     # a caller that dropped the views broke the contract
-                if p.grad is None or p.grad.data_ptr() != self.accum.data_ptr() + 4 * o:
+                # (a zero-element view reports data_ptr() 0 wherever it points: there is nothing it could alias)
+                if p.grad is None or (p.numel() > 0 and p.grad.data_ptr() != self.accum.data_ptr() + 4 * o):
                     raise RuntimeError("p.grad no longer aliases the packed accumulator (zero_grad(set_to_none=True)?)")
             lr = self.lr_fn(g)
             self.plan.step_packed(0, self.param_slab.data_ptr(), self.accum.data_ptr(), self.m.data_ptr(), self.v.data_ptr(),

@@ -1,0 +1,347 @@
+"""The apply kernels' instantiation space, the schedule constants the tests aim at, and a train op stepped in lock-step
+with its composed oracle.
+
+* ``matrix_cases()`` / ``instantiation(case)``: every dispatch key of ``gaccum_abi.cu`` (optimizer x mode x gradients or
+  not x layout and dtype x EMA) and the kernel template each one launches.  ``tests/test_kernel_inventory.py`` checks that
+  this mapping covers exactly the apply kernels in the built library; ``tests/test_gpu_apply_matrix.py`` runs every case.
+* ``Schedule``: the tile and CTA bookkeeping of the clip-apply and the LAMB kernels, for tests that place tiles on their
+  boundaries (``tests/test_gpu_schedule_edges.py``).
+* ``reference_op``: the expected values, composed from the existing oracles (``oracle_np.ReferenceTrainOp``,
+  ``LossScaledReferenceTrainOp``, ``LambReferenceTrainOp``); a 16-bit model is the fp32 oracle fed the upcast gradients.
+* ``LockStep``: one train op on the GPU and its oracle, stepped together and compared after every micro-step.
+
+Importable without torch (the inventory test runs without a GPU).  Test infrastructure only.
+"""
+from __future__ import annotations
+
+import itertools
+from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
+
+import numpy as np
+
+import oracle_np as onp
+from ema_oracle import Ema
+from lamb_oracle import LambReferenceTrainOp
+from loss_scale_oracle import LossScaledReferenceTrainOp
+
+F32 = np.float32
+
+# ---- the dispatch keys ------------------------------------------------------------------------------------------------
+VARIANTS = ("adamw", "adam", "lamb")
+MODES = ("noclip", "clip", "ls_noclip", "ls_clip")
+# layout -> (pointer-table capacity CAP, 16-bit model H, parameter dtype).  CAP 0 is gaccum_step_packed (fp32 only).
+LAYOUTS: Dict[str, Tuple[int, bool, str]] = {
+    "packed": (0, False, "fp32"),
+    "t256_fp32": (256, False, "fp32"), "t256_bf16": (256, True, "bf16"), "t256_fp16": (256, True, "fp16"),
+    "t1920_fp32": (1920, False, "fp32"), "t1920_bf16": (1920, True, "bf16"), "t1920_fp16": (1920, True, "fp16"),
+}
+
+# gaccum_kernels.cuh kLsOff / kLsClip / kLsNoClip and gaccum_lamb.cuh kLamb*: the mode template argument of each kernel
+CLIP_LS_ARG = {"clip": "kLsOff", "ls_clip": "kLsClip", "ls_noclip": "kLsNoClip"}
+LAMB_MODE_ARG = {"noclip": "kLambNoClip", "clip": "kLambClip", "ls_clip": "kLambLsClip", "ls_noclip": "kLambLsNoClip"}
+
+
+class Case(NamedTuple):
+    variant: str
+    mode: str
+    has_g: bool
+    layout: str
+    ema: bool
+
+    @property
+    def id(self) -> str:
+        return f"{self.variant}-{self.mode}-{'g' if self.has_g else 'nog'}-{self.layout}-{'ema' if self.ema else 'noema'}"
+
+
+def matrix_cases() -> List[Case]:
+    return [Case(*k) for k in itertools.product(VARIANTS, MODES, (True, False), LAYOUTS, (False, True))]
+
+
+def instantiation(case: Case, consts: Dict[str, int]) -> Tuple[str, Tuple[int, ...]]:
+    """The kernel template and its arguments that ``gaccum_abi.cu`` launches for ``case``; ``consts`` maps the
+    kernels' mode constants (kLs*, kLamb*) to their values."""
+    cap, h, _ = LAYOUTS[case.layout]
+    g, h, e = int(case.has_g), int(h), int(case.ema)
+    if case.variant == "lamb":
+        return "lamb_apply_kernel", (g, cap, consts[LAMB_MODE_ARG[case.mode]], h, e)
+    v = 0 if case.variant == "adamw" else 1
+    if case.mode == "noclip":
+        return "apply_kernel", (v, g, cap, h, e)
+    return "apply_clip_kernel", (v, g, cap, consts[CLIP_LS_ARG[case.mode]], h, e)
+
+
+# ---- the schedules ----------------------------------------------------------------------------------------------------
+class Schedule:
+    """The tile and CTA bookkeeping of the cooperative apply kernels on a GPU with ``sms`` SMs.
+    ``tests/test_kernel_inventory.py`` reads the four constants out of csrc/*.cuh and compares them with these."""
+    TILE = 2048                # gaccum_kernels.cuh kTile = kThreads * 4 * kUnroll: elements per tile
+    GROUPS = 3                 # gaccum_kernels.cuh kGroups: consumer groups per clip-apply CTA
+    STASH_TILES = {False: 4,   # gaccum_kernels.cuh kStashTiles: a group's own tiles whose a' stays in shared memory
+                   True: 3}    # ... ClipLayout<true>::kStashTiles: an EMA launch's larger pass-2 slot leaves room for 3
+    LAMB_BLOCKS_PER_SM = 3     # gaccum_lamb.cuh kLambBlocksPerSm
+
+    def __init__(self, sms: int):
+        self.sms = sms
+
+    def clip_groups(self, nt: int) -> int:
+        """G: the clip-apply's grid is min(sms, ceil(nt / 3)) CTAs of 3 groups (gaccum_abi.cu launch_apply_clip)."""
+        return self.GROUPS * max(1, min(self.sms, -(-nt // self.GROUPS)))
+
+    def pool_lo(self, nt: int, ema: bool) -> int:
+        """The first tile drawn from the ticket counters; group b's own tiles are b + j*G, j < kStashTiles."""
+        return min(nt, self.STASH_TILES[ema] * self.clip_groups(nt))
+
+    def lamb_ranges(self, nt: int) -> List[Tuple[int, int]]:
+        """LAMB CTA c owns tiles [nt*c/grid, nt*(c+1)/grid), grid = min(3*sms, nt) (gaccum_lamb.cuh)."""
+        grid = max(1, min(self.LAMB_BLOCKS_PER_SM * self.sms, nt))
+        return [(nt * c // grid, nt * (c + 1) // grid) for c in range(grid)]
+
+
+def num_tiles(numels: Sequence[int]) -> int:
+    return sum(-(-int(n) // Schedule.TILE) for n in numels)
+
+
+# ---- the composed oracle ----------------------------------------------------------------------------------------------
+CLIP = 0.5                     # clipping modes: small enough that every window's clip scale is < 1
+SCHED = dict(init_lr=1e-2, num_train_steps=40, num_warmup_steps=4)
+LS_CFG = (16.0, 2.0, 2)        # initial scale, multiplier, growth interval: S grows after the second applied window
+
+
+def oracle_hparams(variant: str, mode: str) -> onp.HParams:
+    clip = CLIP if mode in ("clip", "ls_clip") else 0.0
+    if variant == "lamb":
+        return onp.HParams(variant=2, clip_norm=clip)
+    if variant == "adam":
+        return onp.HParams(variant=onp.VARIANT_ADAM, epsilon=1e-8, weight_decay_rate=0.0, clip_norm=clip)
+    return onp.HParams(clip_norm=clip)
+
+
+def reference_op(variant: str, mode: str, params, names, N: int, adapt: Optional[Sequence[bool]] = None,
+                 ls_cfg=LS_CFG):
+    """The oracle of one dispatch key: ReferenceTrainOp, LossScaledReferenceTrainOp or LambReferenceTrainOp."""
+    hp = oracle_hparams(variant, mode)
+    params = [np.array(p, dtype=F32, copy=True) for p in params]
+    ls = mode.startswith("ls_")
+    lskw = dict(initial_scale=ls_cfg[0], multiplier=ls_cfg[1], growth_interval=ls_cfg[2]) if ls else {}
+    if variant == "lamb":
+        return LambReferenceTrainOp(params, names, hp, N, adapt=adapt, **lskw, **SCHED)
+    if ls:
+        return LossScaledReferenceTrainOp(params, names, hp, N, **lskw, **SCHED)
+    return onp.ReferenceTrainOp(params, names, hp, N, **SCHED)
+
+
+def rel_err(x, ref) -> float:
+    x = np.asarray(x, np.float64); ref = np.asarray(ref, np.float64)
+    if x.size == 0:
+        return 0.0
+    return float(np.max(np.abs(x - ref)) / max(float(np.max(np.abs(ref))), 1e-30))
+
+
+def _bits_equal(x: np.ndarray, y: np.ndarray) -> bool:
+    return x.shape == y.shape and np.array_equal(np.ascontiguousarray(x).view(np.uint32),
+                                                 np.ascontiguousarray(y, dtype=F32).view(np.uint32))
+
+
+# ---- one train op and its oracle in lock-step -------------------------------------------------------------------------
+class LockStep:
+    """A train op on cuda:0 and its composed oracle, stepped together.
+
+    ``layout`` is "packed" (PackedTrainOp; with ``has_g`` the apply gets a gradient slab through ``plan.step_packed``) or
+    "table" (GaccumTrainOp; without ``has_g`` every micro-step is ``accumulate_only`` and an apply step adds
+    ``apply_only(None)``).  ``views`` places tensor i (parameter and gradients) ``views[i]`` elements past an aligned
+    address; ``nograd`` lists tensors that never get a gradient; ``zero`` tensors start at 0.  ``adapt_exclude`` is
+    LAMB's layer-adaptation exclusion list (default: the weight-decay one).
+
+    After every micro-step ``check`` compares: accumulators bit for bit; p (the master weights of a 16-bit model), m
+    and v bit for bit while no window has clipped and the variant is not LAMB, else within 1e-5; the global norm and
+    clip scale within 3e-6; trust ratios within 1e-6; the average bit for bit against ``Ema`` fed the kernel's own
+    weights; the model copy bit for bit against the RNE rounding of the kernel's master weights; the loss-scaling block
+    and the beta powers exactly.
+    """
+
+    def __init__(self, man, variant: str, mode: str, layout: str = "table", dtype: str = "fp32", has_g: bool = True,
+                 ema: Optional[Tuple[float, bool]] = None, N: int = 3, seed: int = 0, views: Optional[Dict[int, int]] = None,
+                 nograd: Sequence[int] = (), zero: Sequence[int] = (), adapt_exclude: Optional[Sequence[str]] = None):
+        import torch
+        import gaccum_b200 as g
+        from gaccum_b200.train_op import GaccumTrainOp, PackedTrainOp
+        self.torch, self.g = torch, g
+        self.man, self.variant, self.mode, self.layout, self.has_g, self.N = man, variant, mode, layout, has_g, N
+        self.dtype = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16}[dtype]
+        self.views, self.nograd = dict(views or {}), set(nograd)
+        self.rng = np.random.default_rng(seed)
+        names = [n for n, _ in man]
+        params = []
+        for i, (_, s) in enumerate(man):
+            x = np.zeros(s, F32) if i in zero else self.rng.normal(0, 0.05, s).astype(F32)
+            params.append(torch.from_numpy(x).to(self.dtype))          # 16-bit: the model starts representable
+        hpo = oracle_hparams(variant, mode)
+        hp = g.HParams(hpo.variant, 0, hpo.beta1, hpo.beta2, hpo.epsilon, hpo.weight_decay_rate, hpo.clip_norm)
+        self.ls = mode.startswith("ls_")
+        lsc = g.LossScaleConfig(*LS_CFG) if self.ls else None
+        emac = g.EmaConfig(*ema) if ema is not None else None
+        lr_fn = lambda s: g.learning_rate(SCHED["init_lr"], SCHED["num_train_steps"], SCHED["num_warmup_steps"], s)
+        kw = dict(loss_scale=lsc, ema=emac, exclude_from_layer_adaptation=adapt_exclude)
+        if layout == "packed":
+            assert dtype == "fp32" and not self.views
+            self.op = PackedTrainOp([p.cuda() for p in params], names, hp, N, lr_fn, **kw)
+            self.gslab = torch.zeros_like(self.op.accum) if has_g else None
+        else:
+            self.op = GaccumTrainOp([self._device(i, p) for i, p in enumerate(params)], names, hp, N, lr_fn, **kw)
+        self.cap = 0 if layout == "packed" else (256 if len(man) <= 256 else 1920)
+        adapt = self.op.adapt if variant == "lamb" else None
+        self.ref = reference_op(variant, mode, [p.float().numpy() for p in params], names, N, adapt=adapt)
+        self.tracker = Ema(self._weights(), *ema) if ema is not None else None
+        self.clipped = False                 # some window so far had a clip scale other than 1
+
+    # -- inputs -----------------------------------------------------------------------------------------------------
+    def _device(self, i: int, t):
+        """Tensor i's parameter or gradient on the GPU, at its view offset."""
+        torch = self.torch
+        off = self.views.get(i)
+        if off is None:
+            return t.cuda()
+        buf = torch.zeros(t.numel() + off + 8, dtype=t.dtype, device="cuda")
+        v = buf[off:off + t.numel()].view(t.shape)
+        v.copy_(t)
+        return v
+
+    def grads(self, sigma: float = 0.1, inf_at: Optional[Tuple[int, int]] = None):
+        """This micro-step's gradients (fp32, unscaled), None for the tensors without one."""
+        out = [None if i in self.nograd else self.rng.normal(0, sigma, s).astype(F32) for i, (_, s) in enumerate(self.man)]
+        if inf_at is not None:
+            out[inf_at[0]].reshape(-1)[inf_at[1]] = np.inf
+        return out
+
+    # -- one micro-step ---------------------------------------------------------------------------------------------
+    def step(self, grads) -> bool:
+        torch, op = self.torch, self.op
+        S = F32(self.ref.scale) if self.ls else F32(1.0)
+        host, dev = [], []
+        for i, x in enumerate(grads):
+            if x is None:
+                host.append(None); dev.append(None)
+                continue
+            with np.errstate(over="ignore", invalid="ignore"):
+                t = torch.from_numpy(x * S).to(self.dtype)                 # gradients of loss * S, in the model's dtype
+            host.append(t.float().numpy())                                   # ... what the oracle sees: their upcast
+            dev.append(self._device(i, t))
+        info = self.ref.run(host)
+        g = op.global_step
+        applied = self.g.is_apply_step(g, self.N)
+        if self.layout == "packed":
+            if self.has_g:
+                self.gslab.zero_()
+                for i, t in enumerate(dev):
+                    if t is not None:
+                        op._view(self.gslab, i).copy_(t)
+                lr = op.lr_fn(g)
+                op.plan.step_packed(self.gslab.data_ptr(), op.param_slab.data_ptr(), op.accum.data_ptr(), op.m.data_ptr(),
+                                    op.v.data_ptr(), op._step_args(g, lr), -1, op._stream())
+                if applied:
+                    op._advance_beta_powers()
+                op.global_step = g + 1
+            else:
+                for p, t in zip(op.params, dev):
+                    if t is not None:
+                        p.grad.add_(t)
+                assert op.step() == applied
+        elif self.has_g:
+            assert op.run(dev) == applied
+        else:
+            op.accumulate_only(dev)
+            if applied:
+                op.apply_only(None)
+            op.global_step = g + 1
+        assert info.applied == applied
+        self.check(info)
+        return applied
+
+    def run(self, steps: int, inf_at: Optional[Tuple[int, int, int]] = None, sigma: float = 0.1) -> None:
+        """``steps`` micro-steps; ``inf_at = (step, tensor, element)`` puts one inf into that gradient."""
+        for s in range(steps):
+            self.step(self.grads(sigma, inf_at[1:] if inf_at is not None and inf_at[0] == s else None))
+
+    # -- what the kernel left ---------------------------------------------------------------------------------------
+    def _slab(self, slab) -> List[np.ndarray]:
+        host = slab.cpu().numpy()
+        return [host[o:o + int(np.prod(s))].reshape(s) for o, (_, s) in zip(self.op.plan.offsets, self.man)]
+
+    def _weights(self) -> List[np.ndarray]:
+        op = self.op
+        if getattr(op, "master", None) is not None:
+            return self._slab(op.master)
+        if self.layout == "packed":
+            return self._slab(op.param_slab)
+        flat = self.torch.cat([p.detach().reshape(-1).float() for p in op.params]).cpu().numpy()
+        out, o = [], 0
+        for _, s in self.man:
+            n = int(np.prod(s))
+            out.append(flat[o:o + n].reshape(s)); o += n
+        return out
+
+    def skipped(self) -> bool:
+        return bool(getattr(self.ref, "last_skipped", False))
+
+    def check(self, info) -> None:
+        torch, op, ref = self.torch, self.op, self.ref
+        torch.cuda.synchronize()
+        names = [n for n, _ in self.man]
+        for i, a in enumerate(self._slab(op.accum)):
+            assert _bits_equal(a, ref.accum[i]), f"accumulator of {names[i]}"
+        if info.applied and not self.skipped() and (self.mode in ("clip", "ls_clip")) and info.clip_scale != F32(1.0):
+            self.clipped = True
+        exact = self.variant != "lamb" and not self.clipped
+        weights = self._weights()
+        for what, got, exp in (("p", weights, ref.params), ("m", self._slab(op.m), ref.m), ("v", self._slab(op.v), ref.v)):
+            # not bit-exact: within 1e-5 of the model's largest |value|.  Per tensor that would be too tight for the
+            # oracle itself: its global norm adds the per-tensor sums in fp32 one by one (off by up to ~1e-6 with 300
+            # tensors; the kernel's sum is exact), and a 1-element tensor whose m nearly cancels magnifies that.
+            scale = max([float(np.max(np.abs(e))) for e in exp if e.size] + [1e-30])
+            for i in range(len(self.man)):
+                if exact:
+                    assert _bits_equal(got[i], exp[i]), f"{what} of {names[i]}"
+                elif got[i].size:
+                    err = float(np.max(np.abs(got[i].astype(np.float64) - exp[i])))
+                    assert err <= 1e-5 * scale, f"{what} of {names[i]}: {err / scale}"
+        if getattr(op, "master", None) is not None:
+            for i, p in enumerate(op.params):
+                assert torch.equal(p.view(torch.int16), op.master_view(i).to(self.dtype).view(torch.int16)), \
+                    f"model copy of {names[i]}"
+        if info.applied:
+            st = op.stats()
+            assert st["applied"] and F32(st["lr"]) == F32(info.lr)
+            if self.mode not in ("clip", "ls_clip"):
+                assert (st["global_norm"], st["clip_scale"]) == (0.0, 1.0)
+            else:
+                for k, e in (("global_norm", info.global_norm), ("clip_scale", info.clip_scale)):
+                    if np.isfinite(e):
+                        assert abs(st[k] - float(e)) <= 3e-6 * abs(float(e)), (k, st[k], e)
+                    else:
+                        assert not np.isfinite(st[k]), (k, st[k], e)
+            if self.variant == "lamb":
+                r = op.trust_ratios()
+                exp = np.array(ref.ratios, F32)
+                # within 1e-6; once a window has clipped, 2e-4: a 1-element tensor whose u nearly cancels turns the
+                # ~1e-6 difference of the two global norms (above) into up to ~1e-4 in r = |p| / |u|
+                rtol = 2e-4 if self.clipped else 1e-6
+                bad = np.abs(r.astype(np.float64) - exp) > rtol * np.abs(exp)
+                assert not bad.any(), [(names[i], r[i], exp[i]) for i in np.flatnonzero(bad)]
+        if self.ls:
+            s = op.loss_scale_state()
+            assert (F32(s["scale"]), s["good_windows"], s["skipped_windows"], s["last_skipped"]) == \
+                (ref.scale, ref.good_windows, ref.skipped_windows, ref.last_skipped)
+        if self.variant in ("adam", "lamb"):
+            if self.ls:
+                words = op._ls_state.cpu().numpy()
+                b1, b2 = words[4], words[5]
+            else:
+                b1, b2 = F32(op.beta1_power), F32(op.beta2_power)
+            assert (b1, b2) == (F32(ref.beta1_power), F32(ref.beta2_power))
+        if self.tracker is not None:
+            if info.applied and not self.skipped():
+                self.tracker.average(weights)
+            for i, e in enumerate(self._slab(op.ema)):
+                assert _bits_equal(e, self.tracker.avg[i]), f"average of {names[i]}"
+            es = op.ema_state()
+            assert es["num_updates"] == self.tracker.num_updates and F32(es["decay"]) == self.tracker.decay
