@@ -90,7 +90,7 @@ struct gaccum_plan {
   gaccum_ema_state* ema_state = nullptr;
   unsigned int* d_ema_done = nullptr;      // apply_kernel: CTAs of the launch that are through (zero between launches)
   std::mutex mu;
-  std::map<const void*, int> grid_cache;   // kernel -> co-resident grid size
+  std::map<const void*, int> grid_cache;   // cooperative kernel -> CTAs that fit on one SM (fit)
 };
 
 static int build_layout(gaccum_plan* pl) {
@@ -159,16 +159,24 @@ static Scalars make_scalars(const gaccum_hparams& hp, const gaccum_step_args* a)
 // ------------------------------------------------------------------------------------------
 // launch helpers
 // ------------------------------------------------------------------------------------------
-static int grid_for(gaccum_plan* pl, const void* fn, int* out) {
+// The CTAs of `threads` threads and `smem` bytes of dynamic shared memory that fit on one SM, found once per kernel
+// (which also sets the kernel's dynamic shared memory limit).  A cooperative kernel's grid must be co-resident, and the
+// grid of the clip-apply and LAMB kernels depends on the plan alone (their barrier counter advances by gridDim.x), so a
+// kernel that fits fewer than `need` CTAs per SM is an error, never a smaller grid.
+static int fit(gaccum_plan* pl, const void* fn, const char* name, int threads, int smem, int need, int* per_sm) {
   std::lock_guard<std::mutex> lk(pl->mu);
   auto it = pl->grid_cache.find(fn);
-  if (it != pl->grid_cache.end()) { *out = it->second; return GACCUM_OK; }
-  int per_sm = 0;
-  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kThreads, 0));
-  if (per_sm < 1) return fail(GACCUM_ECUDA, "kernel does not fit on an SM");
-  int g = std::min(per_sm * pl->num_sms, pl->max_grid);
-  pl->grid_cache[fn] = g;
-  *out = g;
+  if (it == pl->grid_cache.end()) {
+    if (smem > 0) CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    int n = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, threads, (size_t)smem));
+    if (n < need) {
+      return need == 1 ? fail(GACCUM_ECUDA, "%s does not fit on an SM (%d B dynamic shared memory)", name, smem)
+                       : fail(GACCUM_ECUDA, "%s fits %d CTAs per SM, it needs %d", name, n, need);
+    }
+    it = pl->grid_cache.emplace(fn, n).first;
+  }
+  *per_sm = it->second;
   return GACCUM_OK;
 }
 
@@ -184,157 +192,45 @@ static int launch_accumulate(gaccum_plan* pl, KernelParams<CAP>& prm, bool from_
   return GACCUM_OK;
 }
 
-// the KernelParams inside an apply kernel's parameter block
-template <int CAP>
-static KernelParams<CAP>& base_params(KernelParams<CAP>& p) { return p; }
-template <int CAP>
-static KernelParams<CAP>& base_params(EmaKernelParams<CAP>& p) { return p.k; }
-
-template <int VARIANT, bool HAS_G, int CAP, bool H, bool EMA>
-static int launch_apply_noclip(gaccum_plan* pl, ApplyParams<CAP, EMA>& ap, cudaStream_t st) {
-  const int grid = std::max(1, base_params(ap).num_tiles);
-  apply_kernel<VARIANT, HAS_G, CAP, H, EMA><<<grid, kThreads, 0, st>>>(ap);
-  CUDA_TRY(cudaGetLastError());
-  return GACCUM_OK;
-}
-
-// clip-apply: one cooperative launch, ONE 864-thread CTA per SM (ring + stash take nearly all of the SM's shared
-// memory, so a second CTA could never be co-resident -- the grid is clamped to the SM count)
-template <int VARIANT, bool HAS_G, int CAP, int LS, bool H, bool EMA>
-static int launch_apply_clip(gaccum_plan* pl, ApplyParams<CAP, EMA>& ap, cudaStream_t st) {
-  const void* fn = (const void*)&apply_clip_kernel<VARIANT, HAS_G, CAP, LS, H, EMA>;
-  KernelParams<CAP>& prm = base_params(ap);
-  {
-    std::lock_guard<std::mutex> lk(pl->mu);
-    if (pl->grid_cache.find(fn) == pl->grid_cache.end()) {
-      CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kClipSmemBytes));
-      int per_sm = 0;
-      CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kClipThreads, (size_t)kClipSmemBytes));
-      if (per_sm < 1) return fail(GACCUM_ECUDA, "apply_clip_kernel does not fit on an SM (%d B dynamic shared memory)", kClipSmemBytes);
-      pl->grid_cache[fn] = pl->num_sms;
-    }
-  }
-  // the grid must be the same for every launch on this plan: the consumers' barrier counter advances by gridDim.x
-  const int grid = std::max(1, std::min(pl->num_sms, ((int)pl->tiles.size() + kGroups - 1) / kGroups));
-  prm.barrier = pl->d_barrier;
-  prm.counters = pl->d_counters;
-  void* args[] = {(void*)&ap};
-  CUDA_TRY(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kClipThreads), args, (size_t)kClipSmemBytes, st));
-  return GACCUM_OK;
-}
-
-// Loss scaling always takes the two-pass kernel: the single-pass apply_kernel stores p, m and v before it could know
-// whether the window overflowed.
+// The apply step: the kernel of the plan's (variant, mode) and its launch shape.  Loss scaling always takes a
+// cooperative kernel: the single-pass apply_kernel stores p, m and v before it could know whether the window overflowed.
+//   apply_kernel       AdamWeightDecay / Adam in kNoClip: one tile per CTA
+//   apply_clip_kernel  AdamWeightDecay / Adam in every other mode: ONE 864-thread CTA per SM (ring + stash take nearly
+//                      all of the SM's shared memory, so a second CTA could never be co-resident), min(SMs, ceil(nt/3))
+//   lamb_apply_kernel  LAMB in every mode: kLambBlocksPerSm CTAs per SM, min(kLambBlocksPerSm x SMs, nt)
 template <int CAP, bool H, bool EMA>
-static int launch_apply_loss_scaled(gaccum_plan* pl, ApplyParams<CAP, EMA>& ap, bool has_g, bool clip, cudaStream_t st) {
-  const int key = (pl->hp.variant == GACCUM_ADAM ? 4 : 0) | (clip ? 2 : 0) | (has_g ? 1 : 0);
-  switch (key) {
-    case 0: return launch_apply_clip<0, false, CAP, kLsNoClip, H, EMA>(pl, ap, st);
-    case 1: return launch_apply_clip<0, true, CAP, kLsNoClip, H, EMA>(pl, ap, st);
-    case 2: return launch_apply_clip<0, false, CAP, kLsClip, H, EMA>(pl, ap, st);
-    case 3: return launch_apply_clip<0, true, CAP, kLsClip, H, EMA>(pl, ap, st);
-    case 4: return launch_apply_clip<1, false, CAP, kLsNoClip, H, EMA>(pl, ap, st);
-    case 5: return launch_apply_clip<1, true, CAP, kLsNoClip, H, EMA>(pl, ap, st);
-    case 6: return launch_apply_clip<1, false, CAP, kLsClip, H, EMA>(pl, ap, st);
-    default: return launch_apply_clip<1, true, CAP, kLsClip, H, EMA>(pl, ap, st);
-  }
-}
-
-// GACCUM_LAMB: one cooperative launch of kLambBlocksPerSm CTAs per SM (gaccum_lamb.cuh).  The grid depends on the plan
-// only -- the barrier counter advances by gridDim.x per barrier -- so every instantiation must fit kLambBlocksPerSm
-// CTAs on an SM; one that does not is an error, never a smaller grid.
-template <bool HAS_G, int CAP, int MODE, bool H, bool EMA>
-static int launch_lamb_kernel(gaccum_plan* pl, LambApplyParams<CAP, EMA>& lp, cudaStream_t st) {
-  const void* fn = (const void*)&lamb_apply_kernel<HAS_G, CAP, MODE, H, EMA>;
-  {
-    std::lock_guard<std::mutex> lk(pl->mu);
-    if (pl->grid_cache.find(fn) == pl->grid_cache.end()) {
-      int per_sm = 0;
-      CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kThreads, 0));
-      if (per_sm < kLambBlocksPerSm)
-        return fail(GACCUM_ECUDA, "lamb_apply_kernel fits %d CTAs per SM, it needs %d", per_sm, kLambBlocksPerSm);
-      pl->grid_cache[fn] = kLambBlocksPerSm;
-    }
-  }
-  const int grid = std::max(1, std::min(pl->num_sms * kLambBlocksPerSm, (int)pl->tiles.size()));
-  void* args[] = {(void*)&lp};
-  CUDA_TRY(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kThreads), args, 0, st));
-  return GACCUM_OK;
-}
-
-template <int CAP, bool H, bool EMA>
-static int launch_lamb(gaccum_plan* pl, const KernelParams<CAP>& prm, const EmaParams& ema, bool has_g, const gaccum_step_args* a,
-                       cudaStream_t st) {
-  LambApplyParams<CAP, EMA>* lp = new (std::nothrow) LambApplyParams<CAP, EMA>();
-  if (!lp) return fail(GACCUM_ENOMEM, "out of host memory");
-  lp->k = prm;
-  if constexpr (EMA) lp->ema = ema;
-  lp->k.barrier = pl->d_barrier;
-  lp->k.counters = pl->d_counters;
-  lp->lamb.acc = pl->d_lamb_acc;
-  lp->lamb.ratios = pl->d_ratios;
-  lp->lamb.adapt = pl->d_adapt;
-  lp->lamb.num_tensors = pl->T;
-  lp->lamb.beta1_power = a ? a->beta1_power : 0.0f;
-  lp->lamb.beta2_power = a ? a->beta2_power : 0.0f;
+static int launch_apply(gaccum_plan* pl, KernelParams<CAP>& prm, cudaStream_t st) {
   const bool clip = pl->hp.clip_norm > 0.0;
-  const int mode = pl->ls_on ? (clip ? kLambLsClip : kLambLsNoClip) : (clip ? kLambClip : kLambNoClip);
-  int rc;
-  switch (mode * 2 + (has_g ? 1 : 0)) {
-    case 0: rc = launch_lamb_kernel<false, CAP, kLambNoClip, H, EMA>(pl, *lp, st); break;
-    case 1: rc = launch_lamb_kernel<true, CAP, kLambNoClip, H, EMA>(pl, *lp, st); break;
-    case 2: rc = launch_lamb_kernel<false, CAP, kLambClip, H, EMA>(pl, *lp, st); break;
-    case 3: rc = launch_lamb_kernel<true, CAP, kLambClip, H, EMA>(pl, *lp, st); break;
-    case 4: rc = launch_lamb_kernel<false, CAP, kLambLsClip, H, EMA>(pl, *lp, st); break;
-    case 5: rc = launch_lamb_kernel<true, CAP, kLambLsClip, H, EMA>(pl, *lp, st); break;
-    case 6: rc = launch_lamb_kernel<false, CAP, kLambLsNoClip, H, EMA>(pl, *lp, st); break;
-    default: rc = launch_lamb_kernel<true, CAP, kLambLsNoClip, H, EMA>(pl, *lp, st); break;
+  const int mode = pl->ls_on ? (clip ? kLsClip : kLsNoClip) : (clip ? kClip : kNoClip);
+  const int nt = (int)pl->tiles.size();
+  const bool adam = pl->hp.variant == GACCUM_ADAM;
+  if (pl->hp.variant != GACCUM_LAMB && mode == kNoClip) {
+    if (adam) apply_kernel<1, CAP, H, EMA><<<std::max(1, nt), kThreads, 0, st>>>(prm);
+    else apply_kernel<0, CAP, H, EMA><<<std::max(1, nt), kThreads, 0, st>>>(prm);
+    CUDA_TRY(cudaGetLastError());
+    return GACCUM_OK;
   }
-  delete lp;
-  return rc;
-}
-
-template <int CAP, bool H, bool EMA>
-static int launch_apply_params(gaccum_plan* pl, ApplyParams<CAP, EMA>& ap, bool has_g, cudaStream_t st) {
-  const bool clip = pl->hp.clip_norm > 0.0;
-  if (pl->ls_on) return launch_apply_loss_scaled<CAP, H, EMA>(pl, ap, has_g, clip, st);
-  const int key = (pl->hp.variant == GACCUM_ADAM ? 4 : 0) | (clip ? 2 : 0) | (has_g ? 1 : 0);
-  switch (key) {
-    case 0: return launch_apply_noclip<0, false, CAP, H, EMA>(pl, ap, st);
-    case 1: return launch_apply_noclip<0, true, CAP, H, EMA>(pl, ap, st);
-    case 2: return launch_apply_clip<0, false, CAP, kLsOff, H, EMA>(pl, ap, st);
-    case 3: return launch_apply_clip<0, true, CAP, kLsOff, H, EMA>(pl, ap, st);
-    case 4: return launch_apply_noclip<1, false, CAP, H, EMA>(pl, ap, st);
-    case 5: return launch_apply_noclip<1, true, CAP, H, EMA>(pl, ap, st);
-    case 6: return launch_apply_clip<1, false, CAP, kLsOff, H, EMA>(pl, ap, st);
-    default: return launch_apply_clip<1, true, CAP, kLsOff, H, EMA>(pl, ap, st);
-  }
-}
-
-static EmaParams ema_params_of(const gaccum_plan* pl) {
-  EmaParams e{};
-  e.slab = pl->ema_slab;
-  e.state = reinterpret_cast<EmaState*>(pl->ema_state);
-  e.done = pl->d_ema_done;
-  e.decay = (float)pl->ema_cfg.decay;
-  e.num_updates = pl->ema_cfg.num_updates;
-  return e;
-}
-
-template <int CAP, bool H = false>
-static int launch_apply(gaccum_plan* pl, KernelParams<CAP>& prm, bool has_g, const gaccum_step_args* a, cudaStream_t st) {
-  if (!pl->ema_on) {
-    if (pl->hp.variant == GACCUM_LAMB) return launch_lamb<CAP, H, false>(pl, prm, EmaParams{}, has_g, a, st);
-    return launch_apply_params<CAP, H, false>(pl, prm, has_g, st);
-  }
-  if (pl->hp.variant == GACCUM_LAMB) return launch_lamb<CAP, H, true>(pl, prm, ema_params_of(pl), has_g, a, st);
-  EmaKernelParams<CAP>* ep = new (std::nothrow) EmaKernelParams<CAP>();
-  if (!ep) return fail(GACCUM_ENOMEM, "out of host memory");
-  ep->k = prm;
-  ep->ema = ema_params_of(pl);
-  const int rc = launch_apply_params<CAP, H, true>(pl, *ep, has_g, st);
-  delete ep;
-  return rc;
+  static_assert(kNoClip == 0 && kClip == 1 && kLsClip == 2 && kLsNoClip == 3, "the tables are indexed by mode");
+  static const void* const lamb[4] = {
+      (const void*)&lamb_apply_kernel<CAP, kNoClip, H, EMA>, (const void*)&lamb_apply_kernel<CAP, kClip, H, EMA>,
+      (const void*)&lamb_apply_kernel<CAP, kLsClip, H, EMA>, (const void*)&lamb_apply_kernel<CAP, kLsNoClip, H, EMA>};
+  static const void* const clip_apply[2][4] = {   // [VARIANT][mode]
+      {nullptr, (const void*)&apply_clip_kernel<0, CAP, kClip, H, EMA>, (const void*)&apply_clip_kernel<0, CAP, kLsClip, H, EMA>,
+       (const void*)&apply_clip_kernel<0, CAP, kLsNoClip, H, EMA>},
+      {nullptr, (const void*)&apply_clip_kernel<1, CAP, kClip, H, EMA>, (const void*)&apply_clip_kernel<1, CAP, kLsClip, H, EMA>,
+       (const void*)&apply_clip_kernel<1, CAP, kLsNoClip, H, EMA>}};
+  const bool is_lamb = pl->hp.variant == GACCUM_LAMB;
+  const void* fn = is_lamb ? lamb[mode] : clip_apply[adam ? 1 : 0][mode];
+  const int threads = is_lamb ? kThreads : kClipThreads;
+  const int smem = is_lamb ? 0 : kClipSmemBytes;
+  int per_sm = 0;
+  if (int rc = fit(pl, fn, is_lamb ? "lamb_apply_kernel" : "apply_clip_kernel", threads, smem, is_lamb ? kLambBlocksPerSm : 1, &per_sm))
+    return rc;
+  const int grid = is_lamb ? std::max(1, std::min(pl->num_sms * kLambBlocksPerSm, nt))
+                           : std::max(1, std::min(pl->num_sms, (nt + kGroups - 1) / kGroups));
+  void* args[] = {(void*)&prm};
+  CUDA_TRY(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(threads), args, (size_t)smem, st));
+  return GACCUM_OK;
 }
 
 static inline bool aligned16_host(const void* p) { return ((uintptr_t)p & 15u) == 0; }
@@ -352,17 +248,19 @@ static int check_compute(gaccum_plan* pl, const float* accum, const float* m, co
 
 template <int CAP>
 static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, float* m, float* v,
-                        const Scalars& sc) {
+                        const gaccum_step_args* a) {
   prm.tiles = pl->d_tiles;
   prm.num_tiles = (int32_t)pl->tiles.size();
   prm.accum = accum;
   prm.m = m;
   prm.v = v;
+  prm.barrier = pl->d_barrier;
+  prm.counters = pl->d_counters;
 #ifdef GACCUM_EXPERIMENTS
   prm.debug = pl->d_debug;
 #endif
   prm.stats = pl->d_stats;
-  prm.sc = sc;
+  prm.sc = make_scalars(pl->hp, a);
   if (pl->ls_on) {
     prm.ls.state = reinterpret_cast<LossScaleState*>(pl->ls_state);
     prm.ls.multiplier = (float)pl->ls_cfg.multiplier;
@@ -370,6 +268,17 @@ static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, f
   }
   prm.half.master = pl->master;
   prm.half.bf16 = pl->param_dtype == GACCUM_DTYPE_BF16;
+  prm.lamb.acc = pl->d_lamb_acc;
+  prm.lamb.ratios = pl->d_ratios;
+  prm.lamb.adapt = pl->d_adapt;
+  prm.lamb.num_tensors = pl->T;
+  prm.lamb.beta1_power = a ? a->beta1_power : 0.0f;
+  prm.lamb.beta2_power = a ? a->beta2_power : 0.0f;
+  prm.ema.slab = pl->ema_slab;
+  prm.ema.state = reinterpret_cast<EmaState*>(pl->ema_state);
+  prm.ema.done = pl->d_ema_done;
+  prm.ema.decay = (float)pl->ema_cfg.decay;
+  prm.ema.num_updates = pl->ema_cfg.num_updates;
 }
 
 template <int CAP>
@@ -409,7 +318,7 @@ static int do_accumulate_tab(gaccum_plan* pl, const float* const* grads, float* 
                              const gaccum_step_args* a, cudaStream_t st) {
   KernelParams<CAP>* prm = new (std::nothrow) KernelParams<CAP>();
   if (!prm) return fail(GACCUM_ENOMEM, "out of host memory");
-  fill_common(pl, *prm, accum, nullptr, nullptr, make_scalars(pl->hp, a));
+  fill_common(pl, *prm, accum, nullptr, nullptr, a);
   int rc = fill_table(pl, prm->tab, grads, nullptr);
   if (rc == GACCUM_OK) {
     rc = pl->master ? launch_accumulate<CAP, true>(pl, *prm, first_of_window(a), st)
@@ -424,11 +333,11 @@ static int do_apply_tab(gaccum_plan* pl, const float* const* grads, float* const
                         float* m, float* v, const gaccum_step_args* a, cudaStream_t st) {
   KernelParams<CAP>* prm = new (std::nothrow) KernelParams<CAP>();
   if (!prm) return fail(GACCUM_ENOMEM, "out of host memory");
-  fill_common(pl, *prm, accum, m, v, make_scalars(pl->hp, a));
+  fill_common(pl, *prm, accum, m, v, a);
   int rc = fill_table(pl, prm->tab, grads, params);
   if (rc == GACCUM_OK) {
-    rc = pl->master ? launch_apply<CAP, true>(pl, *prm, grads != nullptr, a, st)
-                    : launch_apply<CAP, false>(pl, *prm, grads != nullptr, a, st);
+    if (pl->master) rc = pl->ema_on ? launch_apply<CAP, true, true>(pl, *prm, st) : launch_apply<CAP, true, false>(pl, *prm, st);
+    else rc = pl->ema_on ? launch_apply<CAP, false, true>(pl, *prm, st) : launch_apply<CAP, false, false>(pl, *prm, st);
   }
   delete prm;
   return rc;
@@ -790,7 +699,7 @@ int gaccum_step_packed(gaccum_plan* pl, const float* grad_slab, float* param_sla
   DeviceGuard guard(pl->device);
   cudaStream_t st = (cudaStream_t)stream;
   KernelParams<0> prm{};
-  fill_common(pl, prm, accum, m, v, make_scalars(pl->hp, a));
+  fill_common(pl, prm, accum, m, v, a);
   prm.tab.g = grad_slab;
   prm.tab.p = param_slab;
   if (!apply) {
@@ -799,7 +708,7 @@ int gaccum_step_packed(gaccum_plan* pl, const float* grad_slab, float* param_sla
     return launch_accumulate(pl, prm, force_branch < 0 && first_of_window(a), st);
   }
   if (!param_slab || !aligned16_host(param_slab)) return fail(GACCUM_EINVAL, "param_slab must be a 16-byte aligned device pointer");
-  return launch_apply(pl, prm, grad_slab != nullptr, a, st);
+  return pl->ema_on ? launch_apply<0, false, true>(pl, prm, st) : launch_apply<0, false, false>(pl, prm, st);
 }
 
 // contiguous tile ranges with (nearly) equal element counts: boundary r = first tile whose cumulative
@@ -885,10 +794,10 @@ static int do_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float*
   prm->epoch = epoch;
   for (int32_t t = 0; t < pl->T; ++t) prm->tab.g[t] = grads ? grads[t] : nullptr;
   const void* fn = pl->hp.variant == GACCUM_ADAM ? (const void*)&dp_apply_kernel<1, CAP> : (const void*)&dp_apply_kernel<0, CAP>;
-  int grid = 0;
-  int rc = grid_for(pl, fn, &grid);
+  int per_sm = 0;
+  int rc = fit(pl, fn, "dp_apply_kernel", kThreads, 0, 1, &per_sm);
   if (rc == GACCUM_OK) {
-    grid = std::max(1, std::min(grid, prm->num_tiles));
+    const int grid = std::max(1, std::min({per_sm * pl->num_sms, pl->max_grid, prm->num_tiles}));
     void* args[] = {(void*)prm};
     cudaError_t e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kThreads), args, 0, st);
     if (e != cudaSuccess) rc = fail(GACCUM_ECUDA, "cudaLaunchCooperativeKernel(dp_apply_kernel) failed: %s", cudaGetErrorString(e));

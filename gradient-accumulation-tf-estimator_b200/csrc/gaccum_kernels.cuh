@@ -11,8 +11,8 @@
 //   apply_clip_kernel    the apply branch WITH tf.clip_by_global_norm                  (36 B/elem)
 //                        optimization.py:80-88, 128-177.  The global norm of ALL tensors is needed before
 //                        ANY element can be updated: one cooperative launch, two passes around a grid
-//                        barrier (described at the kernel).  Its loss-scaled instantiations (LS != kLsOff) also
-//                        unscale by 1/S and skip the whole window when a' or the norm is not finite; with
+//                        barrier (described at the kernel).  Its loss-scaled instantiations (kLsClip, kLsNoClip)
+//                        also unscale by 1/S and skip the whole window when a' or the norm is not finite; with
 //                        clipping off they run the same two passes with the norm and the clip multiply compiled out.
 // Arithmetic uses round-to-nearest intrinsics (__fmul_rn, __fadd_rn, __fdiv_rn, __fsqrt_rn) so nvcc
 // cannot contract mul+add into FMA: the reference graph is un-fused, one rounding per TF op, and we
@@ -32,8 +32,6 @@
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-
-#include <type_traits>
 
 namespace gaccum {
 namespace cg = cooperative_groups;
@@ -97,9 +95,12 @@ struct LossScaleParams {
   float multiplier;           // a power of two >= 2
   int32_t growth_interval;    // applied windows before S grows
 };
-constexpr int kLsOff = 0;       // no loss scaling
-constexpr int kLsClip = 1;      // loss scaling + tf.clip_by_global_norm
-constexpr int kLsNoClip = 2;    // loss scaling without clipping: pass 1 only looks for non-finite elements of a'
+// The mode of the cooperative apply kernels (MODE): apply_clip_kernel has every mode but kNoClip, lamb_apply_kernel all
+constexpr int kNoClip = 0;      // neither clipping nor loss scaling
+constexpr int kClip = 1;        // tf.clip_by_global_norm
+constexpr int kLsClip = 2;      // loss scaling + tf.clip_by_global_norm
+constexpr int kLsNoClip = 3;    // loss scaling without clipping: pass 1 only looks for non-finite elements of a'
+__host__ __device__ constexpr bool loss_scaled(int mode) { return mode == kLsClip || mode == kLsNoClip; }
 
 // A 16-bit model (gaccum_plan_set_param_dtype): the pointer table's g[] and p[] point at bf16 or fp16 tensors.  Kept
 // after LossScaleParams, so every member of the fp32 instantiations sits where it does without it.
@@ -108,6 +109,36 @@ struct HalfParams {
   int32_t bf16;       // 1: bf16, 0: fp16
 };
 
+// GACCUM_LAMB (gaccum_lamb.cuh): the per-tensor accumulators and the trust ratios
+struct LambParams {
+  struct LambTensorAcc* acc;   // 2 sets x num_tensors
+  float* ratios;           // num_tensors: r of the last applied window (gaccum_read_trust_ratios)
+  const uint8_t* adapt;    // num_tensors: 1 = layer adaptation (gaccum_plan_set_layer_adaptation)
+  int32_t num_tensors;
+  float beta1_power;       // TF1's beta powers of this step (loss-scaled launches use the device block's)
+  float beta2_power;
+};
+
+// gaccum_ema_state (gaccum.h): caller-owned device memory, written by gaccum_ema_init and afterwards only by the apply
+// launches of an EMA plan
+struct EmaState {
+  long long num_updates;   // n: windows averaged so far
+  float decay;             // d of the last averaged window
+  float reserved;
+};
+static_assert(sizeof(EmaState) == 16, "gaccum_ema_state is 16 bytes");
+
+// The exponential moving average of the weights (gaccum_plan_set_ema)
+struct EmaParams {
+  float* slab;             // the averages, a slab in the plan's layout (16-byte aligned)
+  EmaState* state;
+  unsigned int* done;      // apply_kernel: CTAs of the launch that are through (0 between launches)
+  float decay;             // fp32(decay)
+  int32_t num_updates;     // 1: d = min(decay, (1 + n) / (10 + n))
+};
+
+// Every kernel's parameter block.  Each feature's parameters follow those of the features before it, so adding them
+// moved no member an existing kernel reads.
 template <int CAP>
 struct KernelParams {
   const TileDesc* tiles;
@@ -123,44 +154,12 @@ struct KernelParams {
 #endif
   Scalars sc;
   PtrTable<CAP> tab;
-  LossScaleParams ls;   // apply_clip_kernel with LS != kLsOff only
+  LossScaleParams ls;   // loss-scaled modes (kLsClip, kLsNoClip) only
   HalfParams half;      // kernels with H = true only
+  LambParams lamb;      // lamb_apply_kernel only
+  EmaParams ema;        // kernels with EMA = true only
 };
-
-// gaccum_ema_state (gaccum.h): caller-owned device memory, written by gaccum_ema_init and afterwards only by the apply
-// launches of an EMA plan
-struct EmaState {
-  long long num_updates;   // n: windows averaged so far
-  float decay;             // d of the last averaged window
-  float reserved;
-};
-static_assert(sizeof(EmaState) == 16, "gaccum_ema_state is 16 bytes");
-
-// The exponential moving average of the weights (gaccum_plan_set_ema).  The apply kernels of an EMA plan take
-// EmaKernelParams: KernelParams as every other kernel sees it, then these, so no existing parameter block moves.
-struct EmaParams {
-  float* slab;             // the averages, a slab in the plan's layout (16-byte aligned)
-  EmaState* state;
-  unsigned int* done;      // apply_kernel: CTAs of the launch that are through (0 between launches)
-  float decay;             // fp32(decay)
-  int32_t num_updates;     // 1: d = min(decay, (1 + n) / (10 + n))
-};
-template <int CAP>
-struct EmaKernelParams {
-  KernelParams<CAP> k;
-  EmaParams ema;
-};
-// the parameter block of an apply kernel with (EMA) or without an EMA
-template <int CAP, bool EMA>
-using ApplyParams = typename std::conditional<EMA, EmaKernelParams<CAP>, KernelParams<CAP>>::type;
-template <int CAP>
-__device__ __forceinline__ const KernelParams<CAP>& kparams(const KernelParams<CAP>& p) { return p; }
-template <int CAP>
-__device__ __forceinline__ const KernelParams<CAP>& kparams(const EmaKernelParams<CAP>& p) { return p.k; }
-template <int CAP>
-__device__ __forceinline__ const EmaParams* ema_params(const KernelParams<CAP>&) { return nullptr; }
-template <int CAP>
-__device__ __forceinline__ const EmaParams* ema_params(const EmaKernelParams<CAP>& p) { return &p.ema; }
+static_assert(sizeof(KernelParams<1920>) <= 32764, "kernel parameters must fit the 32 KB limit");
 
 // What every CTA of an EMA launch derives from the state as the launch finds it (TF1 ExponentialMovingAverage, one
 // correctly rounded fp32 op per TF op): d = fp32(decay), in num_updates mode d = min(d, (1 + fp32(n)) / (10 + fp32(n)));
@@ -374,44 +373,38 @@ __device__ __forceinline__ float add_sq(float acc, const float4 x, const Scalars
 __device__ __forceinline__ float unscale(float a, float inv_s, const Scalars& sc) {
   return __fmul_rn(normalize(a, sc.nf, sc.inv_nf), inv_s);
 }
-template <int LS>
+template <int MODE>
 __device__ __forceinline__ float ls_pass1(float acc, float x, float inv_s, bool& bad, const Scalars& sc) {
   bad |= !(fabsf(x) <= 3.402823466e38f);
-  if constexpr (LS == kLsClip) {
+  if constexpr (MODE == kLsClip) {
     const float c = unscale(x, inv_s, sc);
     acc = fmaf(c, c, acc);
   }
   return acc;
 }
-template <int LS>
+template <int MODE>
 __device__ __forceinline__ float ls_pass1(float acc, const float4 x, float inv_s, bool& bad, const Scalars& sc) {
-  return ls_pass1<LS>(ls_pass1<LS>(ls_pass1<LS>(ls_pass1<LS>(acc, x.x, inv_s, bad, sc), x.y, inv_s, bad, sc), x.z, inv_s, bad, sc),
-                      x.w, inv_s, bad, sc);
+  return ls_pass1<MODE>(ls_pass1<MODE>(ls_pass1<MODE>(ls_pass1<MODE>(acc, x.x, inv_s, bad, sc), x.y, inv_s, bad, sc), x.z, inv_s, bad, sc),
+                        x.w, inv_s, bad, sc);
 }
-// pass 2 of the clip kernel on one element: c = a'/N (unscaled under loss scaling), times the clip scale s unless
-// clipping is off, then one Adam step
-template <int VARIANT, int LS>
-__device__ __forceinline__ void update_elem2(float a, float s, float inv_s, float& p, float& m, float& v, bool decay,
-                                             const Scalars& sc) {
-  if constexpr (LS == kLsOff) {
-    update_elem<VARIANT>(a, true, s, p, m, v, decay, sc);
-  } else {
-    float c = unscale(a, inv_s, sc);
-    if constexpr (LS == kLsClip) c = __fmul_rn(c, s);
-    adam_elem<VARIANT>(c, p, m, v, decay, sc);
-  }
+// c of one element of a' in the cooperative kernels: (1.0*a')/N, unscaled by 1/S under loss scaling, times the clip
+// scale s when clipping
+template <int MODE>
+__device__ __forceinline__ float mode_c(float a, float s, float inv_s, const Scalars& sc) {
+  if constexpr (MODE == kNoClip) return normalize(a, sc.nf, sc.inv_nf);
+  else if constexpr (MODE == kClip) return __fmul_rn(normalize(a, sc.nf, sc.inv_nf), s);
+  else if constexpr (MODE == kLsClip) return __fmul_rn(unscale(a, inv_s, sc), s);
+  else return unscale(a, inv_s, sc);
 }
-template <int VARIANT, int LS>
-__device__ __forceinline__ void update_vec2(const float4 a, float s, float inv_s, float4& p, float4& m, float4& v, bool decay,
-                                            const Scalars& sc) {
-  if constexpr (LS == kLsOff) {
-    update_vec<VARIANT>(a, true, s, p, m, v, decay, sc);
-  } else {
-    update_elem2<VARIANT, LS>(a.x, s, inv_s, p.x, m.x, v.x, decay, sc);
-    update_elem2<VARIANT, LS>(a.y, s, inv_s, p.y, m.y, v.y, decay, sc);
-    update_elem2<VARIANT, LS>(a.z, s, inv_s, p.z, m.z, v.z, decay, sc);
-    update_elem2<VARIANT, LS>(a.w, s, inv_s, p.w, m.w, v.w, decay, sc);
-  }
+// pass 2 of the clip kernel on 4 elements: c of a', then one Adam step each.  A function of its own: written out at the
+// call site, nvcc schedules the AdamWeightDecay instantiations differently (more instructions, different registers).
+template <int VARIANT, int MODE>
+__device__ __forceinline__ void adam_vec(const float4 a, float s, float inv_s, float4& p, float4& m, float4& v, bool decay,
+                                         const Scalars& sc) {
+  adam_elem<VARIANT>(mode_c<MODE>(a.x, s, inv_s, sc), p.x, m.x, v.x, decay, sc);
+  adam_elem<VARIANT>(mode_c<MODE>(a.y, s, inv_s, sc), p.y, m.y, v.y, decay, sc);
+  adam_elem<VARIANT>(mode_c<MODE>(a.z, s, inv_s, sc), p.z, m.z, v.z, decay, sc);
+  adam_elem<VARIANT>(mode_c<MODE>(a.w, s, inv_s, sc), p.w, m.w, v.w, decay, sc);
 }
 
 // tf.clip_by_global_norm (TF 1.15): scale = clip * min(1/gn, 1/clip) + (gn - gn)
@@ -496,15 +489,14 @@ __global__ void ema_init_kernel(EmaState* st, long long num_updates) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// apply without clipping: one pass.  HAS_G = false applies the accumulators as they are.
+// apply without clipping: one pass.  A tensor without a gradient applies its accumulator as it is.
 // ---------------------------------------------------------------------------------------------
 // H: p is the master slab (always 16-byte aligned); the model copy is stored after it.
 // EMA: the average e (slab `ema`, always 16-byte aligned) is read with p and stored after it: e - (e - p) * c.
-template <int VARIANT, bool LOAD_G, bool H, int CAP, bool EMA = false>
+template <int VARIANT, bool H, int CAP, bool EMA = false>
 __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams<CAP>& prm, float* ema = nullptr,
                                             const float ema_c = 0.f) {
-  Grad<H> g;
-  if constexpr (LOAD_G) g = Grad<H>(prm, d);
+  const Grad<H> g(prm, d);
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
   float* __restrict__ m = prm.m + soff;
@@ -526,12 +518,12 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
   walk_tile(d.len, (H || aligned16(p)) && (g.g == nullptr || g.vec_ok()) ? d.len >> 2 : 0u, threadIdx.x,
             [&](int u, uint32_t i) {
               va[u] = __ldcs(a4 + i); vp[u] = __ldcs(p4 + i); vm[u] = __ldcs(m4 + i); vv[u] = __ldcs(v4 + i);
-              if (LOAD_G && g.g) vg[u] = g.vec(i);
+              if (g.g) vg[u] = g.vec(i);
               if constexpr (EMA) ve[u] = __ldcs(e4 + i);
             },
             [] {},
             [&](int u, uint32_t i) {
-              if (LOAD_G && g.g) va[u] = add_rn(va[u], vg[u]);
+              if (g.g) va[u] = add_rn(va[u], vg[u]);
               update_vec<VARIANT>(va[u], false, 0.f, vp[u], vm[u], vv[u], decay, sc);
               __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
@@ -540,7 +532,7 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
             },
             [&](uint32_t i) {
               float ax = a[i], px = p[i], mx = m[i], vx = v[i];
-              if (LOAD_G && g.g) ax = __fadd_rn(ax, g.elem(i));
+              if (g.g) ax = __fadd_rn(ax, g.elem(i));
               update_elem<VARIANT>(ax, false, 0.f, px, mx, vx, decay, sc);
               p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
               if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
@@ -550,18 +542,17 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
 
 // EMA: every CTA reads n (thread 0, before its tile); the CTA that finishes last -- a counter of finished CTAs, so
 // every other CTA of the launch has read n by then -- writes n + 1 and d, and resets the counter for the next launch.
-template <int VARIANT, bool HAS_G, int CAP, bool H = false, bool EMA = false>
+template <int VARIANT, int CAP, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads)
-apply_kernel(const __grid_constant__ ApplyParams<CAP, EMA> ap) {
-  const KernelParams<CAP>& prm = kparams(ap);
+apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   if constexpr (!EMA) {
-    if ((int)blockIdx.x < prm.num_tiles) update_tile<VARIANT, HAS_G, H>(prm.tiles[blockIdx.x], prm);
+    if ((int)blockIdx.x < prm.num_tiles) update_tile<VARIANT, H>(prm.tiles[blockIdx.x], prm);
   } else {
-    const EmaParams& ep = *ema_params(ap);
+    const EmaParams& ep = prm.ema;
     __shared__ EmaLaunch s_ema;
     if (threadIdx.x == 0) ema_load(ep, s_ema);
     __syncthreads();
-    if ((int)blockIdx.x < prm.num_tiles) update_tile<VARIANT, HAS_G, H, CAP, true>(prm.tiles[blockIdx.x], prm, ep.slab, s_ema.c);
+    if ((int)blockIdx.x < prm.num_tiles) update_tile<VARIANT, H, CAP, true>(prm.tiles[blockIdx.x], prm, ep.slab, s_ema.c);
     if (threadIdx.x == 0) {
       __threadfence();
       if (atomicAdd(ep.done, 1u) == gridDim.x - 1u) {
@@ -719,10 +710,11 @@ __device__ __forceinline__ uint32_t bulk_vecs2(const TileDesc& d, const float* p
 }
 
 // a' of a tile may be parked in the stash only if BOTH passes take the vector path for it and it is a full tile
-template <bool HAS_G, bool H, int CAP>
+template <bool H, int CAP>
 __device__ __forceinline__ bool stash_ok(const TileDesc& d, const KernelParams<CAP>& prm) {
   bool ok = d.len == (uint32_t)kTile && aligned16(update_ptr<H>(prm, d));
-  if constexpr (HAS_G) { const Grad<H> g(prm, d); ok = ok && (g.g == nullptr || aligned16(g.g)); }
+  const Grad<H> g(prm, d);
+  ok = ok && (g.g == nullptr || aligned16(g.g));
   return ok;
 }
 
@@ -805,10 +797,10 @@ __device__ __forceinline__ void ls_load(const LossScaleState* st, LossScaleState
 // thread 0 after the barrier, from the launch-wide counters (`bins`: their accumulator, copied where the thread reads
 // it): the clip scale s and the global norm gn (1 and 0 without clipping) and, loss-scaled, whether the window is
 // skipped -- an element of a' or, with clipping, gn is not finite.  Every CTA computes the same values.
-template <int LS>
+template <int MODE>
 __device__ __forceinline__ void window_decision(const LaunchCounters* ctr, const unsigned long long* bins, const float clip,
                                                 float& s, float& gn, int& skip) {
-  if constexpr (LS == kLsNoClip) {
+  if constexpr (MODE == kLsNoClip) {
     s = 1.f;                                              // no clipping: stats as the un-clipped apply writes them
     gn = 0.f;
     skip = (__ldcg(&ctr->nonfinite) & kElemNonfinite) != 0;
@@ -818,7 +810,7 @@ __device__ __forceinline__ void window_decision(const LaunchCounters* ctr, const
     const float g_norm = __fsqrt_rn((float)tot);          // tf.linalg.global_norm
     s = clip_scale(g_norm, clip);
     gn = g_norm;
-    if constexpr (LS != kLsOff) skip = (nonfinite & kElemNonfinite) != 0 || !(fabsf(g_norm) <= 3.402823466e38f);
+    if constexpr (loss_scaled(MODE)) skip = (nonfinite & kElemNonfinite) != 0 || !(fabsf(g_norm) <= 3.402823466e38f);
   }
 }
 // block 0's thread 0 at the very end of a loss-scaled launch: TF 2 DynamicLossScale, counted in windows (gaccum.h,
@@ -853,13 +845,12 @@ __device__ __forceinline__ void ls_finish(const LossScaleParams& ls, const LossS
 
 // ---- pass 1, consumer side: one tile out of slot [G | a]; returns this THREAD's partial of sum((a'/N)^2) ----
 // A tile the producer did not copy (nvec == 0), and the < 4 tail elements of any tile, travel through global memory.
-// Loss-scaled (LS != kLsOff): the partial is of sum(((a'/N)(1/S))^2) (none without clipping), and `bad` is set when an
-// element of a' is not finite.
-template <bool HAS_G, int LS, bool H, int CAP>
+// Loss-scaled (kLsClip, kLsNoClip): the partial is of sum(((a'/N)(1/S))^2) (none without clipping), and `bad` is set
+// when an element of a' is not finite.
+template <int MODE, bool H, int CAP>
 __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float4* slot, uint64_t* empty,
                                            float4* const stash, const uint64_t pol, const float inv_s, bool& bad) {
-  Grad<H> g;
-  if constexpr (HAS_G) g = Grad<H>(prm, d);
+  const Grad<H> g(prm, d);
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
   float4* a4 = reinterpret_cast<float4*>(a);
   float acc = 0.f;
@@ -873,14 +864,14 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
                 if (stash == nullptr) st_policy(a4 + i, x[u], pol);
               }
               if (stash != nullptr) stash[i] = x[u];
-              if constexpr (LS == kLsOff) acc = add_sq(acc, x[u], prm.sc);
-              else acc = ls_pass1<LS>(acc, x[u], inv_s, bad, prm.sc);
+              if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, x[u], prm.sc);
+              else acc = ls_pass1<MODE>(acc, x[u], inv_s, bad, prm.sc);
             },
             [&](uint32_t i) {
               float xs = a[i];
               if (g.g) { xs = __fadd_rn(xs, g.elem(i)); a[i] = xs; }
-              if constexpr (LS == kLsOff) acc = add_sq(acc, xs, prm.sc);
-              else acc = ls_pass1<LS>(acc, xs, inv_s, bad, prm.sc);
+              if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, xs, prm.sc);
+              else acc = ls_pass1<MODE>(acc, xs, inv_s, bad, prm.sc);
             });
   return acc;
 }
@@ -890,7 +881,7 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
 // Loss-scaled: `sc` carries the alpha computed from the device's beta powers, and a skipped window (`skip`) stores
 // a = 0 and nothing else.  H: p is the master slab, and the model copy is stored after it (not on a skipped window).
 // EMA: the slot is [p | m | v | a' | e], and e - (e - p) * c is stored after p (not on a skipped window).
-template <int VARIANT, int LS, bool H, int CAP, bool EMA = false>
+template <int VARIANT, int MODE, bool H, int CAP, bool EMA = false>
 __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelParams<CAP>& prm, const float s, const float4* slot,
                                              uint64_t* empty, const float4* const stash, const Scalars& sc, const float inv_s,
                                              const bool skip, float* ema = nullptr, const float ema_c = 0.f) {
@@ -904,7 +895,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
   bool bf16 = false;
   if constexpr (H) { q = model_ptr(prm, d); bf16 = prm.half.bf16 != 0; }
   const bool decay = (d.tensor_flags >> 31) != 0;
-  const bool write = LS == kLsOff || !skip;
+  const bool write = !loss_scaled(MODE) || !skip;
   float4* a4 = reinterpret_cast<float4*>(a);
   float4* m4 = reinterpret_cast<float4*>(m);
   float4* v4 = reinterpret_cast<float4*>(v);
@@ -920,7 +911,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
             [&] { __syncwarp(); if ((threadIdx.x & 31) == 0) mbar_arrive(empty); },
             [&](int u, uint32_t i) {
               if (write) {
-                update_vec2<VARIANT, LS>(va[u], s, inv_s, vp[u], vm[u], vv[u], decay, sc);
+                adam_vec<VARIANT, MODE>(va[u], s, inv_s, vp[u], vm[u], vv[u], decay, sc);
                 __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
                 if constexpr (H) store_model4(q, i, vp[u], bf16);
                 if constexpr (EMA) __stcs(e4 + i, ema_vec(ve[u], vp[u], ema_c));
@@ -930,7 +921,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
             [&](uint32_t i) {
               if (write) {
                 float px = p[i], mx = m[i], vx = v[i];
-                update_elem2<VARIANT, LS>(a[i], s, inv_s, px, mx, vx, decay, sc);
+                adam_elem<VARIANT>(mode_c<MODE>(a[i], s, inv_s, sc), px, mx, vx, decay, sc);
                 p[i] = px; m[i] = mx; v[i] = vx;
                 if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
                 if constexpr (EMA) e[i] = ema_elem(e[i], px, ema_c);
@@ -945,7 +936,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
 // fit without spilling; the plain-Adam ones with clipping (VARIANT 1, used only when tf_adam is combined with
 // clip_norm > 0) spill 8-20 bytes per thread to local memory (ptxas -v).  What that costs has not been measured.
 //
-// Loss scaling (LS != kLsOff, gaccum_plan_set_loss_scale).  Thread 0 of every CTA reads S, the counters and the beta
+// Loss scaling (kLsClip, kLsNoClip; gaccum_plan_set_loss_scale).  Thread 0 of every CTA reads S, the counters and the beta
 // powers from prm.ls.state during set-up, i.e. before its CTA arrives at the grid barrier; pass 1 ORs kElemNonfinite
 // into the launch's counters when an element of a' is not finite.  After the barrier every CTA takes the same decision
 // from the same launch-wide flags: skip iff an element was non-finite or, with clipping, gn is.  A skipped window
@@ -958,14 +949,13 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
 // EMA: ClipLayout<true> -- pass 2's producer moves e by bulk copy as the fifth stream of the slot.  Thread 0 of every
 // CTA reads n during set-up, before its CTA arrives at the grid barrier; block 0's thread 0 writes n + 1 and d at the
 // very end, on an applied window only, as it writes the loss-scaling state.
-template <int VARIANT, bool HAS_G, int CAP, int LS = kLsOff, bool H = false, bool EMA = false>
+template <int VARIANT, int CAP, int MODE, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kClipThreads, 1)
-apply_clip_kernel(const __grid_constant__ ApplyParams<CAP, EMA> ap) {
+apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   using L = ClipLayout<EMA>;
   constexpr int kRingVecs = L::kRingVecs, kP2SlotVecs = L::kP2SlotVecs, kP2Slots = L::kP2Slots, kRingBytes = L::kRingBytes;
   constexpr int kStashTiles = L::kStashTiles, kStashVecs = L::kStashVecs;
-  const KernelParams<CAP>& prm = kparams(ap);
-  const EmaParams* const ema = ema_params(ap);
+  const EmaParams* const ema = &prm.ema;   // read through a pointer: without it nvcc adds instructions to one EMA instantiation
   EmaLaunch* s_ema = nullptr;            // EMA: n, d and c as this launch found them
   if constexpr (EMA) {
     __shared__ EmaLaunch s_ema_launch;
@@ -1023,7 +1013,7 @@ apply_clip_kernel(const __grid_constant__ ApplyParams<CAP, EMA> ap) {
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    if constexpr (LS != kLsOff) {
+    if constexpr (loss_scaled(MODE)) {
       ls_load(prm.ls.state, s_ls);
       if constexpr (VARIANT == 1) {
         // make_scalars' op order: lr * sqrt(1 - b2^t) / (1 - b1^t), one rounding per op
@@ -1054,8 +1044,7 @@ apply_clip_kernel(const __grid_constant__ ApplyParams<CAP, EMA> ap) {
     {
       RingPos rp;
       auto issue = [&](const TileDesc& dl) {                               // lane 0 only
-        Grad<H> g;
-        if constexpr (HAS_G) g = Grad<H>(prm, dl);
+        const Grad<H> g(prm, dl);
         const uint32_t nvec = bulk_vecs(dl, g);
         uint64_t* full = &s_full1[grp][rp.slot];
 #ifdef GACCUM_EXPERIMENTS
@@ -1166,7 +1155,7 @@ apply_clip_kernel(const __grid_constant__ ApplyParams<CAP, EMA> ap) {
         const TileDesc d = prm.tiles[tile];
         const float* p = update_ptr<H>(prm, d);
         const uint32_t nvec = bulk_vecs2(d, p);
-        const bool in_stash = stash_slot != kNoStash && stash_ok<HAS_G, H>(d, prm);
+        const bool in_stash = stash_slot != kNoStash && stash_ok<H>(d, prm);
         if (!in_stash && !past_barrier) {                                        // an own tile whose a' had to go to global memory
           mbar_wait(&s_go[grp], 0);
           asm volatile("fence.proxy.async;" ::: "memory");
@@ -1213,7 +1202,7 @@ apply_clip_kernel(const __grid_constant__ ApplyParams<CAP, EMA> ap) {
     // ---- pass 1: whatever tiles the producer hands over, until its end marker ----
     unsigned int my_nonfinite = 0;
     float inv_s = 1.0f;
-    if constexpr (LS != kLsOff) inv_s = __fdiv_rn(1.0f, s_ls.scale);   // exact: S is a power of two
+    if constexpr (loss_scaled(MODE)) inv_s = __fdiv_rn(1.0f, s_ls.scale);   // exact: S is a power of two
     {
       RingPos rp;
       int n_seen = 0;
@@ -1230,13 +1219,13 @@ apply_clip_kernel(const __grid_constant__ ApplyParams<CAP, EMA> ap) {
         // the stash takes the group's own tiles j < kStashTiles (the first ones it is handed) when they are FULL,
         // vector-path tiles (the same predicate the producer evaluates in pass 2)
         const bool own = n_seen < n_st;
-        const bool park = own && stash_ok<HAS_G, H>(meta.d, prm);
+        const bool park = own && stash_ok<H>(meta.d, prm);
         float4* const st = park ? stash + (size_t)n_seen * (kTile / 4) : nullptr;
         bool bad = false;
-        const float part = norm_tile<HAS_G, LS, H>(meta.d, prm, ring + (size_t)rp.slot * kP1SlotVecs, &s_empty1[grp][rp.slot], st,
+        const float part = norm_tile<MODE, H>(meta.d, prm, ring + (size_t)rp.slot * kP1SlotVecs, &s_empty1[grp][rp.slot], st,
                                                 pol_last, inv_s, bad);
-        if constexpr (LS != kLsOff) { if (bad) my_nonfinite |= kElemNonfinite; }
-        if constexpr (LS != kLsNoClip) {
+        if constexpr (loss_scaled(MODE)) { if (bad) my_nonfinite |= kElemNonfinite; }
+        if constexpr (MODE != kLsNoClip) {
           // warp total in fp64, fixed butterfly order; lane 0 adds it EXACTLY into its warp's accumulator
           double w = (double)part;
 #pragma unroll
@@ -1270,16 +1259,16 @@ apply_clip_kernel(const __grid_constant__ ApplyParams<CAP, EMA> ap) {
     if (leader) mbar_arrive(&s_go[grp]);                     // this group's producer may now fetch pool tiles
     stamp(2);
     // ---- every CTA evaluates the same exact sum the same way: bit-identical gn and clip scale everywhere ----
-    if constexpr (LS != kLsNoClip) {
+    if constexpr (MODE != kLsNoClip) {
       if (threadIdx.x < kAccBins) s_bins[0][threadIdx.x] = __ldcg(&ctr->bins[threadIdx.x]);
       named_bar_sync(1, kConsumerThreads);
     }
-    if (threadIdx.x == 0) window_decision<LS>(ctr, s_bins[0], prm.sc.clip, s_bcast[0], s_bcast[1], s_skip);
+    if (threadIdx.x == 0) window_decision<MODE>(ctr, s_bins[0], prm.sc.clip, s_bcast[0], s_bcast[1], s_skip);
     named_bar_sync(1, kConsumerThreads);
     const float s = s_bcast[0];
     bool skip = false;
-    if constexpr (LS != kLsOff) skip = s_skip != 0;
-    const Scalars& sc = (LS != kLsOff && VARIANT == 1) ? s_sc : prm.sc;
+    if constexpr (loss_scaled(MODE)) skip = s_skip != 0;
+    const Scalars& sc = (loss_scaled(MODE) && VARIANT == 1) ? s_sc : prm.sc;
     // ---- pass 2: whatever tiles the producer hands over, until its end marker ----
     {
       RingPos rp;
@@ -1289,18 +1278,18 @@ apply_clip_kernel(const __grid_constant__ ApplyParams<CAP, EMA> ap) {
         if (meta.d.len == 0) break;
         const float4* const st = meta.stash_slot != kNoStash ? stash + (size_t)meta.stash_slot * (kTile / 4) : nullptr;
         if constexpr (EMA) {
-          update_tile2<VARIANT, LS, H, CAP, true>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot],
-                                                  st, sc, inv_s, skip, ema->slab, s_ema->c);
+          update_tile2<VARIANT, MODE, H, CAP, true>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot],
+                                                    st, sc, inv_s, skip, ema->slab, s_ema->c);
         } else {
-          update_tile2<VARIANT, LS, H>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st, sc, inv_s,
-                                    skip);
+          update_tile2<VARIANT, MODE, H>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st, sc, inv_s,
+                                      skip);
         }
         rp.advance(kP2Slots);
       }
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) {
       prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s;
-      if constexpr (LS != kLsOff) ls_finish<VARIANT == 1>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
+      if constexpr (loss_scaled(MODE)) ls_finish<VARIANT == 1>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
       if constexpr (EMA) { if (!skip) ema_finish(*ema, *s_ema); }
     }
   }

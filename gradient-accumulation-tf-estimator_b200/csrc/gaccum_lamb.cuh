@@ -28,10 +28,6 @@
 
 namespace gaccum {
 
-constexpr int kLambNoClip = 0;     // no clipping, no loss scaling: phases 2 and 3 only
-constexpr int kLambClip = 1;       // tf.clip_by_global_norm
-constexpr int kLambLsClip = 2;     // loss scaling + clipping
-constexpr int kLambLsNoClip = 3;   // loss scaling without clipping: phase 1 only looks for non-finite elements of a'
 constexpr int kLambBlocksPerSm = 3;
 
 // sum(p^2) and sum(u^2) of one tensor in one launch, exact (acc_add); nonfinite as LaunchCounters::nonfinite bits 0-1
@@ -42,50 +38,11 @@ struct LambTensorAcc {
 };
 static_assert(sizeof(LambTensorAcc) % 8 == 0, "cleared in 8-byte words");
 
-struct LambParams {
-  LambTensorAcc* acc;      // 2 sets x num_tensors
-  float* ratios;           // num_tensors: r of the last applied window (gaccum_read_trust_ratios)
-  const uint8_t* adapt;    // num_tensors: 1 = layer adaptation (gaccum_plan_set_layer_adaptation)
-  int32_t num_tensors;
-  float beta1_power;       // TF1's beta powers of this step (loss-scaled launches use the device block's)
-  float beta2_power;
-};
-
-// KernelParams stays as every other kernel sees it; LAMB's own parameters follow it
-template <int CAP>
-struct LambKernelParams {
-  KernelParams<CAP> k;
-  LambParams lamb;
-};
-static_assert(sizeof(LambKernelParams<1920>) <= 32764, "kernel parameters must fit the 32 KB limit");
-// ... and with an EMA (gaccum_plan_set_ema), the EMA's after LAMB's
-template <int CAP>
-struct LambEmaKernelParams {
-  KernelParams<CAP> k;
-  LambParams lamb;
-  EmaParams ema;
-};
-static_assert(sizeof(LambEmaKernelParams<1920>) <= 32764, "kernel parameters must fit the 32 KB limit");
-template <int CAP, bool EMA>
-using LambApplyParams = typename std::conditional<EMA, LambEmaKernelParams<CAP>, LambKernelParams<CAP>>::type;
-template <int CAP>
-__device__ __forceinline__ const EmaParams* ema_params(const LambEmaKernelParams<CAP>& p) { return &p.ema; }
-template <int CAP>
-__device__ __forceinline__ const EmaParams* ema_params(const LambKernelParams<CAP>&) { return nullptr; }
-
 // what phase 2 needs besides Scalars: the clip scale, 1/S, and the bias corrections 1 - beta^t
 struct LambCoef {
   float s, inv_s, omb1p, omb2p;
 };
 
-// c of one element of a': (1.0*a')/N, unscaled by 1/S under loss scaling, times the clip scale when clipping
-template <int MODE>
-__device__ __forceinline__ float lamb_c(float a, const LambCoef& k, const Scalars& sc) {
-  if constexpr (MODE == kLambNoClip) return normalize(a, sc.nf, sc.inv_nf);
-  else if constexpr (MODE == kLambClip) return __fmul_rn(normalize(a, sc.nf, sc.inv_nf), k.s);
-  else if constexpr (MODE == kLambLsClip) return __fmul_rn(unscale(a, k.inv_s, sc), k.s);
-  else return unscale(a, k.inv_s, sc);
-}
 // m, v and the update u of one element (gaccum.h, GACCUM_LAMB): one correctly rounded op per TF op
 __device__ __forceinline__ float lamb_u(float c, float p, float& m, float& v, bool decay, const Scalars& sc, const LambCoef& k) {
   m = __fadd_rn(__fmul_rn(sc.b1, m), __fmul_rn(sc.omb1, c));
@@ -102,10 +59,9 @@ __device__ __forceinline__ double add_sq64(double acc, const float4 x) {
 }
 
 // ---- phase 1: a' = a + G stored back; returns this thread's fp32 partial of the global norm (as norm_tile) ----
-template <bool HAS_G, int LS, bool H, int CAP>
+template <int MODE, bool H, int CAP>
 __device__ __forceinline__ float lamb_norm_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float inv_s, bool& bad) {
-  Grad<H> g;
-  if constexpr (HAS_G) g = Grad<H>(prm, d);
+  const Grad<H> g(prm, d);
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
   float4* a4 = reinterpret_cast<float4*>(a);
   float acc = 0.f;
@@ -115,14 +71,14 @@ __device__ __forceinline__ float lamb_norm_tile(const TileDesc& d, const KernelP
             [] {},
             [&](int u, uint32_t i) {
               if (g.g) { x[u] = add_rn(x[u], gg[u]); a4[i] = x[u]; }
-              if constexpr (LS == kLsOff) acc = add_sq(acc, x[u], prm.sc);
-              else acc = ls_pass1<LS>(acc, x[u], inv_s, bad, prm.sc);
+              if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, x[u], prm.sc);
+              else acc = ls_pass1<MODE>(acc, x[u], inv_s, bad, prm.sc);
             },
             [&](uint32_t i) {
               float xs = a[i];
               if (g.g) { xs = __fadd_rn(xs, g.elem(i)); a[i] = xs; }
-              if constexpr (LS == kLsOff) acc = add_sq(acc, xs, prm.sc);
-              else acc = ls_pass1<LS>(acc, xs, inv_s, bad, prm.sc);
+              if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, xs, prm.sc);
+              else acc = ls_pass1<MODE>(acc, xs, inv_s, bad, prm.sc);
             });
   return acc;
 }
@@ -155,10 +111,10 @@ __device__ __forceinline__ void lamb_update_tile(const TileDesc& d, const Kernel
             [&](int u, uint32_t i) {
               if (LOAD_G && g.g) va[u] = add_rn(va[u], vg[u]);
               float4 w;
-              w.x = lamb_u(lamb_c<MODE>(va[u].x, k, sc), vp[u].x, vm[u].x, vv[u].x, decay, sc, k);
-              w.y = lamb_u(lamb_c<MODE>(va[u].y, k, sc), vp[u].y, vm[u].y, vv[u].y, decay, sc, k);
-              w.z = lamb_u(lamb_c<MODE>(va[u].z, k, sc), vp[u].z, vm[u].z, vv[u].z, decay, sc, k);
-              w.w = lamb_u(lamb_c<MODE>(va[u].w, k, sc), vp[u].w, vm[u].w, vv[u].w, decay, sc, k);
+              w.x = lamb_u(mode_c<MODE>(va[u].x, k.s, k.inv_s, sc), vp[u].x, vm[u].x, vv[u].x, decay, sc, k);
+              w.y = lamb_u(mode_c<MODE>(va[u].y, k.s, k.inv_s, sc), vp[u].y, vm[u].y, vv[u].y, decay, sc, k);
+              w.z = lamb_u(mode_c<MODE>(va[u].z, k.s, k.inv_s, sc), vp[u].z, vm[u].z, vv[u].z, decay, sc, k);
+              w.w = lamb_u(mode_c<MODE>(va[u].w, k.s, k.inv_s, sc), vp[u].w, vm[u].w, vv[u].w, decay, sc, k);
               __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]); a4[i] = w;
               sp = add_sq64(sp, vp[u]); su = add_sq64(su, w);
             },
@@ -166,7 +122,7 @@ __device__ __forceinline__ void lamb_update_tile(const TileDesc& d, const Kernel
               float ax = a[i], mx = m[i], vx = v[i];
               const float px = p[i];
               if (LOAD_G && g.g) ax = __fadd_rn(ax, g.elem(i));
-              const float w = lamb_u(lamb_c<MODE>(ax, k, sc), px, mx, vx, decay, sc, k);
+              const float w = lamb_u(mode_c<MODE>(ax, k.s, k.inv_s, sc), px, mx, vx, decay, sc, k);
               m[i] = mx; v[i] = vx; a[i] = w;
               sp = add_sq64(sp, px); su = add_sq64(su, w);
             });
@@ -228,16 +184,13 @@ __device__ __forceinline__ double warp_sum(double w) {
 
 // EMA: thread 0 of every CTA reads n during set-up; block 0's thread 0 writes n + 1 and d at the very end, past the
 // grid barriers, on an applied window only.
-template <bool HAS_G, int CAP, int MODE, bool H = false, bool EMA = false>
+template <int CAP, int MODE, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads, kLambBlocksPerSm)
-lamb_apply_kernel(const __grid_constant__ LambApplyParams<CAP, EMA> lp) {
-  constexpr int LS = MODE == kLambLsClip ? kLsClip : MODE == kLambLsNoClip ? kLsNoClip : kLsOff;
-  constexpr bool kPhase1 = MODE != kLambNoClip;
+lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
+  constexpr bool kPhase1 = MODE != kNoClip;
   constexpr unsigned long long kBarriers = kPhase1 ? 3 : 2;
   constexpr int kWarps = kThreads / 32;
-  const KernelParams<CAP>& prm = lp.k;
-  const LambParams& lb = lp.lamb;
-  const EmaParams* const ema = ema_params(lp);
+  const LambParams& lb = prm.lamb;
   EmaLaunch* s_ema = nullptr;            // EMA: n, d and c as this launch found them
   if constexpr (EMA) {
     __shared__ EmaLaunch s_ema_launch;
@@ -263,8 +216,8 @@ lamb_apply_kernel(const __grid_constant__ LambApplyParams<CAP, EMA> lp) {
     s_bcast[0] = 1.f;
     s_bcast[1] = 0.f;
     s_skip = 0;
-    if constexpr (LS != kLsOff) ls_load(prm.ls.state, s_ls);
-    if constexpr (EMA) ema_load(*ema, *s_ema);
+    if constexpr (loss_scaled(MODE)) ls_load(prm.ls.state, s_ls);
+    if constexpr (EMA) ema_load(prm.ema, *s_ema);
   }
   for (int i = threadIdx.x; i < kWarps * 2 * kAccBins; i += kThreads) (&s_bins[0][0][0])[i] = 0ull;
   __syncthreads();
@@ -279,7 +232,7 @@ lamb_apply_kernel(const __grid_constant__ LambApplyParams<CAP, EMA> lp) {
   }
   float inv_s = 1.0f;
   float b1p = lb.beta1_power, b2p = lb.beta2_power;
-  if constexpr (LS != kLsOff) {
+  if constexpr (loss_scaled(MODE)) {
     inv_s = __fdiv_rn(1.0f, s_ls.scale);   // exact: S is a power of two
     b1p = s_ls.beta1_power;
     b2p = s_ls.beta2_power;
@@ -290,13 +243,13 @@ lamb_apply_kernel(const __grid_constant__ LambApplyParams<CAP, EMA> lp) {
     bool bad = false;
     unsigned int nonfinite = 0;
     for (int t = t_lo; t < t_hi; ++t) {
-      const float part = lamb_norm_tile<HAS_G, LS, H>(prm.tiles[t], prm, inv_s, bad);
-      if constexpr (LS != kLsNoClip) {
+      const float part = lamb_norm_tile<MODE, H>(prm.tiles[t], prm, inv_s, bad);
+      if constexpr (MODE != kLsNoClip) {
         const double w = warp_sum((double)part);
         if (lane == 0) acc_add(s_bins[warp][0], nonfinite, w);
       }
     }
-    if constexpr (LS != kLsOff) { if (bad) nonfinite |= kElemNonfinite; }
+    if constexpr (loss_scaled(MODE)) { if (bad) nonfinite |= kElemNonfinite; }
     if (nonfinite) atomicOr(&s_nonfinite[0], nonfinite);
     __syncthreads();
     if (threadIdx.x < kAccBins) {
@@ -311,11 +264,11 @@ lamb_apply_kernel(const __grid_constant__ LambApplyParams<CAP, EMA> lp) {
       grid_barrier(prm.barrier);
     }
     __syncthreads();
-    if constexpr (LS != kLsNoClip) {
+    if constexpr (MODE != kLsNoClip) {
       if (threadIdx.x < kAccBins) s_bins[0][1][threadIdx.x] = __ldcg(&ctr->bins[threadIdx.x]);
       __syncthreads();
     }
-    if (threadIdx.x == 0) window_decision<LS>(ctr, s_bins[0][1], prm.sc.clip, s_bcast[0], s_bcast[1], s_skip);
+    if (threadIdx.x == 0) window_decision<MODE>(ctr, s_bins[0][1], prm.sc.clip, s_bcast[0], s_bcast[1], s_skip);
     __syncthreads();
     if (threadIdx.x < kAccBins) s_bins[0][1][threadIdx.x] = 0ull;
     __syncthreads();
@@ -350,7 +303,7 @@ lamb_apply_kernel(const __grid_constant__ LambApplyParams<CAP, EMA> lp) {
         cur_adapt = lb.adapt[ti] != 0;
       }
       double sp = 0.0, su = 0.0;
-      lamb_update_tile<MODE, HAS_G && !kPhase1, H>(d, prm, coef, sp, su);
+      lamb_update_tile<MODE, !kPhase1, H>(d, prm, coef, sp, su);
       if (cur_adapt) {
         sp = warp_sum(sp);
         su = warp_sum(su);
@@ -395,14 +348,14 @@ lamb_apply_kernel(const __grid_constant__ LambApplyParams<CAP, EMA> lp) {
   for (int t = t_lo; t < t_hi; ++t) {
     const TileDesc d = prm.tiles[t];
     const float rlr = skip ? 0.f : __fmul_rn(__ldcg(&lb.ratios[d.tensor_flags & 0x7fffffffu]), prm.sc.lr);   // ratio * lr first
-    if constexpr (EMA) lamb_write_tile<H, CAP, true>(d, prm, rlr, !skip, ema->slab, s_ema->c);
+    if constexpr (EMA) lamb_write_tile<H, CAP, true>(d, prm, rlr, !skip, prm.ema.slab, s_ema->c);
     else lamb_write_tile<H>(d, prm, rlr, !skip);
   }
 
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s_bcast[0];
-    if constexpr (LS != kLsOff) ls_finish<true>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
-    if constexpr (EMA) { if (!skip) ema_finish(*ema, *s_ema); }
+    if constexpr (loss_scaled(MODE)) ls_finish<true>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
+    if constexpr (EMA) { if (!skip) ema_finish(prm.ema, *s_ema); }
   }
 }
 

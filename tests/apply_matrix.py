@@ -36,9 +36,8 @@ LAYOUTS: Dict[str, Tuple[int, bool, str]] = {
     "t1920_fp32": (1920, False, "fp32"), "t1920_bf16": (1920, True, "bf16"), "t1920_fp16": (1920, True, "fp16"),
 }
 
-# gaccum_kernels.cuh kLsOff / kLsClip / kLsNoClip and gaccum_lamb.cuh kLamb*: the mode template argument of each kernel
-CLIP_LS_ARG = {"clip": "kLsOff", "ls_clip": "kLsClip", "ls_noclip": "kLsNoClip"}
-LAMB_MODE_ARG = {"noclip": "kLambNoClip", "clip": "kLambClip", "ls_clip": "kLambLsClip", "ls_noclip": "kLambLsNoClip"}
+# gaccum_kernels.cuh kNoClip / kClip / kLsClip / kLsNoClip: the MODE template argument of the cooperative kernels
+MODE_ARG = {"noclip": "kNoClip", "clip": "kClip", "ls_clip": "kLsClip", "ls_noclip": "kLsNoClip"}
 
 
 class Case(NamedTuple):
@@ -59,15 +58,17 @@ def matrix_cases() -> List[Case]:
 
 def instantiation(case: Case, consts: Dict[str, int]) -> Tuple[str, Tuple[int, ...]]:
     """The kernel template and its arguments that ``gaccum_abi.cu`` launches for ``case``; ``consts`` maps the
-    kernels' mode constants (kLs*, kLamb*) to their values."""
+    kernels' mode constants (MODE_ARG) to their values.  With or without gradients, a case runs the same kernel: a
+    tensor without a gradient is one whose gradient pointer is NULL."""
     cap, h, _ = LAYOUTS[case.layout]
-    g, h, e = int(case.has_g), int(h), int(case.ema)
+    h, e = int(h), int(case.ema)
+    mode = consts[MODE_ARG[case.mode]]
     if case.variant == "lamb":
-        return "lamb_apply_kernel", (g, cap, consts[LAMB_MODE_ARG[case.mode]], h, e)
+        return "lamb_apply_kernel", (cap, mode, h, e)
     v = 0 if case.variant == "adamw" else 1
     if case.mode == "noclip":
-        return "apply_kernel", (v, g, cap, h, e)
-    return "apply_clip_kernel", (v, g, cap, consts[CLIP_LS_ARG[case.mode]], h, e)
+        return "apply_kernel", (v, cap, h, e)
+    return "apply_clip_kernel", (v, cap, mode, h, e)
 
 
 # ---- the schedules ----------------------------------------------------------------------------------------------------
@@ -84,7 +85,7 @@ class Schedule:
         self.sms = sms
 
     def clip_groups(self, nt: int) -> int:
-        """G: the clip-apply's grid is min(sms, ceil(nt / 3)) CTAs of 3 groups (gaccum_abi.cu launch_apply_clip)."""
+        """G: the clip-apply's grid is min(sms, ceil(nt / 3)) CTAs of 3 groups (gaccum_abi.cu launch_apply)."""
         return self.GROUPS * max(1, min(self.sms, -(-nt // self.GROUPS)))
 
     def pool_lo(self, nt: int, ema: bool) -> int:

@@ -3,7 +3,7 @@
 One case per dispatch key of gaccum_abi.cu: optimizer (AdamWeightDecay, Adam, LAMB) x mode (no clip, clip, loss scaling
 without and with clip) x with gradients (``run``) or without (``accumulate_only`` + ``apply_only(None)``) x layout and
 dtype (packed CAP 0 fp32; CAP 256 and 1920 in fp32, bf16, fp16) x EMA off / on -- 336 cases, which between them launch
-each of the library's 240 apply instantiations (tests/test_kernel_inventory.py checks that mapping against the binary).
+each of the library's 120 apply instantiations (tests/test_kernel_inventory.py checks that mapping against the binary).
 
 Each case trains a small model with tails, a multi-tile tensor, one element, a tensor without a gradient and a
 zero-element tensor (CAP 1920: plus 300 tiny tensors) at N = 3 for ten micro-steps -- four applied windows.  Loss-scaled

@@ -73,7 +73,7 @@ def test_schedule_constants_match_the_kernels():
     assert (c["kClipSmemBytes"] - ring_bytes) // (c["kGroups"] * c["kTile"] * 4) == Schedule.STASH_TILES[True]
 
 
-def test_matrix_covers_every_apply_instantiation():
+def test_matrix_covers_every_apply_instantiation_with_or_without_gradients():
     consts = _constants()
     cases = matrix_cases()
     assert len(cases) == 336 and len(set(cases)) == 336
@@ -82,8 +82,11 @@ def test_matrix_covers_every_apply_instantiation():
     built = [e for e in entries if e[0] in APPLY_KERNELS]
     assert len(built) == len(set(built)), "an apply instantiation appears twice"
     assert set(built) == claimed, (sorted(set(built) - claimed), sorted(claimed - set(built)))
-    # bf16 and fp16 share their instantiations: 5 (CAP, H) pairs x 2 (EMA) x (4 + 12 + 8) kernels
-    assert len(claimed) == 5 * 2 * 24 == 240
+    # bf16 and fp16 share their instantiations: 5 (CAP, H) pairs x 2 (EMA) x (2 + 6 + 4) kernels
+    assert len(claimed) == 5 * 2 * 12 == 120
+    # a case without gradients runs the kernel of the same case with them
+    for c in cases:
+        assert instantiation(c, consts) == instantiation(c._replace(has_g=not c.has_g), consts)
     others = {}
     for name, _ in entries:
         if name not in APPLY_KERNELS:
@@ -92,11 +95,11 @@ def test_matrix_covers_every_apply_instantiation():
 
 
 @pytest.mark.parametrize("layout", sorted(LAYOUTS))
-def test_every_layout_reaches_its_own_instantiations(layout):
+def test_every_layout_reaches_its_own_24_instantiations(layout):
     """Different layouts of one (CAP, H) pair -- bf16 and fp16 -- map to the same kernels, all others to disjoint ones."""
     consts = _constants()
     mine = {instantiation(c, consts) for c in matrix_cases() if c.layout == layout}
-    assert len(mine) == 48
+    assert len(mine) == 24
     for other in LAYOUTS:
         theirs = {instantiation(c, consts) for c in matrix_cases() if c.layout == other}
         if LAYOUTS[other][:2] == LAYOUTS[layout][:2]:
