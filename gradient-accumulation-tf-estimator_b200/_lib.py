@@ -2,6 +2,7 @@
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 import re
 from typing import List, Optional, Sequence
@@ -163,6 +164,7 @@ def _load():
         "gaccum_read_trust_ratios": (C.c_int, [vp, vp, vp]),
         "gaccum_plan_set_ema": (C.c_int, [vp, C.POINTER(EmaConfig), vp, vp]),
         "gaccum_ema_init": (C.c_int, [vp, vp, i64, vp]),
+        "gaccum_plan_set_lr_multipliers": (C.c_int, [vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -231,6 +233,21 @@ def adaptation_mask(names: Sequence[str], exclude: Optional[Sequence[str]]) -> L
     is found (Python ``re.search``) in its name with a trailing ``:<digits>`` stripped.  Unlike the decay mask it does not
     depend on the weight-decay rate."""
     return [not any(re.search(r, _variable_name(n)) is not None for r in exclude or ()) for n in names]
+
+
+def lr_multiplier_array(mult: Sequence[float], num_tensors: int):
+    """The T per-tensor learning-rate multipliers as the kernels see them: an np.float32 array, each value rounded to
+    fp32 once.  ValueError for the wrong length, or a value that is negative, not finite, or overflows fp32."""
+    import numpy as np
+    vals = [float(x) for x in mult]
+    if len(vals) != num_tensors:
+        raise ValueError(f"{len(vals)} learning-rate multipliers for {num_tensors} tensors")
+    with np.errstate(over="ignore"):
+        out = np.array(vals, dtype=np.float64).astype(np.float32)
+    for i, (x, x32) in enumerate(zip(vals, out)):
+        if not (math.isfinite(x) and x >= 0.0 and np.isfinite(x32)):
+            raise ValueError(f"learning-rate multiplier {i} is {x!r}: it must be finite and >= 0, and fit fp32")
+    return out
 
 
 def decay_mask_c(names: Sequence[str], weight_decay_rate: float,
@@ -340,6 +357,12 @@ class Plan:
 
     def ema_init(self, device_state: int, num_updates: int = 0, stream: int = 0) -> None:
         _check(_load().gaccum_ema_init(self._h, device_state or None, int(num_updates), stream))
+
+    def set_lr_multipliers(self, mult: Sequence[float]) -> None:
+        """Tensor t trains with lr_t = fp32(lr * mult[t]) (before the first compute call; default 1.0 everywhere)."""
+        m32 = lr_multiplier_array(mult, self.T)
+        arr = (C.c_float * max(self.T, 1))(*m32.tolist())
+        _check(_load().gaccum_plan_set_lr_multipliers(self._h, C.cast(arr, C.c_void_p)))
 
     def close(self) -> None:
         if getattr(self, "_h", None):

@@ -89,6 +89,11 @@ struct gaccum_plan {
   float* ema_slab = nullptr;
   gaccum_ema_state* ema_state = nullptr;
   unsigned int* d_ema_done = nullptr;      // apply_kernel: CTAs of the launch that are through (zero between launches)
+  // per-tensor learning-rate multipliers (gaccum_plan_set_lr_multipliers): 1.0 unless set, the device copy exists on every
+  // device plan because every apply kernel reads it
+  bool lr_mult_set = false;
+  std::vector<float> lr_mult;
+  float* d_lr_mult = nullptr;
   std::mutex mu;
   std::map<const void*, int> grid_cache;   // cooperative kernel -> CTAs that fit on one SM (fit)
 };
@@ -279,6 +284,17 @@ static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, f
   prm.ema.done = pl->d_ema_done;
   prm.ema.decay = (float)pl->ema_cfg.decay;
   prm.ema.num_updates = pl->ema_cfg.num_updates;
+  prm.lrm.mult = pl->d_lr_mult;
+  prm.lrm.bc2 = 1.0f;
+  prm.lrm.bc1 = 1.0f;
+  if (a && pl->hp.variant == GACCUM_ADAM) {
+    // make_scalars' t2 and t4: the alpha of a tile is (lr_t * bc2) / bc1
+    volatile float t1 = 1.0f - a->beta2_power;
+    volatile float t2 = sqrtf(t1);
+    volatile float t4 = 1.0f - a->beta1_power;
+    prm.lrm.bc2 = t2;
+    prm.lrm.bc1 = t4;
+  }
 }
 
 template <int CAP>
@@ -352,7 +368,7 @@ static int check_args(const gaccum_step_args* a) {
 
 static void free_plan_device(gaccum_plan* pl) {
   cudaFree(pl->d_tiles); cudaFree(pl->d_partials); cudaFree(pl->d_stats); cudaFree(pl->d_dp_sync); cudaFree(pl->d_barrier); cudaFree(pl->d_counters);
-  cudaFree(pl->d_adapt); cudaFree(pl->d_lamb_acc); cudaFree(pl->d_ratios); cudaFree(pl->d_ema_done);
+  cudaFree(pl->d_adapt); cudaFree(pl->d_lamb_acc); cudaFree(pl->d_ratios); cudaFree(pl->d_ema_done); cudaFree(pl->d_lr_mult);
 #ifdef GACCUM_EXPERIMENTS
   cudaFree(pl->d_debug);
 #endif
@@ -448,6 +464,7 @@ int gaccum_plan_create(gaccum_plan** out, int32_t T, const int64_t* numels, cons
   pl->decay.assign((size_t)T, 0);
   if (hp->variant != GACCUM_ADAM && decay) pl->decay.assign(decay, decay + T);
   if (hp->variant == GACCUM_LAMB) pl->adapt.assign((size_t)T, 1);   // every tensor adapts unless told otherwise
+  pl->lr_mult.assign((size_t)T, 1.0f);
   if (int rc = build_layout(pl)) { delete pl; return rc; }
   pl->device = -1;
   if (device >= 0) {
@@ -478,6 +495,9 @@ int gaccum_plan_create(gaccum_plan** out, int32_t T, const int64_t* numels, cons
     if (e == cudaSuccess) e = cudaMemset(pl->d_stats, 0, sizeof(gaccum_stats));
     if (e == cudaSuccess) e = cudaMalloc(&pl->d_ema_done, sizeof(unsigned int));
     if (e == cudaSuccess) e = cudaMemset(pl->d_ema_done, 0, sizeof(unsigned int));
+    if (e == cudaSuccess) e = cudaMalloc(&pl->d_lr_mult, (size_t)std::max(1, T) * sizeof(float));
+    if (e == cudaSuccess && T > 0)
+      e = cudaMemcpy(pl->d_lr_mult, pl->lr_mult.data(), (size_t)T * sizeof(float), cudaMemcpyHostToDevice);
     if (hp->variant == GACCUM_LAMB) {
       const size_t nt = (size_t)std::max(1, T);
       const std::vector<float> ones(nt, 1.0f);
@@ -634,6 +654,28 @@ int gaccum_ema_init(gaccum_plan* pl, gaccum_ema_state* device_state, int64_t num
 
 static int refuse_ema(const gaccum_plan* pl, const char* what) {
   return pl && pl->ema_on ? fail(GACCUM_EINVAL, "%s does not support a moving average (gaccum_plan_set_ema)", what) : GACCUM_OK;
+}
+
+int gaccum_plan_set_lr_multipliers(gaccum_plan* pl, const float* mult) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (!mult && pl->T > 0) return fail(GACCUM_EINVAL, "mult is NULL");
+  if (pl->computed) return fail(GACCUM_EINVAL, "learning-rate multipliers can only be set before the plan's first compute call");
+  for (int32_t t = 0; t < pl->T; ++t)
+    if (!(std::isfinite(mult[t]) && mult[t] >= 0.0f))
+      return fail(GACCUM_EINVAL, "mult[%d] = %g: learning-rate multipliers must be finite and >= 0", t, (double)mult[t]);
+  if (pl->device >= 0 && pl->T > 0) {
+    DeviceGuard guard(pl->device);
+    CUDA_TRY(cudaMemcpy(pl->d_lr_mult, mult, sizeof(float) * (size_t)pl->T, cudaMemcpyHostToDevice));
+  }
+  pl->lr_mult.assign(mult, mult + pl->T);
+  pl->lr_mult_set = true;
+  return GACCUM_OK;
+}
+
+static int refuse_lr_mult(const gaccum_plan* pl, const char* what) {
+  return pl && pl->lr_mult_set
+             ? fail(GACCUM_EINVAL, "%s does not support learning-rate multipliers (gaccum_plan_set_lr_multipliers)", what)
+             : GACCUM_OK;
 }
 
 static int refuse_half(const gaccum_plan* pl, const char* what) {
@@ -813,6 +855,7 @@ int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* co
   if (int rc = refuse_lamb(pl, "the fused data-parallel apply")) return rc;
   if (int rc = refuse_half(pl, "the fused data-parallel apply")) return rc;
   if (int rc = refuse_ema(pl, "the fused data-parallel apply")) return rc;
+  if (int rc = refuse_lr_mult(pl, "the fused data-parallel apply")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (comm->world < 2 || comm->world > GACCUM_MAX_RANKS || comm->rank < 0 || comm->rank >= comm->world)
     return fail(GACCUM_EINVAL, "world must be 2..%d and 0 <= rank < world", GACCUM_MAX_RANKS);
@@ -839,6 +882,7 @@ int gaccum_step_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* con
   if (int rc = refuse_lamb(pl, "the fused data-parallel step")) return rc;
   if (int rc = refuse_half(pl, "the fused data-parallel step")) return rc;
   if (int rc = refuse_ema(pl, "the fused data-parallel step")) return rc;
+  if (int rc = refuse_lr_mult(pl, "the fused data-parallel step")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (int rc = check_args(a)) return rc;
   if (!grads) return fail(GACCUM_EINVAL, "grads is NULL");
@@ -922,6 +966,7 @@ int gaccum_host_session_create(gaccum_host_session** out, gaccum_plan* pl) {
   if (int rc = refuse_half(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_lamb(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_ema(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse_lr_mult(pl, "the host-buffer session")) return rc;
   if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): libgaccum has no CPU fallback, a CUDA device is required");
   DeviceGuard guard(pl->device);
   gaccum_host_session* s = new (std::nothrow) gaccum_host_session();
@@ -1033,6 +1078,7 @@ int gaccum_step_host(gaccum_host_session* s, const float* const* host_grads, flo
   if (int rc = refuse_half(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_lamb(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_ema(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse_lr_mult(pl, "the host-buffer session")) return rc;
   DeviceGuard guard(pl->device);
   const int b = (int)(s->calls & 1);
   ++s->calls;

@@ -137,6 +137,15 @@ struct EmaParams {
   int32_t num_updates;     // 1: d = min(decay, (1 + n) / (10 + n))
 };
 
+// Per-tensor learning-rate multipliers (gaccum_plan_set_lr_multipliers).  Every plan has the table (1.0 unless set), so
+// no kernel is specialised on it: each apply kernel reads mult[t] once per tile and uses the tile's lr_t = lr * mult[t]
+// -- GACCUM_ADAM: alpha_t = (lr_t * bc2) / bc1, make_scalars' op order -- where Scalars' lr / alpha would go.
+struct LrMultParams {
+  const float* mult;       // num_tensors
+  float bc2;               // GACCUM_ADAM: sqrtf(1 - beta2_power) of this step (loss-scaled launches use the device block's)
+  float bc1;               // GACCUM_ADAM: 1 - beta1_power
+};
+
 // Every kernel's parameter block.  Each feature's parameters follow those of the features before it, so adding them
 // moved no member an existing kernel reads.
 template <int CAP>
@@ -158,6 +167,7 @@ struct KernelParams {
   HalfParams half;      // kernels with H = true only
   LambParams lamb;      // lamb_apply_kernel only
   EmaParams ema;        // kernels with EMA = true only
+  LrMultParams lrm;     // apply kernels only
 };
 static_assert(sizeof(KernelParams<1920>) <= 32764, "kernel parameters must fit the 32 KB limit");
 
@@ -316,44 +326,71 @@ __device__ __forceinline__ float normalize(float a, float nf, float inv_nf) {
   return inv_nf != 0.f ? __fmul_rn(a, inv_nf) : __fdiv_rn(a, nf);
 }
 
+// rate: the learning rate (VARIANT 0) or alpha (VARIANT 1) the update uses -- Scalars' own, or the tile's lr_t / alpha_t
+// (LrMultParams)
 template <int VARIANT>
 __device__ __forceinline__ void adam_elem(float c, float& p, float& m, float& v, bool decay,
-                                          const Scalars& sc) {
+                                          const Scalars& sc, const float& rate) {
   if constexpr (VARIANT == 0) {
     // optimization.py:151-171
     const float m2 = __fadd_rn(__fmul_rn(sc.b1, m), __fmul_rn(sc.omb1, c));
     const float v2 = __fadd_rn(__fmul_rn(sc.b2, v), __fmul_rn(sc.omb2, __fmul_rn(c, c)));
     float u = __fdiv_rn(m2, __fadd_rn(__fsqrt_rn(v2), sc.eps));
     if (decay) u = __fadd_rn(u, __fmul_rn(sc.wd, p));
-    p = __fsub_rn(p, __fmul_rn(sc.lr, u));
+    p = __fsub_rn(p, __fmul_rn(rate, u));
     m = m2;
     v = v2;
   } else {
     // TF1 ApplyAdam: m += (g-m)(1-b1); v += (g*g-v)(1-b2); var -= (m*alpha)/(sqrt(v)+eps)
     const float m2 = __fadd_rn(m, __fmul_rn(__fsub_rn(c, m), sc.omb1));
     const float v2 = __fadd_rn(v, __fmul_rn(__fsub_rn(__fmul_rn(c, c), v), sc.omb2));
-    p = __fsub_rn(p, __fdiv_rn(__fmul_rn(m2, sc.alpha), __fadd_rn(__fsqrt_rn(v2), sc.eps)));
+    p = __fsub_rn(p, __fdiv_rn(__fmul_rn(m2, rate), __fadd_rn(__fsqrt_rn(v2), sc.eps)));
     m = m2;
     v = v2;
   }
 }
+template <int VARIANT>
+__device__ __forceinline__ const float& sc_rate(const Scalars& sc) { return VARIANT == 0 ? sc.lr : sc.alpha; }
+
+// The tile's rate for tensor multiplier `mult`: lr_t = lr * mult, one correctly rounded multiply; GACCUM_ADAM:
+// alpha_t = (lr_t * sqrt(1 - b2^t)) / (1 - b1^t), with bc2 and bc1 those two bias-correction terms.  mult == 1 gives
+// Scalars' lr / alpha bit for bit.
+template <int VARIANT>
+__device__ __forceinline__ float tile_rate(const float lr, const float mult, const float bc2, const float bc1) {
+  const float lr_t = __fmul_rn(lr, mult);
+  if constexpr (VARIANT == 0) return lr_t;
+  else return __fdiv_rn(__fmul_rn(lr_t, bc2), bc1);
+}
+__device__ __forceinline__ float tensor_mult(const LrMultParams& lrm, const TileDesc& d) {
+  return __ldg(lrm.mult + (d.tensor_flags & 0x7fffffffu));
+}
 
 // optimization.py:83-85: c = a/N, times the clip scale s if `scaled` (never a multiply by 1: it could change a NaN's
-// payload), then one Adam step of p, m, v
+// payload), then one Adam step of p, m, v with `rate` (default: Scalars' lr / alpha)
+template <int VARIANT>
+__device__ __forceinline__ void update_elem(float a, bool scaled, float s, float& p, float& m, float& v, bool decay,
+                                            const Scalars& sc, const float& rate) {
+  float c = normalize(a, sc.nf, sc.inv_nf);
+  if (scaled) c = __fmul_rn(c, s);
+  adam_elem<VARIANT>(c, p, m, v, decay, sc, rate);
+}
 template <int VARIANT>
 __device__ __forceinline__ void update_elem(float a, bool scaled, float s, float& p, float& m, float& v, bool decay,
                                             const Scalars& sc) {
-  float c = normalize(a, sc.nf, sc.inv_nf);
-  if (scaled) c = __fmul_rn(c, s);
-  adam_elem<VARIANT>(c, p, m, v, decay, sc);
+  update_elem<VARIANT>(a, scaled, s, p, m, v, decay, sc, sc_rate<VARIANT>(sc));
+}
+template <int VARIANT>
+__device__ __forceinline__ void update_vec(const float4 a, bool scaled, float s, float4& p, float4& m, float4& v, bool decay,
+                                           const Scalars& sc, const float& rate) {
+  update_elem<VARIANT>(a.x, scaled, s, p.x, m.x, v.x, decay, sc, rate);
+  update_elem<VARIANT>(a.y, scaled, s, p.y, m.y, v.y, decay, sc, rate);
+  update_elem<VARIANT>(a.z, scaled, s, p.z, m.z, v.z, decay, sc, rate);
+  update_elem<VARIANT>(a.w, scaled, s, p.w, m.w, v.w, decay, sc, rate);
 }
 template <int VARIANT>
 __device__ __forceinline__ void update_vec(const float4 a, bool scaled, float s, float4& p, float4& m, float4& v, bool decay,
                                            const Scalars& sc) {
-  update_elem<VARIANT>(a.x, scaled, s, p.x, m.x, v.x, decay, sc);
-  update_elem<VARIANT>(a.y, scaled, s, p.y, m.y, v.y, decay, sc);
-  update_elem<VARIANT>(a.z, scaled, s, p.z, m.z, v.z, decay, sc);
-  update_elem<VARIANT>(a.w, scaled, s, p.w, m.w, v.w, decay, sc);
+  update_vec<VARIANT>(a, scaled, s, p, m, v, decay, sc, sc_rate<VARIANT>(sc));
 }
 
 __device__ __forceinline__ float4 add_rn(const float4 a, const float4 b) {
@@ -400,11 +437,11 @@ __device__ __forceinline__ float mode_c(float a, float s, float inv_s, const Sca
 // call site, nvcc schedules the AdamWeightDecay instantiations differently (more instructions, different registers).
 template <int VARIANT, int MODE>
 __device__ __forceinline__ void adam_vec(const float4 a, float s, float inv_s, float4& p, float4& m, float4& v, bool decay,
-                                         const Scalars& sc) {
-  adam_elem<VARIANT>(mode_c<MODE>(a.x, s, inv_s, sc), p.x, m.x, v.x, decay, sc);
-  adam_elem<VARIANT>(mode_c<MODE>(a.y, s, inv_s, sc), p.y, m.y, v.y, decay, sc);
-  adam_elem<VARIANT>(mode_c<MODE>(a.z, s, inv_s, sc), p.z, m.z, v.z, decay, sc);
-  adam_elem<VARIANT>(mode_c<MODE>(a.w, s, inv_s, sc), p.w, m.w, v.w, decay, sc);
+                                         const Scalars& sc, const float& rate) {
+  adam_elem<VARIANT>(mode_c<MODE>(a.x, s, inv_s, sc), p.x, m.x, v.x, decay, sc, rate);
+  adam_elem<VARIANT>(mode_c<MODE>(a.y, s, inv_s, sc), p.y, m.y, v.y, decay, sc, rate);
+  adam_elem<VARIANT>(mode_c<MODE>(a.z, s, inv_s, sc), p.z, m.z, v.z, decay, sc, rate);
+  adam_elem<VARIANT>(mode_c<MODE>(a.w, s, inv_s, sc), p.w, m.w, v.w, decay, sc, rate);
 }
 
 // tf.clip_by_global_norm (TF 1.15): scale = clip * min(1/gn, 1/clip) + (gn - gn)
@@ -508,6 +545,7 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
   if constexpr (H) { q = model_ptr(prm, d); bf16 = prm.half.bf16 != 0; }
   const bool decay = (d.tensor_flags >> 31) != 0;
   const Scalars& sc = prm.sc;
+  const float rate = tile_rate<VARIANT>(sc.lr, tensor_mult(prm.lrm, d), prm.lrm.bc2, prm.lrm.bc1);
   float4* a4 = reinterpret_cast<float4*>(a);
   float4* m4 = reinterpret_cast<float4*>(m);
   float4* v4 = reinterpret_cast<float4*>(v);
@@ -524,7 +562,7 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
             [] {},
             [&](int u, uint32_t i) {
               if (g.g) va[u] = add_rn(va[u], vg[u]);
-              update_vec<VARIANT>(va[u], false, 0.f, vp[u], vm[u], vv[u], decay, sc);
+              update_vec<VARIANT>(va[u], false, 0.f, vp[u], vm[u], vv[u], decay, sc, rate);
               __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
               if constexpr (H) store_model4(q, i, vp[u], bf16);
@@ -533,7 +571,7 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
             [&](uint32_t i) {
               float ax = a[i], px = p[i], mx = m[i], vx = v[i];
               if (g.g) ax = __fadd_rn(ax, g.elem(i));
-              update_elem<VARIANT>(ax, false, 0.f, px, mx, vx, decay, sc);
+              update_elem<VARIANT>(ax, false, 0.f, px, mx, vx, decay, sc, rate);
               p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
               if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
               if constexpr (EMA) e[i] = ema_elem(e[i], px, ema_c);
@@ -642,7 +680,9 @@ constexpr int kTicketBatch = 4;                   // pass-1 tickets a producer d
 struct __align__(16) SlotMeta {
   TileDesc d;          // len == 0: end of the pass
   uint32_t stash_slot; // pass 2: a' is parked in this stash slot of the group (kNoStash: it is in the slot's 4th quarter / in global memory)
+  float rate;          // pass 2: the tile's lr_t (AdamWeightDecay) or alpha_t (Adam), tile_rate
 };
+static_assert(sizeof(SlotMeta) == 32, "the rate sits in what was padding: static shared memory is unchanged");
 // exact accumulation of non-negative doubles: 68 bins of 32 payload bits in 64-bit containers cover the whole
 // binary64 range (2^-1074 .. 2^1024); a container overflows only after 2^31 additions
 constexpr int kAccBins = 68;
@@ -878,13 +918,15 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
 
 // ---- pass 2, consumer side: one tile out of slot [p | m | v | a']; a' from the slot or from the stash ----
 // The caller has waited on the slot's `full` barrier (it had to, to learn which tile this is).
-// Loss-scaled: `sc` carries the alpha computed from the device's beta powers, and a skipped window (`skip`) stores
-// a = 0 and nothing else.  H: p is the master slab, and the model copy is stored after it (not on a skipped window).
+// `rate` is the tile's lr_t / alpha_t (SlotMeta::rate; loss-scaled Adam: from the device's beta powers).
+// Loss-scaled: a skipped window (`skip`) stores a = 0 and nothing else.  H: p is the master slab, and the model copy is
+// stored after it (not on a skipped window).
 // EMA: the slot is [p | m | v | a' | e], and e - (e - p) * c is stored after p (not on a skipped window).
 template <int VARIANT, int MODE, bool H, int CAP, bool EMA = false>
 __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelParams<CAP>& prm, const float s, const float4* slot,
-                                             uint64_t* empty, const float4* const stash, const Scalars& sc, const float inv_s,
+                                             uint64_t* empty, const float4* const stash, const float rate, const float inv_s,
                                              const bool skip, float* ema = nullptr, const float ema_c = 0.f) {
+  const Scalars& sc = prm.sc;
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
   float* __restrict__ m = prm.m + soff;
@@ -911,7 +953,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
             [&] { __syncwarp(); if ((threadIdx.x & 31) == 0) mbar_arrive(empty); },
             [&](int u, uint32_t i) {
               if (write) {
-                adam_vec<VARIANT, MODE>(va[u], s, inv_s, vp[u], vm[u], vv[u], decay, sc);
+                adam_vec<VARIANT, MODE>(va[u], s, inv_s, vp[u], vm[u], vv[u], decay, sc, rate);
                 __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
                 if constexpr (H) store_model4(q, i, vp[u], bf16);
                 if constexpr (EMA) __stcs(e4 + i, ema_vec(ve[u], vp[u], ema_c));
@@ -921,7 +963,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
             [&](uint32_t i) {
               if (write) {
                 float px = p[i], mx = m[i], vx = v[i];
-                adam_elem<VARIANT>(mode_c<MODE>(a[i], s, inv_s, sc), px, mx, vx, decay, sc);
+                adam_elem<VARIANT>(mode_c<MODE>(a[i], s, inv_s, sc), px, mx, vx, decay, sc, rate);
                 p[i] = px; m[i] = mx; v[i] = vx;
                 if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
                 if constexpr (EMA) e[i] = ema_elem(e[i], px, ema_c);
@@ -966,7 +1008,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   __shared__ unsigned int s_nonfinite;
   __shared__ float s_bcast[2];
   __shared__ LossScaleState s_ls;        // loss-scaled: the state as this launch found it
-  __shared__ Scalars s_sc;               // loss-scaled GACCUM_ADAM: prm.sc with alpha from the device's beta powers
+  __shared__ float s_bc[2];              // loss-scaled GACCUM_ADAM: bc2, bc1 (LrMultParams) from the device's beta powers
   __shared__ int s_skip;
   __shared__ uint32_t s_set;
   __shared__ __align__(8) uint64_t s_full1[kGroups][kP1Slots], s_empty1[kGroups][kP1Slots];
@@ -1016,10 +1058,9 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     if constexpr (loss_scaled(MODE)) {
       ls_load(prm.ls.state, s_ls);
       if constexpr (VARIANT == 1) {
-        // make_scalars' op order: lr * sqrt(1 - b2^t) / (1 - b1^t), one rounding per op
-        s_sc = prm.sc;
-        s_sc.alpha = __fdiv_rn(__fmul_rn(prm.sc.lr, __fsqrt_rn(__fsub_rn(1.0f, s_ls.beta2_power))),
-                               __fsub_rn(1.0f, s_ls.beta1_power));
+        // make_scalars' terms: alpha_t = (lr_t * sqrt(1 - b2^t)) / (1 - b1^t), one rounding per op (tile_rate)
+        s_bc[0] = __fsqrt_rn(__fsub_rn(1.0f, s_ls.beta2_power));
+        s_bc[1] = __fsub_rn(1.0f, s_ls.beta1_power);
       }
     }
     if constexpr (EMA) ema_load(*ema, *s_ema);
@@ -1134,6 +1175,10 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
       RingPos rp;
       int jb = 0;
       bool past_barrier = false;
+      // the bias corrections of the tiles' alpha_t (GACCUM_ADAM): the step's, or under loss scaling the device block's,
+      // which thread 0 wrote before the set-up barrier
+      float bc2 = prm.lrm.bc2, bc1 = prm.lrm.bc1;
+      if constexpr (loss_scaled(MODE) && VARIANT == 1) { bc2 = s_bc[0]; bc1 = s_bc[1]; }
       const unsigned long long pool_n = (unsigned long long)max(0, nt - pool_lo);
       while (true) {
         int tile;
@@ -1166,6 +1211,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         SlotMeta* meta = &s_meta2[grp][rp.slot];
         meta->d = d;
         meta->stash_slot = in_stash ? stash_slot : kNoStash;
+        meta->rate = tile_rate<VARIANT>(prm.sc.lr, tensor_mult(prm.lrm, d), bc2, bc1);
         if (nvec > 0) {
           const size_t soff = (size_t)d.soff32 * kSlabAlign;
           float4* dst = ring + (size_t)rp.slot * kP2SlotVecs;
@@ -1268,7 +1314,6 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     const float s = s_bcast[0];
     bool skip = false;
     if constexpr (loss_scaled(MODE)) skip = s_skip != 0;
-    const Scalars& sc = (loss_scaled(MODE) && VARIANT == 1) ? s_sc : prm.sc;
     // ---- pass 2: whatever tiles the producer hands over, until its end marker ----
     {
       RingPos rp;
@@ -1279,10 +1324,10 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         const float4* const st = meta.stash_slot != kNoStash ? stash + (size_t)meta.stash_slot * (kTile / 4) : nullptr;
         if constexpr (EMA) {
           update_tile2<VARIANT, MODE, H, CAP, true>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot],
-                                                    st, sc, inv_s, skip, ema->slab, s_ema->c);
+                                                    st, meta.rate, inv_s, skip, ema->slab, s_ema->c);
         } else {
-          update_tile2<VARIANT, MODE, H>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st, sc, inv_s,
-                                      skip);
+          update_tile2<VARIANT, MODE, H>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st, meta.rate,
+                                      inv_s, skip);
         }
         rp.advance(kP2Slots);
       }

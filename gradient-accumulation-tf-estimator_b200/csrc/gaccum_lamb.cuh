@@ -13,7 +13,8 @@
 //            another tensor -- the sums do not depend on which CTA reduced which tile
 //   barrier  one warp per tensor turns its two sums into r, stored in the plan's ratio array
 //   barrier
-//   phase 3  read p and u, store p - (r*lr)*u (fp32, or the master weights plus their RNE model copy) and a = +0
+//   phase 3  read p and u, store p - (r*lr_t)*u (fp32, or the master weights plus their RNE model copy) and a = +0;
+//            lr_t = lr * mult[t], the tensor's learning-rate multiplier (LrMultParams), read once per tile
 //
 // A skipped window (loss scaling) runs neither phase 2 nor the ratio step: it stores a = +0 and nothing else, so the
 // ratios of the last applied window stay.  Bytes: phase 2 reads a', p, m, v (and G) and writes m, v, u; phase 3 reads
@@ -347,7 +348,9 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   // ---- phase 3: the parameters and a = +0 ----
   for (int t = t_lo; t < t_hi; ++t) {
     const TileDesc d = prm.tiles[t];
-    const float rlr = skip ? 0.f : __fmul_rn(__ldcg(&lb.ratios[d.tensor_flags & 0x7fffffffu]), prm.sc.lr);   // ratio * lr first
+    // ratio * lr_t first, lr_t = lr * mult[t] (LrMultParams)
+    const float rlr = skip ? 0.f : __fmul_rn(__ldcg(&lb.ratios[d.tensor_flags & 0x7fffffffu]),
+                                             tile_rate<0>(prm.sc.lr, tensor_mult(prm.lrm, d), 0.f, 1.f));
     if constexpr (EMA) lamb_write_tile<H, CAP, true>(d, prm, rlr, !skip, prm.ema.slab, s_ema->c);
     else lamb_write_tile<H>(d, prm, rlr, !skip);
   }

@@ -89,11 +89,14 @@ class FusedDataParallelTrainOp:
 
     def __init__(self, params: Sequence[torch.Tensor], names: Sequence[str], hp, accum_n: int, lr_fn,
                  process_group=None, exclude_from_weight_decay=("LayerNorm", "layer_norm", "bias"),
-                 global_step: int = 0, loss_scale=None, ema=None):
+                 global_step: int = 0, loss_scale=None, ema=None, lr_multipliers=None):
         import torch.distributed._symmetric_memory as symm
         from .train_op import GaccumTrainOp
         if ema is not None:
             raise ValueError("the fused data-parallel train op does not keep a moving average of the weights; "
+                             "use dp_mode='allreduce'")
+        if lr_multipliers is not None:
+            raise ValueError("the fused data-parallel train op does not support per-tensor learning-rate multipliers; "
                              "use dp_mode='allreduce'")
         if loss_scale is not None:
             raise ValueError("the fused data-parallel train op does not support loss scaling; use dp_mode='allreduce'")

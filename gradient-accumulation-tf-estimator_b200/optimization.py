@@ -19,7 +19,8 @@ There is no CPU fallback: variables must be CUDA tensors.
 from __future__ import annotations
 
 import os
-from typing import Callable, Iterable, List, Optional, Sequence, Tuple, Union
+import re
+from typing import Callable, Dict, Iterable, List, Optional, Sequence, Tuple, Union
 
 import torch
 
@@ -39,6 +40,9 @@ optimizer_type = "adam"
 # The decay of an exponential moving average of the weights (ExponentialMovingAverage), off by default; create_optimizer
 # reads it.
 moving_average_decay: Optional[float] = None
+# ELECTRA's layer-wise learning-rate decay (layerwise_lr_multipliers), off by default; create_optimizer reads it and takes
+# the number of encoder layers from the trainable variables' names.
+layerwise_lr_decay: Optional[float] = None
 
 LossLike = Union[torch.Tensor, Callable[[], torch.Tensor]]
 LrLike = Union[float, Callable[[int], float]]
@@ -48,19 +52,60 @@ def _lr_callable(lr: LrLike) -> Callable[[int], float]:
     return lr if callable(lr) else (lambda step, _v=float(lr): _v)
 
 
+def layerwise_lr_multipliers(layer_decay: float, num_layers: int) -> Dict[str, float]:
+    """ELECTRA's layer-wise learning-rate decay (``_get_layer_lrs``) as multipliers of the scheduled lr, keyed by
+    variable-name substring: the embeddings get ``layer_decay ** (L + 2)``, encoder layer i ``layer_decay ** (L + 1 - i)``
+    and the task head (``task_specific/``) 1.  The powers are Python doubles; each is rounded to fp32 once, as TF
+    converts the constant it multiplies the learning rate by."""
+    L = int(num_layers)
+    depths = {"/embeddings/": 0, "/embeddings_project/": 0, "task_specific/": L + 2}
+    for i in range(L):
+        depths[f"encoder/layer_{i}/"] = i + 1
+    return {key: float(layer_decay) ** (L + 2 - depth) for key, depth in depths.items()}
+
+
+def lr_multipliers_for(names: Sequence[str], multipliers: Optional[Dict[str, float]]) -> Optional[List[float]]:
+    """The per-tensor list of ``multipliers`` (ELECTRA's key -> rate dict, as multipliers of the scheduled lr): each
+    variable takes the multiplier of the key that is a substring of its name.  Two deliberate departures from ELECTRA:
+    a variable that matches no key trains at the scheduled lr (1.0) -- ELECTRA raises, so BERT's pooler and
+    ``output_weights`` would each need a key -- and a variable that matches two keys raises ValueError -- ELECTRA would
+    silently update it once per key.  None stays None: the train op then keeps a single learning rate."""
+    if multipliers is None:
+        return None
+    out = []
+    for name in names:
+        keys = [k for k in multipliers if k in name]
+        if len(keys) > 1:
+            raise ValueError(f"variable {name!r} matches more than one learning-rate key: {keys}")
+        out.append(float(multipliers[keys[0]]) if keys else 1.0)
+    return out
+
+
+def _num_encoder_layers(names: Sequence[str]) -> int:
+    """1 + the largest i of an ``encoder/layer_<i>/`` in the names."""
+    layers = [int(m.group(1)) for n in names for m in [re.search(r"encoder/layer_(\d+)/", n)] if m is not None]
+    if not layers:
+        raise ValueError("layerwise_lr_decay is set, but no trainable variable is named like encoder/layer_<i>/")
+    return max(layers) + 1
+
+
 def bert_learning_rate(init_lr: float, num_train_steps: int, num_warmup_steps: Optional[int]) -> Callable[[int], float]:
     """optimization.py:29-54 as a function of the pre-increment global step (fp32 op order)."""
     return lambda step: _lib.learning_rate(init_lr, num_train_steps, num_warmup_steps, step)
 
 
 class _OptimizerBase:
-    """What both optimizers share: turning (grad, var) pairs into one kernel launch."""
+    """What every optimizer shares: turning (grad, var) pairs into one kernel launch.  ``lr_multipliers`` is ELECTRA's
+    per-variable learning-rate dict as multipliers of the scheduled lr (``lr_multipliers_for``): a constructor argument
+    of LAMBOptimizer and AdamOptimizer, an attribute to set on AdamWeightDecayOptimizer (whose constructor keeps the
+    reference's signature).  It is read when the train op is built."""
     variant = ADAM_WEIGHT_DECAY
 
     def _hparams(self, clip: float) -> HParams:
         raise NotImplementedError
 
-    def __init__(self):
+    def __init__(self, lr_multipliers: Optional[Dict[str, float]] = None):
+        self.lr_multipliers = dict(lr_multipliers) if lr_multipliers is not None else None
         self._direct_op: Optional[GaccumTrainOp] = None
         self._direct_key = None
 
@@ -81,7 +126,8 @@ class _OptimizerBase:
             self._direct_op = GaccumTrainOp([v.tensor for v in vars_], [v.name for v in vars_],
                                             self._hparams(0.0), 1, _lr_callable(self.learning_rate),
                                             exclude_from_weight_decay=getattr(self, "exclude_from_weight_decay", None),
-                                            exclude_from_layer_adaptation=getattr(self, "exclude_from_layer_adaptation", None))
+                                            exclude_from_layer_adaptation=getattr(self, "exclude_from_layer_adaptation", None),
+                                            lr_multipliers=lr_multipliers_for([v.name for v in vars_], self.lr_multipliers))
             self._direct_key = key
         op = self._direct_op
         gs = graph.get_global_step()
@@ -100,6 +146,7 @@ class AdamWeightDecayOptimizer(_OptimizerBase):
 
     def __init__(self, learning_rate: LrLike, weight_decay_rate=0.0, beta_1=0.9, beta_2=0.999, epsilon=1e-6,
                  exclude_from_weight_decay: Optional[Sequence[str]] = None, name="AdamWeightDecayOptimizer"):
+        # the reference's signature: per-variable learning rates are set as the ``lr_multipliers`` attribute
         super().__init__()
         self.learning_rate = learning_rate
         self.weight_decay_rate = weight_decay_rate
@@ -129,8 +176,9 @@ class LAMBOptimizer(_OptimizerBase):
 
     def __init__(self, learning_rate: LrLike, weight_decay_rate=0.01, beta_1=0.9, beta_2=0.999, epsilon=1e-6,
                  exclude_from_weight_decay: Optional[Sequence[str]] = None,
-                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None, name="LAMBOptimizer"):
-        super().__init__()
+                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None, name="LAMBOptimizer",
+                 lr_multipliers: Optional[Dict[str, float]] = None):
+        super().__init__(lr_multipliers)
         self.learning_rate = learning_rate
         self.weight_decay_rate = weight_decay_rate
         self.beta_1 = beta_1
@@ -159,8 +207,9 @@ class AdamOptimizer(_OptimizerBase):
     """``tf.train.AdamOptimizer`` as the example scripts use it (02:41, 04:42, another-example.py:135)."""
     variant = ADAM
 
-    def __init__(self, learning_rate: LrLike = 0.001, beta1=0.9, beta2=0.999, epsilon=1e-8, name="Adam"):
-        super().__init__()
+    def __init__(self, learning_rate: LrLike = 0.001, beta1=0.9, beta2=0.999, epsilon=1e-8, name="Adam",
+                 lr_multipliers: Optional[Dict[str, float]] = None):
+        super().__init__(lr_multipliers)
         self.learning_rate = learning_rate
         self.beta1, self.beta2, self.epsilon, self.name = beta1, beta2, epsilon, name
 
@@ -220,6 +269,7 @@ class TrainOp:
             if hp.variant == LAMB else {}
         self.ema = ema
         ema_cfg = ema.config() if ema is not None else None
+        mult = lr_multipliers_for(names, getattr(optimizer, "lr_multipliers", None))
         self.dp = None
         if process_group is not None:
             # reference 04: MultiWorkerMirroredStrategy.  "fused": the exchange happens inside the apply
@@ -228,15 +278,15 @@ class TrainOp:
             pg = None if process_group is True else process_group
             if dp_mode == "fused":
                 self.dp = FusedDataParallelTrainOp(tensors, names, hp, accum_n, lr_fn, pg, exclude, int(global_step),
-                                                   loss_scale=loss_scale, ema=ema_cfg)
+                                                   loss_scale=loss_scale, ema=ema_cfg, lr_multipliers=mult)
                 self.engine = self.dp.engine
             else:
                 self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step),
-                                            loss_scale=loss_scale, ema=ema_cfg, **adapt_kw)
+                                            loss_scale=loss_scale, ema=ema_cfg, lr_multipliers=mult, **adapt_kw)
                 self.dp = DataParallelTrainOp(self.engine, pg)
         else:
             self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step),
-                                        loss_scale=loss_scale, ema=ema_cfg, **adapt_kw)
+                                        loss_scale=loss_scale, ema=ema_cfg, lr_multipliers=mult, **adapt_kw)
         if ema is not None:
             ema._train_op = self
         self.last_loss: Optional[torch.Tensor] = None
@@ -303,6 +353,8 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
     With the module attribute ``optimizer_type = "lamb"`` the optimizer is a LAMBOptimizer with the same
     hyper-parameters and exclusions (layer adaptation excludes what weight decay excludes).  With the module attribute
     ``moving_average_decay`` set, the train op keeps an ExponentialMovingAverage of the variables (``train_op.ema``).
+    With the module attribute ``layerwise_lr_decay`` set, each variable trains at ELECTRA's layer-wise decayed rate
+    (``layerwise_lr_multipliers``), the number of encoder layers taken from the trainable variables' names.
     """
     if use_tpu:
         # optimization.py:67-68 wraps the optimizer in tf.contrib.tpu.CrossShardOptimizer: TPU-only.
@@ -310,11 +362,16 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
     global_step = graph.get_or_create_global_step()
     if optimizer_type not in ("adam", "lamb"):
         raise ValueError(f"optimizer_type must be 'adam' or 'lamb' (got {optimizer_type!r})")
+    mult = None
+    if layerwise_lr_decay is not None:
+        mult = layerwise_lr_multipliers(layerwise_lr_decay,
+                                        _num_encoder_layers([v.name for v in graph.trainable_variables()]))
     cls = LAMBOptimizer if optimizer_type == "lamb" else AdamWeightDecayOptimizer
     optimizer = cls(
         learning_rate=bert_learning_rate(init_lr, num_train_steps, num_warmup_steps),
         weight_decay_rate=0.01, beta_1=0.9, beta_2=0.999, epsilon=1e-6,
         exclude_from_weight_decay=["LayerNorm", "layer_norm", "bias"])
+    optimizer.lr_multipliers = mult
     ema = ExponentialMovingAverage(moving_average_decay) if moving_average_decay is not None else None
     return gradient_accumulation_train_op(loss, optimizer, gradient_accumulation_multiplier,
                                           clip_norm=clip_norm, global_step=global_step, loss_scale=loss_scale, ema=ema)

@@ -93,11 +93,14 @@ class _DeviceTrainOp(_TrainOpCore):
     """A train op whose parameters live on one CUDA device and whose Adam moments are packed HBM slabs."""
 
     def __init__(self, params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step,
-                 loss_scale: Optional[LossScaleConfig] = None, exclude_from_layer_adaptation=None):
+                 loss_scale: Optional[LossScaleConfig] = None, exclude_from_layer_adaptation=None,
+                 lr_multipliers: Optional[Sequence[float]] = None):
         self.ema: Optional[torch.Tensor] = None          # the moving average of the weights, when one is kept
         self._ema_state: Optional[torch.Tensor] = None
         if not params:
             raise ValueError("no trainable variables")
+        # checked before the plan exists, so a bad table fails without touching the device
+        mult = _lib.lr_multiplier_array(lr_multipliers, len(params)) if lr_multipliers is not None else None
         self.device = params[0].device
         if self.device.type != "cuda":
             raise _lib.GaccumError(_lib.ENODEVICE, "parameters must live on a CUDA device: the train_op has no CPU fallback")
@@ -105,6 +108,12 @@ class _DeviceTrainOp(_TrainOpCore):
                          self.device.index or 0, exclude_from_layer_adaptation)
         self.m = self._zeros_slab()
         self.v = self._zeros_slab()
+        # per-tensor learning rates lr_t = fp32(lr * mult[t]) (gaccum_plan_set_lr_multipliers); configuration, not state:
+        # checkpoints do not store them
+        self._lr_multipliers = np.ones(len(params), np.float32) if mult is None else mult
+        self._lr_multipliers.flags.writeable = False
+        if mult is not None:
+            self.plan.set_lr_multipliers(mult)
         if loss_scale is not None:
             # gaccum_loss_scale_state: 8 x 4 bytes; `loss_scale` views its first word, S, so a producer can write
             # (loss * op.loss_scale).backward() without reading S back to the host
@@ -123,6 +132,12 @@ class _DeviceTrainOp(_TrainOpCore):
         self._ema_state = torch.zeros(2, dtype=torch.int64, device=self.device)    # gaccum_ema_state: 16 bytes
         self.plan.set_ema(cfg, self.ema.data_ptr(), self._ema_state.data_ptr())
         self.plan.ema_init(self._ema_state.data_ptr(), 0, self._stream())
+
+    @property
+    def lr_multipliers(self) -> np.ndarray:
+        """Tensor t's learning-rate multiplier: the apply trains it with lr_t = fp32(lr * mult[t]) (np.float32,
+        read-only; ones unless ``lr_multipliers`` was given)."""
+        return self._lr_multipliers
 
     def _zeros_slab(self) -> torch.Tensor:
         return torch.zeros(max(self.plan.padded_size, 32), dtype=torch.float32, device=self.device)
@@ -243,14 +258,15 @@ class GaccumTrainOp(_DeviceTrainOp):
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, accum: Optional[torch.Tensor] = None,
                  loss_scale: Optional[LossScaleConfig] = None,
-                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None):
+                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None,
+                 lr_multipliers: Optional[Sequence[float]] = None):
         dtypes = {p.dtype for p in params}
         if len(dtypes) > 1 and dtypes & set(_HALF_DTYPES):
             raise ValueError(f"parameters of mixed dtypes ({', '.join(sorted(str(d) for d in dtypes))}): "
                              "a 16-bit model must be all bf16 or all fp16")
         self.param_dtype = params[0].dtype if len(dtypes) == 1 and params[0].dtype in _HALF_DTYPES else torch.float32
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale,
-                         exclude_from_layer_adaptation)
+                         exclude_from_layer_adaptation, lr_multipliers)
         for p in self.params:
             if p.dtype != self.param_dtype or not p.is_contiguous() or p.device != self.device:
                 if self.param_dtype != torch.float32:
@@ -507,11 +523,12 @@ class PackedTrainOp(_DeviceTrainOp):
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, loss_scale: Optional[LossScaleConfig] = None,
-                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None):
+                 exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None,
+                 lr_multipliers: Optional[Sequence[float]] = None):
         # autograd accumulates a 16-bit parameter's gradient in its own dtype: it cannot add into an fp32 slab
         _refuse_half(params, "PackedTrainOp")
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale,
-                         exclude_from_layer_adaptation)
+                         exclude_from_layer_adaptation, lr_multipliers)
         self.param_slab = self._zeros_slab()
         self.accum = self._zeros_slab()
         with torch.no_grad():
@@ -582,9 +599,11 @@ class HostTrainOp(_TrainOpCore):
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, device: int = 0, loss_scale: Optional[LossScaleConfig] = None,
-                 ema: Optional[EmaConfig] = None):
+                 ema: Optional[EmaConfig] = None, lr_multipliers: Optional[Sequence[float]] = None):
         if ema is not None:
             raise ValueError("HostTrainOp does not keep a moving average of the weights; use GaccumTrainOp")
+        if lr_multipliers is not None:
+            raise ValueError("HostTrainOp does not support per-tensor learning-rate multipliers; use GaccumTrainOp")
         if loss_scale is not None:   # host-resident models have no fp16 autocast: nothing to loss-scale
             raise ValueError("HostTrainOp does not support loss scaling")
         if hp.variant == LAMB:

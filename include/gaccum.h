@@ -61,7 +61,8 @@ extern "C" {
  *     r  = 1
  *     if adapt[i]:  wn = ||p||, un = ||u||   (p before the update; ||x|| = sqrtf(fp32(sum x^2)))
  *                   r  = (wn > 0 && un > 0) ? wn / un : 1
- *     p  = p - (r*lr)*u              the scalar product first, as `ratio * lr * update` evaluates
+ *     p  = p - (r*lr)*u              the scalar product first, as `ratio * lr * update` evaluates (lr: the tensor's lr_t
+ *                                    with gaccum_plan_set_lr_multipliers)
  * The beta powers are TF1 Adam's running fp32 products (beta_power *= beta after every APPLIED window, starting at
  * fp32(beta)), not pow(beta, t): gaccum_step_args.beta{1,2}_power, or under loss scaling the device block's, which the
  * apply advances on windows it does not skip.  decay[] is gaccum_plan_create's mask; adapt[] is set with
@@ -265,6 +266,25 @@ GACCUM_API int gaccum_plan_set_ema(gaccum_plan* plan, const gaccum_ema_config* c
  * `stream`.  The plan must keep an EMA, and `device_state` must be the block given to gaccum_plan_set_ema (GACCUM_EINVAL
  * otherwise: the apply reads that one). */
 GACCUM_API int gaccum_ema_init(gaccum_plan* plan, gaccum_ema_state* device_state, int64_t num_updates, gaccum_stream_t stream);
+
+/* Per-tensor learning rates (layer-wise learning-rate decay, parameter groups): tensor t trains with
+ *     lr_t = fp32(lr * mult[t])                 one correctly rounded fp32 multiply, as TF's `learning_rate * python_float`
+ * in place of the step's lr, wherever the variant uses it:
+ *     GACCUM_ADAM_WEIGHT_DECAY   p = p - lr_t*u                        (u includes the decay term, as in ELECTRA)
+ *     GACCUM_ADAM                alpha_t = (lr_t * sqrt(1 - beta2_power)) / (1 - beta1_power), make_scalars' op order
+ *                                (loss-scaled: the device block's beta powers)
+ *     GACCUM_LAMB                p = p - (r*lr_t)*u
+ * mult[t] is an fp32 value, finite and >= 0; 1.0 for every tensor without a call.  Nothing else depends on the
+ * multipliers, bit for bit: the accumulators, the global norm, the clip scale, the trust ratios, the loss-scaling decision
+ * and state, the beta powers, the EMA rule and the stats (gaccum_stats.lr stays the step's lr).  Since x * 1.0f == x, a
+ * plan whose multipliers are all 1 computes exactly what a plan without the call computes; a tensor with multiplier 0
+ * keeps its weights while its m and v advance.
+ * `mult` is num_tensors floats in host memory, copied -- synchronously into the plan's device memory on a device plan.
+ * GACCUM_EINVAL for NULL, a NaN, an infinity or a negative value, and after the plan's first compute call, like
+ * gaccum_plan_set_loss_scale; combines with the other setters in any order.  gaccum_algorithmic_bytes is unchanged: the
+ * num_tensors x 4-byte table is plan metadata, as the tile table is.  gaccum_step_dp, gaccum_apply_dp,
+ * gaccum_host_session_create and gaccum_step_host refuse a plan on which it was called with GACCUM_EINVAL. */
+GACCUM_API int gaccum_plan_set_lr_multipliers(gaccum_plan* plan, const float* mult);
 
 /* ---- the hot path --------------------------------------------------------------------- */
 /* One micro-step of the train_op (optimization.py:91-94): if gaccum_is_apply_step() the apply
