@@ -165,6 +165,7 @@ def _load():
         "gaccum_plan_set_ema": (C.c_int, [vp, C.POINTER(EmaConfig), vp, vp]),
         "gaccum_ema_init": (C.c_int, [vp, vp, i64, vp]),
         "gaccum_plan_set_lr_multipliers": (C.c_int, [vp, vp]),
+        "gaccum_plan_set_window_weight": (C.c_int, [vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -363,6 +364,11 @@ class Plan:
         m32 = lr_multiplier_array(mult, self.T)
         arr = (C.c_float * max(self.T, 1))(*m32.tolist())
         _check(_load().gaccum_plan_set_lr_multipliers(self._h, C.cast(arr, C.c_void_p)))
+
+    def set_window_weight(self, device_state: int) -> None:
+        """Divide each window by the producer's total weight W instead of N (before the first compute call):
+        ``device_state`` points to the 16-byte gaccum_window_weight_state in device memory, zeroed to start."""
+        _check(_load().gaccum_plan_set_window_weight(self._h, device_state or None))
 
     def close(self) -> None:
         if getattr(self, "_h", None):

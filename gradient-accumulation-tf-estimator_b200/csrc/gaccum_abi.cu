@@ -94,6 +94,9 @@ struct gaccum_plan {
   bool lr_mult_set = false;
   std::vector<float> lr_mult;
   float* d_lr_mult = nullptr;
+  // per-window normalisation by the producer's total weight (gaccum_plan_set_window_weight); set only while `computed`
+  // is false
+  gaccum_window_weight_state* ww_state = nullptr;
   std::mutex mu;
   std::map<const void*, int> grid_cache;   // cooperative kernel -> CTAs that fit on one SM (fit)
 };
@@ -295,6 +298,7 @@ static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, f
     prm.lrm.bc2 = t2;
     prm.lrm.bc1 = t4;
   }
+  prm.ww.state = reinterpret_cast<WindowWeightState*>(pl->ww_state);
 }
 
 template <int CAP>
@@ -678,6 +682,21 @@ static int refuse_lr_mult(const gaccum_plan* pl, const char* what) {
              : GACCUM_OK;
 }
 
+int gaccum_plan_set_window_weight(gaccum_plan* pl, gaccum_window_weight_state* state) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (!state || !aligned16_host(state)) return fail(GACCUM_EINVAL, "state must be a 16-byte aligned device pointer");
+  if (pl->computed) return fail(GACCUM_EINVAL, "the window weight can only be set before the plan's first compute call");
+  static_assert(sizeof(gaccum_window_weight_state) == sizeof(WindowWeightState), "header and kernel disagree");
+  pl->ww_state = state;
+  return GACCUM_OK;
+}
+
+static int refuse_window_weight(const gaccum_plan* pl, const char* what) {
+  return pl && pl->ww_state
+             ? fail(GACCUM_EINVAL, "%s does not support a window weight (gaccum_plan_set_window_weight)", what)
+             : GACCUM_OK;
+}
+
 static int refuse_half(const gaccum_plan* pl, const char* what) {
   return pl && pl->master ? fail(GACCUM_EINVAL, "%s does not support 16-bit parameters (gaccum_plan_set_param_dtype)", what)
                           : GACCUM_OK;
@@ -856,6 +875,7 @@ int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* co
   if (int rc = refuse_half(pl, "the fused data-parallel apply")) return rc;
   if (int rc = refuse_ema(pl, "the fused data-parallel apply")) return rc;
   if (int rc = refuse_lr_mult(pl, "the fused data-parallel apply")) return rc;
+  if (int rc = refuse_window_weight(pl, "the fused data-parallel apply")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (comm->world < 2 || comm->world > GACCUM_MAX_RANKS || comm->rank < 0 || comm->rank >= comm->world)
     return fail(GACCUM_EINVAL, "world must be 2..%d and 0 <= rank < world", GACCUM_MAX_RANKS);
@@ -883,6 +903,7 @@ int gaccum_step_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* con
   if (int rc = refuse_half(pl, "the fused data-parallel step")) return rc;
   if (int rc = refuse_ema(pl, "the fused data-parallel step")) return rc;
   if (int rc = refuse_lr_mult(pl, "the fused data-parallel step")) return rc;
+  if (int rc = refuse_window_weight(pl, "the fused data-parallel step")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (int rc = check_args(a)) return rc;
   if (!grads) return fail(GACCUM_EINVAL, "grads is NULL");
@@ -967,6 +988,7 @@ int gaccum_host_session_create(gaccum_host_session** out, gaccum_plan* pl) {
   if (int rc = refuse_lamb(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_ema(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_lr_mult(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse_window_weight(pl, "the host-buffer session")) return rc;
   if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): libgaccum has no CPU fallback, a CUDA device is required");
   DeviceGuard guard(pl->device);
   gaccum_host_session* s = new (std::nothrow) gaccum_host_session();
@@ -1079,6 +1101,7 @@ int gaccum_step_host(gaccum_host_session* s, const float* const* host_grads, flo
   if (int rc = refuse_lamb(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_ema(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_lr_mult(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse_window_weight(pl, "the host-buffer session")) return rc;
   DeviceGuard guard(pl->device);
   const int b = (int)(s->calls & 1);
   ++s->calls;

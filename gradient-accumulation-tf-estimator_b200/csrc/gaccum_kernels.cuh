@@ -146,6 +146,20 @@ struct LrMultParams {
   float bc1;               // GACCUM_ADAM: 1 - beta1_power
 };
 
+// gaccum_window_weight_state (gaccum.h): caller-owned device memory.  The producer adds each micro-batch's weight into
+// `weight`; every apply launch of a weighted plan divides by it, then stores last_weight = W and weight = +0.
+struct WindowWeightState {
+  float weight;            // W: the running window's total weight
+  float last_weight;       // W of the last apply launch
+  float reserved[2];
+};
+static_assert(sizeof(WindowWeightState) == 16, "gaccum_window_weight_state is 16 bytes");
+
+// Per-window normalisation (gaccum_plan_set_window_weight): c = a'/W in place of a'/N.  state == NULL: divide by N.
+struct WindowWeightParams {
+  WindowWeightState* state;
+};
+
 // Every kernel's parameter block.  Each feature's parameters follow those of the features before it, so adding them
 // moved no member an existing kernel reads.
 template <int CAP>
@@ -168,6 +182,7 @@ struct KernelParams {
   LambParams lamb;      // lamb_apply_kernel only
   EmaParams ema;        // kernels with EMA = true only
   LrMultParams lrm;     // apply kernels only
+  WindowWeightParams ww;  // apply kernels only
 };
 static_assert(sizeof(KernelParams<1920>) <= 32764, "kernel parameters must fit the 32 KB limit");
 
@@ -326,6 +341,30 @@ __device__ __forceinline__ float normalize(float a, float nf, float inv_nf) {
   return inv_nf != 0.f ? __fmul_rn(a, inv_nf) : __fdiv_rn(a, nf);
 }
 
+// The divisor D of c = (1.0*a')/D, as normalize() takes it: fp32(N) from Scalars, or a weighted plan's window weight W.
+// The functions that normalise take either (Scalars or Divisor: both have nf and inv_nf).
+struct Divisor {
+  float nf;       // D
+  float inv_nf;   // 1/D when D is a normal power of two (exact), else 0 -> the kernels divide
+};
+// W as a divisor: the rule make_scalars applies to N, so a / W is always the correctly rounded quotient.  A W that is
+// zero, negative, subnormal or not finite is divided by as it is (IEEE results, as a NaN gradient propagates).
+__device__ __forceinline__ Divisor weight_divisor(float W) {
+  const uint32_t bits = __float_as_uint(W), e = (bits >> 23) & 0xffu;
+  return Divisor{W, ((bits & 0x007fffffu) == 0u && e != 0u && e != 0xffu) ? __fdiv_rn(1.0f, W) : 0.f};
+}
+// The divisor of one apply launch: W as the state holds it when the launch starts (weighted plans), else N.  Read by
+// one thread of each CTA before any CTA can reach window_finish.
+template <typename KP>
+__device__ __forceinline__ Divisor launch_divisor(const KP& prm) {
+  return prm.ww.state ? weight_divisor(__ldcg(&prm.ww.state->weight)) : Divisor{prm.sc.nf, prm.sc.inv_nf};
+}
+// Once every CTA of the launch has read W: record it, and start the next window at +0 (applied or skipped alike)
+__device__ __forceinline__ void window_finish(WindowWeightState* st, float W) {
+  st->last_weight = W;
+  st->weight = 0.f;
+}
+
 // rate: the learning rate (VARIANT 0) or alpha (VARIANT 1) the update uses -- Scalars' own, or the tile's lr_t / alpha_t
 // (LrMultParams)
 template <int VARIANT>
@@ -365,83 +404,86 @@ __device__ __forceinline__ float tensor_mult(const LrMultParams& lrm, const Tile
   return __ldg(lrm.mult + (d.tensor_flags & 0x7fffffffu));
 }
 
-// optimization.py:83-85: c = a/N, times the clip scale s if `scaled` (never a multiply by 1: it could change a NaN's
-// payload), then one Adam step of p, m, v with `rate` (default: Scalars' lr / alpha)
-template <int VARIANT>
+// optimization.py:83-85: c = a/D (dv: N, or the window weight W), times the clip scale s if `scaled` (never a multiply
+// by 1: it could change a NaN's payload), then one Adam step of p, m, v with `rate` (default: Scalars' lr / alpha)
+template <int VARIANT, typename D>
 __device__ __forceinline__ void update_elem(float a, bool scaled, float s, float& p, float& m, float& v, bool decay,
-                                            const Scalars& sc, const float& rate) {
-  float c = normalize(a, sc.nf, sc.inv_nf);
+                                            const Scalars& sc, const float& rate, const D& dv) {
+  float c = normalize(a, dv.nf, dv.inv_nf);
   if (scaled) c = __fmul_rn(c, s);
   adam_elem<VARIANT>(c, p, m, v, decay, sc, rate);
 }
 template <int VARIANT>
 __device__ __forceinline__ void update_elem(float a, bool scaled, float s, float& p, float& m, float& v, bool decay,
                                             const Scalars& sc) {
-  update_elem<VARIANT>(a, scaled, s, p, m, v, decay, sc, sc_rate<VARIANT>(sc));
+  update_elem<VARIANT>(a, scaled, s, p, m, v, decay, sc, sc_rate<VARIANT>(sc), sc);
 }
-template <int VARIANT>
+template <int VARIANT, typename D>
 __device__ __forceinline__ void update_vec(const float4 a, bool scaled, float s, float4& p, float4& m, float4& v, bool decay,
-                                           const Scalars& sc, const float& rate) {
-  update_elem<VARIANT>(a.x, scaled, s, p.x, m.x, v.x, decay, sc, rate);
-  update_elem<VARIANT>(a.y, scaled, s, p.y, m.y, v.y, decay, sc, rate);
-  update_elem<VARIANT>(a.z, scaled, s, p.z, m.z, v.z, decay, sc, rate);
-  update_elem<VARIANT>(a.w, scaled, s, p.w, m.w, v.w, decay, sc, rate);
+                                           const Scalars& sc, const float& rate, const D& dv) {
+  update_elem<VARIANT>(a.x, scaled, s, p.x, m.x, v.x, decay, sc, rate, dv);
+  update_elem<VARIANT>(a.y, scaled, s, p.y, m.y, v.y, decay, sc, rate, dv);
+  update_elem<VARIANT>(a.z, scaled, s, p.z, m.z, v.z, decay, sc, rate, dv);
+  update_elem<VARIANT>(a.w, scaled, s, p.w, m.w, v.w, decay, sc, rate, dv);
 }
 template <int VARIANT>
 __device__ __forceinline__ void update_vec(const float4 a, bool scaled, float s, float4& p, float4& m, float4& v, bool decay,
                                            const Scalars& sc) {
-  update_vec<VARIANT>(a, scaled, s, p, m, v, decay, sc, sc_rate<VARIANT>(sc));
+  update_vec<VARIANT>(a, scaled, s, p, m, v, decay, sc, sc_rate<VARIANT>(sc), sc);
 }
 
 __device__ __forceinline__ float4 add_rn(const float4 a, const float4 b) {
   return make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w));
 }
-// acc + (x/N)^2: one element of a thread's fp32 partial of the global norm
-__device__ __forceinline__ float add_sq(float acc, float x, const Scalars& sc) {
-  const float n = normalize(x, sc.nf, sc.inv_nf);
+// acc + (x/D)^2: one element of a thread's fp32 partial of the global norm
+template <typename D>
+__device__ __forceinline__ float add_sq(float acc, float x, const D& dv) {
+  const float n = normalize(x, dv.nf, dv.inv_nf);
   return fmaf(n, n, acc);
 }
-__device__ __forceinline__ float add_sq(float acc, const float4 x, const Scalars& sc) {
-  return add_sq(add_sq(add_sq(add_sq(acc, x.x, sc), x.y, sc), x.z, sc), x.w, sc);
+template <typename D>
+__device__ __forceinline__ float add_sq(float acc, const float4 x, const D& dv) {
+  return add_sq(add_sq(add_sq(add_sq(acc, x.x, dv), x.y, dv), x.z, dv), x.w, dv);
 }
 
-// Loss scaling: the accumulators hold sums of S*g.  c = ((1.0*a')/N) * (1/S), two correctly rounded ops; S is a power of
+// Loss scaling: the accumulators hold sums of S*g.  c = ((1.0*a')/D) * (1/S), two correctly rounded ops; S is a power of
 // two, so the multiply is exact wherever c is a normal number.  Pass 1 also notes any non-finite element of a'.
-__device__ __forceinline__ float unscale(float a, float inv_s, const Scalars& sc) {
-  return __fmul_rn(normalize(a, sc.nf, sc.inv_nf), inv_s);
+template <typename D>
+__device__ __forceinline__ float unscale(float a, float inv_s, const D& dv) {
+  return __fmul_rn(normalize(a, dv.nf, dv.inv_nf), inv_s);
 }
-template <int MODE>
-__device__ __forceinline__ float ls_pass1(float acc, float x, float inv_s, bool& bad, const Scalars& sc) {
+template <int MODE, typename D>
+__device__ __forceinline__ float ls_pass1(float acc, float x, float inv_s, bool& bad, const D& dv) {
   bad |= !(fabsf(x) <= 3.402823466e38f);
   if constexpr (MODE == kLsClip) {
-    const float c = unscale(x, inv_s, sc);
+    const float c = unscale(x, inv_s, dv);
     acc = fmaf(c, c, acc);
   }
   return acc;
 }
-template <int MODE>
-__device__ __forceinline__ float ls_pass1(float acc, const float4 x, float inv_s, bool& bad, const Scalars& sc) {
-  return ls_pass1<MODE>(ls_pass1<MODE>(ls_pass1<MODE>(ls_pass1<MODE>(acc, x.x, inv_s, bad, sc), x.y, inv_s, bad, sc), x.z, inv_s, bad, sc),
-                        x.w, inv_s, bad, sc);
+template <int MODE, typename D>
+__device__ __forceinline__ float ls_pass1(float acc, const float4 x, float inv_s, bool& bad, const D& dv) {
+  return ls_pass1<MODE>(ls_pass1<MODE>(ls_pass1<MODE>(ls_pass1<MODE>(acc, x.x, inv_s, bad, dv), x.y, inv_s, bad, dv), x.z, inv_s, bad, dv),
+                        x.w, inv_s, bad, dv);
 }
-// c of one element of a' in the cooperative kernels: (1.0*a')/N, unscaled by 1/S under loss scaling, times the clip
+// c of one element of a' in the cooperative kernels: (1.0*a')/D, unscaled by 1/S under loss scaling, times the clip
 // scale s when clipping
-template <int MODE>
-__device__ __forceinline__ float mode_c(float a, float s, float inv_s, const Scalars& sc) {
-  if constexpr (MODE == kNoClip) return normalize(a, sc.nf, sc.inv_nf);
-  else if constexpr (MODE == kClip) return __fmul_rn(normalize(a, sc.nf, sc.inv_nf), s);
-  else if constexpr (MODE == kLsClip) return __fmul_rn(unscale(a, inv_s, sc), s);
-  else return unscale(a, inv_s, sc);
+template <int MODE, typename D>
+__device__ __forceinline__ float mode_c(float a, float s, float inv_s, const D& dv) {
+  if constexpr (MODE == kNoClip) return normalize(a, dv.nf, dv.inv_nf);
+  else if constexpr (MODE == kClip) return __fmul_rn(normalize(a, dv.nf, dv.inv_nf), s);
+  else if constexpr (MODE == kLsClip) return __fmul_rn(unscale(a, inv_s, dv), s);
+  else return unscale(a, inv_s, dv);
 }
 // pass 2 of the clip kernel on 4 elements: c of a', then one Adam step each.  A function of its own: written out at the
 // call site, nvcc schedules the AdamWeightDecay instantiations differently (more instructions, different registers).
 template <int VARIANT, int MODE>
 __device__ __forceinline__ void adam_vec(const float4 a, float s, float inv_s, float4& p, float4& m, float4& v, bool decay,
-                                         const Scalars& sc, const float& rate) {
-  adam_elem<VARIANT>(mode_c<MODE>(a.x, s, inv_s, sc), p.x, m.x, v.x, decay, sc, rate);
-  adam_elem<VARIANT>(mode_c<MODE>(a.y, s, inv_s, sc), p.y, m.y, v.y, decay, sc, rate);
-  adam_elem<VARIANT>(mode_c<MODE>(a.z, s, inv_s, sc), p.z, m.z, v.z, decay, sc, rate);
-  adam_elem<VARIANT>(mode_c<MODE>(a.w, s, inv_s, sc), p.w, m.w, v.w, decay, sc, rate);
+                                         const Scalars& sc, const float& rate, const Divisor& dv) {
+  adam_elem<VARIANT>(mode_c<MODE>(a.x, s, inv_s, dv), p.x, m.x, v.x, decay, sc, rate);
+  adam_elem<VARIANT>(mode_c<MODE>(a.y, s, inv_s, dv), p.y, m.y, v.y, decay, sc, rate);
+  adam_elem<VARIANT>(mode_c<MODE>(a.z, s, inv_s, dv), p.z, m.z, v.z, decay, sc, rate);
+  adam_elem<VARIANT>(mode_c<MODE>(a.w, s, inv_s, dv), p.w, m.w, v.w, decay, sc, rate);
 }
 
 // tf.clip_by_global_norm (TF 1.15): scale = clip * min(1/gn, 1/clip) + (gn - gn)
@@ -530,9 +572,10 @@ __global__ void ema_init_kernel(EmaState* st, long long num_updates) {
 // ---------------------------------------------------------------------------------------------
 // H: p is the master slab (always 16-byte aligned); the model copy is stored after it.
 // EMA: the average e (slab `ema`, always 16-byte aligned) is read with p and stored after it: e - (e - p) * c.
+// dv: the launch's divisor (N, or the window weight W).
 template <int VARIANT, bool H, int CAP, bool EMA = false>
-__device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams<CAP>& prm, float* ema = nullptr,
-                                            const float ema_c = 0.f) {
+__device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams<CAP>& prm, const Divisor dv,
+                                            float* ema = nullptr, const float ema_c = 0.f) {
   const Grad<H> g(prm, d);
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
@@ -562,7 +605,7 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
             [] {},
             [&](int u, uint32_t i) {
               if (g.g) va[u] = add_rn(va[u], vg[u]);
-              update_vec<VARIANT>(va[u], false, 0.f, vp[u], vm[u], vv[u], decay, sc, rate);
+              update_vec<VARIANT>(va[u], false, 0.f, vp[u], vm[u], vv[u], decay, sc, rate, dv);
               __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
               if constexpr (H) store_model4(q, i, vp[u], bf16);
@@ -571,32 +614,46 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
             [&](uint32_t i) {
               float ax = a[i], px = p[i], mx = m[i], vx = v[i];
               if (g.g) ax = __fadd_rn(ax, g.elem(i));
-              update_elem<VARIANT>(ax, false, 0.f, px, mx, vx, decay, sc, rate);
+              update_elem<VARIANT>(ax, false, 0.f, px, mx, vx, decay, sc, rate, dv);
               p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
               if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
               if constexpr (EMA) e[i] = ema_elem(e[i], px, ema_c);
             });
 }
 
-// EMA: every CTA reads n (thread 0, before its tile); the CTA that finishes last -- a counter of finished CTAs, so
-// every other CTA of the launch has read n by then -- writes n + 1 and d, and resets the counter for the next launch.
+// EMA and window weight: every CTA reads n and W (thread 0, before its tile); the CTA that finishes last -- a counter of
+// finished CTAs, so every other CTA of the launch has read n and W by then -- writes n + 1 and d, last_weight = W and
+// W = +0, and resets the counter for the next launch.  One counter (EmaParams::done) serves both.
 template <int VARIANT, int CAP, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads)
 apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
-  if constexpr (!EMA) {
-    if ((int)blockIdx.x < prm.num_tiles) update_tile<VARIANT, H>(prm.tiles[blockIdx.x], prm);
-  } else {
-    const EmaParams& ep = prm.ema;
-    __shared__ EmaLaunch s_ema;
-    if (threadIdx.x == 0) ema_load(ep, s_ema);
-    __syncthreads();
-    if ((int)blockIdx.x < prm.num_tiles) update_tile<VARIANT, H, CAP, true>(prm.tiles[blockIdx.x], prm, ep.slab, s_ema.c);
+  const EmaParams& ep = prm.ema;
+  WindowWeightState* const ww = prm.ww.state;
+  __shared__ Divisor s_dv;
+  EmaLaunch* s_ema = nullptr;
+  if constexpr (EMA) {
+    __shared__ EmaLaunch s_ema_launch;
+    s_ema = &s_ema_launch;
+  }
+  const bool counted = EMA || ww != nullptr;   // launch-uniform
+  if (counted) {
     if (threadIdx.x == 0) {
-      __threadfence();
-      if (atomicAdd(ep.done, 1u) == gridDim.x - 1u) {
-        ema_finish(ep, s_ema);
-        *ep.done = 0u;
-      }
+      if constexpr (EMA) ema_load(ep, *s_ema);
+      s_dv = launch_divisor(prm);
+    }
+    __syncthreads();
+  }
+  const Divisor dv = ww ? s_dv : Divisor{prm.sc.nf, prm.sc.inv_nf};
+  if ((int)blockIdx.x < prm.num_tiles) {
+    if constexpr (EMA) update_tile<VARIANT, H, CAP, true>(prm.tiles[blockIdx.x], prm, dv, ep.slab, s_ema->c);
+    else update_tile<VARIANT, H>(prm.tiles[blockIdx.x], prm, dv);
+  }
+  if (counted && threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(ep.done, 1u) == gridDim.x - 1u) {
+      if constexpr (EMA) ema_finish(ep, *s_ema);
+      if (ww) window_finish(ww, s_dv.nf);
+      *ep.done = 0u;
     }
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -889,7 +946,8 @@ __device__ __forceinline__ void ls_finish(const LossScaleParams& ls, const LossS
 // when an element of a' is not finite.
 template <int MODE, bool H, int CAP>
 __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float4* slot, uint64_t* empty,
-                                           float4* const stash, const uint64_t pol, const float inv_s, bool& bad) {
+                                           float4* const stash, const uint64_t pol, const float inv_s, bool& bad,
+                                           const Divisor& dv) {
   const Grad<H> g(prm, d);
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
   float4* a4 = reinterpret_cast<float4*>(a);
@@ -904,14 +962,14 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
                 if (stash == nullptr) st_policy(a4 + i, x[u], pol);
               }
               if (stash != nullptr) stash[i] = x[u];
-              if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, x[u], prm.sc);
-              else acc = ls_pass1<MODE>(acc, x[u], inv_s, bad, prm.sc);
+              if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, x[u], dv);
+              else acc = ls_pass1<MODE>(acc, x[u], inv_s, bad, dv);
             },
             [&](uint32_t i) {
               float xs = a[i];
               if (g.g) { xs = __fadd_rn(xs, g.elem(i)); a[i] = xs; }
-              if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, xs, prm.sc);
-              else acc = ls_pass1<MODE>(acc, xs, inv_s, bad, prm.sc);
+              if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, xs, dv);
+              else acc = ls_pass1<MODE>(acc, xs, inv_s, bad, dv);
             });
   return acc;
 }
@@ -925,7 +983,7 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
 template <int VARIANT, int MODE, bool H, int CAP, bool EMA = false>
 __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelParams<CAP>& prm, const float s, const float4* slot,
                                              uint64_t* empty, const float4* const stash, const float rate, const float inv_s,
-                                             const bool skip, float* ema = nullptr, const float ema_c = 0.f) {
+                                             const bool skip, const Divisor& dv, float* ema = nullptr, const float ema_c = 0.f) {
   const Scalars& sc = prm.sc;
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
@@ -953,7 +1011,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
             [&] { __syncwarp(); if ((threadIdx.x & 31) == 0) mbar_arrive(empty); },
             [&](int u, uint32_t i) {
               if (write) {
-                adam_vec<VARIANT, MODE>(va[u], s, inv_s, vp[u], vm[u], vv[u], decay, sc, rate);
+                adam_vec<VARIANT, MODE>(va[u], s, inv_s, vp[u], vm[u], vv[u], decay, sc, rate, dv);
                 __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
                 if constexpr (H) store_model4(q, i, vp[u], bf16);
                 if constexpr (EMA) __stcs(e4 + i, ema_vec(ve[u], vp[u], ema_c));
@@ -963,7 +1021,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
             [&](uint32_t i) {
               if (write) {
                 float px = p[i], mx = m[i], vx = v[i];
-                adam_elem<VARIANT>(mode_c<MODE>(a[i], s, inv_s, sc), px, mx, vx, decay, sc, rate);
+                adam_elem<VARIANT>(mode_c<MODE>(a[i], s, inv_s, dv), px, mx, vx, decay, sc, rate);
                 p[i] = px; m[i] = mx; v[i] = vx;
                 if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
                 if constexpr (EMA) e[i] = ema_elem(e[i], px, ema_c);
@@ -991,6 +1049,10 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
 // EMA: ClipLayout<true> -- pass 2's producer moves e by bulk copy as the fifth stream of the slot.  Thread 0 of every
 // CTA reads n during set-up, before its CTA arrives at the grid barrier; block 0's thread 0 writes n + 1 and d at the
 // very end, on an applied window only, as it writes the loss-scaling state.
+//
+// Window weight (gaccum_plan_set_window_weight): thread 0 of every CTA reads W during set-up into s_dv (N on other
+// plans), which both passes' consumers read tile by tile; block 0's thread 0 writes last_weight = W and W = +0 at the
+// very end, on applied and skipped windows alike.
 template <int VARIANT, int CAP, int MODE, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kClipThreads, 1)
 apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
@@ -1009,6 +1071,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   __shared__ float s_bcast[2];
   __shared__ LossScaleState s_ls;        // loss-scaled: the state as this launch found it
   __shared__ float s_bc[2];              // loss-scaled GACCUM_ADAM: bc2, bc1 (LrMultParams) from the device's beta powers
+  __shared__ Divisor s_dv;               // the launch's divisor: N, or W as this launch found it
   __shared__ int s_skip;
   __shared__ uint32_t s_set;
   __shared__ __align__(8) uint64_t s_full1[kGroups][kP1Slots], s_empty1[kGroups][kP1Slots];
@@ -1064,6 +1127,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
       }
     }
     if constexpr (EMA) ema_load(*ema, *s_ema);
+    s_dv = launch_divisor(prm);
   }
   for (int i = threadIdx.x; i < (kConsumerThreads / 32) * kAccBins; i += kClipThreads) (&s_bins[0][0])[i] = 0ull;
   __syncthreads();
@@ -1269,7 +1333,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         float4* const st = park ? stash + (size_t)n_seen * (kTile / 4) : nullptr;
         bool bad = false;
         const float part = norm_tile<MODE, H>(meta.d, prm, ring + (size_t)rp.slot * kP1SlotVecs, &s_empty1[grp][rp.slot], st,
-                                                pol_last, inv_s, bad);
+                                                pol_last, inv_s, bad, s_dv);
         if constexpr (loss_scaled(MODE)) { if (bad) my_nonfinite |= kElemNonfinite; }
         if constexpr (MODE != kLsNoClip) {
           // warp total in fp64, fixed butterfly order; lane 0 adds it EXACTLY into its warp's accumulator
@@ -1324,10 +1388,10 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         const float4* const st = meta.stash_slot != kNoStash ? stash + (size_t)meta.stash_slot * (kTile / 4) : nullptr;
         if constexpr (EMA) {
           update_tile2<VARIANT, MODE, H, CAP, true>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot],
-                                                    st, meta.rate, inv_s, skip, ema->slab, s_ema->c);
+                                                    st, meta.rate, inv_s, skip, s_dv, ema->slab, s_ema->c);
         } else {
           update_tile2<VARIANT, MODE, H>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st, meta.rate,
-                                      inv_s, skip);
+                                      inv_s, skip, s_dv);
         }
         rp.advance(kP2Slots);
       }
@@ -1336,6 +1400,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
       prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s;
       if constexpr (loss_scaled(MODE)) ls_finish<VARIANT == 1>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
       if constexpr (EMA) { if (!skip) ema_finish(*ema, *s_ema); }
+      if (prm.ww.state) window_finish(prm.ww.state, s_dv.nf);
     }
   }
   __syncthreads();

@@ -61,7 +61,8 @@ __device__ __forceinline__ double add_sq64(double acc, const float4 x) {
 
 // ---- phase 1: a' = a + G stored back; returns this thread's fp32 partial of the global norm (as norm_tile) ----
 template <int MODE, bool H, int CAP>
-__device__ __forceinline__ float lamb_norm_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float inv_s, bool& bad) {
+__device__ __forceinline__ float lamb_norm_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float inv_s, bool& bad,
+                                                const Divisor& dv) {
   const Grad<H> g(prm, d);
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
   float4* a4 = reinterpret_cast<float4*>(a);
@@ -72,14 +73,14 @@ __device__ __forceinline__ float lamb_norm_tile(const TileDesc& d, const KernelP
             [] {},
             [&](int u, uint32_t i) {
               if (g.g) { x[u] = add_rn(x[u], gg[u]); a4[i] = x[u]; }
-              if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, x[u], prm.sc);
-              else acc = ls_pass1<MODE>(acc, x[u], inv_s, bad, prm.sc);
+              if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, x[u], dv);
+              else acc = ls_pass1<MODE>(acc, x[u], inv_s, bad, dv);
             },
             [&](uint32_t i) {
               float xs = a[i];
               if (g.g) { xs = __fadd_rn(xs, g.elem(i)); a[i] = xs; }
-              if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, xs, prm.sc);
-              else acc = ls_pass1<MODE>(acc, xs, inv_s, bad, prm.sc);
+              if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, xs, dv);
+              else acc = ls_pass1<MODE>(acc, xs, inv_s, bad, dv);
             });
   return acc;
 }
@@ -88,7 +89,7 @@ __device__ __forceinline__ float lamb_norm_tile(const TileDesc& d, const KernelP
 // LOAD_G: there was no phase 1, so a' = a + G is formed here.  H: p is the master slab.
 template <int MODE, bool LOAD_G, bool H, int CAP>
 __device__ __forceinline__ void lamb_update_tile(const TileDesc& d, const KernelParams<CAP>& prm, const LambCoef& k,
-                                                 double& sp, double& su) {
+                                                 const Divisor& dv, double& sp, double& su) {
   Grad<H> g;
   if constexpr (LOAD_G) g = Grad<H>(prm, d);
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
@@ -112,10 +113,10 @@ __device__ __forceinline__ void lamb_update_tile(const TileDesc& d, const Kernel
             [&](int u, uint32_t i) {
               if (LOAD_G && g.g) va[u] = add_rn(va[u], vg[u]);
               float4 w;
-              w.x = lamb_u(mode_c<MODE>(va[u].x, k.s, k.inv_s, sc), vp[u].x, vm[u].x, vv[u].x, decay, sc, k);
-              w.y = lamb_u(mode_c<MODE>(va[u].y, k.s, k.inv_s, sc), vp[u].y, vm[u].y, vv[u].y, decay, sc, k);
-              w.z = lamb_u(mode_c<MODE>(va[u].z, k.s, k.inv_s, sc), vp[u].z, vm[u].z, vv[u].z, decay, sc, k);
-              w.w = lamb_u(mode_c<MODE>(va[u].w, k.s, k.inv_s, sc), vp[u].w, vm[u].w, vv[u].w, decay, sc, k);
+              w.x = lamb_u(mode_c<MODE>(va[u].x, k.s, k.inv_s, dv), vp[u].x, vm[u].x, vv[u].x, decay, sc, k);
+              w.y = lamb_u(mode_c<MODE>(va[u].y, k.s, k.inv_s, dv), vp[u].y, vm[u].y, vv[u].y, decay, sc, k);
+              w.z = lamb_u(mode_c<MODE>(va[u].z, k.s, k.inv_s, dv), vp[u].z, vm[u].z, vv[u].z, decay, sc, k);
+              w.w = lamb_u(mode_c<MODE>(va[u].w, k.s, k.inv_s, dv), vp[u].w, vm[u].w, vv[u].w, decay, sc, k);
               __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]); a4[i] = w;
               sp = add_sq64(sp, vp[u]); su = add_sq64(su, w);
             },
@@ -123,7 +124,7 @@ __device__ __forceinline__ void lamb_update_tile(const TileDesc& d, const Kernel
               float ax = a[i], mx = m[i], vx = v[i];
               const float px = p[i];
               if (LOAD_G && g.g) ax = __fadd_rn(ax, g.elem(i));
-              const float w = lamb_u(mode_c<MODE>(ax, k.s, k.inv_s, sc), px, mx, vx, decay, sc, k);
+              const float w = lamb_u(mode_c<MODE>(ax, k.s, k.inv_s, dv), px, mx, vx, decay, sc, k);
               m[i] = mx; v[i] = vx; a[i] = w;
               sp = add_sq64(sp, px); su = add_sq64(su, w);
             });
@@ -184,7 +185,8 @@ __device__ __forceinline__ double warp_sum(double w) {
 }
 
 // EMA: thread 0 of every CTA reads n during set-up; block 0's thread 0 writes n + 1 and d at the very end, past the
-// grid barriers, on an applied window only.
+// grid barriers, on an applied window only.  Window weight: thread 0 of every CTA reads W during set-up (s_dv); block
+// 0's thread 0 writes last_weight = W and W = +0 at the very end, on applied and skipped windows alike.
 template <int CAP, int MODE, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads, kLambBlocksPerSm)
 lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
@@ -201,6 +203,7 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   __shared__ unsigned int s_nonfinite[2];
   __shared__ LossScaleState s_ls;
   __shared__ float s_bcast[2];
+  __shared__ Divisor s_dv;               // the launch's divisor: N, or W as this launch found it
   __shared__ int s_skip;
   __shared__ uint32_t s_set;
 
@@ -219,10 +222,13 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     s_skip = 0;
     if constexpr (loss_scaled(MODE)) ls_load(prm.ls.state, s_ls);
     if constexpr (EMA) ema_load(prm.ema, *s_ema);
+    s_dv = launch_divisor(prm);
   }
   for (int i = threadIdx.x; i < kWarps * 2 * kAccBins; i += kThreads) (&s_bins[0][0][0])[i] = 0ull;
   __syncthreads();
   const uint32_t set = s_set;
+  // the launch's divisor, held in registers: read from shared memory at every use it slowed the unweighted apply 1.6-2.2 %
+  const Divisor dv = s_dv;
   LaunchCounters* const ctr = prm.counters + set;
   LambTensorAcc* const tacc = lb.acc + (size_t)set * lb.num_tensors;
   clear_other_counters(prm.counters, set);
@@ -244,7 +250,7 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     bool bad = false;
     unsigned int nonfinite = 0;
     for (int t = t_lo; t < t_hi; ++t) {
-      const float part = lamb_norm_tile<MODE, H>(prm.tiles[t], prm, inv_s, bad);
+      const float part = lamb_norm_tile<MODE, H>(prm.tiles[t], prm, inv_s, bad, dv);
       if constexpr (MODE != kLsNoClip) {
         const double w = warp_sum((double)part);
         if (lane == 0) acc_add(s_bins[warp][0], nonfinite, w);
@@ -304,7 +310,7 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         cur_adapt = lb.adapt[ti] != 0;
       }
       double sp = 0.0, su = 0.0;
-      lamb_update_tile<MODE, !kPhase1, H>(d, prm, coef, sp, su);
+      lamb_update_tile<MODE, !kPhase1, H>(d, prm, coef, dv, sp, su);
       if (cur_adapt) {
         sp = warp_sum(sp);
         su = warp_sum(su);
@@ -359,6 +365,7 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s_bcast[0];
     if constexpr (loss_scaled(MODE)) ls_finish<true>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
     if constexpr (EMA) { if (!skip) ema_finish(prm.ema, *s_ema); }
+    if (prm.ww.state) window_finish(prm.ww.state, s_dv.nf);
   }
 }
 

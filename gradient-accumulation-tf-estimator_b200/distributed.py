@@ -13,6 +13,11 @@ bit-identical without an extra norm exchange.  Under loss scaling the same holds
 taken from the all-reduced accumulators, so an overflow on one rank makes every rank skip.  The producer keeps 04's convention of dividing the
 loss by ``num_workers``.  (04's second reduction inside ``apply_gradients`` -- SURVEY.md 5.8 -- is
 not reproduced.)
+
+A weighted engine (window_weight=True: each window divided by its total weight W) has its W summed over ranks together
+with the accumulators on the apply step, so the apply divides the global batch's summed loss gradient by the global
+batch's total weight: the per-token mean of the whole global batch.  Its producer must therefore NOT divide the loss by
+``num_workers``: each rank differentiates its own summed loss and adds its own weights.
 """
 from __future__ import annotations
 
@@ -23,6 +28,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib
+from .train_op import WINDOW_WEIGHT_KEY
 
 
 class DataParallelTrainOp:
@@ -37,33 +43,55 @@ class DataParallelTrainOp:
         self.world = dist.get_world_size(self.group) if dist.is_initialized() else 1
         self.allreduces = 0
 
+    def _weighted(self) -> bool:
+        return getattr(self.engine, "window_weight", None) is not None
+
     def state_dict(self):
-        """Replicated moments are already complete on every rank; the rank-local accumulators are summed (04:55)."""
+        """Replicated moments are already complete on every rank; the rank-local accumulators are summed (04:55), and so
+        is a weighted engine's running window weight W."""
         e = self.engine
         if self.world == 1:
             return e.state_dict()
         acc = e.accum.clone()
         dist.all_reduce(acc, op=dist.ReduceOp.SUM, group=self.group)
+        w = None
+        if self._weighted():
+            w = e.window_weight.detach().clone().reshape(1)
+            dist.all_reduce(w, op=dist.ReduceOp.SUM, group=self.group)
         saved, e.accum = e.accum, acc
         try:
-            return e.state_dict()
+            sd = e.state_dict()
         finally:
             e.accum = saved
+        if w is not None:
+            sd[WINDOW_WEIGHT_KEY] = w.reshape(()).cpu()
+        return sd
 
     def load_state_dict(self, sd, strict: bool = True) -> None:
+        """Rank 0 takes the summed accumulators (and W); the other ranks continue the window from zero."""
         self.engine.load_state_dict(sd, strict)
         if self.world > 1 and dist.get_rank(self.group) != 0:
             self.engine.accum.zero_()
+            if self._weighted():
+                with torch.no_grad():
+                    self.engine.window_weight.zero_()
 
-    def run(self, grads: Sequence[Optional[torch.Tensor]]) -> bool:
+    def run(self, grads: Sequence[Optional[torch.Tensor]], weight=None) -> bool:
+        """One micro-step; a weighted engine takes this rank's micro-batch weight, as ``GaccumTrainOp.run`` does."""
         e = self.engine
+        kw = {} if weight is None else {"weight": weight}
         if self.world == 1:
-            return e.run(grads)
+            return e.run(grads, **kw)
         g = e.global_step
         if not _lib.is_apply_step(g, e.N):       # optimization.py:91 predicate, accumulate branch
-            return e.run(grads)
+            return e.run(grads, **kw)
+        if weight is not None or self._weighted():
+            e._add_weight(weight)                # this rank's last micro-batch, before W is summed
         e.accumulate_only(grads)                 # 04:58
         dist.all_reduce(e.accum, op=dist.ReduceOp.SUM, group=self.group)   # 04:55, once per window
+        if self._weighted():
+            # the global batch's total weight: every rank divides the summed accumulators by the same W
+            dist.all_reduce(e.window_weight.view(1), op=dist.ReduceOp.SUM, group=self.group)
         self.allreduces += 1
         e.apply_only(None)                       # 04:59-66 on the summed accumulators
         e.global_step = g + 1                    # 04:74
@@ -89,9 +117,11 @@ class FusedDataParallelTrainOp:
 
     def __init__(self, params: Sequence[torch.Tensor], names: Sequence[str], hp, accum_n: int, lr_fn,
                  process_group=None, exclude_from_weight_decay=("LayerNorm", "layer_norm", "bias"),
-                 global_step: int = 0, loss_scale=None, ema=None, lr_multipliers=None):
+                 global_step: int = 0, loss_scale=None, ema=None, lr_multipliers=None, window_weight: bool = False):
         import torch.distributed._symmetric_memory as symm
         from .train_op import GaccumTrainOp
+        if window_weight:
+            raise ValueError("the fused data-parallel train op does not support a window weight; use dp_mode='allreduce'")
         if ema is not None:
             raise ValueError("the fused data-parallel train op does not keep a moving average of the weights; "
                              "use dp_mode='allreduce'")

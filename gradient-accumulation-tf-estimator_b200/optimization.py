@@ -43,6 +43,9 @@ moving_average_decay: Optional[float] = None
 # ELECTRA's layer-wise learning-rate decay (layerwise_lr_multipliers), off by default; create_optimizer reads it and takes
 # the number of encoder layers from the trainable variables' names.
 layerwise_lr_decay: Optional[float] = None
+# Divide each window by its total weight (typically its number of loss tokens) instead of N: the loss callable returns
+# (summed loss, weight).  Off by default; create_optimizer reads it.
+window_weight = False
 
 LossLike = Union[torch.Tensor, Callable[[], torch.Tensor]]
 LrLike = Union[float, Callable[[int], float]]
@@ -256,8 +259,9 @@ class TrainOp:
     def __init__(self, loss: LossLike, tvars: Sequence[graph.Variable], optimizer: _OptimizerBase,
                  accum_n: int, clip: Optional[float], global_step: graph.GlobalStep, process_group=None,
                  dp_mode: str = "fused", loss_scale: Optional[LossScaleConfig] = None,
-                 ema: Optional[ExponentialMovingAverage] = None):
+                 ema: Optional[ExponentialMovingAverage] = None, window_weight: bool = False):
         self.loss = loss
+        self.window_weight = bool(window_weight)
         self.tvars = list(tvars)
         self.optimizer = optimizer
         self.global_step = global_step
@@ -278,18 +282,22 @@ class TrainOp:
             pg = None if process_group is True else process_group
             if dp_mode == "fused":
                 self.dp = FusedDataParallelTrainOp(tensors, names, hp, accum_n, lr_fn, pg, exclude, int(global_step),
-                                                   loss_scale=loss_scale, ema=ema_cfg, lr_multipliers=mult)
+                                                   loss_scale=loss_scale, ema=ema_cfg, lr_multipliers=mult,
+                                                   window_weight=window_weight)
                 self.engine = self.dp.engine
             else:
                 self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step),
-                                            loss_scale=loss_scale, ema=ema_cfg, lr_multipliers=mult, **adapt_kw)
+                                            loss_scale=loss_scale, ema=ema_cfg, lr_multipliers=mult,
+                                            window_weight=window_weight, **adapt_kw)
                 self.dp = DataParallelTrainOp(self.engine, pg)
         else:
             self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step),
-                                        loss_scale=loss_scale, ema=ema_cfg, lr_multipliers=mult, **adapt_kw)
+                                        loss_scale=loss_scale, ema=ema_cfg, lr_multipliers=mult,
+                                        window_weight=window_weight, **adapt_kw)
         if ema is not None:
             ema._train_op = self
         self.last_loss: Optional[torch.Tensor] = None
+        self._weight = None          # window_weight: the weight the loss callable returned with last_loss
 
     @property
     def accum_n(self) -> int:
@@ -306,17 +314,28 @@ class TrainOp:
 
     def gradients(self) -> List[Optional[torch.Tensor]]:
         """``tf.gradients(loss, tvars)`` (optimization.py:71): evaluated every micro-step.  Under loss scaling these
-        are the gradients of ``loss * S``, S read on the device; ``last_loss`` stays unscaled."""
+        are the gradients of ``loss * S``, S read on the device; ``last_loss`` stays unscaled.  With ``window_weight``
+        the loss is a pair (summed loss, weight): the gradients are those of the summed loss, ``last_loss`` is the
+        summed loss as returned, and the weight goes to the next ``run_with_grads``."""
         loss = self.loss() if callable(self.loss) else self.loss
+        if self.window_weight:
+            if not (isinstance(loss, (tuple, list)) and len(loss) == 2):
+                raise ValueError("with window_weight=True the loss must be a pair (summed loss, weight)")
+            loss, self._weight = loss
         self.last_loss = loss.detach()
         if self.engine.loss_scale is not None:
             loss = loss * self.engine.loss_scale
         grads = torch.autograd.grad(loss, [v.tensor for v in self.tvars], allow_unused=True)
         return [None if g is None else g.contiguous() for g in grads]
 
-    def run_with_grads(self, grads: Sequence[Optional[torch.Tensor]]) -> bool:
+    def run_with_grads(self, grads: Sequence[Optional[torch.Tensor]], weight=None) -> bool:
+        """One micro-step with ``grads``; with ``window_weight`` it takes the micro-batch's weight -- by default the one
+        the loss callable returned to the last ``gradients()``."""
+        if weight is None and self.window_weight:
+            weight, self._weight = self._weight, None
         self.engine.global_step = int(self.global_step)
-        applied = self.dp.run(grads) if self.dp is not None else self.engine.run(grads)
+        kw = {} if weight is None else {"weight": weight}
+        applied = self.dp.run(grads, **kw) if self.dp is not None else self.engine.run(grads, **kw)
         self.global_step.assign(self.engine.global_step)          # optimization.py:102-103
         return applied
 
@@ -331,17 +350,19 @@ def gradient_accumulation_train_op(loss: LossLike, optimizer: _OptimizerBase, gr
                                    clip_norm: Optional[float] = None, global_step: Optional[graph.GlobalStep] = None,
                                    tvars: Optional[Sequence[graph.Variable]] = None, process_group=None,
                                    dp_mode: str = "fused", loss_scale: Optional[LossScaleConfig] = None,
-                                   ema: Optional[ExponentialMovingAverage] = None) -> TrainOp:
+                                   ema: Optional[ExponentialMovingAverage] = None, window_weight: bool = False) -> TrainOp:
     """The recipe the example scripts inline (02:47-73, 04:48-74, another-example.py:126-155):
     N from ``params``, optimizer given, no clipping unless asked.  ``loss_scale`` turns on dynamic loss scaling for
     fp16 mixed precision: gradients are taken of ``loss * S`` and a window that overflows is skipped on the device.
-    ``ema`` keeps an exponential moving average of the trainable variables, updated by the apply step."""
+    ``ema`` keeps an exponential moving average of the trainable variables, updated by the apply step.
+    ``window_weight`` divides each window by its total weight instead of N: ``loss`` returns (summed loss, weight), the
+    weight typically the micro-batch's number of loss tokens, so a window trains on the per-token mean of its tokens."""
     gs = global_step or graph.get_or_create_global_step()
     tv = list(tvars) if tvars is not None else graph.trainable_variables()
     if not tv:
         raise ValueError("no trainable variables registered (graph.add_variable / graph.register_module)")
     return TrainOp(loss, tv, optimizer, int(gradient_accumulation_multiplier), clip_norm, gs, process_group, dp_mode,
-                   loss_scale, ema)
+                   loss_scale, ema, window_weight)
 
 
 def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
@@ -355,6 +376,8 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
     ``moving_average_decay`` set, the train op keeps an ExponentialMovingAverage of the variables (``train_op.ema``).
     With the module attribute ``layerwise_lr_decay`` set, each variable trains at ELECTRA's layer-wise decayed rate
     (``layerwise_lr_multipliers``), the number of encoder layers taken from the trainable variables' names.
+    With the module attribute ``window_weight`` set, ``loss`` returns (summed loss, weight) and each window is divided by
+    its total weight instead of N.
     """
     if use_tpu:
         # optimization.py:67-68 wraps the optimizer in tf.contrib.tpu.CrossShardOptimizer: TPU-only.
@@ -374,4 +397,5 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
     optimizer.lr_multipliers = mult
     ema = ExponentialMovingAverage(moving_average_decay) if moving_average_decay is not None else None
     return gradient_accumulation_train_op(loss, optimizer, gradient_accumulation_multiplier,
-                                          clip_norm=clip_norm, global_step=global_step, loss_scale=loss_scale, ema=ema)
+                                          clip_norm=clip_norm, global_step=global_step, loss_scale=loss_scale, ema=ema,
+                                          window_weight=window_weight)

@@ -388,6 +388,8 @@ _BETA_POWERS = (ADAM, LAMB)      # variants that keep TF1's beta1_power / beta2_
 
 
 _EMA, _EMA_STEP = "/ExponentialMovingAverage", "ExponentialMovingAverage/num_updates"
+# the running total weight of the current window (a train op with window_weight=True): an fp32 scalar
+_WINDOW_WEIGHT = "gradient_accumulation/window_weight"
 
 
 def _accum_name(i: int) -> str:
@@ -413,15 +415,18 @@ def to_reference_names(state: Dict[str, object], names: Sequence[str], variant: 
         for n in names:
             out[n + _EMA] = arr(state[n + _EMA])
         out[_EMA_STEP] = arr(state[_EMA_STEP], np.int64)
+    if _WINDOW_WEIGHT in state:
+        out[_WINDOW_WEIGHT] = arr(state[_WINDOW_WEIGHT], np.float32).reshape(())
     return out
 
 
 def from_reference_names(tensors: Dict[str, np.ndarray], names: Sequence[str], variant: int, strict: bool = True,
-                         ema: bool = False) -> Dict[str, np.ndarray]:
+                         ema: bool = False, window_weight: bool = False) -> Dict[str, np.ndarray]:
     """{reference Saver key: array} -> the dictionary train_op.load_state_dict() takes.  A checkpoint written before the
     optimizer existed (a pre-trained BERT: parameters only) loads with strict=False: moments and accumulators stay zero.
     The moving averages (``<var>/ExponentialMovingAverage``, ``ExponentialMovingAverage/num_updates``) are taken when
-    present, and required in strict mode when ``ema`` is True (a train op that keeps them)."""
+    present, and required in strict mode when ``ema`` is True (a train op that keeps them).  The window's running weight
+    (``gradient_accumulation/window_weight``, fp32) likewise, required in strict mode when ``window_weight`` is True."""
     m_s, v_s = _SLOTS[variant]
     out: Dict[str, np.ndarray] = {"global_step": np.asarray(tensors.get("global_step", 0), dtype=np.int64)}
     for i, n in enumerate(names):
@@ -441,6 +446,10 @@ def from_reference_names(tensors: Dict[str, np.ndarray], names: Sequence[str], v
             out[k] = tensors[k]
         elif strict and ema:
             raise KeyError(f"checkpoint has no tensor {k!r}")
+    if _WINDOW_WEIGHT in tensors:
+        out[_WINDOW_WEIGHT] = np.asarray(tensors[_WINDOW_WEIGHT], np.float32).reshape(())
+    elif strict and window_weight:
+        raise KeyError(f"checkpoint has no tensor {_WINDOW_WEIGHT!r}")
     return out
 
 
@@ -537,7 +546,8 @@ def restore(prefix_or_dir: str, train_op, names: Optional[Sequence[str]] = None,
         raise FileNotFoundError(f"no checkpoint state in {prefix_or_dir}")
     eng = _engine_of(train_op)
     names = list(names if names is not None else eng.names)
-    sd = from_reference_names(read_bundle(prefix), names, int(eng.hp.variant), strict, getattr(eng, "ema", None) is not None)
+    sd = from_reference_names(read_bundle(prefix), names, int(eng.hp.variant), strict, getattr(eng, "ema", None) is not None,
+                              getattr(eng, "window_weight", None) is not None)
     train_op.load_state_dict({k: torch.from_numpy(np.array(v, order="C")) for k, v in sd.items()}, strict)
     return prefix
 

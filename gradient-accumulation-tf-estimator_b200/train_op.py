@@ -42,6 +42,10 @@ def _pinned_zeros(n: int) -> torch.Tensor:
         return t
 
 
+# the state_dict key of a weighted train op's running window weight W (an fp32 scalar)
+WINDOW_WEIGHT_KEY = "gradient_accumulation/window_weight"
+
+
 def _stats_dict(buf: torch.Tensor) -> Dict[str, float]:
     """The 16-byte gaccum_stats block as ``stats()`` reports it."""
     a, lr, gn, s = buf.tolist()
@@ -94,7 +98,7 @@ class _DeviceTrainOp(_TrainOpCore):
 
     def __init__(self, params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step,
                  loss_scale: Optional[LossScaleConfig] = None, exclude_from_layer_adaptation=None,
-                 lr_multipliers: Optional[Sequence[float]] = None):
+                 lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False):
         self.ema: Optional[torch.Tensor] = None          # the moving average of the weights, when one is kept
         self._ema_state: Optional[torch.Tensor] = None
         if not params:
@@ -121,6 +125,14 @@ class _DeviceTrainOp(_TrainOpCore):
             self.plan.set_loss_scale(loss_scale, self._ls_state.data_ptr())
             self.plan.loss_scale_init(self._ls_state.data_ptr(), self._stream())
             self.loss_scale = self._ls_state[0]
+        self._ww_state: Optional[torch.Tensor] = None
+        self.window_weight: Optional[torch.Tensor] = None
+        if window_weight:
+            # gaccum_window_weight_state: 4 x 4 bytes, zeroed; `window_weight` views its first word, W, so a producer adds
+            # each micro-batch's weight on the device (op.window_weight += count) without a host round trip
+            self._ww_state = torch.zeros(4, dtype=torch.float32, device=self.device)
+            self.plan.set_window_weight(self._ww_state.data_ptr())
+            self.window_weight = self._ww_state[0]
 
     def _init_ema(self, cfg: EmaConfig, weights: Callable[[int], torch.Tensor]) -> None:
         """Keep an exponential moving average of ``weights(i)`` (the fp32 weights the apply updates).  TF initialises
@@ -138,6 +150,48 @@ class _DeviceTrainOp(_TrainOpCore):
         """Tensor t's learning-rate multiplier: the apply trains it with lr_t = fp32(lr * mult[t]) (np.float32,
         read-only; ones unless ``lr_multipliers`` was given)."""
         return self._lr_multipliers
+
+    def window_weight_state(self) -> Dict[str, float]:
+        """Synchronously read the window-weight block: weight (W, the running window's total so far) and last_weight
+        (the W the last apply step divided by)."""
+        if self._ww_state is None:
+            raise ValueError("this train op does not weight its windows (window_weight=False)")
+        words = self._ww_state.cpu()
+        return {"weight": float(words[0]), "last_weight": float(words[1])}
+
+    def _add_weight(self, weight, stream: Optional[int] = None) -> None:
+        """Add a micro-batch's weight into W (an fp32 add on the op's stream), after checking it against the op: a
+        weighted op needs one on every micro-step, an unweighted op takes none."""
+        if self._ww_state is None:
+            if weight is not None:
+                raise ValueError("a weight was given to a train op that divides each window by N (window_weight=False)")
+            return
+        if weight is None:
+            raise ValueError("this train op divides each window by its total weight (window_weight=True): "
+                             "every micro-step needs its weight")
+        ctx = torch.cuda.stream(torch.cuda.ExternalStream(stream, device=self.device)) if stream is not None \
+            else contextlib.nullcontext()
+        if isinstance(weight, torch.Tensor):
+            weight = weight.to(device=self.device, dtype=torch.float32)   # fp32(w) first: the add is an fp32 add
+        else:
+            weight = float(np.float32(weight))
+        with ctx, torch.no_grad():
+            self.window_weight.add_(weight)
+
+    def _window_weight_state_dict(self, out: Dict[str, torch.Tensor]) -> None:
+        """The running W: a checkpoint taken mid-window needs it, as it needs the accumulators."""
+        out[WINDOW_WEIGHT_KEY] = self._ww_state[0].detach().cpu().clone()
+
+    def _load_window_weight(self, sd: Dict[str, torch.Tensor], strict: bool) -> None:
+        """W from a checkpoint; non-strict, a checkpoint without it starts the window at W = 0."""
+        if WINDOW_WEIGHT_KEY in sd:
+            w = torch.as_tensor(sd[WINDOW_WEIGHT_KEY], dtype=torch.float32).reshape(())
+        elif strict:
+            raise KeyError(WINDOW_WEIGHT_KEY)
+        else:
+            w = torch.zeros((), dtype=torch.float32)
+        with torch.no_grad():
+            self._ww_state[0].copy_(w)
 
     def _zeros_slab(self) -> torch.Tensor:
         return torch.zeros(max(self.plan.padded_size, 32), dtype=torch.float32, device=self.device)
@@ -259,14 +313,14 @@ class GaccumTrainOp(_DeviceTrainOp):
                  global_step: int = 0, accum: Optional[torch.Tensor] = None,
                  loss_scale: Optional[LossScaleConfig] = None,
                  exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None,
-                 lr_multipliers: Optional[Sequence[float]] = None):
+                 lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False):
         dtypes = {p.dtype for p in params}
         if len(dtypes) > 1 and dtypes & set(_HALF_DTYPES):
             raise ValueError(f"parameters of mixed dtypes ({', '.join(sorted(str(d) for d in dtypes))}): "
                              "a 16-bit model must be all bf16 or all fp16")
         self.param_dtype = params[0].dtype if len(dtypes) == 1 and params[0].dtype in _HALF_DTYPES else torch.float32
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale,
-                         exclude_from_layer_adaptation, lr_multipliers)
+                         exclude_from_layer_adaptation, lr_multipliers, window_weight)
         for p in self.params:
             if p.dtype != self.param_dtype or not p.is_contiguous() or p.device != self.device:
                 if self.param_dtype != torch.float32:
@@ -317,8 +371,11 @@ class GaccumTrainOp(_DeviceTrainOp):
             self._param_key = key
 
     # -- one micro-step -------------------------------------------------------------------
-    def run(self, grads: Sequence[Optional[torch.Tensor]]) -> bool:
-        """One ``session.run(train_op)`` (optimization.py:91-104).  Returns True if it applied."""
+    def run(self, grads: Sequence[Optional[torch.Tensor]], weight=None) -> bool:
+        """One ``session.run(train_op)`` (optimization.py:91-104).  Returns True if it applied.  A weighted op
+        (window_weight=True) takes the micro-batch's weight -- a number or a device scalar, typically its count of loss
+        tokens -- and adds it into W before the step; ``grads`` are then the gradients of the summed loss."""
+        self._add_weight(weight)
         self._refresh_param_table()
         return self.run_bound(self._grad_table(grads))
 
@@ -453,6 +510,8 @@ class GaccumTrainOp(_DeviceTrainOp):
             for i, n in enumerate(self.names):
                 out[n + "/ExponentialMovingAverage"] = self.ema_view(i).clone()
             out["ExponentialMovingAverage/num_updates"] = torch.tensor(self.ema_state()["num_updates"], dtype=torch.int64)
+        if self._ww_state is not None:
+            self._window_weight_state_dict(out)
         return out
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True) -> None:
@@ -473,6 +532,8 @@ class GaccumTrainOp(_DeviceTrainOp):
             self.beta2_power = float(sd["beta2_power"])
         if self.ema is not None:
             self._load_ema_state(sd, strict)
+        if self._ww_state is not None:
+            self._load_window_weight(sd, strict)
         if self.master is not None:
             self._refresh_model()
 
@@ -524,11 +585,11 @@ class PackedTrainOp(_DeviceTrainOp):
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, loss_scale: Optional[LossScaleConfig] = None,
                  exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None,
-                 lr_multipliers: Optional[Sequence[float]] = None):
+                 lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False):
         # autograd accumulates a 16-bit parameter's gradient in its own dtype: it cannot add into an fp32 slab
         _refuse_half(params, "PackedTrainOp")
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale,
-                         exclude_from_layer_adaptation, lr_multipliers)
+                         exclude_from_layer_adaptation, lr_multipliers, window_weight)
         self.param_slab = self._zeros_slab()
         self.accum = self._zeros_slab()
         with torch.no_grad():
@@ -543,9 +604,11 @@ class PackedTrainOp(_DeviceTrainOp):
             self._init_ema(ema, lambda i: self._view(self.param_slab, i))
         self.launches = 0
 
-    def step(self, stream: Optional[int] = None) -> bool:
+    def step(self, stream: Optional[int] = None, weight=None) -> bool:
         """One ``session.run(train_op)`` AFTER the backward pass has added this micro-batch's gradient into
-        ``p.grad`` (== accum).  Returns True if it applied (optimization.py:91, pre-increment predicate)."""
+        ``p.grad`` (== accum).  Returns True if it applied (optimization.py:91, pre-increment predicate).  A weighted op
+        (window_weight=True) takes the micro-batch's weight, as ``GaccumTrainOp.run`` does."""
+        self._add_weight(weight, stream)
         g = self.global_step
         applied = _lib.is_apply_step(g, self.N)
         if applied:
@@ -599,9 +662,12 @@ class HostTrainOp(_TrainOpCore):
                  lr_fn: Callable[[int], float],
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, device: int = 0, loss_scale: Optional[LossScaleConfig] = None,
-                 ema: Optional[EmaConfig] = None, lr_multipliers: Optional[Sequence[float]] = None):
+                 ema: Optional[EmaConfig] = None, lr_multipliers: Optional[Sequence[float]] = None,
+                 window_weight: bool = False):
         if ema is not None:
             raise ValueError("HostTrainOp does not keep a moving average of the weights; use GaccumTrainOp")
+        if window_weight:
+            raise ValueError("HostTrainOp does not support a window weight; use GaccumTrainOp")
         if lr_multipliers is not None:
             raise ValueError("HostTrainOp does not support per-tensor learning-rate multipliers; use GaccumTrainOp")
         if loss_scale is not None:   # host-resident models have no fp16 autocast: nothing to loss-scale

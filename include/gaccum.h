@@ -286,6 +286,37 @@ GACCUM_API int gaccum_ema_init(gaccum_plan* plan, gaccum_ema_state* device_state
  * gaccum_host_session_create and gaccum_step_host refuse a plan on which it was called with GACCUM_EINVAL. */
 GACCUM_API int gaccum_plan_set_lr_multipliers(gaccum_plan* plan, const float* mult);
 
+/* Per-token normalisation of each accumulation window (token-level losses such as masked-LM pretraining).  Dividing
+ * by N averages the micro-batches' mean losses; that equals the gradient of the large batch a window stands for only
+ * when every micro-batch carries the same loss weight.  With this setter each window is divided by its total weight:
+ *   - the producer differentiates the SUMMED loss of each micro-batch, and adds that micro-batch's weight w_i (its
+ *     number of loss tokens, typically; any fp32 value) into `weight` with fp32 adds, on the device;
+ *   - the apply step computes c = a' / W in place of (1.0 * a') / N.  If W is a normal power of two this is an exact
+ *     multiply by 1/W, else a correctly rounded division -- the rule the unweighted apply uses for N -- so c is always
+ *     the correctly rounded a' / W.  Everything after it is unchanged: * 1/S under loss scaling, the global norm and
+ *     the clip scale (computed on c), every variant's update, the EMA, the learning-rate multipliers, the stats;
+ *   - N still decides where a window ends (gaccum_is_apply_step); it no longer divides.  The reference divides the
+ *     one-micro-batch window at global_step 0 by N; a weighted plan divides it by its own W;
+ *   - every apply launch, applied or skipped by loss scaling, stores last_weight = W and resets weight = +0.
+ *     Accumulate steps never touch the block;
+ *   - the producer must have added ALL of the window's weights -- the apply step's own micro-batch included -- before
+ *     the apply step is enqueued on the stream.  The total can arrive at the end of the window: nothing is read on the
+ *     host, so the window can be captured in a CUDA graph together with the producer's adds.
+ * A W that is not positive and finite is the caller's error.  The library reads no device data on the host, so IEEE
+ * results propagate (W = 0 gives infinities and NaNs in c), as a NaN gradient propagates in the reference; with loss
+ * scaling and clipping on, the non-finite global norm skips such a window.
+ * `state` is caller-owned device memory, 16-byte aligned; zeroed memory is the starting state.  The setter is host-only
+ * and reads nothing through the pointer.  GACCUM_EINVAL for NULL or a misaligned block, and after the plan's first
+ * compute call; combines with the other setters in any order.  gaccum_step, gaccum_apply and gaccum_step_packed honour
+ * it; gaccum_step_dp, gaccum_apply_dp, gaccum_host_session_create and gaccum_step_host refuse such a plan with
+ * GACCUM_EINVAL.  gaccum_algorithmic_bytes is unchanged (the block is 16 bytes per window). */
+typedef struct gaccum_window_weight_state {
+  float weight;       /* W: the running window's total weight, added by the producer */
+  float last_weight;  /* W of the last apply launch (written by the apply) */
+  float reserved[2];
+} gaccum_window_weight_state;
+GACCUM_API int gaccum_plan_set_window_weight(gaccum_plan* plan, gaccum_window_weight_state* state);
+
 /* ---- the hot path --------------------------------------------------------------------- */
 /* One micro-step of the train_op (optimization.py:91-94): if gaccum_is_apply_step() the apply
  * branch (assign_add -> /N -> clip_by_global_norm -> apply_gradients -> zero; :80-88), else
