@@ -99,6 +99,24 @@ class EmaConfig(C.Structure):
         super().__init__(float(decay), int(num_updates), int(reserved))
 
 
+class ScheduleConfig(C.Structure):
+    """gaccum_schedule_config: create_optimizer's learning-rate schedule (optimization.py:29-52), evaluated on the device
+    by every launch of a device-scheduled plan (``end_lr`` 0 and ``power`` 1 are the only values it takes)."""
+    _fields_ = [("init_lr", C.c_double), ("num_train_steps", C.c_int64), ("num_warmup_steps", C.c_int64),
+                ("end_lr", C.c_double), ("power", C.c_double)]
+
+    def __init__(self, init_lr: float, num_train_steps: int, num_warmup_steps: Optional[int] = 0,
+                 end_lr: float = 0.0, power: float = 1.0):
+        super().__init__(float(init_lr), int(num_train_steps), int(num_warmup_steps or 0), float(end_lr), float(power))
+
+
+class ScheduleState(C.Structure):
+    """gaccum_schedule_state: the 48-byte device block of a device-scheduled plan."""
+    _fields_ = [("global_step", C.c_int64), ("num_train_steps", C.c_int64), ("num_warmup_steps", C.c_int64),
+                ("init_lr", C.c_float), ("end_lr", C.c_float), ("power", C.c_float), ("beta1_power", C.c_float),
+                ("beta2_power", C.c_float), ("refused", C.c_int32)]
+
+
 _lib = None
 
 
@@ -166,6 +184,8 @@ def _load():
         "gaccum_ema_init": (C.c_int, [vp, vp, i64, vp]),
         "gaccum_plan_set_lr_multipliers": (C.c_int, [vp, vp]),
         "gaccum_plan_set_window_weight": (C.c_int, [vp, vp]),
+        "gaccum_plan_set_device_schedule": (C.c_int, [vp, C.POINTER(ScheduleConfig), vp]),
+        "gaccum_schedule_init": (C.c_int, [vp, vp, i64, C.c_float, C.c_float, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -369,6 +389,16 @@ class Plan:
         """Divide each window by the producer's total weight W instead of N (before the first compute call):
         ``device_state`` points to the 16-byte gaccum_window_weight_state in device memory, zeroed to start."""
         _check(_load().gaccum_plan_set_window_weight(self._h, device_state or None))
+
+    def set_device_schedule(self, cfg: ScheduleConfig, block: int) -> None:
+        """Keep global_step, the learning rate and the beta powers on the device (before the first compute call):
+        ``block`` points to the 48-byte gaccum_schedule_state in device memory that ``schedule_init`` fills."""
+        _check(_load().gaccum_plan_set_device_schedule(self._h, C.byref(cfg), block or None))
+
+    def schedule_init(self, block: int, global_step: int, beta1_power: float, beta2_power: float,
+                      stream: int = 0) -> None:
+        _check(_load().gaccum_schedule_init(self._h, block or None, int(global_step), float(beta1_power),
+                                            float(beta2_power), stream))
 
     def close(self) -> None:
         if getattr(self, "_h", None):

@@ -97,6 +97,9 @@ struct gaccum_plan {
   // per-window normalisation by the producer's total weight (gaccum_plan_set_window_weight); set only while `computed`
   // is false
   gaccum_window_weight_state* ww_state = nullptr;
+  // the device schedule (gaccum_plan_set_device_schedule); set only while `computed` is false
+  gaccum_schedule_config sched_cfg{};
+  gaccum_schedule_state* sched_state = nullptr;
   std::mutex mu;
   std::map<const void*, int> grid_cache;   // cooperative kernel -> CTAs that fit on one SM (fit)
 };
@@ -299,6 +302,9 @@ static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, f
     prm.lrm.bc1 = t4;
   }
   prm.ww.state = reinterpret_cast<WindowWeightState*>(pl->ww_state);
+  prm.sched.state = reinterpret_cast<ScheduleState*>(pl->sched_state);
+  prm.sched.done = pl->d_ema_done;
+  prm.sched.accum_n = a ? a->accum_n : 1;
 }
 
 template <int CAP>
@@ -716,6 +722,49 @@ int gaccum_loss_scale_init(gaccum_plan* pl, gaccum_loss_scale_state* device_stat
   return GACCUM_OK;
 }
 
+int gaccum_plan_set_device_schedule(gaccum_plan* pl, const gaccum_schedule_config* cfg, gaccum_schedule_state* block) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (!cfg) return fail(GACCUM_EINVAL, "cfg is NULL");
+  if (!block || !aligned16_host(block)) return fail(GACCUM_EINVAL, "block must be a 16-byte aligned device pointer");
+  if (pl->computed) return fail(GACCUM_EINVAL, "the device schedule can only be set before the plan's first compute call");
+  if (!std::isfinite(cfg->init_lr)) return fail(GACCUM_EINVAL, "init_lr must be finite (got %g)", cfg->init_lr);
+  if (cfg->num_train_steps < 0 || cfg->num_warmup_steps < 0)
+    return fail(GACCUM_EINVAL, "num_train_steps and num_warmup_steps must be >= 0 (got %lld, %lld)",
+                (long long)cfg->num_train_steps, (long long)cfg->num_warmup_steps);
+  if (cfg->end_lr != 0.0 || cfg->power != 1.0)
+    return fail(GACCUM_EINVAL, "the device schedule is create_optimizer's: end_lr must be 0 and power 1 (got %g, %g)",
+                cfg->end_lr, cfg->power);
+  static_assert(sizeof(gaccum_schedule_state) == sizeof(ScheduleState), "header and kernel disagree");
+  pl->sched_cfg = *cfg;
+  pl->sched_state = block;
+  return GACCUM_OK;
+}
+
+int gaccum_schedule_init(gaccum_plan* pl, gaccum_schedule_state* block, int64_t global_step, float beta1_power,
+                         float beta2_power, gaccum_stream_t stream) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (!pl->sched_state) return fail(GACCUM_EINVAL, "this plan has no device schedule (gaccum_plan_set_device_schedule)");
+  if (block != pl->sched_state)
+    return fail(GACCUM_EINVAL, "block is not the one given to gaccum_plan_set_device_schedule, which the launches read");
+  if (global_step < 0) return fail(GACCUM_EINVAL, "global_step must be >= 0 (got %lld)", (long long)global_step);
+  if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): a CUDA device is required");
+  ScheduleState s{};
+  s.global_step = (long long)global_step;
+  s.num_train_steps = (long long)pl->sched_cfg.num_train_steps;
+  s.num_warmup_steps = (long long)pl->sched_cfg.num_warmup_steps;
+  s.init_lr = (float)pl->sched_cfg.init_lr;
+  s.end_lr = (float)pl->sched_cfg.end_lr;
+  s.power = (float)pl->sched_cfg.power;
+  if (!pl->ls_on) {          // under loss scaling the beta powers live in the loss-scaling block
+    s.beta1_power = beta1_power;
+    s.beta2_power = beta2_power;
+  }
+  DeviceGuard guard(pl->device);
+  // a copy from pageable memory: stream-ordered, and `s` is staged before the call returns
+  CUDA_TRY(cudaMemcpyAsync(block, &s, sizeof s, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  return GACCUM_OK;
+}
+
 static int accumulate_impl(gaccum_plan* pl, const float* const* grads, float* accum,
                            const gaccum_step_args* a, gaccum_stream_t stream) {
   if (int rc = check_compute(pl, accum, nullptr, nullptr, false)) return rc;
@@ -726,12 +775,30 @@ static int accumulate_impl(gaccum_plan* pl, const float* const* grads, float* ac
                             : do_accumulate_tab<kCapLarge>(pl, grads, accum, a, st);
 }
 
+static int refuse_schedule(const gaccum_plan* pl, const char* what) {
+  return pl && pl->sched_state
+             ? fail(GACCUM_EINVAL, "%s does not support a device schedule (gaccum_plan_set_device_schedule)", what)
+             : GACCUM_OK;
+}
+
 int gaccum_accumulate(gaccum_plan* pl, const float* const* grads, float* accum, gaccum_stream_t stream) {
+  // without step arguments the launch cannot check global_step against its branch: a device-scheduled plan steps with
+  // gaccum_step
+  if (int rc = refuse_schedule(pl, "gaccum_accumulate")) return rc;
   return accumulate_impl(pl, grads, accum, nullptr, stream);
 }
 
+static int apply_impl(gaccum_plan* pl, const float* const* grads, float* const* params, float* accum,
+                      float* m, float* v, const gaccum_step_args* a, gaccum_stream_t stream);
+
 int gaccum_apply(gaccum_plan* pl, const float* const* grads, float* const* params, float* accum,
                  float* m, float* v, const gaccum_step_args* a, gaccum_stream_t stream) {
+  if (int rc = refuse_schedule(pl, "gaccum_apply")) return rc;
+  return apply_impl(pl, grads, params, accum, m, v, a, stream);
+}
+
+static int apply_impl(gaccum_plan* pl, const float* const* grads, float* const* params, float* accum,
+                      float* m, float* v, const gaccum_step_args* a, gaccum_stream_t stream) {
   if (int rc = check_compute(pl, accum, m, v, true)) return rc;
   if (int rc = check_args(a)) return rc;
   if (!params) return fail(GACCUM_EINVAL, "params is NULL");
@@ -745,7 +812,7 @@ int gaccum_step(gaccum_plan* pl, const float* const* grads, float* const* params
                 float* m, float* v, const gaccum_step_args* a, gaccum_stream_t stream) {
   if (int rc = check_args(a)) return rc;
   if (!grads) return fail(GACCUM_EINVAL, "grads is NULL");
-  if (gaccum_is_apply_step(a->global_step, a->accum_n)) return gaccum_apply(pl, grads, params, accum, m, v, a, stream);
+  if (gaccum_is_apply_step(a->global_step, a->accum_n)) return apply_impl(pl, grads, params, accum, m, v, a, stream);
   return accumulate_impl(pl, grads, accum, a, stream);
 }
 
@@ -754,6 +821,8 @@ int gaccum_step_packed(gaccum_plan* pl, const float* grad_slab, float* param_sla
                        gaccum_stream_t stream) {
   if (int rc = refuse_half(pl, "gaccum_step_packed")) return rc;
   if (int rc = check_args(a)) return rc;
+  if (pl && pl->sched_state && force_branch >= 0)
+    return fail(GACCUM_EINVAL, "a device-scheduled plan takes its branch from global_step: force_branch must be -1 (got %d)", force_branch);
   const bool apply = force_branch < 0 ? gaccum_is_apply_step(a->global_step, a->accum_n) != 0 : force_branch != 0;
   if (int rc = check_compute(pl, accum, m, v, apply)) return rc;
   if (grad_slab && !aligned16_host(grad_slab)) return fail(GACCUM_EINVAL, "grad_slab must be 16-byte aligned");
@@ -764,6 +833,11 @@ int gaccum_step_packed(gaccum_plan* pl, const float* grad_slab, float* param_sla
   prm.tab.g = grad_slab;
   prm.tab.p = param_slab;
   if (!apply) {
+    if (!grad_slab && pl->sched_state) {
+      // the gradients are already in accum (PackedTrainOp): one CTA only advances the device schedule
+      prm.num_tiles = 0;
+      return launch_accumulate(pl, prm, false, st);
+    }
     if (!grad_slab) return fail(GACCUM_EINVAL, "grad_slab is NULL on an accumulate step");
     // a forced branch says nothing about what the previous micro-step did: only the scheduled one may skip reading a
     return launch_accumulate(pl, prm, force_branch < 0 && first_of_window(a), st);
@@ -876,6 +950,7 @@ int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* co
   if (int rc = refuse_ema(pl, "the fused data-parallel apply")) return rc;
   if (int rc = refuse_lr_mult(pl, "the fused data-parallel apply")) return rc;
   if (int rc = refuse_window_weight(pl, "the fused data-parallel apply")) return rc;
+  if (int rc = refuse_schedule(pl, "the fused data-parallel apply")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (comm->world < 2 || comm->world > GACCUM_MAX_RANKS || comm->rank < 0 || comm->rank >= comm->world)
     return fail(GACCUM_EINVAL, "world must be 2..%d and 0 <= rank < world", GACCUM_MAX_RANKS);
@@ -904,6 +979,7 @@ int gaccum_step_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* con
   if (int rc = refuse_ema(pl, "the fused data-parallel step")) return rc;
   if (int rc = refuse_lr_mult(pl, "the fused data-parallel step")) return rc;
   if (int rc = refuse_window_weight(pl, "the fused data-parallel step")) return rc;
+  if (int rc = refuse_schedule(pl, "the fused data-parallel step")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (int rc = check_args(a)) return rc;
   if (!grads) return fail(GACCUM_EINVAL, "grads is NULL");
@@ -989,6 +1065,7 @@ int gaccum_host_session_create(gaccum_host_session** out, gaccum_plan* pl) {
   if (int rc = refuse_ema(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_lr_mult(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_window_weight(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse_schedule(pl, "the host-buffer session")) return rc;
   if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): libgaccum has no CPU fallback, a CUDA device is required");
   DeviceGuard guard(pl->device);
   gaccum_host_session* s = new (std::nothrow) gaccum_host_session();
@@ -1102,6 +1179,7 @@ int gaccum_step_host(gaccum_host_session* s, const float* const* host_grads, flo
   if (int rc = refuse_ema(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_lr_mult(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_window_weight(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse_schedule(pl, "the host-buffer session")) return rc;
   DeviceGuard guard(pl->device);
   const int b = (int)(s->calls & 1);
   ++s->calls;

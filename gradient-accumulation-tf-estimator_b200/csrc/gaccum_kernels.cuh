@@ -160,6 +160,28 @@ struct WindowWeightParams {
   WindowWeightState* state;
 };
 
+// gaccum_schedule_state (gaccum.h): caller-owned device memory, written by gaccum_schedule_init and afterwards only by
+// the launches of a device-scheduled plan
+struct ScheduleState {
+  long long global_step;        // the pre-increment step of the next launch
+  long long num_train_steps;
+  long long num_warmup_steps;
+  float init_lr;                // fp32(init_lr)
+  float end_lr;                 // 0
+  float power;                  // 1
+  float beta1_power, beta2_power;   // GACCUM_ADAM, GACCUM_LAMB without loss scaling (else the loss-scaling block's)
+  int32_t refused;              // 1 once a launch found global_step selecting the other branch: every launch is a no-op
+};
+static_assert(sizeof(ScheduleState) == 48, "gaccum_schedule_state is 48 bytes");
+
+// The device schedule (gaccum_plan_set_device_schedule).  state == NULL: the host's lr and beta powers (Scalars,
+// LrMultParams, LambParams).  A launch-uniform branch, not a template flag: no kernel is specialised on it.
+struct ScheduleParams {
+  ScheduleState* state;
+  unsigned int* done;      // CTAs of the launch that are through (EmaParams::done: launches on a plan are serialised)
+  int32_t accum_n;         // N: the launch checks that global_step selects its branch
+};
+
 // Every kernel's parameter block.  Each feature's parameters follow those of the features before it, so adding them
 // moved no member an existing kernel reads.
 template <int CAP>
@@ -183,8 +205,64 @@ struct KernelParams {
   EmaParams ema;        // kernels with EMA = true only
   LrMultParams lrm;     // apply kernels only
   WindowWeightParams ww;  // apply kernels only
+  ScheduleParams sched;   // every kernel
 };
 static_assert(sizeof(KernelParams<1920>) <= 32764, "kernel parameters must fit the 32 KB limit");
+
+// What a launch of a device-scheduled plan derives from the block as it finds it (thread 0 of every CTA, before any CTA
+// can write it): the step g, its learning rate, the beta powers, and whether the launch may run at all.
+struct SchedLaunch {
+  long long g;
+  float lr;
+  float bc2, bc1;          // GACCUM_ADAM: sqrt(1 - beta2_power), 1 - beta1_power (LrMultParams' terms)
+  float b1p, b2p;
+  int ok;                  // g selects this launch's branch and no earlier launch was refused
+};
+// optimization.py:29-54 exactly as gaccum_learning_rate evaluates it on the host: polynomial decay (end 0, power 1) of
+// min(g, T) over T, then, with a warm-up, (1 - is_warmup) * lr + is_warmup * (init_lr * (int32(g) / int32(W))).  One
+// correctly rounded fp32 op per TF op; int64 -> fp32 and int32 -> fp32 conversions round to nearest.
+__device__ __forceinline__ float schedule_lr(const float init_lr, const long long T, const long long W, const long long g) {
+  float gs = __ll2float_rn(g);
+  const float ds = __ll2float_rn(T);
+  if (gs > ds) gs = ds;
+  const float p = __fdiv_rn(gs, ds);
+  float lr = __fmul_rn(init_lr, __fsub_rn(1.0f, p));
+  if (W != 0) {
+    const int gi = (int)g, wi = (int)W;
+    const float pct = __fdiv_rn(__int2float_rn(gi), __int2float_rn(wi));
+    const float wlr = __fmul_rn(init_lr, pct);
+    const float isw = gi < wi ? 1.0f : 0.0f;
+    lr = __fadd_rn(__fmul_rn(__fsub_rn(1.0f, isw), lr), __fmul_rn(isw, wlr));
+  }
+  return lr;
+}
+__device__ __forceinline__ void sched_load(const ScheduleParams& sp, const bool apply, SchedLaunch& sl) {
+  const ScheduleState* st = sp.state;
+  const long long g = __ldcg(&st->global_step);
+  sl.g = g;
+  sl.lr = schedule_lr(__ldcg(&st->init_lr), __ldcg(&st->num_train_steps), __ldcg(&st->num_warmup_steps), g);
+  sl.b1p = __ldcg(&st->beta1_power);
+  sl.b2p = __ldcg(&st->beta2_power);
+  sl.bc2 = __fsqrt_rn(__fsub_rn(1.0f, sl.b2p));
+  sl.bc1 = __fsub_rn(1.0f, sl.b1p);
+  sl.ok = __ldcg(&st->refused) == 0 && ((((int)g % sp.accum_n) == 0) == apply);   // gaccum_is_apply_step
+}
+// One thread, once no CTA of the launch will read the block again: the next step, and (betas) TF1's beta powers
+// advanced with one fp32 multiply each, as after an applied window
+__device__ __forceinline__ void sched_finish(const ScheduleParams& sp, const SchedLaunch& sl, const bool betas, const float b1,
+                                             const float b2) {
+  ScheduleState* st = sp.state;
+  st->global_step = sl.g + 1;
+  if (betas) {
+    st->beta1_power = __fmul_rn(sl.b1p, b1);
+    st->beta2_power = __fmul_rn(sl.b2p, b2);
+  }
+}
+// A launch whose branch global_step does not select (a captured graph whose start is not a window start) changes
+// nothing; block 0 marks the schedule refused, so every later launch is a no-op too and the host can report it.
+__device__ __forceinline__ void sched_refuse(const ScheduleParams& sp) {
+  if (blockIdx.x == 0 && threadIdx.x == 0) sp.state->refused = 1;
+}
 
 // What every CTA of an EMA launch derives from the state as the launch finds it (TF1 ExponentialMovingAverage, one
 // correctly rounded fp32 op per TF op): d = fp32(decay), in num_updates mode d = min(d, (1 + fp32(n)) / (10 + fp32(n)));
@@ -544,6 +622,23 @@ __device__ __forceinline__ void accumulate_tile(const TileDesc d, const KernelPa
 template <int CAP, bool FROM_ZERO, bool H = false>
 __global__ void __launch_bounds__(kThreads)
 accumulate_kernel(const __grid_constant__ KernelParams<CAP> prm) {
+  if (prm.sched.state) {
+    // device schedule: every CTA checks the step before its tile; the last one through advances it
+    __shared__ SchedLaunch s_sl;
+    if (threadIdx.x == 0) sched_load(prm.sched, false, s_sl);
+    __syncthreads();
+    if (!s_sl.ok) { sched_refuse(prm.sched); return; }
+    if ((int)blockIdx.x < prm.num_tiles) accumulate_tile<FROM_ZERO, H>(prm.tiles[blockIdx.x], prm);
+    if (threadIdx.x == 0) {
+      if (blockIdx.x == 0) { prm.stats[0] = 0.f; prm.stats[1] = s_sl.lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f; }
+      __threadfence();
+      if (atomicAdd(prm.sched.done, 1u) == gridDim.x - 1u) {
+        sched_finish(prm.sched, s_sl, false, 0.f, 0.f);
+        *prm.sched.done = 0u;
+      }
+    }
+    return;
+  }
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     prm.stats[0] = 0.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f;
   }
@@ -573,8 +668,11 @@ __global__ void ema_init_kernel(EmaState* st, long long num_updates) {
 // H: p is the master slab (always 16-byte aligned); the model copy is stored after it.
 // EMA: the average e (slab `ema`, always 16-byte aligned) is read with p and stored after it: e - (e - p) * c.
 // dv: the launch's divisor (N, or the window weight W).
+// lr, bc2, bc1: the step's learning rate and GACCUM_ADAM's bias-correction terms (Scalars / LrMultParams, or the device
+// schedule's).
 template <int VARIANT, bool H, int CAP, bool EMA = false>
 __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams<CAP>& prm, const Divisor dv,
+                                            const float lr, const float bc2, const float bc1,
                                             float* ema = nullptr, const float ema_c = 0.f) {
   const Grad<H> g(prm, d);
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
@@ -588,7 +686,7 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
   if constexpr (H) { q = model_ptr(prm, d); bf16 = prm.half.bf16 != 0; }
   const bool decay = (d.tensor_flags >> 31) != 0;
   const Scalars& sc = prm.sc;
-  const float rate = tile_rate<VARIANT>(sc.lr, tensor_mult(prm.lrm, d), prm.lrm.bc2, prm.lrm.bc1);
+  const float rate = tile_rate<VARIANT>(lr, tensor_mult(prm.lrm, d), bc2, bc1);
   float4* a4 = reinterpret_cast<float4*>(a);
   float4* m4 = reinterpret_cast<float4*>(m);
   float4* v4 = reinterpret_cast<float4*>(v);
@@ -635,29 +733,36 @@ apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     __shared__ EmaLaunch s_ema_launch;
     s_ema = &s_ema_launch;
   }
-  const bool counted = EMA || ww != nullptr;   // launch-uniform
+  __shared__ SchedLaunch s_sl;
+  const bool sched = prm.sched.state != nullptr;   // launch-uniform
+  const bool counted = EMA || ww != nullptr || sched;
   if (counted) {
     if (threadIdx.x == 0) {
       if constexpr (EMA) ema_load(ep, *s_ema);
       s_dv = launch_divisor(prm);
+      if (sched) sched_load(prm.sched, true, s_sl);
     }
     __syncthreads();
+    if (sched && !s_sl.ok) { sched_refuse(prm.sched); return; }
   }
   const Divisor dv = ww ? s_dv : Divisor{prm.sc.nf, prm.sc.inv_nf};
+  const float lr = sched ? s_sl.lr : prm.sc.lr;
+  const float bc2 = sched ? s_sl.bc2 : prm.lrm.bc2, bc1 = sched ? s_sl.bc1 : prm.lrm.bc1;
   if ((int)blockIdx.x < prm.num_tiles) {
-    if constexpr (EMA) update_tile<VARIANT, H, CAP, true>(prm.tiles[blockIdx.x], prm, dv, ep.slab, s_ema->c);
-    else update_tile<VARIANT, H>(prm.tiles[blockIdx.x], prm, dv);
+    if constexpr (EMA) update_tile<VARIANT, H, CAP, true>(prm.tiles[blockIdx.x], prm, dv, lr, bc2, bc1, ep.slab, s_ema->c);
+    else update_tile<VARIANT, H>(prm.tiles[blockIdx.x], prm, dv, lr, bc2, bc1);
   }
   if (counted && threadIdx.x == 0) {
     __threadfence();
     if (atomicAdd(ep.done, 1u) == gridDim.x - 1u) {
       if constexpr (EMA) ema_finish(ep, *s_ema);
       if (ww) window_finish(ww, s_dv.nf);
+      if (sched) sched_finish(prm.sched, s_sl, VARIANT == 1, prm.sc.b1, prm.sc.b2);
       *ep.done = 0u;
     }
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) {
-    prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f;
+    prm.stats[0] = 1.f; prm.stats[1] = lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f;
   }
 }
 
@@ -1072,6 +1177,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   __shared__ LossScaleState s_ls;        // loss-scaled: the state as this launch found it
   __shared__ float s_bc[2];              // loss-scaled GACCUM_ADAM: bc2, bc1 (LrMultParams) from the device's beta powers
   __shared__ Divisor s_dv;               // the launch's divisor: N, or W as this launch found it
+  __shared__ SchedLaunch s_sl;           // device schedule: the step as this launch found it
   __shared__ int s_skip;
   __shared__ uint32_t s_set;
   __shared__ __align__(8) uint64_t s_full1[kGroups][kP1Slots], s_empty1[kGroups][kP1Slots];
@@ -1128,9 +1234,12 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     }
     if constexpr (EMA) ema_load(*ema, *s_ema);
     s_dv = launch_divisor(prm);
+    if (prm.sched.state) sched_load(prm.sched, true, s_sl);
   }
   for (int i = threadIdx.x; i < (kConsumerThreads / 32) * kAccBins; i += kClipThreads) (&s_bins[0][0])[i] = 0ull;
   __syncthreads();
+  // device schedule: every CTA read the same step, so all of them leave here or none does (before any barrier)
+  if (prm.sched.state && !s_sl.ok) { sched_refuse(prm.sched); return; }
   LaunchCounters* const ctr = prm.counters + s_set;
   clear_other_counters(prm.counters, s_set);
 
@@ -1241,7 +1350,8 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
       bool past_barrier = false;
       // the bias corrections of the tiles' alpha_t (GACCUM_ADAM): the step's, or under loss scaling the device block's,
       // which thread 0 wrote before the set-up barrier
-      float bc2 = prm.lrm.bc2, bc1 = prm.lrm.bc1;
+      float bc2 = prm.lrm.bc2, bc1 = prm.lrm.bc1, lr = prm.sc.lr;
+      if (prm.sched.state) { lr = s_sl.lr; bc2 = s_sl.bc2; bc1 = s_sl.bc1; }    // the device schedule's step
       if constexpr (loss_scaled(MODE) && VARIANT == 1) { bc2 = s_bc[0]; bc1 = s_bc[1]; }
       const unsigned long long pool_n = (unsigned long long)max(0, nt - pool_lo);
       while (true) {
@@ -1275,7 +1385,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         SlotMeta* meta = &s_meta2[grp][rp.slot];
         meta->d = d;
         meta->stash_slot = in_stash ? stash_slot : kNoStash;
-        meta->rate = tile_rate<VARIANT>(prm.sc.lr, tensor_mult(prm.lrm, d), bc2, bc1);
+        meta->rate = tile_rate<VARIANT>(lr, tensor_mult(prm.lrm, d), bc2, bc1);
         if (nvec > 0) {
           const size_t soff = (size_t)d.soff32 * kSlabAlign;
           float4* dst = ring + (size_t)rp.slot * kP2SlotVecs;
@@ -1397,10 +1507,12 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
       }
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) {
-      prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s;
+      prm.stats[0] = 1.f; prm.stats[1] = prm.sched.state ? s_sl.lr : prm.sc.lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s;
       if constexpr (loss_scaled(MODE)) ls_finish<VARIANT == 1>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
       if constexpr (EMA) { if (!skip) ema_finish(*ema, *s_ema); }
       if (prm.ww.state) window_finish(prm.ww.state, s_dv.nf);
+      // loss-scaled: the beta powers live in the loss-scaling block, which ls_finish advanced
+      if (prm.sched.state) sched_finish(prm.sched, s_sl, !loss_scaled(MODE) && VARIANT == 1, prm.sc.b1, prm.sc.b2);
     }
   }
   __syncthreads();

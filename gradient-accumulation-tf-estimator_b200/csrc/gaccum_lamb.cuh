@@ -204,6 +204,7 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   __shared__ LossScaleState s_ls;
   __shared__ float s_bcast[2];
   __shared__ Divisor s_dv;               // the launch's divisor: N, or W as this launch found it
+  __shared__ SchedLaunch s_sl;           // device schedule: the step as this launch found it
   __shared__ int s_skip;
   __shared__ uint32_t s_set;
 
@@ -223,9 +224,12 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     if constexpr (loss_scaled(MODE)) ls_load(prm.ls.state, s_ls);
     if constexpr (EMA) ema_load(prm.ema, *s_ema);
     s_dv = launch_divisor(prm);
+    if (prm.sched.state) sched_load(prm.sched, true, s_sl);
   }
   for (int i = threadIdx.x; i < kWarps * 2 * kAccBins; i += kThreads) (&s_bins[0][0][0])[i] = 0ull;
   __syncthreads();
+  // device schedule: every CTA read the same step, so all of them leave here or none does (before any barrier)
+  if (prm.sched.state && !s_sl.ok) { sched_refuse(prm.sched); return; }
   const uint32_t set = s_set;
   // the launch's divisor, held in registers: read from shared memory at every use it slowed the unweighted apply 1.6-2.2 %
   const Divisor dv = s_dv;
@@ -239,6 +243,8 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   }
   float inv_s = 1.0f;
   float b1p = lb.beta1_power, b2p = lb.beta2_power;
+  const float lr = prm.sched.state ? s_sl.lr : prm.sc.lr;
+  if (prm.sched.state) { b1p = s_sl.b1p; b2p = s_sl.b2p; }
   if constexpr (loss_scaled(MODE)) {
     inv_s = __fdiv_rn(1.0f, s_ls.scale);   // exact: S is a power of two
     b1p = s_ls.beta1_power;
@@ -356,16 +362,18 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     const TileDesc d = prm.tiles[t];
     // ratio * lr_t first, lr_t = lr * mult[t] (LrMultParams)
     const float rlr = skip ? 0.f : __fmul_rn(__ldcg(&lb.ratios[d.tensor_flags & 0x7fffffffu]),
-                                             tile_rate<0>(prm.sc.lr, tensor_mult(prm.lrm, d), 0.f, 1.f));
+                                             tile_rate<0>(lr, tensor_mult(prm.lrm, d), 0.f, 1.f));
     if constexpr (EMA) lamb_write_tile<H, CAP, true>(d, prm, rlr, !skip, prm.ema.slab, s_ema->c);
     else lamb_write_tile<H>(d, prm, rlr, !skip);
   }
 
   if (blockIdx.x == 0 && threadIdx.x == 0) {
-    prm.stats[0] = 1.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s_bcast[0];
+    prm.stats[0] = 1.f; prm.stats[1] = lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s_bcast[0];
     if constexpr (loss_scaled(MODE)) ls_finish<true>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
     if constexpr (EMA) { if (!skip) ema_finish(prm.ema, *s_ema); }
     if (prm.ww.state) window_finish(prm.ww.state, s_dv.nf);
+    // loss-scaled: the beta powers live in the loss-scaling block, which ls_finish advanced
+    if (prm.sched.state) sched_finish(prm.sched, s_sl, !loss_scaled(MODE), prm.sc.b1, prm.sc.b2);
   }
 }
 

@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import ADAM, ADAM_WEIGHT_DECAY, LAMB, EmaConfig, HParams, LossScaleConfig, Plan, StepArgs
+from ._lib import ADAM, ADAM_WEIGHT_DECAY, LAMB, EmaConfig, HParams, LossScaleConfig, Plan, ScheduleConfig, StepArgs
 
 
 def _f32(x) -> float:
@@ -40,6 +40,22 @@ def _pinned_zeros(n: int) -> torch.Tensor:
         return t.pin_memory()
     except Exception:
         return t
+
+
+def _window_position(g: int, n: int) -> int:
+    """The position of micro-step g in its window: the step cast to int32 (as gaccum_is_apply_step does), modulo N."""
+    return ((int(g) + 0x80000000) % 0x100000000 - 0x80000000) % n
+
+
+class ScheduleLr:
+    """The learning rate of a device-scheduled train op as a host function (for logging and comparisons): the same
+    fp32 evaluation of create_optimizer's schedule the device performs (gaccum_learning_rate)."""
+
+    def __init__(self, cfg: ScheduleConfig):
+        self.cfg = cfg
+
+    def __call__(self, step: int) -> float:
+        return _lib.learning_rate(self.cfg.init_lr, self.cfg.num_train_steps, self.cfg.num_warmup_steps, step)
 
 
 # the state_dict key of a weighted train op's running window weight W (an fp32 scalar)
@@ -98,9 +114,11 @@ class _DeviceTrainOp(_TrainOpCore):
 
     def __init__(self, params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step,
                  loss_scale: Optional[LossScaleConfig] = None, exclude_from_layer_adaptation=None,
-                 lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False):
+                 lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False,
+                 device_schedule: Optional[ScheduleConfig] = None):
         self.ema: Optional[torch.Tensor] = None          # the moving average of the weights, when one is kept
         self._ema_state: Optional[torch.Tensor] = None
+        self._sched_state: Optional[torch.Tensor] = None  # the device schedule's block, when one is kept
         if not params:
             raise ValueError("no trainable variables")
         # checked before the plan exists, so a bad table fails without touching the device
@@ -133,6 +151,90 @@ class _DeviceTrainOp(_TrainOpCore):
             self._ww_state = torch.zeros(4, dtype=torch.float32, device=self.device)
             self.plan.set_window_weight(self._ww_state.data_ptr())
             self.window_weight = self._ww_state[0]
+        if device_schedule is not None:
+            # gaccum_schedule_state: 6 x 8 bytes.  From here on global_step, the lr and (without loss scaling) the beta
+            # powers live on the device; the host keeps only the position in the window, which picks the branch
+            if lr_fn is not None and not isinstance(lr_fn, ScheduleLr):
+                raise ValueError("a device-scheduled train op computes its learning rate on the device: pass "
+                                 "lr_fn=None (or device_schedule_lr(cfg))")
+            self.lr_fn = ScheduleLr(device_schedule)
+            self._sched_state = torch.zeros(6, dtype=torch.int64, device=self.device)
+            self.plan.set_device_schedule(device_schedule, self._sched_state.data_ptr())
+            self._capturing = False
+            self._write_schedule(self._step, self.beta1_power, self.beta2_power)
+
+    # -- global_step: a host int, or the device schedule's counter ---------------------------------------------------
+    @property
+    def global_step(self) -> int:
+        """The pre-increment step of the next micro-step.  With a device schedule this is a SYNCHRONOUS read of the
+        device counter: a training loop that wants the step without waiting reads ``global_step_tensor`` instead."""
+        if self._sched_state is None:
+            return self._step
+        return self.schedule_state()["global_step"]
+
+    @global_step.setter
+    def global_step(self, g: int) -> None:
+        self._step = int(g)
+        if getattr(self, "_sched_state", None) is not None:
+            st = self._read_schedule()      # keeps the beta powers; a refused schedule starts afresh
+            self._write_schedule(self._step, st["beta1_power"], st["beta2_power"])
+
+    @property
+    def device_schedule(self) -> bool:
+        return self._sched_state is not None
+
+    @property
+    def global_step_tensor(self) -> torch.Tensor:
+        """The device counter as a 0-d int64 CUDA tensor (a view: no copy, no sync).  Device-scheduled ops only."""
+        if self._sched_state is None:
+            raise ValueError("this train op keeps global_step on the host (device_schedule=None)")
+        return self._sched_state[0]
+
+    def _write_schedule(self, g: int, beta1_power: float, beta2_power: float) -> None:
+        """gaccum_schedule_init: the step, the beta powers (ignored under loss scaling, whose block holds them) and
+        refused = 0, stream-ordered on the current stream."""
+        self.plan.schedule_init(self._sched_state.data_ptr(), g, beta1_power, beta2_power, self._stream())
+        self._phase = _window_position(g, self.N)
+
+    def schedule_state(self) -> Dict[str, float]:
+        """Synchronously read the device schedule: global_step, beta1_power and beta2_power (under loss scaling the
+        loss-scaling block's) and refused.  Raises RuntimeError if a launch was refused (see gaccum.h)."""
+        if self._sched_state is None:
+            raise ValueError("this train op keeps global_step on the host (device_schedule=None)")
+        out = self._read_schedule()
+        if out["refused"]:
+            raise RuntimeError(f"the device schedule refused a launch at global_step {out['global_step']}: it found the "
+                               "step selecting the other branch (a CUDA graph captured or replayed across a window "
+                               "boundary?).  Every launch since was a no-op; nothing after that step was computed")
+        return out
+
+    def _read_schedule(self) -> Dict[str, float]:
+        words = self._sched_state.cpu()
+        f, i = words.view(torch.float32), words.view(torch.int32)
+        out = {"global_step": int(words[0]), "beta1_power": float(f[9]), "beta2_power": float(f[10]),
+               "refused": bool(i[11])}
+        if self._ls_state is not None:
+            ls = self._ls_state.cpu()
+            out["beta1_power"], out["beta2_power"] = float(ls[4]), float(ls[5])
+        return out
+
+    def _scheduled_step_args(self) -> StepArgs:
+        """The host's share of a device-scheduled micro-step: its position in the window (all the branch and the
+        first-accumulate decision depend on).  A CUDA graph must start at a window start: refused here when the
+        capture follows eager micro-steps; a graph that starts or ends mid-window is always refused by the device when
+        replayed (gaccum.h: `refused`)."""
+        capturing = torch.cuda.is_current_stream_capturing()
+        if capturing and not self._capturing and self._phase != 0:
+            raise ValueError(f"a CUDA graph of a device-scheduled train op must start at a window start: this capture "
+                             f"starts at micro-step {self._phase} of a window of {self.N}")
+        self._capturing = capturing
+        return StepArgs(self._phase, self.N, 0, 0.0, 0.0, 0.0, 0.0)
+
+    def _scheduled_after(self) -> bool:
+        applied = self._phase == 0
+        self._phase = (self._phase + 1) % self.N
+        self.last_applied = applied
+        return applied
 
     def _init_ema(self, cfg: EmaConfig, weights: Callable[[int], torch.Tensor]) -> None:
         """Keep an exponential moving average of ``weights(i)`` (the fp32 weights the apply updates).  TF initialises
@@ -313,14 +415,15 @@ class GaccumTrainOp(_DeviceTrainOp):
                  global_step: int = 0, accum: Optional[torch.Tensor] = None,
                  loss_scale: Optional[LossScaleConfig] = None,
                  exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None,
-                 lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False):
+                 lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False,
+                 device_schedule: Optional[ScheduleConfig] = None):
         dtypes = {p.dtype for p in params}
         if len(dtypes) > 1 and dtypes & set(_HALF_DTYPES):
             raise ValueError(f"parameters of mixed dtypes ({', '.join(sorted(str(d) for d in dtypes))}): "
                              "a 16-bit model must be all bf16 or all fp16")
         self.param_dtype = params[0].dtype if len(dtypes) == 1 and params[0].dtype in _HALF_DTYPES else torch.float32
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale,
-                         exclude_from_layer_adaptation, lr_multipliers, window_weight)
+                         exclude_from_layer_adaptation, lr_multipliers, window_weight, device_schedule)
         for p in self.params:
             if p.dtype != self.param_dtype or not p.is_contiguous() or p.device != self.device:
                 if self.param_dtype != torch.float32:
@@ -391,6 +494,12 @@ class GaccumTrainOp(_DeviceTrainOp):
     def run_bound(self, grad_table, stream: Optional[int] = None) -> bool:
         """``run`` with a pointer table from ``bind`` (no per-step Python work over T tensors).
         Parameters must not have been re-allocated since construction / the last ``run``."""
+        if self._sched_state is not None:
+            # device schedule: the launch reads the step, lr and beta powers from the block and advances them
+            args = self._scheduled_step_args()
+            self.plan.step(grad_table, self._param_ptrs, self._accum_ptr, self._m_ptr, self._v_ptr, args,
+                           self._stream(stream))
+            return self._scheduled_after()
         g = self.global_step
         lr = self.lr_fn(g)
         if stream is None:
@@ -401,10 +510,12 @@ class GaccumTrainOp(_DeviceTrainOp):
 
     def accumulate_only(self, grads: Sequence[Optional[torch.Tensor]]) -> None:
         """The false branch alone (used by the data-parallel driver); does not touch global_step."""
+        self._refuse_schedule("accumulate_only")
         self.plan.accumulate(self._grad_table(grads), self.accum.data_ptr(), self._stream())
 
     def apply_only(self, grads: Optional[Sequence[Optional[torch.Tensor]]] = None) -> None:
         """The true branch alone; ``grads=None`` applies the accumulators as they are."""
+        self._refuse_schedule("apply_only")
         lr = _f32(self.lr_fn(self.global_step))
         self._refresh_param_table()
         self.plan.apply(self._grad_table(grads) if grads is not None else None, self._param_ptrs,
@@ -435,6 +546,10 @@ class GaccumTrainOp(_DeviceTrainOp):
         self._k_done, self._d2h_done = torch.cuda.Event(), torch.cuda.Event()
         self._host_calls = 0
         self._stats_ring = _pinned_zeros(4)
+
+    def _refuse_schedule(self, what: str) -> None:
+        if self._sched_state is not None:
+            raise ValueError(f"{what} does not support a device schedule: a device-scheduled train op steps with run()")
 
     def run_host(self, host_grads: Sequence[Optional[torch.Tensor]],
                  host_params_out: Optional[Sequence[torch.Tensor]] = None) -> bool:
@@ -494,15 +609,18 @@ class GaccumTrainOp(_DeviceTrainOp):
         """Per-tensor copies under the reference's names (optimization.py:78, 137-148).  A 16-bit model stores its
         fp32 master weights under the variables' names, as TF mixed precision saves its fp32 variables, so fp32 and
         16-bit checkpoints load into each other."""
-        out: Dict[str, torch.Tensor] = {"global_step": torch.tensor(self.global_step, dtype=torch.int64)}
+        sched = self.schedule_state() if self._sched_state is not None else None
+        g = self.global_step if sched is None else sched["global_step"]
+        out: Dict[str, torch.Tensor] = {"global_step": torch.tensor(g, dtype=torch.int64)}
         for i, n in enumerate(self.names):
             out[n] = self.params[i].detach().clone() if self.master is None else self.master_view(i).clone()
             out[n + "/adam_m"] = self.m_view(i).clone()
             out[n + "/adam_v"] = self.v_view(i).clone()
             out[n + "/accum_grad"] = self.accum_view(i).clone()
         if self.hp.variant in (ADAM, LAMB):
-            out["beta1_power"] = torch.tensor(self.beta1_power, dtype=torch.float32)
-            out["beta2_power"] = torch.tensor(self.beta2_power, dtype=torch.float32)
+            b1, b2 = (self.beta1_power, self.beta2_power) if sched is None else (sched["beta1_power"], sched["beta2_power"])
+            out["beta1_power"] = torch.tensor(b1, dtype=torch.float32)
+            out["beta2_power"] = torch.tensor(b2, dtype=torch.float32)
         if self._ls_state is not None:
             self._loss_scale_state_dict(out)
         if self.ema is not None:
@@ -530,6 +648,8 @@ class GaccumTrainOp(_DeviceTrainOp):
         elif self.hp.variant in (ADAM, LAMB) and "beta1_power" in sd:
             self.beta1_power = float(sd["beta1_power"])
             self.beta2_power = float(sd["beta2_power"])
+            if self._sched_state is not None:        # the beta powers' home is the schedule block
+                self._write_schedule(int(sd["global_step"]), self.beta1_power, self.beta2_power)
         if self.ema is not None:
             self._load_ema_state(sd, strict)
         if self._ww_state is not None:
@@ -585,11 +705,12 @@ class PackedTrainOp(_DeviceTrainOp):
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, loss_scale: Optional[LossScaleConfig] = None,
                  exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None,
-                 lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False):
+                 lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False,
+                 device_schedule: Optional[ScheduleConfig] = None):
         # autograd accumulates a 16-bit parameter's gradient in its own dtype: it cannot add into an fp32 slab
         _refuse_half(params, "PackedTrainOp")
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale,
-                         exclude_from_layer_adaptation, lr_multipliers, window_weight)
+                         exclude_from_layer_adaptation, lr_multipliers, window_weight, device_schedule)
         self.param_slab = self._zeros_slab()
         self.accum = self._zeros_slab()
         with torch.no_grad():
@@ -609,13 +730,25 @@ class PackedTrainOp(_DeviceTrainOp):
         ``p.grad`` (== accum).  Returns True if it applied (optimization.py:91, pre-increment predicate).  A weighted op
         (window_weight=True) takes the micro-batch's weight, as ``GaccumTrainOp.run`` does."""
         self._add_weight(weight, stream)
-        g = self.global_step
+        sched = self._sched_state is not None
+        args = self._scheduled_step_args() if sched else None
+        g = self._phase if sched else self.global_step
         applied = _lib.is_apply_step(g, self.N)
+        if sched and not applied:
+            # the gradients are already in accum: the launch only advances the device schedule (one CTA)
+            self.plan.step_packed(0, 0, self.accum.data_ptr(), 0, 0, args, -1, self._stream(stream))
+            self.launches += 1
+            return self._scheduled_after()
         if applied:
             for p, o in zip(self.params, self.plan.offsets):     # a caller that dropped the views broke the contract
                 # (a zero-element view reports data_ptr() 0 wherever it points: there is nothing it could alias)
                 if p.grad is None or (p.numel() > 0 and p.grad.data_ptr() != self.accum.data_ptr() + 4 * o):
                     raise RuntimeError("p.grad no longer aliases the packed accumulator (zero_grad(set_to_none=True)?)")
+            if sched:
+                self.plan.step_packed(0, self.param_slab.data_ptr(), self.accum.data_ptr(), self.m.data_ptr(),
+                                      self.v.data_ptr(), args, -1, self._stream(stream))
+                self.launches += 1
+                return self._scheduled_after()
             lr = self.lr_fn(g)
             self.plan.step_packed(0, self.param_slab.data_ptr(), self.accum.data_ptr(), self.m.data_ptr(), self.v.data_ptr(),
                                   self._step_args(g, lr), 1, self._stream(stream))
@@ -663,7 +796,9 @@ class HostTrainOp(_TrainOpCore):
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, device: int = 0, loss_scale: Optional[LossScaleConfig] = None,
                  ema: Optional[EmaConfig] = None, lr_multipliers: Optional[Sequence[float]] = None,
-                 window_weight: bool = False):
+                 window_weight: bool = False, device_schedule: Optional[ScheduleConfig] = None):
+        if device_schedule is not None:
+            raise ValueError("HostTrainOp does not support a device schedule; use GaccumTrainOp")
         if ema is not None:
             raise ValueError("HostTrainOp does not keep a moving average of the weights; use GaccumTrainOp")
         if window_weight:

@@ -317,6 +317,60 @@ typedef struct gaccum_window_weight_state {
 } gaccum_window_weight_state;
 GACCUM_API int gaccum_plan_set_window_weight(gaccum_plan* plan, gaccum_window_weight_state* state);
 
+/* The device schedule: global_step, the learning rate and TF1's beta powers kept on the device, so a CUDA graph of one
+ * window of micro-steps (producer + train op) can be replayed for the whole run.  Off unless set; a plan without it
+ * takes lr and the beta powers from gaccum_step_args, exactly as before.
+ *   - The block (gaccum_schedule_state, caller-owned device memory) holds the step, the beta powers and the schedule
+ *     constants; gaccum_schedule_init writes it, afterwards only the launches do.
+ *   - Every launch of gaccum_step / gaccum_step_packed reads g = global_step, computes
+ *         lr = gaccum_learning_rate(init_lr, num_train_steps, num_warmup_steps, g)
+ *     with the same fp32 ops in the same order (bit for bit the host's lr; create_optimizer's polynomial decay with
+ *     end_lr = 0 and power = 1, optimization.py:29-52), uses it wherever gaccum_step_args.lr would go (the per-tensor
+ *     multipliers then apply as before, lr_t = fp32(lr * mult[t])), writes it to the stats, and stores
+ *     global_step = g + 1 -- accumulate launches and windows that loss scaling skips included.
+ *   - The beta powers have ONE home.  Without loss scaling it is this block: an applied window of GACCUM_ADAM or
+ *     GACCUM_LAMB uses them, then multiplies each by fp32(beta) once (TF1 AdamOptimizer._finish).  Under loss scaling it
+ *     is the loss-scaling block (gaccum_loss_scale_state.beta{1,2}_power), as without a device schedule; this block's
+ *     beta fields are then 0 and unused.
+ *   - The host still chooses the branch, from gaccum_step_args.global_step and accum_n as before.  Only that step's
+ *     position in its window matters, g mod N: a window is always the same N launches (N - 1 accumulates, the first
+ *     without reading the accumulators, then an apply), so a graph captured over whole windows replays correctly with
+ *     any g.  Each launch checks that g selects its branch ((int32)g % N == 0 exactly for an apply).  A launch that
+ *     finds otherwise -- e.g. a replayed graph whose capture did not start at a window start, or did not end at a window
+ *     end -- changes nothing and sets `refused`; from then on every launch on the plan is a no-op, until
+ *     gaccum_schedule_init rewrites the block.  gaccum_step_args.lr and .beta{1,2}_power are ignored.
+ *   - gaccum_step_packed must use force_branch = -1; on an accumulate step its grad_slab may be NULL (the gradients
+ *     are already in accum): the launch then only advances the schedule.
+ * gaccum_plan_set_device_schedule is host-only: validates `cfg` (end_lr must be 0 and power 1) and keeps `block`
+ * (16-byte aligned; not dereferenced here).  Allowed only before the plan's first compute call; combines with the other
+ * setters in any order.  gaccum_accumulate and gaccum_apply (no step to check), gaccum_step_dp, gaccum_apply_dp,
+ * gaccum_host_session_create and gaccum_step_host refuse such a plan with GACCUM_EINVAL. */
+typedef struct gaccum_schedule_config {
+  double init_lr;           /* optimization.py:29, rounded to fp32 as the host schedule does */
+  int64_t num_train_steps;  /* >= 0 */
+  int64_t num_warmup_steps; /* >= 0; 0: no warm-up */
+  double end_lr;            /* must be 0 */
+  double power;             /* must be 1 */
+} gaccum_schedule_config;
+typedef struct gaccum_schedule_state {
+  int64_t global_step;      /* the pre-increment step of the next launch */
+  int64_t num_train_steps;
+  int64_t num_warmup_steps;
+  float init_lr;            /* fp32(init_lr) */
+  float end_lr;             /* 0 */
+  float power;              /* 1 */
+  float beta1_power;        /* without loss scaling: TF1's beta1^t (see above) */
+  float beta2_power;
+  int32_t refused;          /* 1 once a launch found global_step selecting the other branch */
+} gaccum_schedule_state;    /* 48 bytes */
+GACCUM_API int gaccum_plan_set_device_schedule(gaccum_plan* plan, const gaccum_schedule_config* cfg,
+                                               gaccum_schedule_state* block);
+/* Writes the block on `stream` (stream-ordered; the call returns once the host values are staged): global_step,
+ * beta{1,2}_power (ignored under loss scaling: they live in the loss-scaling block), the plan's schedule constants and
+ * refused = 0.  `block` must be the one given to gaccum_plan_set_device_schedule. */
+GACCUM_API int gaccum_schedule_init(gaccum_plan* plan, gaccum_schedule_state* block, int64_t global_step,
+                                    float beta1_power, float beta2_power, gaccum_stream_t stream);
+
 /* ---- the hot path --------------------------------------------------------------------- */
 /* One micro-step of the train_op (optimization.py:91-94): if gaccum_is_apply_step() the apply
  * branch (assign_add -> /N -> clip_by_global_norm -> apply_gradients -> zero; :80-88), else
