@@ -186,6 +186,7 @@ def _load():
         "gaccum_plan_set_window_weight": (C.c_int, [vp, vp]),
         "gaccum_plan_set_device_schedule": (C.c_int, [vp, C.POINTER(ScheduleConfig), vp]),
         "gaccum_schedule_init": (C.c_int, [vp, vp, i64, C.c_float, C.c_float, vp]),
+        "gaccum_plan_set_tensor_norms": (C.c_int, [vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -399,6 +400,11 @@ class Plan:
                       stream: int = 0) -> None:
         _check(_load().gaccum_schedule_init(self._h, block or None, int(global_step), float(beta1_power),
                                             float(beta2_power), stream))
+
+    def set_tensor_norms(self, device_out: int) -> None:
+        """Write per-tensor gradient, weight and update norms on every apply (before the first compute call):
+        ``device_out`` points to 3 x T floats of 16-byte aligned device memory, row t = (gradient, weight, update)."""
+        _check(_load().gaccum_plan_set_tensor_norms(self._h, device_out or None))
 
     def close(self) -> None:
         if getattr(self, "_h", None):

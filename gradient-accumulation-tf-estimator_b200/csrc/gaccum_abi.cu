@@ -100,6 +100,10 @@ struct gaccum_plan {
   // the device schedule (gaccum_plan_set_device_schedule); set only while `computed` is false
   gaccum_schedule_config sched_cfg{};
   gaccum_schedule_state* sched_state = nullptr;
+  // per-tensor norms of the apply step (gaccum_plan_set_tensor_norms); set only while `computed` is false.  d_norms holds
+  // the partials, the chunk tables and the counters of NormParams in one allocation
+  NormParams norms{};
+  void* d_norms = nullptr;
   std::mutex mu;
   std::map<const void*, int> grid_cache;   // cooperative kernel -> CTAs that fit on one SM (fit)
 };
@@ -305,6 +309,7 @@ static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, f
   prm.sched.state = reinterpret_cast<ScheduleState*>(pl->sched_state);
   prm.sched.done = pl->d_ema_done;
   prm.sched.accum_n = a ? a->accum_n : 1;
+  prm.norms = pl->norms;
 }
 
 template <int CAP>
@@ -379,6 +384,7 @@ static int check_args(const gaccum_step_args* a) {
 static void free_plan_device(gaccum_plan* pl) {
   cudaFree(pl->d_tiles); cudaFree(pl->d_partials); cudaFree(pl->d_stats); cudaFree(pl->d_dp_sync); cudaFree(pl->d_barrier); cudaFree(pl->d_counters);
   cudaFree(pl->d_adapt); cudaFree(pl->d_lamb_acc); cudaFree(pl->d_ratios); cudaFree(pl->d_ema_done); cudaFree(pl->d_lr_mult);
+  cudaFree(pl->d_norms);
 #ifdef GACCUM_EXPERIMENTS
   cudaFree(pl->d_debug);
 #endif
@@ -765,6 +771,65 @@ int gaccum_schedule_init(gaccum_plan* pl, gaccum_schedule_state* block, int64_t 
   return GACCUM_OK;
 }
 
+int gaccum_plan_set_tensor_norms(gaccum_plan* pl, float* device_out) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (!device_out || !aligned16_host(device_out)) return fail(GACCUM_EINVAL, "device_out must be a 16-byte aligned device pointer");
+  if (pl->device < 0) return fail(GACCUM_EINVAL, "layout-only plan (device=-1): per-tensor norms need a device plan");
+  if (pl->computed) return fail(GACCUM_EINVAL, "per-tensor norms can only be set before the plan's first compute call");
+  // the tables of NormParams: tensor t's tiles and chunks of up to kNormChunk of them
+  const int32_t T = pl->T;
+  const int64_t nt = (int64_t)pl->tiles.size();
+  std::vector<int32_t> tile_begin((size_t)T + 1, 0), chunk_begin((size_t)T + 1, 0), chunk_tensor;
+  for (int32_t t = 0; t < T; ++t) {
+    const int64_t tiles = (pl->numel[t] + kTile - 1) / kTile;
+    tile_begin[t + 1] = tile_begin[t] + (int32_t)tiles;
+    const int64_t chunks = (tiles + kNormChunk - 1) / kNormChunk;
+    chunk_begin[t + 1] = chunk_begin[t] + (int32_t)chunks;
+    chunk_tensor.insert(chunk_tensor.end(), (size_t)chunks, t);
+  }
+  if (tile_begin[T] != nt) return fail(GACCUM_EINVAL, "internal error: the tile table does not match the tensors");
+  const int64_t nc = chunk_begin[T];
+  // doubles first (8-byte aligned), then the int32 tables and the counters
+  const size_t b_tile = sizeof(double) * (size_t)nt * kNormCols * kNormWarps;
+  const size_t b_chunk = sizeof(double) * (size_t)nc * kNormCols;
+  const size_t b_ints = sizeof(int32_t) * (2 * ((size_t)T + 1) + 2 * (size_t)nc + (size_t)T);
+  DeviceGuard guard(pl->device);
+  if (pl->d_norms) { cudaFree(pl->d_norms); pl->d_norms = nullptr; pl->norms = NormParams{}; }
+  void* blk = nullptr;
+  CUDA_TRY(cudaMalloc(&blk, b_tile + b_chunk + b_ints + 16));
+  NormParams np{};
+  np.tile_part = reinterpret_cast<double*>(blk);
+  np.chunk_part = reinterpret_cast<double*>(reinterpret_cast<char*>(blk) + b_tile);
+  int32_t* ints = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(blk) + b_tile + b_chunk);
+  np.tile_begin = ints;
+  np.chunk_begin = ints + (T + 1);
+  np.chunk_tensor = ints + 2 * (T + 1);
+  np.chunk_done = reinterpret_cast<unsigned int*>(ints + 2 * (T + 1) + nc);
+  np.tensor_done = reinterpret_cast<unsigned int*>(ints + 2 * (T + 1) + 2 * nc);
+  np.num_chunks = (int32_t)nc;
+  np.out = device_out;
+  cudaError_t e = cudaMemset(ints, 0, b_ints);
+  if (e == cudaSuccess) e = cudaMemcpy(ints, tile_begin.data(), sizeof(int32_t) * ((size_t)T + 1), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(ints + (T + 1), chunk_begin.data(), sizeof(int32_t) * ((size_t)T + 1), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && nc > 0)
+    e = cudaMemcpy(ints + 2 * (T + 1), chunk_tensor.data(), sizeof(int32_t) * (size_t)nc, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && T > 0) e = cudaMemset(device_out, 0, sizeof(float) * kNormCols * (size_t)T);   // 0 before the first apply
+  if (e == cudaSuccess) e = cudaStreamSynchronize(0);   // the memsets are stream-ordered: done before the setter returns
+  if (e != cudaSuccess) {
+    cudaFree(blk);
+    return fail(GACCUM_ECUDA, "tensor-norm setup failed: %s", cudaGetErrorString(e));
+  }
+  pl->d_norms = blk;
+  pl->norms = np;
+  return GACCUM_OK;
+}
+
+static int refuse_norms(const gaccum_plan* pl, const char* what) {
+  return pl && pl->norms.out
+             ? fail(GACCUM_EINVAL, "%s does not support per-tensor norms (gaccum_plan_set_tensor_norms)", what)
+             : GACCUM_OK;
+}
+
 static int accumulate_impl(gaccum_plan* pl, const float* const* grads, float* accum,
                            const gaccum_step_args* a, gaccum_stream_t stream) {
   if (int rc = check_compute(pl, accum, nullptr, nullptr, false)) return rc;
@@ -951,6 +1016,7 @@ int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* co
   if (int rc = refuse_lr_mult(pl, "the fused data-parallel apply")) return rc;
   if (int rc = refuse_window_weight(pl, "the fused data-parallel apply")) return rc;
   if (int rc = refuse_schedule(pl, "the fused data-parallel apply")) return rc;
+  if (int rc = refuse_norms(pl, "the fused data-parallel apply")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (comm->world < 2 || comm->world > GACCUM_MAX_RANKS || comm->rank < 0 || comm->rank >= comm->world)
     return fail(GACCUM_EINVAL, "world must be 2..%d and 0 <= rank < world", GACCUM_MAX_RANKS);
@@ -980,6 +1046,7 @@ int gaccum_step_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* con
   if (int rc = refuse_lr_mult(pl, "the fused data-parallel step")) return rc;
   if (int rc = refuse_window_weight(pl, "the fused data-parallel step")) return rc;
   if (int rc = refuse_schedule(pl, "the fused data-parallel step")) return rc;
+  if (int rc = refuse_norms(pl, "the fused data-parallel step")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (int rc = check_args(a)) return rc;
   if (!grads) return fail(GACCUM_EINVAL, "grads is NULL");
@@ -1066,6 +1133,7 @@ int gaccum_host_session_create(gaccum_host_session** out, gaccum_plan* pl) {
   if (int rc = refuse_lr_mult(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_window_weight(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_schedule(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse_norms(pl, "the host-buffer session")) return rc;
   if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): libgaccum has no CPU fallback, a CUDA device is required");
   DeviceGuard guard(pl->device);
   gaccum_host_session* s = new (std::nothrow) gaccum_host_session();
@@ -1180,6 +1248,7 @@ int gaccum_step_host(gaccum_host_session* s, const float* const* host_grads, flo
   if (int rc = refuse_lr_mult(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_window_weight(pl, "the host-buffer session")) return rc;
   if (int rc = refuse_schedule(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse_norms(pl, "the host-buffer session")) return rc;
   DeviceGuard guard(pl->device);
   const int b = (int)(s->calls & 1);
   ++s->calls;

@@ -25,6 +25,9 @@
 //
 // Exponential moving average of the weights (template flag EMA, gaccum_plan_set_ema): every apply kernel also reads the
 // average e and stores e - (e - p) * c after p, on applied windows only (+8 B/elem); see EmaParams.
+//
+// Per-tensor norms (launch-uniform, gaccum_plan_set_tensor_norms): every apply kernel also sums c^2, p^2 and (p - p')^2
+// per tile into plan scratch and reduces them per tensor in a fixed order; see NormParams.
 #pragma once
 
 #include <cooperative_groups.h>
@@ -182,6 +185,30 @@ struct ScheduleParams {
   int32_t accum_n;         // N: the launch checks that global_step selects its branch
 };
 
+// Per-tensor norms of the apply step (gaccum_plan_set_tensor_norms).  out == NULL: off.  A launch-uniform branch, not a
+// template flag: no kernel is specialised on it.  The reduction is deterministic without atomics on the sums:
+//   1. the apply kernels store, for every tile, column (gradient, weight, update) and warp of the 256 threads that walked
+//      the tile, the warp's fp64 total of its threads' fp32 partials (tile_part; plain stores, each slot written once);
+//   2. a chunk of up to kNormChunk consecutive tiles of one tensor is summed by one warp, tile by tile and warp by warp
+//      in that order (chunk_part), once all its tiles are written;
+//   3. the tensor's chunks are summed in chunk order by the warp that finishes its last chunk (a counter per tensor),
+//      and out[3t + k] = sqrtf(fp32(sum)).
+// Every order is fixed by the tile table alone, so the values do not depend on which CTA, group or path took a tile.
+constexpr int kNormCols = 3;                     // gradient, weight, update
+constexpr int kNormWarps = kThreads / 32;        // warps of the 256 threads that walk one tile
+constexpr int kNormChunk = 32;                   // tiles per chunk: one per lane of the summing warp
+struct NormParams {
+  float* out;                  // num_tensors x 3, caller-owned
+  double* tile_part;           // num_tiles x kNormCols x kNormWarps
+  double* chunk_part;          // num_chunks x kNormCols
+  const int32_t* tile_begin;   // num_tensors + 1: tensor t owns tiles [tile_begin[t], tile_begin[t + 1])
+  const int32_t* chunk_begin;  // num_tensors + 1: ... and chunks [chunk_begin[t], chunk_begin[t + 1])
+  const int32_t* chunk_tensor; // num_chunks
+  unsigned int* chunk_done;    // num_chunks: apply_kernel's tiles of the chunk that are through (0 between launches)
+  unsigned int* tensor_done;   // num_tensors: chunks of the tensor that are summed (0 between launches)
+  int32_t num_chunks;
+};
+
 // Every kernel's parameter block.  Each feature's parameters follow those of the features before it, so adding them
 // moved no member an existing kernel reads.
 template <int CAP>
@@ -206,6 +233,7 @@ struct KernelParams {
   LrMultParams lrm;     // apply kernels only
   WindowWeightParams ww;  // apply kernels only
   ScheduleParams sched;   // every kernel
+  NormParams norms;       // apply kernels only
 };
 static_assert(sizeof(KernelParams<1920>) <= 32764, "kernel parameters must fit the 32 KB limit");
 
@@ -513,6 +541,15 @@ __device__ __forceinline__ void update_vec(const float4 a, bool scaled, float s,
 __device__ __forceinline__ float4 add_rn(const float4 a, const float4 b) {
   return make_float4(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z), __fadd_rn(a.w, b.w));
 }
+// per-tensor norms (NormParams): a thread's fp32 partial of one tile's column: acc + x^2, and acc + (p - q)^2 with the fp32 difference
+__device__ __forceinline__ float sq_acc(float acc, float x) { return fmaf(x, x, acc); }
+__device__ __forceinline__ float sq_acc(float acc, const float4 x) {
+  return sq_acc(sq_acc(sq_acc(sq_acc(acc, x.x), x.y), x.z), x.w);
+}
+__device__ __forceinline__ float diff_sq_acc(float acc, float p, float q) {
+  const float d = __fsub_rn(p, q);
+  return fmaf(d, d, acc);
+}
 // acc + (x/D)^2: one element of a thread's fp32 partial of the global norm
 template <typename D>
 __device__ __forceinline__ float add_sq(float acc, float x, const D& dv) {
@@ -571,6 +608,86 @@ __device__ __forceinline__ float clip_scale(float gn, float clip) {
   float mn = inv < invc ? inv : invc;
   if (inv != inv) mn = inv;
   return __fadd_rn(__fmul_rn(clip, mn), __fsub_rn(gn, gn));
+}
+
+// ---- per-tensor norms (NormParams) ----------------------------------------------------------------------------
+// warp total of a per-thread double, fixed butterfly order (lane 0's value is the one every caller uses)
+__device__ __forceinline__ double warp_sum(double w) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) w += __shfl_xor_sync(0xffffffffu, w, o);
+  return w;
+}
+// the whole warp: its fp64 total of the threads' partials `part` of (tile, col), stored by lane 0
+__device__ __forceinline__ void norm_store(const NormParams& np, const int tile, const int col, const int warp, const float part) {
+  const double w = warp_sum((double)part);
+  if ((threadIdx.x & 31) == 0) np.tile_part[((size_t)tile * kNormCols + col) * kNormWarps + warp] = w;
+}
+// The whole warp, once every tile of chunk c is stored: the chunk's sums (lane l takes tile l of the chunk and adds its
+// warps' partials in order; then the butterfly), and, if this is the tensor's last chunk to be summed, the tensor's norms
+// from its chunks in chunk order.  The finishing warp resets the tensor's counter for the next launch.
+__device__ __noinline__ void norm_chunk(const NormParams& np, const int c) {
+  const int lane = (int)threadIdx.x & 31;
+  const int t = __ldg(np.chunk_tensor + c);
+  const int cb = __ldg(np.chunk_begin + t), ce = __ldg(np.chunk_begin + t + 1);
+  const int tile = __ldg(np.tile_begin + t) + (c - cb) * kNormChunk + lane;
+  double s[kNormCols] = {0.0, 0.0, 0.0};
+  if (tile < __ldg(np.tile_begin + t + 1)) {
+    const double* tp = np.tile_part + (size_t)tile * kNormCols * kNormWarps;
+#pragma unroll
+    for (int k = 0; k < kNormCols; ++k)
+#pragma unroll
+      for (int w = 0; w < kNormWarps; ++w) s[k] += __ldcg(tp + k * kNormWarps + w);
+  }
+#pragma unroll
+  for (int k = 0; k < kNormCols; ++k) s[k] = warp_sum(s[k]);
+  unsigned int last = 0;
+  if (lane == 0) {
+#pragma unroll
+    for (int k = 0; k < kNormCols; ++k) np.chunk_part[(size_t)c * kNormCols + k] = s[k];
+    __threadfence();
+    last = atomicAdd(np.tensor_done + t, 1u) == (unsigned int)(ce - cb - 1);
+  }
+  if (!__shfl_sync(0xffffffffu, last, 0)) return;
+  __threadfence();
+  double r[kNormCols] = {0.0, 0.0, 0.0};
+  for (int k = cb + lane; k < ce; k += 32) {
+#pragma unroll
+    for (int j = 0; j < kNormCols; ++j) r[j] += __ldcg(np.chunk_part + (size_t)k * kNormCols + j);
+  }
+#pragma unroll
+  for (int j = 0; j < kNormCols; ++j) r[j] = warp_sum(r[j]);
+  if (lane == 0) {
+#pragma unroll
+    for (int j = 0; j < kNormCols; ++j) np.out[(size_t)t * kNormCols + j] = __fsqrt_rn((float)r[j]);
+    np.tensor_done[t] = 0u;
+  }
+}
+// Every warp of a cooperative launch, past a grid barrier that follows the last tile_part store: every chunk, `gw` the
+// warp's index among `nw`
+__device__ __forceinline__ void norm_finish_all(const NormParams& np, const int gw, const int nw) {
+  for (int c = gw; c < np.num_chunks; c += nw) norm_chunk(np, c);
+}
+// apply_kernel, one tile per CTA, after every warp stored the tile's partials: thread 0 counts the tile into its chunk;
+// the CTA that completes the chunk sums it with warp 0
+__device__ __forceinline__ void norm_arrive_tile(const NormParams& np, const TileDesc& d, const int tile) {
+  __shared__ int s_chunk;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const int t = (int)(d.tensor_flags & 0x7fffffffu);
+    const int tb = __ldg(np.tile_begin + t), te = __ldg(np.tile_begin + t + 1);
+    const int j = (tile - tb) / kNormChunk;
+    const int c = __ldg(np.chunk_begin + t) + j;
+    const int n = min(kNormChunk, te - tb - j * kNormChunk);
+    __threadfence();
+    const bool last = atomicAdd(np.chunk_done + c, 1u) == (unsigned int)(n - 1);
+    if (last) np.chunk_done[c] = 0u;
+    s_chunk = last ? c : -1;
+  }
+  __syncthreads();
+  if (s_chunk >= 0 && threadIdx.x < 32) {
+    __threadfence();
+    norm_chunk(np, s_chunk);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -670,10 +787,15 @@ __global__ void ema_init_kernel(EmaState* st, long long num_updates) {
 // dv: the launch's divisor (N, or the window weight W).
 // lr, bc2, bc1: the step's learning rate and GACCUM_ADAM's bias-correction terms (Scalars / LrMultParams, or the device
 // schedule's).
+// norms (launch-uniform, NormParams): the thread's fp32 partials of c^2 (c before any clip scale), p^2 (p before the
+// update) and (p - p')^2 go into `np_`.
+struct NormPart {
+  float g = 0.f, w = 0.f, u = 0.f;
+};
 template <int VARIANT, bool H, int CAP, bool EMA = false>
 __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams<CAP>& prm, const Divisor dv,
-                                            const float lr, const float bc2, const float bc1,
-                                            float* ema = nullptr, const float ema_c = 0.f) {
+                                            const float lr, const float bc2, const float bc1, const bool norms,
+                                            NormPart& np_, float* ema = nullptr, const float ema_c = 0.f) {
   const Grad<H> g(prm, d);
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
@@ -703,7 +825,13 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
             [] {},
             [&](int u, uint32_t i) {
               if (g.g) va[u] = add_rn(va[u], vg[u]);
+              float4 pb;
+              if (norms) { np_.g = add_sq(np_.g, va[u], dv); np_.w = sq_acc(np_.w, vp[u]); pb = vp[u]; }
               update_vec<VARIANT>(va[u], false, 0.f, vp[u], vm[u], vv[u], decay, sc, rate, dv);
+              if (norms) {
+                np_.u = diff_sq_acc(diff_sq_acc(diff_sq_acc(diff_sq_acc(np_.u, pb.x, vp[u].x), pb.y, vp[u].y), pb.z, vp[u].z),
+                                    pb.w, vp[u].w);
+              }
               __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
               if constexpr (H) store_model4(q, i, vp[u], bf16);
@@ -712,7 +840,10 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
             [&](uint32_t i) {
               float ax = a[i], px = p[i], mx = m[i], vx = v[i];
               if (g.g) ax = __fadd_rn(ax, g.elem(i));
+              const float pb = px;
+              if (norms) { np_.g = add_sq(np_.g, ax, dv); np_.w = sq_acc(np_.w, px); }
               update_elem<VARIANT>(ax, false, 0.f, px, mx, vx, decay, sc, rate, dv);
+              if (norms) np_.u = diff_sq_acc(np_.u, pb, px);
               p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
               if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
               if constexpr (EMA) e[i] = ema_elem(e[i], px, ema_c);
@@ -748,9 +879,19 @@ apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   const Divisor dv = ww ? s_dv : Divisor{prm.sc.nf, prm.sc.inv_nf};
   const float lr = sched ? s_sl.lr : prm.sc.lr;
   const float bc2 = sched ? s_sl.bc2 : prm.lrm.bc2, bc1 = sched ? s_sl.bc1 : prm.lrm.bc1;
+  const bool norms = prm.norms.out != nullptr;     // launch-uniform
   if ((int)blockIdx.x < prm.num_tiles) {
-    if constexpr (EMA) update_tile<VARIANT, H, CAP, true>(prm.tiles[blockIdx.x], prm, dv, lr, bc2, bc1, ep.slab, s_ema->c);
-    else update_tile<VARIANT, H>(prm.tiles[blockIdx.x], prm, dv, lr, bc2, bc1);
+    const TileDesc d = prm.tiles[blockIdx.x];
+    NormPart part;
+    if constexpr (EMA) update_tile<VARIANT, H, CAP, true>(d, prm, dv, lr, bc2, bc1, norms, part, ep.slab, s_ema->c);
+    else update_tile<VARIANT, H>(d, prm, dv, lr, bc2, bc1, norms, part);
+    if (norms) {
+      const int warp = (int)threadIdx.x >> 5;
+      norm_store(prm.norms, (int)blockIdx.x, 0, warp, part.g);
+      norm_store(prm.norms, (int)blockIdx.x, 1, warp, part.w);
+      norm_store(prm.norms, (int)blockIdx.x, 2, warp, part.u);
+      norm_arrive_tile(prm.norms, d, (int)blockIdx.x);
+    }
   }
   if (counted && threadIdx.x == 0) {
     __threadfence();
@@ -843,8 +984,9 @@ struct __align__(16) SlotMeta {
   TileDesc d;          // len == 0: end of the pass
   uint32_t stash_slot; // pass 2: a' is parked in this stash slot of the group (kNoStash: it is in the slot's 4th quarter / in global memory)
   float rate;          // pass 2: the tile's lr_t (AdamWeightDecay) or alpha_t (Adam), tile_rate
+  uint32_t tile;       // the tile's index in the table (per-tensor norms)
 };
-static_assert(sizeof(SlotMeta) == 32, "the rate sits in what was padding: static shared memory is unchanged");
+static_assert(sizeof(SlotMeta) == 32, "the rate and the tile index sit in what was padding: static shared memory is unchanged");
 // exact accumulation of non-negative doubles: 68 bins of 32 payload bits in 64-bit containers cover the whole
 // binary64 range (2^-1074 .. 2^1024); a container overflows only after 2^31 additions
 constexpr int kAccBins = 68;
@@ -1049,10 +1191,11 @@ __device__ __forceinline__ void ls_finish(const LossScaleParams& ls, const LossS
 // A tile the producer did not copy (nvec == 0), and the < 4 tail elements of any tile, travel through global memory.
 // Loss-scaled (kLsClip, kLsNoClip): the partial is of sum(((a'/N)(1/S))^2) (none without clipping), and `bad` is set
 // when an element of a' is not finite.
+// norms (kLsNoClip only; launch-uniform): the partial of sum(((a'/N)(1/S))^2) is formed as kLsClip forms it.
 template <int MODE, bool H, int CAP>
 __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float4* slot, uint64_t* empty,
                                            float4* const stash, const uint64_t pol, const float inv_s, bool& bad,
-                                           const Divisor& dv) {
+                                           const Divisor& dv, const bool norms) {
   const Grad<H> g(prm, d);
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
   float4* a4 = reinterpret_cast<float4*>(a);
@@ -1068,12 +1211,14 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
               }
               if (stash != nullptr) stash[i] = x[u];
               if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, x[u], dv);
+              else if (MODE == kLsNoClip && norms) acc = ls_pass1<kLsClip>(acc, x[u], inv_s, bad, dv);
               else acc = ls_pass1<MODE>(acc, x[u], inv_s, bad, dv);
             },
             [&](uint32_t i) {
               float xs = a[i];
               if (g.g) { xs = __fadd_rn(xs, g.elem(i)); a[i] = xs; }
               if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, xs, dv);
+              else if (MODE == kLsNoClip && norms) acc = ls_pass1<kLsClip>(acc, xs, inv_s, bad, dv);
               else acc = ls_pass1<MODE>(acc, xs, inv_s, bad, dv);
             });
   return acc;
@@ -1085,10 +1230,15 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
 // Loss-scaled: a skipped window (`skip`) stores a = 0 and nothing else.  H: p is the master slab, and the model copy is
 // stored after it (not on a skipped window).
 // EMA: the slot is [p | m | v | a' | e], and e - (e - p) * c is stored after p (not on a skipped window).
+// norms (launch-uniform): the slot is kept for norm_tile2 instead of being released after the loads, and the tile's
+// elements in it are made those norm_tile2 reads -- p before the update in the slot's p quarter (where the vector path
+// already has it), the stored p' in its m quarter (consumed by then), element i at float i -- so that no value is kept
+// alive across the update, whose registers are the kernel's limit.
 template <int VARIANT, int MODE, bool H, int CAP, bool EMA = false>
-__device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelParams<CAP>& prm, const float s, const float4* slot,
+__device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelParams<CAP>& prm, const float s, float4* slot,
                                              uint64_t* empty, const float4* const stash, const float rate, const float inv_s,
-                                             const bool skip, const Divisor& dv, float* ema = nullptr, const float ema_c = 0.f) {
+                                             const bool skip, const Divisor& dv, const bool norms,
+                                             float* ema = nullptr, const float ema_c = 0.f) {
   const Scalars& sc = prm.sc;
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
@@ -1113,26 +1263,62 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
               va[u] = stash != nullptr ? stash[i] : slot[3 * (kTile / 4) + i];
               if constexpr (EMA) ve[u] = slot[4 * (kTile / 4) + i];
             },
-            [&] { __syncwarp(); if ((threadIdx.x & 31) == 0) mbar_arrive(empty); },
+            [&] { if (!norms) { __syncwarp(); if ((threadIdx.x & 31) == 0) mbar_arrive(empty); } },
             [&](int u, uint32_t i) {
               if (write) {
                 adam_vec<VARIANT, MODE>(va[u], s, inv_s, vp[u], vm[u], vv[u], decay, sc, rate, dv);
                 __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
                 if constexpr (H) store_model4(q, i, vp[u], bf16);
                 if constexpr (EMA) __stcs(e4 + i, ema_vec(ve[u], vp[u], ema_c));
+                if (norms) slot[kTile / 4 + i] = vp[u];
               }
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
             },
             [&](uint32_t i) {
+              float* const sf = reinterpret_cast<float*>(slot);
               if (write) {
                 float px = p[i], mx = m[i], vx = v[i];
+                if (norms) sf[i] = px;
                 adam_elem<VARIANT>(mode_c<MODE>(a[i], s, inv_s, dv), px, mx, vx, decay, sc, rate);
                 p[i] = px; m[i] = mx; v[i] = vx;
+                if (norms) sf[kTile + i] = px;
                 if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
                 if constexpr (EMA) e[i] = ema_elem(e[i], px, ema_c);
+              } else if (norms) {
+                sf[i] = p[i];
               }
               a[i] = 0.f;
             });
+}
+// norms, after update_tile2: the tile's partials of p^2 (p before the update) and, unless the window is skipped,
+// (p - p')^2 from what update_tile2 left in the slot.  Each thread reads exactly the elements it wrote (walk_tile's
+// assignment, nvec as update_tile2 took it), so no barrier is needed.  Then the slot goes back to the producer: it was
+// written through the generic proxy and the producer's next bulk copy into it is an async-proxy write, hence the proxy
+// fence before the release.
+__device__ __forceinline__ void norm_tile2(const TileDesc& d, const uint32_t nvec, const float4* slot, uint64_t* empty,
+                                           const bool skip, float& nw, float& nu) {
+  const uint32_t tid = threadIdx.x & (kThreads - 1);
+#pragma unroll
+  for (int u = 0; u < kUnroll; ++u) {
+    const uint32_t i = u * kThreads + tid;
+    if (i < nvec) {
+      const float4 pb = slot[i];
+      nw = sq_acc(nw, pb);
+      if (!skip) {
+        const float4 pn = slot[kTile / 4 + i];
+        nu = diff_sq_acc(diff_sq_acc(diff_sq_acc(diff_sq_acc(nu, pb.x, pn.x), pb.y, pn.y), pb.z, pn.z), pb.w, pn.w);
+      }
+    }
+  }
+  const float* const sf = reinterpret_cast<const float*>(slot);
+  for (uint32_t i = (nvec << 2) + tid; i < d.len; i += kThreads) {
+    const float pb = sf[i];
+    nw = sq_acc(nw, pb);
+    if (!skip) nu = diff_sq_acc(nu, pb, sf[kTile + i]);
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(empty);
 }
 
 // Dynamic shared memory of apply_clip_kernel (kClipSmemBytes): 3 groups x kRingVecs float4 of ring, then
@@ -1211,9 +1397,11 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   stamp(0);
 
   // ---- set-up: which counter set this launch uses, mbarriers, accumulator -----------------------------------
+  const bool norms = prm.norms.out != nullptr;   // launch-uniform: one more grid barrier at the end of the launch
   if (threadIdx.x == 0) {
-    // every CTA that has not yet arrived at this launch's barrier reads a value in [k*grid, (k+1)*grid)
-    const unsigned long long k = ld_acquire_gpu_u64(prm.barrier) / gridDim.x;
+    // every CTA that has not yet arrived at this launch's first barrier reads a value in [k*B*grid, (k*B+1)*grid), B the
+    // launch's barriers
+    const unsigned long long k = ld_acquire_gpu_u64(prm.barrier) / ((unsigned long long)gridDim.x * (norms ? 2ull : 1ull));
     s_set = (uint32_t)(k & 1ull);
     s_nonfinite = 0;
 #pragma unroll
@@ -1257,7 +1445,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     //      descriptor loads of a batch overlap), single tickets near the end so that no SM is left holding a batch ----
     {
       RingPos rp;
-      auto issue = [&](const TileDesc& dl) {                               // lane 0 only
+      auto issue = [&](const TileDesc& dl, const int tile) {               // lane 0 only
         const Grad<H> g(prm, dl);
         const uint32_t nvec = bulk_vecs(dl, g);
         uint64_t* full = &s_full1[grp][rp.slot];
@@ -1270,6 +1458,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
 #endif
         SlotMeta* meta = &s_meta1[grp][rp.slot];
         meta->d = dl;
+        meta->tile = (uint32_t)tile;
         if (nvec > 0) {
           float4* dst = ring + (size_t)rp.slot * kP1SlotVecs;
           if constexpr (H) {
@@ -1297,7 +1486,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         if (lane < n_st) d = prm.tiles[b + lane * G];                        // own tiles' descriptors, one per lane
         for (int l = 0; l < n_st; ++l) {
           const TileDesc dl = shuffled(d, l);
-          if (lane == 0) issue(dl);
+          if (lane == 0) issue(dl, b + l * G);
           rp.advance(kP1Slots);
         }
       }
@@ -1317,7 +1506,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
           if (tl >= nt) { done = true; continue; }       // lanes get their tickets in no particular order: a valid one may follow
           last = tl;
           const TileDesc dl = shuffled(d, l);
-          if (lane == 0) issue(dl);
+          if (lane == 0) issue(dl, (int)tl);
           rp.advance(kP1Slots);
         }
       }
@@ -1384,6 +1573,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         mbar_wait(&s_empty2[grp][rp.slot], rp.use & 1u);
         SlotMeta* meta = &s_meta2[grp][rp.slot];
         meta->d = d;
+        meta->tile = (uint32_t)tile;
         meta->stash_slot = in_stash ? stash_slot : kNoStash;
         meta->rate = tile_rate<VARIANT>(lr, tensor_mult(prm.lrm, d), bc2, bc1);
         if (nvec > 0) {
@@ -1443,14 +1633,20 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         float4* const st = park ? stash + (size_t)n_seen * (kTile / 4) : nullptr;
         bool bad = false;
         const float part = norm_tile<MODE, H>(meta.d, prm, ring + (size_t)rp.slot * kP1SlotVecs, &s_empty1[grp][rp.slot], st,
-                                                pol_last, inv_s, bad, s_dv);
+                                                pol_last, inv_s, bad, s_dv, norms);
         if constexpr (loss_scaled(MODE)) { if (bad) my_nonfinite |= kElemNonfinite; }
-        if constexpr (MODE != kLsNoClip) {
-          // warp total in fp64, fixed butterfly order; lane 0 adds it EXACTLY into its warp's accumulator
+        if (MODE != kLsNoClip || norms) {
+          // warp total in fp64, fixed butterfly order; lane 0 adds it EXACTLY into its warp's accumulator and, with
+          // norms, stores it as the tile's gradient partial of this warp
           double w = (double)part;
 #pragma unroll
           for (int o = 16; o > 0; o >>= 1) w += __shfl_xor_sync(0xffffffffu, w, o);
-          if ((threadIdx.x & 31) == 0) acc_add(s_bins[warp], my_nonfinite, w);
+          if ((threadIdx.x & 31) == 0) {
+            if constexpr (MODE != kLsNoClip) acc_add(s_bins[warp], my_nonfinite, w);
+            if (norms) {
+              prm.norms.tile_part[((size_t)meta.tile * kNormCols) * kNormWarps + (warp & (kNormWarps - 1))] = w;
+            }
+          }
         }
         ++n_seen;
         rp.advance(kP1Slots);
@@ -1498,10 +1694,17 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         const float4* const st = meta.stash_slot != kNoStash ? stash + (size_t)meta.stash_slot * (kTile / 4) : nullptr;
         if constexpr (EMA) {
           update_tile2<VARIANT, MODE, H, CAP, true>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot],
-                                                    st, meta.rate, inv_s, skip, s_dv, ema->slab, s_ema->c);
+                                                    st, meta.rate, inv_s, skip, s_dv, norms, ema->slab, s_ema->c);
         } else {
           update_tile2<VARIANT, MODE, H>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st, meta.rate,
-                                      inv_s, skip, s_dv);
+                                      inv_s, skip, s_dv, norms);
+        }
+        if (norms) {
+          float nw = 0.f, nu = 0.f;
+          norm_tile2(meta.d, bulk_vecs2(meta.d, update_ptr<H>(prm, meta.d)), ring + (size_t)rp.slot * kP2SlotVecs,
+                     &s_empty2[grp][rp.slot], loss_scaled(MODE) && skip, nw, nu);
+          norm_store(prm.norms, (int)meta.tile, 1, warp & (kNormWarps - 1), nw);
+          norm_store(prm.norms, (int)meta.tile, 2, warp & (kNormWarps - 1), nu);
         }
         rp.advance(kP2Slots);
       }
@@ -1513,6 +1716,14 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
       if (prm.ww.state) window_finish(prm.ww.state, s_dv.nf);
       // loss-scaled: the beta powers live in the loss-scaling block, which ls_finish advanced
       if (prm.sched.state) sched_finish(prm.sched, s_sl, !loss_scaled(MODE) && VARIANT == 1, prm.sc.b1, prm.sc.b2);
+    }
+    if (norms) {
+      // every tile's partials are stored once all consumers are through pass 2: a second grid barrier, then every
+      // consumer warp of the grid sums chunks
+      named_bar_sync(1, kConsumerThreads);
+      if (threadIdx.x == 0) grid_barrier(prm.barrier);
+      named_bar_sync(1, kConsumerThreads);
+      norm_finish_all(prm.norms, (int)blockIdx.x * (kConsumerThreads / 32) + warp, (int)gridDim.x * (kConsumerThreads / 32));
     }
   }
   __syncthreads();

@@ -60,9 +60,10 @@ __device__ __forceinline__ double add_sq64(double acc, const float4 x) {
 }
 
 // ---- phase 1: a' = a + G stored back; returns this thread's fp32 partial of the global norm (as norm_tile) ----
+// norms (kLsNoClip only; launch-uniform): the partial of sum(((a'/N)(1/S))^2) is formed as kLsClip forms it.
 template <int MODE, bool H, int CAP>
 __device__ __forceinline__ float lamb_norm_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float inv_s, bool& bad,
-                                                const Divisor& dv) {
+                                                const Divisor& dv, const bool norms) {
   const Grad<H> g(prm, d);
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
   float4* a4 = reinterpret_cast<float4*>(a);
@@ -74,22 +75,25 @@ __device__ __forceinline__ float lamb_norm_tile(const TileDesc& d, const KernelP
             [&](int u, uint32_t i) {
               if (g.g) { x[u] = add_rn(x[u], gg[u]); a4[i] = x[u]; }
               if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, x[u], dv);
+              else if (MODE == kLsNoClip && norms) acc = ls_pass1<kLsClip>(acc, x[u], inv_s, bad, dv);
               else acc = ls_pass1<MODE>(acc, x[u], inv_s, bad, dv);
             },
             [&](uint32_t i) {
               float xs = a[i];
               if (g.g) { xs = __fadd_rn(xs, g.elem(i)); a[i] = xs; }
               if constexpr (!loss_scaled(MODE)) acc = add_sq(acc, xs, dv);
+              else if (MODE == kLsNoClip && norms) acc = ls_pass1<kLsClip>(acc, xs, inv_s, bad, dv);
               else acc = ls_pass1<MODE>(acc, xs, inv_s, bad, dv);
             });
   return acc;
 }
 
 // ---- phase 2: m, v and u of one tile (u into the accumulator slab); this thread's sums of p^2 and u^2 ----
-// LOAD_G: there was no phase 1, so a' = a + G is formed here.  H: p is the master slab.
+// LOAD_G: there was no phase 1, so a' = a + G is formed here, and with norms (launch-uniform) the thread's fp32 partial of
+// sum((a'/N)^2) goes into sg.  H: p is the master slab.
 template <int MODE, bool LOAD_G, bool H, int CAP>
 __device__ __forceinline__ void lamb_update_tile(const TileDesc& d, const KernelParams<CAP>& prm, const LambCoef& k,
-                                                 const Divisor& dv, double& sp, double& su) {
+                                                 const Divisor& dv, double& sp, double& su, const bool norms, float& sg) {
   Grad<H> g;
   if constexpr (LOAD_G) g = Grad<H>(prm, d);
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
@@ -112,6 +116,7 @@ __device__ __forceinline__ void lamb_update_tile(const TileDesc& d, const Kernel
             [] {},
             [&](int u, uint32_t i) {
               if (LOAD_G && g.g) va[u] = add_rn(va[u], vg[u]);
+              if (LOAD_G && norms) sg = add_sq(sg, va[u], dv);
               float4 w;
               w.x = lamb_u(mode_c<MODE>(va[u].x, k.s, k.inv_s, dv), vp[u].x, vm[u].x, vv[u].x, decay, sc, k);
               w.y = lamb_u(mode_c<MODE>(va[u].y, k.s, k.inv_s, dv), vp[u].y, vm[u].y, vv[u].y, decay, sc, k);
@@ -124,6 +129,7 @@ __device__ __forceinline__ void lamb_update_tile(const TileDesc& d, const Kernel
               float ax = a[i], mx = m[i], vx = v[i];
               const float px = p[i];
               if (LOAD_G && g.g) ax = __fadd_rn(ax, g.elem(i));
+              if (LOAD_G && norms) sg = add_sq(sg, ax, dv);
               const float w = lamb_u(mode_c<MODE>(ax, k.s, k.inv_s, dv), px, mx, vx, decay, sc, k);
               m[i] = mx; v[i] = vx; a[i] = w;
               sp = add_sq64(sp, px); su = add_sq64(su, w);
@@ -132,9 +138,12 @@ __device__ __forceinline__ void lamb_update_tile(const TileDesc& d, const Kernel
 
 // ---- phase 3: p = p - (r*lr)*u and a = +0 (a = +0 only on a skipped window) ----
 // EMA: e is read with p and u, and e - (e - p) * c stored after p.
+// norms (launch-uniform): the thread's fp32 partials of p^2 (p before the update; on a skipped window p is read for it)
+// and (p - p')^2 go into nw and nu.
 template <bool H, int CAP, bool EMA = false>
 __device__ __forceinline__ void lamb_write_tile(const TileDesc& d, const KernelParams<CAP>& prm, const float rlr, const bool write,
-                                                float* ema = nullptr, const float ema_c = 0.f) {
+                                                const bool norms, float& nw, float& nu, float* ema = nullptr,
+                                                const float ema_c = 0.f) {
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
   float* __restrict__ p = update_ptr<H>(prm, d);
@@ -151,37 +160,44 @@ __device__ __forceinline__ void lamb_write_tile(const TileDesc& d, const KernelP
               if (write) {
                 vu[u] = __ldcs(a4 + i); vp[u] = __ldcs(p4 + i);
                 if constexpr (EMA) ve[u] = __ldcs(e4 + i);
+              } else if (norms) {
+                vp[u] = __ldcs(p4 + i);
               }
             },
             [] {},
             [&](int u, uint32_t i) {
               if (write) {
+                const float4 pb = vp[u];
                 vp[u].x = __fsub_rn(vp[u].x, __fmul_rn(rlr, vu[u].x));
                 vp[u].y = __fsub_rn(vp[u].y, __fmul_rn(rlr, vu[u].y));
                 vp[u].z = __fsub_rn(vp[u].z, __fmul_rn(rlr, vu[u].z));
                 vp[u].w = __fsub_rn(vp[u].w, __fmul_rn(rlr, vu[u].w));
+                if (norms) {
+                  nw = sq_acc(nw, pb);
+                  nu = diff_sq_acc(diff_sq_acc(diff_sq_acc(diff_sq_acc(nu, pb.x, vp[u].x), pb.y, vp[u].y), pb.z, vp[u].z),
+                                   pb.w, vp[u].w);
+                }
                 __stcs(p4 + i, vp[u]);
                 if constexpr (H) store_model4(q, i, vp[u], bf16);
                 if constexpr (EMA) __stcs(e4 + i, ema_vec(ve[u], vp[u], ema_c));
+              } else if (norms) {
+                nw = sq_acc(nw, vp[u]);
               }
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
             },
             [&](uint32_t i) {
               if (write) {
-                const float px = __fsub_rn(p[i], __fmul_rn(rlr, a[i]));
+                const float pb = p[i];
+                const float px = __fsub_rn(pb, __fmul_rn(rlr, a[i]));
+                if (norms) { nw = sq_acc(nw, pb); nu = diff_sq_acc(nu, pb, px); }
                 p[i] = px;
                 if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
                 if constexpr (EMA) e[i] = ema_elem(e[i], px, ema_c);
+              } else if (norms) {
+                nw = sq_acc(nw, p[i]);
               }
               a[i] = 0.f;
             });
-}
-
-// warp total of a per-thread double, fixed butterfly order (every lane gets it)
-__device__ __forceinline__ double warp_sum(double w) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) w += __shfl_xor_sync(0xffffffffu, w, o);
-  return w;
 }
 
 // EMA: thread 0 of every CTA reads n during set-up; block 0's thread 0 writes n + 1 and d at the very end, past the
@@ -191,7 +207,8 @@ template <int CAP, int MODE, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads, kLambBlocksPerSm)
 lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   constexpr bool kPhase1 = MODE != kNoClip;
-  constexpr unsigned long long kBarriers = kPhase1 ? 3 : 2;
+  const bool norms = prm.norms.out != nullptr;   // launch-uniform: one more grid barrier at the end of the launch
+  const unsigned long long kBarriers = (kPhase1 ? 3 : 2) + (norms ? 1 : 0);
   constexpr int kWarps = kThreads / 32;
   const LambParams& lb = prm.lamb;
   EmaLaunch* s_ema = nullptr;            // EMA: n, d and c as this launch found them
@@ -256,10 +273,13 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     bool bad = false;
     unsigned int nonfinite = 0;
     for (int t = t_lo; t < t_hi; ++t) {
-      const float part = lamb_norm_tile<MODE, H>(prm.tiles[t], prm, inv_s, bad, dv);
-      if constexpr (MODE != kLsNoClip) {
+      const float part = lamb_norm_tile<MODE, H>(prm.tiles[t], prm, inv_s, bad, dv, norms);
+      if (MODE != kLsNoClip || norms) {
         const double w = warp_sum((double)part);
-        if (lane == 0) acc_add(s_bins[warp][0], nonfinite, w);
+        if (lane == 0) {
+          if constexpr (MODE != kLsNoClip) acc_add(s_bins[warp][0], nonfinite, w);
+          if (norms) prm.norms.tile_part[((size_t)t * kNormCols) * kNormWarps + warp] = w;
+        }
       }
     }
     if constexpr (loss_scaled(MODE)) { if (bad) nonfinite |= kElemNonfinite; }
@@ -316,7 +336,9 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         cur_adapt = lb.adapt[ti] != 0;
       }
       double sp = 0.0, su = 0.0;
-      lamb_update_tile<MODE, !kPhase1, H>(d, prm, coef, dv, sp, su);
+      float sg = 0.f;
+      lamb_update_tile<MODE, !kPhase1, H>(d, prm, coef, dv, sp, su, norms, sg);
+      if (!kPhase1 && norms) norm_store(prm.norms, t, 0, warp, sg);
       if (cur_adapt) {
         sp = warp_sum(sp);
         su = warp_sum(su);
@@ -363,8 +385,13 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     // ratio * lr_t first, lr_t = lr * mult[t] (LrMultParams)
     const float rlr = skip ? 0.f : __fmul_rn(__ldcg(&lb.ratios[d.tensor_flags & 0x7fffffffu]),
                                              tile_rate<0>(lr, tensor_mult(prm.lrm, d), 0.f, 1.f));
-    if constexpr (EMA) lamb_write_tile<H, CAP, true>(d, prm, rlr, !skip, prm.ema.slab, s_ema->c);
-    else lamb_write_tile<H>(d, prm, rlr, !skip);
+    float nw = 0.f, nu = 0.f;
+    if constexpr (EMA) lamb_write_tile<H, CAP, true>(d, prm, rlr, !skip, norms, nw, nu, prm.ema.slab, s_ema->c);
+    else lamb_write_tile<H>(d, prm, rlr, !skip, norms, nw, nu);
+    if (norms) {
+      norm_store(prm.norms, t, 1, warp, nw);
+      norm_store(prm.norms, t, 2, warp, nu);
+    }
   }
 
   if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -374,6 +401,14 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     if (prm.ww.state) window_finish(prm.ww.state, s_dv.nf);
     // loss-scaled: the beta powers live in the loss-scaling block, which ls_finish advanced
     if (prm.sched.state) sched_finish(prm.sched, s_sl, !loss_scaled(MODE), prm.sc.b1, prm.sc.b2);
+  }
+  if (norms) {
+    // every tile's partials are stored once every CTA is through phase 3: one more grid barrier, then every warp of
+    // the grid sums chunks
+    __syncthreads();
+    if (threadIdx.x == 0) grid_barrier(prm.barrier);
+    __syncthreads();
+    norm_finish_all(prm.norms, (int)blockIdx.x * kWarps + warp, (int)gridDim.x * kWarps);
   }
 }
 

@@ -117,9 +117,12 @@ class FusedDataParallelTrainOp:
 
     def __init__(self, params: Sequence[torch.Tensor], names: Sequence[str], hp, accum_n: int, lr_fn,
                  process_group=None, exclude_from_weight_decay=("LayerNorm", "layer_norm", "bias"),
-                 global_step: int = 0, loss_scale=None, ema=None, lr_multipliers=None, window_weight: bool = False):
+                 global_step: int = 0, loss_scale=None, ema=None, lr_multipliers=None, window_weight: bool = False,
+                 tensor_norms: bool = False):
         import torch.distributed._symmetric_memory as symm
         from .train_op import GaccumTrainOp
+        if tensor_norms:
+            raise ValueError("the fused data-parallel train op does not report per-tensor norms; use dp_mode='allreduce'")
         if window_weight:
             raise ValueError("the fused data-parallel train op does not support a window weight; use dp_mode='allreduce'")
         if ema is not None:

@@ -46,6 +46,9 @@ layerwise_lr_decay: Optional[float] = None
 # Divide each window by its total weight (typically its number of loss tokens) instead of N: the loss callable returns
 # (summed loss, weight).  Off by default; create_optimizer reads it.
 window_weight = False
+# Report per-tensor gradient, weight and update norms from every apply step (``train_op.tensor_norms()``).  Off by
+# default; create_optimizer reads it.
+tensor_norms = False
 
 LossLike = Union[torch.Tensor, Callable[[], torch.Tensor]]
 LrLike = Union[float, Callable[[int], float]]
@@ -259,7 +262,8 @@ class TrainOp:
     def __init__(self, loss: LossLike, tvars: Sequence[graph.Variable], optimizer: _OptimizerBase,
                  accum_n: int, clip: Optional[float], global_step: graph.GlobalStep, process_group=None,
                  dp_mode: str = "fused", loss_scale: Optional[LossScaleConfig] = None,
-                 ema: Optional[ExponentialMovingAverage] = None, window_weight: bool = False):
+                 ema: Optional[ExponentialMovingAverage] = None, window_weight: bool = False,
+                 tensor_norms: bool = False):
         self.loss = loss
         self.window_weight = bool(window_weight)
         self.tvars = list(tvars)
@@ -283,21 +287,28 @@ class TrainOp:
             if dp_mode == "fused":
                 self.dp = FusedDataParallelTrainOp(tensors, names, hp, accum_n, lr_fn, pg, exclude, int(global_step),
                                                    loss_scale=loss_scale, ema=ema_cfg, lr_multipliers=mult,
-                                                   window_weight=window_weight)
+                                                   window_weight=window_weight, tensor_norms=tensor_norms)
                 self.engine = self.dp.engine
             else:
                 self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step),
                                             loss_scale=loss_scale, ema=ema_cfg, lr_multipliers=mult,
-                                            window_weight=window_weight, **adapt_kw)
+                                            window_weight=window_weight, tensor_norms=tensor_norms, **adapt_kw)
                 self.dp = DataParallelTrainOp(self.engine, pg)
         else:
             self.engine = GaccumTrainOp(tensors, names, hp, accum_n, lr_fn, exclude, int(global_step),
                                         loss_scale=loss_scale, ema=ema_cfg, lr_multipliers=mult,
-                                        window_weight=window_weight, **adapt_kw)
+                                        window_weight=window_weight, tensor_norms=tensor_norms, **adapt_kw)
         if ema is not None:
             ema._train_op = self
         self.last_loss: Optional[torch.Tensor] = None
         self._weight = None          # window_weight: the weight the loss callable returned with last_loss
+
+    def tensor_norms(self) -> Dict[str, Tuple[float, float, float]]:
+        """Synchronously read the per-tensor norms of the last apply step, keyed by variable name (``:0`` stripped):
+        (gradient, weight, update) -- ||c|| before the clip scale, ||p|| before the update, ||p_before - p_after||.
+        ValueError unless the train op was built with ``tensor_norms=True``."""
+        vals = self.engine.tensor_norms()
+        return {_lib._variable_name(v.name): (float(r[0]), float(r[1]), float(r[2])) for v, r in zip(self.tvars, vals)}
 
     @property
     def accum_n(self) -> int:
@@ -350,19 +361,21 @@ def gradient_accumulation_train_op(loss: LossLike, optimizer: _OptimizerBase, gr
                                    clip_norm: Optional[float] = None, global_step: Optional[graph.GlobalStep] = None,
                                    tvars: Optional[Sequence[graph.Variable]] = None, process_group=None,
                                    dp_mode: str = "fused", loss_scale: Optional[LossScaleConfig] = None,
-                                   ema: Optional[ExponentialMovingAverage] = None, window_weight: bool = False) -> TrainOp:
+                                   ema: Optional[ExponentialMovingAverage] = None, window_weight: bool = False,
+                                   tensor_norms: bool = False) -> TrainOp:
     """The recipe the example scripts inline (02:47-73, 04:48-74, another-example.py:126-155):
     N from ``params``, optimizer given, no clipping unless asked.  ``loss_scale`` turns on dynamic loss scaling for
     fp16 mixed precision: gradients are taken of ``loss * S`` and a window that overflows is skipped on the device.
     ``ema`` keeps an exponential moving average of the trainable variables, updated by the apply step.
     ``window_weight`` divides each window by its total weight instead of N: ``loss`` returns (summed loss, weight), the
-    weight typically the micro-batch's number of loss tokens, so a window trains on the per-token mean of its tokens."""
+    weight typically the micro-batch's number of loss tokens, so a window trains on the per-token mean of its tokens.
+    ``tensor_norms`` makes every apply step report per-tensor gradient, weight and update norms (``tensor_norms()``)."""
     gs = global_step or graph.get_or_create_global_step()
     tv = list(tvars) if tvars is not None else graph.trainable_variables()
     if not tv:
         raise ValueError("no trainable variables registered (graph.add_variable / graph.register_module)")
     return TrainOp(loss, tv, optimizer, int(gradient_accumulation_multiplier), clip_norm, gs, process_group, dp_mode,
-                   loss_scale, ema, window_weight)
+                   loss_scale, ema, window_weight, tensor_norms)
 
 
 def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
@@ -377,7 +390,8 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
     With the module attribute ``layerwise_lr_decay`` set, each variable trains at ELECTRA's layer-wise decayed rate
     (``layerwise_lr_multipliers``), the number of encoder layers taken from the trainable variables' names.
     With the module attribute ``window_weight`` set, ``loss`` returns (summed loss, weight) and each window is divided by
-    its total weight instead of N.
+    its total weight instead of N.  With the module attribute ``tensor_norms`` set, every apply step reports per-tensor
+    gradient, weight and update norms (``train_op.tensor_norms()``).
     """
     if use_tpu:
         # optimization.py:67-68 wraps the optimizer in tf.contrib.tpu.CrossShardOptimizer: TPU-only.
@@ -398,4 +412,4 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
     ema = ExponentialMovingAverage(moving_average_decay) if moving_average_decay is not None else None
     return gradient_accumulation_train_op(loss, optimizer, gradient_accumulation_multiplier,
                                           clip_norm=clip_norm, global_step=global_step, loss_scale=loss_scale, ema=ema,
-                                          window_weight=window_weight)
+                                          window_weight=window_weight, tensor_norms=tensor_norms)

@@ -115,7 +115,7 @@ class _DeviceTrainOp(_TrainOpCore):
     def __init__(self, params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step,
                  loss_scale: Optional[LossScaleConfig] = None, exclude_from_layer_adaptation=None,
                  lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False,
-                 device_schedule: Optional[ScheduleConfig] = None):
+                 device_schedule: Optional[ScheduleConfig] = None, tensor_norms: bool = False):
         self.ema: Optional[torch.Tensor] = None          # the moving average of the weights, when one is kept
         self._ema_state: Optional[torch.Tensor] = None
         self._sched_state: Optional[torch.Tensor] = None  # the device schedule's block, when one is kept
@@ -162,6 +162,25 @@ class _DeviceTrainOp(_TrainOpCore):
             self.plan.set_device_schedule(device_schedule, self._sched_state.data_ptr())
             self._capturing = False
             self._write_schedule(self._step, self.beta1_power, self.beta2_power)
+        self._norms: Optional[torch.Tensor] = None
+        if tensor_norms:
+            # T x 3 fp32 on the device, rewritten by every apply: statistics, not state (checkpoints do not store them)
+            self._norms = torch.zeros((len(params), 3), dtype=torch.float32, device=self.device)
+            self.plan.set_tensor_norms(self._norms.data_ptr())
+
+    @property
+    def tensor_norms_tensor(self) -> torch.Tensor:
+        """The per-tensor norms of the last apply as a (T, 3) fp32 CUDA tensor -- columns gradient, weight, update --
+        without a copy or a sync (e.g. for a captured loop).  Every apply overwrites it."""
+        if self._norms is None:
+            raise ValueError("this train op does not report per-tensor norms (tensor_norms=False)")
+        return self._norms
+
+    def tensor_norms(self) -> np.ndarray:
+        """Synchronously read the per-tensor norms of the last apply: a (T, 3) np.float32 array in tensor order with
+        columns gradient (||c||, c before the clip scale), weight (||p|| before the update) and update
+        (||p_before - p_after||); zeros before the first apply (gaccum.h, gaccum_plan_set_tensor_norms)."""
+        return self.tensor_norms_tensor.cpu().numpy().copy()
 
     # -- global_step: a host int, or the device schedule's counter ---------------------------------------------------
     @property
@@ -416,14 +435,14 @@ class GaccumTrainOp(_DeviceTrainOp):
                  loss_scale: Optional[LossScaleConfig] = None,
                  exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None,
                  lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False,
-                 device_schedule: Optional[ScheduleConfig] = None):
+                 device_schedule: Optional[ScheduleConfig] = None, tensor_norms: bool = False):
         dtypes = {p.dtype for p in params}
         if len(dtypes) > 1 and dtypes & set(_HALF_DTYPES):
             raise ValueError(f"parameters of mixed dtypes ({', '.join(sorted(str(d) for d in dtypes))}): "
                              "a 16-bit model must be all bf16 or all fp16")
         self.param_dtype = params[0].dtype if len(dtypes) == 1 and params[0].dtype in _HALF_DTYPES else torch.float32
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale,
-                         exclude_from_layer_adaptation, lr_multipliers, window_weight, device_schedule)
+                         exclude_from_layer_adaptation, lr_multipliers, window_weight, device_schedule, tensor_norms)
         for p in self.params:
             if p.dtype != self.param_dtype or not p.is_contiguous() or p.device != self.device:
                 if self.param_dtype != torch.float32:
@@ -706,11 +725,11 @@ class PackedTrainOp(_DeviceTrainOp):
                  global_step: int = 0, loss_scale: Optional[LossScaleConfig] = None,
                  exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None,
                  lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False,
-                 device_schedule: Optional[ScheduleConfig] = None):
+                 device_schedule: Optional[ScheduleConfig] = None, tensor_norms: bool = False):
         # autograd accumulates a 16-bit parameter's gradient in its own dtype: it cannot add into an fp32 slab
         _refuse_half(params, "PackedTrainOp")
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale,
-                         exclude_from_layer_adaptation, lr_multipliers, window_weight, device_schedule)
+                         exclude_from_layer_adaptation, lr_multipliers, window_weight, device_schedule, tensor_norms)
         self.param_slab = self._zeros_slab()
         self.accum = self._zeros_slab()
         with torch.no_grad():
@@ -796,7 +815,10 @@ class HostTrainOp(_TrainOpCore):
                  exclude_from_weight_decay: Optional[Sequence[str]] = ("LayerNorm", "layer_norm", "bias"),
                  global_step: int = 0, device: int = 0, loss_scale: Optional[LossScaleConfig] = None,
                  ema: Optional[EmaConfig] = None, lr_multipliers: Optional[Sequence[float]] = None,
-                 window_weight: bool = False, device_schedule: Optional[ScheduleConfig] = None):
+                 window_weight: bool = False, device_schedule: Optional[ScheduleConfig] = None,
+                 tensor_norms: bool = False):
+        if tensor_norms:
+            raise ValueError("HostTrainOp does not report per-tensor norms; use GaccumTrainOp")
         if device_schedule is not None:
             raise ValueError("HostTrainOp does not support a device schedule; use GaccumTrainOp")
         if ema is not None:

@@ -371,6 +371,34 @@ GACCUM_API int gaccum_plan_set_device_schedule(gaccum_plan* plan, const gaccum_s
 GACCUM_API int gaccum_schedule_init(gaccum_plan* plan, gaccum_schedule_state* block, int64_t global_step,
                                     float beta1_power, float beta2_power, gaccum_stream_t stream);
 
+/* Per-tensor norms of the apply step, for watching a run layer by layer (TF1's add_gradients_summaries /
+ * optimize_loss(summaries=["gradient_norm"])) without extra passes over the slabs.  Off unless set.  Every apply launch
+ * of gaccum_step, gaccum_apply (grads == NULL included) and gaccum_step_packed writes, for every tensor t, row t of
+ * `device_out` (num_tensors x 3 floats, caller-owned device memory, 16-byte aligned):
+ *     [3t + 0]  gradient  ||c_t||: c the window gradient the update consumes BEFORE the clip scale -- (1.0 * a') / N (or
+ *                         a' / W with a window weight), times 1/S under loss scaling: the c whose norm
+ *                         gaccum_stats.global_norm reports -- whether clipping is on or off.  A tensor without a gradient
+ *                         this micro-step reports the norm of its accumulated c.
+ *     [3t + 1]  weight    ||p_t|| of the weights before the update (a 16-bit plan: the fp32 master weights).
+ *     [3t + 2]  update    ||p_before - p_after||, from the per-element fp32 difference of what the apply stored: 0 for a
+ *                         tensor with learning-rate multiplier 0, and 0 everywhere on a window that loss scaling skips.
+ *   ||x|| = sqrtf(fp32(sum x^2)).  Each thread of the kernel sums x^2 of its elements of a tile in fp32 (fmaf, as the
+ *   global norm's partials), a warp adds its threads' sums in fp64 in a fixed butterfly order, and those fp64 values are
+ *   added tile by tile, warp by warp in a fixed order that depends on the tile table only: the values are bit-identical
+ *   from launch to launch, across CUDA-graph replays and whichever CTA took a tile.  Non-finite values propagate (a
+ *   tensor holding an inf reports inf, one holding a NaN reports NaN); a zero-element tensor reports 0.
+ *   A window that loss scaling skips still writes all three columns: the overflowed tensors' gradient norms, the
+ *   unchanged weights' norms and zero update norms.  Every apply launch overwrites the values; after a replayed graph of
+ *   k windows they hold the last window's, as the stats block does.
+ * Nothing else the apply computes depends on the setting, bit for bit.  The setter is host-only: it validates its
+ * arguments, allocates the plan's scratch (per tile 192 bytes of fp64 partials, per 32 tiles 24 bytes, 12 bytes per
+ * tensor of tables and counters) and zeroes `device_out` and waits for that to finish, so the values are 0 before the first apply.
+ * GACCUM_EINVAL for a NULL plan or buffer, a misaligned buffer, a layout-only plan, and after the plan's first compute
+ * call; combines with the other setters in any order.  gaccum_accumulate is unaffected; gaccum_step_dp,
+ * gaccum_apply_dp, gaccum_host_session_create and gaccum_step_host refuse such a plan with GACCUM_EINVAL.
+ * gaccum_algorithmic_bytes is unchanged: the scratch is metadata-sized. */
+GACCUM_API int gaccum_plan_set_tensor_norms(gaccum_plan* plan, float* device_out);
+
 /* ---- the hot path --------------------------------------------------------------------- */
 /* One micro-step of the train_op (optimization.py:91-94): if gaccum_is_apply_step() the apply
  * branch (assign_add -> /N -> clip_by_global_norm -> apply_gradients -> zero; :80-88), else
