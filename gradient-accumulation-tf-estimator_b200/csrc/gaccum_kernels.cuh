@@ -1087,8 +1087,10 @@ __device__ __forceinline__ void acc_add(unsigned long long* bins, unsigned int& 
   bins[q + 1] += lo >> 32;
   bins[q + 2] += hi;
 }
-// the accumulated value as a double (deterministic: carries are propagated low to high, the three leading 32-bit
-// digits are combined in a fixed order; relative error <= 2^-52); executed by one thread
+// the accumulated value as a double ROUNDED TO ODD: its leading 53 bits, the last one ORed with every bit below them
+// (the rest of the three leading 32-bit digits and every lower digit).  53 >= 24 + 2, so the caller's (float) cast then
+// rounds the exact sum to fp32 once -- to nearest, ties to even, inf from FLT_MAX + half an ulp -- where rounding to
+// nearest twice can land one ulp off.  Deterministic (carries propagated low to high); executed by one thread.
 __device__ __forceinline__ double acc_value(const unsigned long long* bins /* kAccBins */, const unsigned int nonfinite) {
   if (nonfinite & 2u) return __longlong_as_double(0x7ff8000000000000ll);
   if (nonfinite & 1u) return __longlong_as_double(0x7ff0000000000000ll);
@@ -1102,16 +1104,23 @@ __device__ __forceinline__ double acc_value(const unsigned long long* bins /* kA
   if (top < 0) return 0.0;
   carry = 0;
   unsigned int g0 = 0, g1 = 0, g2 = 0;                 // digits top-2, top-1, top
+  bool sticky = false;                                 // a digit below top-2 is not zero
   for (int i = 0; i <= top; ++i) {
     const unsigned long long t = bins[i] + carry;
     const unsigned int digit = (unsigned int)(t & 0xffffffffull);
     carry = t >> 32;
+    if (i < top - 2) sticky |= digit != 0u;
     if (i == top - 2) g0 = digit;
     if (i == top - 1) g1 = digit;
     if (i == top) g2 = digit;
   }
-  const double m = ((double)g2 * 4294967296.0 + (double)g1) * 4294967296.0 + (double)g0;
-  return scalbn(m, 32 * (top - 2) - 1074);
+  // the 96 bits g2:g1:g0 shifted left until g2's leading one is bit 63 of `hi`; what falls off joins the sticky bit
+  const int lz = __clz(g2);
+  unsigned long long hi = (((unsigned long long)g2 << 32) | g1) << lz;
+  if (lz) hi |= (unsigned long long)g0 >> (32 - lz);
+  sticky |= (g0 << lz) != 0u;                          // 32-bit shift: the bits of g0 below hi
+  const unsigned long long mant = (hi >> 11) | (unsigned long long)(sticky || (hi & 0x7ffull) != 0ull);
+  return scalbn((double)mant, 32 * (top - 1) - lz - 1074 + 11);
 }
 
 // ---- pieces the cooperative apply kernels share (apply_clip_kernel, lamb_apply_kernel in gaccum_lamb.cuh) ----------

@@ -219,12 +219,34 @@ class StepInfo:
     clip_scale: np.float32 = F32(1.0)
 
 
+@dataclass
+class Reduced:
+    """The scalars a device reduced for one applied window: the global norm gn and, LAMB, the per-tensor trust ratios
+    (r of the tensors without layer adaptation is ignored: it is 1)."""
+    global_norm: np.float32
+    ratios: Optional[Sequence[np.float32]] = None
+
+
 class ReferenceTrainOp:
     """State + one ``run(grads)`` per micro-step, op-for-op as optimization.py:76-104.
 
     ``params`` are updated in place (list of fp32 arrays).  ``names`` feed the decay mask.
     ``lr_fn(g)`` overrides the BERT schedule (variant B scripts use a constant lr).
+
+    Opt-in: set ``reduced`` before the ``run`` of an apply step and that window takes its gn (and LAMB's r) from it
+    instead of reducing them itself; the clip scale and everything after it are still computed here.  Such a window
+    keeps its c before the clip scale in ``window_c`` (LAMB: each adapted tensor's p before the update and u in
+    ``window_pu``).  ``run`` clears ``reduced`` once the window is applied.
     """
+    reduced: Optional[Reduced] = None
+    window_c: Optional[List[np.ndarray]] = None
+
+    def _global_norm(self, c: Sequence[np.ndarray]) -> np.float32:
+        """gn of the window's c: ``reduced.global_norm`` if it was given, else ``global_norm(c)``."""
+        if self.reduced is None:
+            return global_norm(c)
+        self.window_c = list(c)
+        return F32(self.reduced.global_norm)
 
     def __init__(self, params: List[np.ndarray], names: Sequence[str], hp: HParams,
                  accum_n: int, init_lr: float = 0.0, num_train_steps: int = 1,
@@ -266,7 +288,7 @@ class ReferenceTrainOp:
             # :83  1.0*accum_grad / N   (Mul by 1.0 exact, then RealDiv by fp32(N))
             normalized = [np.divide(np.multiply(F32(1.0), a, dtype=F32), nf, dtype=F32) for a in self.accum]
             if hp.clip_norm and hp.clip_norm > 0:                 # :84
-                gn = global_norm(normalized)
+                gn = self._global_norm(normalized)
                 s = clip_scale(gn, hp.clip_norm)
                 clipped = [np.multiply(n, s, dtype=F32) for n in normalized]
                 info.global_norm, info.clip_scale = gn, s
@@ -289,6 +311,7 @@ class ReferenceTrainOp:
                 self.beta2_power = F32(self.beta2_power * F32(hp.beta2))
             for a in self.accum:                                  # :86-87
                 a[...] = F32(0.0)
+            self.reduced = None
         self.global_step = g + 1                                  # :102-103
         return info
 

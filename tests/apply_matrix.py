@@ -15,13 +15,16 @@ Importable without torch (the inventory test runs without a GPU).  Test infrastr
 from __future__ import annotations
 
 import itertools
+import math
+from fractions import Fraction
 from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
+import exact_norm_oracle as eno
 import oracle_np as onp
 from ema_oracle import Ema
-from lamb_oracle import LambReferenceTrainOp
+from lamb_oracle import LambReferenceTrainOp, trust_ratio
 from loss_scale_oracle import LossScaledReferenceTrainOp
 
 F32 = np.float32
@@ -143,6 +146,34 @@ def _bits_equal(x: np.ndarray, y: np.ndarray) -> bool:
                                                  np.ascontiguousarray(y, dtype=F32).view(np.uint32))
 
 
+# a sum of squares the LAMB kernel forms in fp64 (gaccum_lamb.cuh add_sq64) is known far better than this before its
+# one rounding to fp32; only a sum this close to an fp32 rounding boundary may round to the boundary's other side
+LAMB_TIE_REL = 1e-12
+
+
+def check_global_norm(gn: np.float32, c: Sequence[np.ndarray]) -> None:
+    """The clip-apply's gn against the exact sum of squares of the window's c (``exact_norm_oracle.clip_norm_bound``);
+    a non-finite c or sum must give a non-finite gn."""
+    e = sum((eno.exact_sumsq(x) for x in c), Fraction(0))
+    if not isinstance(e, Fraction):
+        assert not np.isfinite(gn), (gn, e)
+        return
+    ref = eno.ref_norm(e)
+    if not np.isfinite(ref):
+        assert not np.isfinite(gn) or float(gn) ** 2 >= float(e) * (1 - 1e-6), (gn, float(e))
+        return
+    n = sum(x.size for x in c)
+    err = abs(float(gn) - math.sqrt(e))
+    assert np.isfinite(gn) and err <= eno.clip_norm_bound(e, n), (float(gn), math.sqrt(e), err, eno.clip_norm_bound(e, n))
+
+
+def trust_ratio_candidates(p: np.ndarray, u: np.ndarray) -> List[np.float32]:
+    """LAMB's r = ||p|| / ||u|| with each norm rounded to fp32 once from its exact sum of squares: one value, or, for
+    a sum within LAMB_TIE_REL of a rounding boundary, the values either side of it gives."""
+    return [trust_ratio(wn, un) for wn in eno.norm_candidates(eno.exact_sumsq(p), LAMB_TIE_REL)
+            for un in eno.norm_candidates(eno.exact_sumsq(u), LAMB_TIE_REL)]
+
+
 # ---- one train op and its oracle in lock-step -------------------------------------------------------------------------
 class LockStep:
     """A train op on cuda:0 and its composed oracle, stepped together.
@@ -158,11 +189,21 @@ class LockStep:
     clip scale within 3e-6; trust ratios within 1e-6; the average bit for bit against ``Ema`` fed the kernel's own
     weights; the model copy bit for bit against the RNE rounding of the kernel's master weights; the loss-scaling block
     and the beta powers exactly.
+
+    ``injected``: on an apply step the kernel runs first, and the oracle takes its global norm and trust ratios
+    (``oracle_np.Reduced``).  Everything the oracle still computes is then compared bit for bit, clipped windows and
+    LAMB included: p, m, v and the clip scale the oracle derives from the kernel's gn.  The reduced scalars themselves
+    are held to exact sums (``exact_norm_oracle``): gn within ``clip_norm_bound`` of sqrt(sum c^2), and r equal to
+    ||p|| / ||u|| with both norms rounded to fp32 once from their exact sums (either side of a tie for a sum that
+    lies within 1e-12 of one).  ``init`` maps tensor indices to their initial values; ``tensor_norms`` turns the
+    train op's per-tensor norms on.
     """
 
     def __init__(self, man, variant: str, mode: str, layout: str = "table", dtype: str = "fp32", has_g: bool = True,
                  ema: Optional[Tuple[float, bool]] = None, N: int = 3, seed: int = 0, views: Optional[Dict[int, int]] = None,
-                 nograd: Sequence[int] = (), zero: Sequence[int] = (), adapt_exclude: Optional[Sequence[str]] = None):
+                 nograd: Sequence[int] = (), zero: Sequence[int] = (), adapt_exclude: Optional[Sequence[str]] = None,
+                 injected: bool = False, init: Optional[Dict[int, np.ndarray]] = None, tensor_norms: bool = False,
+                 ls_cfg=LS_CFG):
         import torch
         import gaccum_b200 as g
         from gaccum_b200.train_op import GaccumTrainOp, PackedTrainOp
@@ -170,19 +211,24 @@ class LockStep:
         self.man, self.variant, self.mode, self.layout, self.has_g, self.N = man, variant, mode, layout, has_g, N
         self.dtype = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16}[dtype]
         self.views, self.nograd = dict(views or {}), set(nograd)
+        self.injected = injected
         self.rng = np.random.default_rng(seed)
         names = [n for n, _ in man]
         params = []
         for i, (_, s) in enumerate(man):
             x = np.zeros(s, F32) if i in zero else self.rng.normal(0, 0.05, s).astype(F32)
+            if init is not None and i in init:
+                x = np.array(init[i], F32).reshape(s)
             params.append(torch.from_numpy(x).to(self.dtype))          # 16-bit: the model starts representable
         hpo = oracle_hparams(variant, mode)
         hp = g.HParams(hpo.variant, 0, hpo.beta1, hpo.beta2, hpo.epsilon, hpo.weight_decay_rate, hpo.clip_norm)
         self.ls = mode.startswith("ls_")
-        lsc = g.LossScaleConfig(*LS_CFG) if self.ls else None
+        lsc = g.LossScaleConfig(*ls_cfg) if self.ls else None
         emac = g.EmaConfig(*ema) if ema is not None else None
         lr_fn = lambda s: g.learning_rate(SCHED["init_lr"], SCHED["num_train_steps"], SCHED["num_warmup_steps"], s)
         kw = dict(loss_scale=lsc, ema=emac, exclude_from_layer_adaptation=adapt_exclude)
+        if tensor_norms:
+            kw["tensor_norms"] = True
         if layout == "packed":
             assert dtype == "fp32" and not self.views
             self.op = PackedTrainOp([p.cuda() for p in params], names, hp, N, lr_fn, **kw)
@@ -191,7 +237,7 @@ class LockStep:
             self.op = GaccumTrainOp([self._device(i, p) for i, p in enumerate(params)], names, hp, N, lr_fn, **kw)
         self.cap = 0 if layout == "packed" else (256 if len(man) <= 256 else 1920)
         adapt = self.op.adapt if variant == "lamb" else None
-        self.ref = reference_op(variant, mode, [p.float().numpy() for p in params], names, N, adapt=adapt)
+        self.ref = reference_op(variant, mode, [p.float().numpy() for p in params], names, N, adapt=adapt, ls_cfg=ls_cfg)
         self.tracker = Ema(self._weights(), *ema) if ema is not None else None
         self.clipped = False                 # some window so far had a clip scale other than 1
 
@@ -227,9 +273,9 @@ class LockStep:
                 t = torch.from_numpy(x * S).to(self.dtype)                 # gradients of loss * S, in the model's dtype
             host.append(t.float().numpy())                                   # ... what the oracle sees: their upcast
             dev.append(self._device(i, t))
-        info = self.ref.run(host)
         g = op.global_step
         applied = self.g.is_apply_step(g, self.N)
+        info = None if self.injected else self.ref.run(host)
         if self.layout == "packed":
             if self.has_g:
                 self.gslab.zero_()
@@ -254,6 +300,12 @@ class LockStep:
             if applied:
                 op.apply_only(None)
             op.global_step = g + 1
+        if self.injected:
+            if applied:
+                st = op.stats()
+                ratios = op.trust_ratios() if self.variant == "lamb" else None
+                self.ref.reduced = onp.Reduced(F32(st["global_norm"]), ratios)
+            info = self.ref.run(host)
         assert info.applied == applied
         self.check(info)
         return applied
@@ -292,7 +344,7 @@ class LockStep:
             assert _bits_equal(a, ref.accum[i]), f"accumulator of {names[i]}"
         if info.applied and not self.skipped() and (self.mode in ("clip", "ls_clip")) and info.clip_scale != F32(1.0):
             self.clipped = True
-        exact = self.variant != "lamb" and not self.clipped
+        exact = self.injected or (self.variant != "lamb" and not self.clipped)
         weights = self._weights()
         for what, got, exp in (("p", weights, ref.params), ("m", self._slab(op.m), ref.m), ("v", self._slab(op.v), ref.v)):
             # not bit-exact: within 1e-5 of the model's largest |value|.  Per tensor that would be too tight for the
@@ -314,13 +366,26 @@ class LockStep:
             assert st["applied"] and F32(st["lr"]) == F32(info.lr)
             if self.mode not in ("clip", "ls_clip"):
                 assert (st["global_norm"], st["clip_scale"]) == (0.0, 1.0)
+            elif self.injected:
+                s, e = F32(st["clip_scale"]), F32(info.clip_scale)
+                assert s.tobytes() == e.tobytes() or (np.isnan(s) and np.isnan(e)), (s, e)    # NaN: any payload
+                check_global_norm(F32(st["global_norm"]), ref.window_c)
             else:
                 for k, e in (("global_norm", info.global_norm), ("clip_scale", info.clip_scale)):
                     if np.isfinite(e):
                         assert abs(st[k] - float(e)) <= 3e-6 * abs(float(e)), (k, st[k], e)
                     else:
                         assert not np.isfinite(st[k]), (k, st[k], e)
-            if self.variant == "lamb":
+            if self.variant == "lamb" and self.injected:
+                if not self.skipped():
+                    adapted = [i for i in range(len(self.man)) if ref.adapt[i]]
+                    r = op.trust_ratios()
+                    assert all(r[i] == 1.0 for i in range(len(self.man)) if not ref.adapt[i])
+                    assert len(ref.window_pu) == len(adapted)
+                    for i, (p, u) in zip(adapted, ref.window_pu):
+                        exp = trust_ratio_candidates(p, u)
+                        assert any(r[i].tobytes() == e.tobytes() for e in exp), (names[i], r[i], exp)
+            elif self.variant == "lamb":
                 r = op.trust_ratios()
                 exp = np.array(ref.ratios, F32)
                 # within 1e-6; once a window has clipped, 2e-4: a 1-element tensor whose u nearly cancels turns the

@@ -34,8 +34,10 @@ def trust_ratio(wn: np.float32, un: np.float32) -> np.float32:
         return F32(wn / un) if (wn > 0 and un > 0) else F32(1.0)
 
 
-def lamb_update(p, m, v, c, lr, beta1, beta2, eps, wd, use_decay, adapt, beta1_power, beta2_power):
-    """One tensor.  Returns (p', m', v', r)."""
+def lamb_update(p, m, v, c, lr, beta1, beta2, eps, wd, use_decay, adapt, beta1_power, beta2_power, ratio=None,
+                record=None):
+    """One tensor.  Returns (p', m', v', r).  ``ratio``: r of an adapted tensor as a device reduced it, used in place
+    of ``trust_ratio(norm(p), norm(u))``; ``record``: a list that (p, u) of an adapted tensor is appended to."""
     b1, b2 = F32(beta1), F32(beta2)
     omb1, omb2 = F32(1.0 - float(beta1)), F32(1.0 - float(beta2))
     next_m = np.add(np.multiply(b1, m, dtype=F32), np.multiply(omb1, c, dtype=F32), dtype=F32)
@@ -46,9 +48,23 @@ def lamb_update(p, m, v, c, lr, beta1, beta2, eps, wd, use_decay, adapt, beta1_p
         u = np.divide(mh, np.add(np.sqrt(vh, dtype=F32), F32(eps), dtype=F32), dtype=F32)
         if use_decay:
             u = np.add(u, np.multiply(F32(wd), p, dtype=F32), dtype=F32)
-        r = trust_ratio(norm(p), norm(u)) if adapt else F32(1.0)
+        if adapt and record is not None:
+            record.append((np.array(p, F32, copy=True), u))
+        if not adapt:
+            r = F32(1.0)
+        else:
+            r = trust_ratio(norm(p), norm(u)) if ratio is None else F32(ratio)
         next_p = np.subtract(p, np.multiply(F32(r * F32(lr)), u, dtype=F32), dtype=F32)
     return next_p, next_m, next_v, r
+
+
+def reduced_ratios(op: onp.ReferenceTrainOp):
+    """(per-tensor r to pass to ``lamb_update``, its ``record`` list) for the window ``op`` is applying: the device's r
+    and a fresh list when ``op.reduced`` is set, else None for every tensor and no record."""
+    T = len(op.params)
+    if op.reduced is None or op.reduced.ratios is None:
+        return [None] * T, None
+    return list(op.reduced.ratios), []
 
 
 def adaptation_mask(names: Sequence[str], exclude: Optional[Sequence[str]]) -> List[bool]:
@@ -93,16 +109,17 @@ class LambReferenceTrainOp(onp.ReferenceTrainOp):
                     c = [np.multiply(x, inv_s, dtype=F32) for x in c]
                     overflow = any(not np.all(np.isfinite(a)) for a in self.accum)
                 if hp.clip_norm and hp.clip_norm > 0:
-                    gn = onp.global_norm(c)
+                    gn = self._global_norm(c)
                     s = onp.clip_scale(gn, hp.clip_norm)
                     info.global_norm, info.clip_scale = gn, s
                     overflow = overflow or (self.ls and not np.isfinite(gn))
                     c = [np.multiply(x, s, dtype=F32) for x in c]
             if not overflow:
+                ratios, self.window_pu = reduced_ratios(self)
                 for i, ci in enumerate(c):
                     p2, m2, v2, r = lamb_update(self.params[i], self.m[i], self.v[i], ci, lr, hp.beta1, hp.beta2,
                                                 hp.epsilon, hp.weight_decay_rate, self.decay[i], self.adapt[i],
-                                                self.beta1_power, self.beta2_power)
+                                                self.beta1_power, self.beta2_power, ratios[i], self.window_pu)
                     self.params[i][...] = p2; self.m[i][...] = m2; self.v[i][...] = v2
                     self.ratios[i] = r
                 self.beta1_power = F32(self.beta1_power * F32(hp.beta1))
@@ -114,5 +131,6 @@ class LambReferenceTrainOp(onp.ReferenceTrainOp):
                 self.last_skipped = overflow
             for a in self.accum:
                 a[...] = F32(0.0)
+            self.reduced = None
         self.global_step = g + 1
         return info

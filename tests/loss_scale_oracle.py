@@ -59,7 +59,7 @@ class LossScaledReferenceTrainOp(onp.ReferenceTrainOp):
                 overflow = any(not np.all(np.isfinite(a)) for a in self.accum)
                 clipping = bool(hp.clip_norm and hp.clip_norm > 0)
                 if clipping:
-                    gn = onp.global_norm(normalized)
+                    gn = self._global_norm(normalized)
                     s = onp.clip_scale(gn, hp.clip_norm)
                     info.global_norm, info.clip_scale = gn, s
                     overflow = overflow or not np.isfinite(gn)
@@ -84,5 +84,6 @@ class LossScaledReferenceTrainOp(onp.ReferenceTrainOp):
             self.last_skipped = overflow
             for a in self.accum:
                 a[...] = F32(0.0)
+            self.reduced = None
         self.global_step = g + 1
         return info

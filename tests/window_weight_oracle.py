@@ -16,7 +16,7 @@ import numpy as np
 
 import oracle_np as onp
 from apply_matrix import LS_CFG, SCHED, oracle_hparams
-from lamb_oracle import lamb_update
+from lamb_oracle import lamb_update, reduced_ratios
 from loss_scale_oracle import update_scale
 from lr_mult_oracle import VARIANT_LAMB, LrMultLockStep, LrMultReferenceTrainOp
 
@@ -58,19 +58,20 @@ class WindowWeightReferenceTrainOp(LrMultReferenceTrainOp):
                     c = [np.multiply(x, inv_s, dtype=F32) for x in c]
                     overflow = any(not np.all(np.isfinite(a)) for a in self.accum)
                 if hp.clip_norm and hp.clip_norm > 0:
-                    gn = onp.global_norm(c)
+                    gn = self._global_norm(c)
                     s = onp.clip_scale(gn, hp.clip_norm)
                     info.global_norm, info.clip_scale = gn, s
                     overflow = overflow or (self.ls and not np.isfinite(gn))
                     if not overflow:
                         c = [np.multiply(x, s, dtype=F32) for x in c]
                 if not overflow:
+                    ratios, self.window_pu = reduced_ratios(self)
                     for i, ci in enumerate(c):
                         lr_t = self.lr_t(lr, i)
                         if hp.variant == VARIANT_LAMB:
                             p2, m2, v2, r = lamb_update(self.params[i], self.m[i], self.v[i], ci, lr_t, hp.beta1, hp.beta2,
                                                         hp.epsilon, hp.weight_decay_rate, self.decay[i], self.adapt[i],
-                                                        self.beta1_power, self.beta2_power)
+                                                        self.beta1_power, self.beta2_power, ratios[i], self.window_pu)
                             self.ratios[i] = r
                         elif hp.variant == onp.VARIANT_ADAM_WEIGHT_DECAY:
                             p2, m2, v2 = onp.adam_weight_decay_update(self.params[i], self.m[i], self.v[i], ci, lr_t,
@@ -90,6 +91,7 @@ class WindowWeightReferenceTrainOp(LrMultReferenceTrainOp):
                 self.last_skipped = overflow
             for a in self.accum:
                 a[...] = F32(0.0)
+            self.reduced = None
             self.last_weight, self.weight = W, F32(0.0)
         self.global_step = g + 1
         return info
