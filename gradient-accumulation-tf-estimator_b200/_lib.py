@@ -222,6 +222,12 @@ def is_apply_step(global_step: int, accum_n: int) -> bool:
     return accum_n > 0 and step32 % accum_n == 0
 
 
+def is_first_accumulate(global_step: int, accum_n: int) -> bool:
+    """The first accumulate of a window, which gaccum_step runs without reading the accumulators (gaccum_abi.cu
+    first_of_window): the step does not apply and the one before it did, both by the int32 predicate."""
+    return not is_apply_step(global_step, accum_n) and is_apply_step(int(global_step) - 1, accum_n)
+
+
 def _c_strs(strs: Sequence[str]):
     arr = (C.c_char_p * len(strs))()
     arr[:] = [s.encode() for s in strs]

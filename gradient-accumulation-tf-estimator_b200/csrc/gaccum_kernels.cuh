@@ -264,7 +264,10 @@ __device__ __forceinline__ float schedule_lr(const float init_lr, const long lon
   }
   return lr;
 }
-__device__ __forceinline__ void sched_load(const ScheduleParams& sp, const bool apply, SchedLaunch& sl) {
+// from_zero: the launch is a first accumulate, which does not read the accumulators; it may run only where the previous
+// step applied and left them at +0 ((int32)(g - 1) % N == 0), else it would overwrite that step's gradients
+__device__ __forceinline__ void sched_load(const ScheduleParams& sp, const bool apply, SchedLaunch& sl,
+                                           const bool from_zero = false) {
   const ScheduleState* st = sp.state;
   const long long g = __ldcg(&st->global_step);
   sl.g = g;
@@ -273,7 +276,8 @@ __device__ __forceinline__ void sched_load(const ScheduleParams& sp, const bool 
   sl.b2p = __ldcg(&st->beta2_power);
   sl.bc2 = __fsqrt_rn(__fsub_rn(1.0f, sl.b2p));
   sl.bc1 = __fsub_rn(1.0f, sl.b1p);
-  sl.ok = __ldcg(&st->refused) == 0 && ((((int)g % sp.accum_n) == 0) == apply);   // gaccum_is_apply_step
+  sl.ok = __ldcg(&st->refused) == 0 && ((((int)g % sp.accum_n) == 0) == apply)    // gaccum_is_apply_step
+          && (!from_zero || ((int)(g - 1) % sp.accum_n) == 0);
 }
 // One thread, once no CTA of the launch will read the block again: the next step, and (betas) TF1's beta powers
 // advanced with one fp32 multiply each, as after an applied window
@@ -286,8 +290,9 @@ __device__ __forceinline__ void sched_finish(const ScheduleParams& sp, const Sch
     st->beta2_power = __fmul_rn(sl.b2p, b2);
   }
 }
-// A launch whose branch global_step does not select (a captured graph whose start is not a window start) changes
-// nothing; block 0 marks the schedule refused, so every later launch is a no-op too and the host can report it.
+// A launch whose branch global_step does not select (a captured graph whose start is not a window start, or a window
+// that straddles the int32 wrap of global_step), or a first accumulate that does not follow an apply, changes nothing;
+// block 0 marks the schedule refused, so every later launch is a no-op too and the host can report it.
 __device__ __forceinline__ void sched_refuse(const ScheduleParams& sp) {
   if (blockIdx.x == 0 && threadIdx.x == 0) sp.state->refused = 1;
 }
@@ -742,7 +747,7 @@ accumulate_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   if (prm.sched.state) {
     // device schedule: every CTA checks the step before its tile; the last one through advances it
     __shared__ SchedLaunch s_sl;
-    if (threadIdx.x == 0) sched_load(prm.sched, false, s_sl);
+    if (threadIdx.x == 0) sched_load(prm.sched, false, s_sl, FROM_ZERO);
     __syncthreads();
     if (!s_sl.ok) { sched_refuse(prm.sched); return; }
     if ((int)blockIdx.x < prm.num_tiles) accumulate_tile<FROM_ZERO, H>(prm.tiles[blockIdx.x], prm);

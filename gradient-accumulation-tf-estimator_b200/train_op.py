@@ -42,9 +42,48 @@ def _pinned_zeros(n: int) -> torch.Tensor:
         return t
 
 
-def _window_position(g: int, n: int) -> int:
-    """The position of micro-step g in its window: the step cast to int32 (as gaccum_is_apply_step does), modulo N."""
-    return ((int(g) + 0x80000000) % 0x100000000 - 0x80000000) % n
+class ScheduleCursor:
+    """The host's share of a device-scheduled train op: the step of its next launch, passed as StepArgs.global_step.
+    gaccum_step takes from it both the branch and whether the launch is a window's first accumulate (which does not read
+    the accumulators), by the int32 predicate the device checks.  The position g mod N is not enough: int32(g) jumps
+    from 2^31 - 1 to -2^31 every 2^32 steps, and unless N is a power of two the window that straddles the jump is longer
+    than N (for N = 3 it applies at 2^31 - 2 and next at 2^31 + 2).
+
+    Captured launches run when the graph is replayed, any number of times, so after a capture the host does not know the
+    step: the first eager launch after it reads the device counter (``read_step``, synchronous), once.  A replay made
+    after that, between eager launches, leaves the tracked step behind by whole windows: the same kernels, except once
+    the replays have carried the device across an int32 wrap, where the next eager launch is refused by the device
+    (loudly: ``schedule_state()`` raises) and writing ``global_step`` resynchronises."""
+
+    def __init__(self, accum_n: int, read_step: Callable[[], int]):
+        self.N, self._read_step = int(accum_n), read_step
+        self.step = 0                   # the next launch's step, while not stale
+        self._stale = False             # a capture launched since the step was last known
+        self._capturing = False
+
+    def reset(self, g: int) -> None:
+        """The device counter was written with g."""
+        self.step, self._stale = int(g), False
+
+    def launch(self, capturing: bool) -> int:
+        """The step of the launch about to be enqueued.  A CUDA graph must start at a window start (an apply step):
+        refused here when the capture follows eager micro-steps; a graph that starts or ends mid-window, or whose replay
+        straddles the int32 wrap, is refused by the device when replayed (gaccum.h: `refused`)."""
+        if capturing:
+            if not self._capturing and not _lib.is_apply_step(self.step, self.N):
+                raise ValueError(f"a CUDA graph of a device-scheduled train op must start at a window start: this "
+                                 f"capture starts at global_step {self.step}, an accumulate step (N = {self.N})")
+            self._stale = True
+        elif self._stale:
+            self.reset(self._read_step())
+        self._capturing = capturing
+        return self.step
+
+    def advance(self) -> bool:
+        """After the launch: True if it was an apply step."""
+        applied = _lib.is_apply_step(self.step, self.N)
+        self.step += 1
+        return applied
 
 
 class ScheduleLr:
@@ -153,14 +192,14 @@ class _DeviceTrainOp(_TrainOpCore):
             self.window_weight = self._ww_state[0]
         if device_schedule is not None:
             # gaccum_schedule_state: 6 x 8 bytes.  From here on global_step, the lr and (without loss scaling) the beta
-            # powers live on the device; the host keeps only the position in the window, which picks the branch
+            # powers live on the device; the host tracks the step only to pick each launch's kernel (ScheduleCursor)
             if lr_fn is not None and not isinstance(lr_fn, ScheduleLr):
                 raise ValueError("a device-scheduled train op computes its learning rate on the device: pass "
                                  "lr_fn=None (or device_schedule_lr(cfg))")
             self.lr_fn = ScheduleLr(device_schedule)
             self._sched_state = torch.zeros(6, dtype=torch.int64, device=self.device)
             self.plan.set_device_schedule(device_schedule, self._sched_state.data_ptr())
-            self._capturing = False
+            self._cursor = ScheduleCursor(self.N, lambda: self._read_schedule()["global_step"])
             self._write_schedule(self._step, self.beta1_power, self.beta2_power)
         self._norms: Optional[torch.Tensor] = None
         if tensor_norms:
@@ -213,7 +252,7 @@ class _DeviceTrainOp(_TrainOpCore):
         """gaccum_schedule_init: the step, the beta powers (ignored under loss scaling, whose block holds them) and
         refused = 0, stream-ordered on the current stream."""
         self.plan.schedule_init(self._sched_state.data_ptr(), g, beta1_power, beta2_power, self._stream())
-        self._phase = _window_position(g, self.N)
+        self._cursor.reset(g)
 
     def schedule_state(self) -> Dict[str, float]:
         """Synchronously read the device schedule: global_step, beta1_power and beta2_power (under loss scaling the
@@ -238,22 +277,14 @@ class _DeviceTrainOp(_TrainOpCore):
         return out
 
     def _scheduled_step_args(self) -> StepArgs:
-        """The host's share of a device-scheduled micro-step: its position in the window (all the branch and the
-        first-accumulate decision depend on).  A CUDA graph must start at a window start: refused here when the
-        capture follows eager micro-steps; a graph that starts or ends mid-window is always refused by the device when
-        replayed (gaccum.h: `refused`)."""
-        capturing = torch.cuda.is_current_stream_capturing()
-        if capturing and not self._capturing and self._phase != 0:
-            raise ValueError(f"a CUDA graph of a device-scheduled train op must start at a window start: this capture "
-                             f"starts at micro-step {self._phase} of a window of {self.N}")
-        self._capturing = capturing
-        return StepArgs(self._phase, self.N, 0, 0.0, 0.0, 0.0, 0.0)
+        """The host's share of a device-scheduled micro-step: its step, from which gaccum_step picks the branch and
+        the first-accumulate kernel (ScheduleCursor.launch)."""
+        g = self._cursor.launch(torch.cuda.is_current_stream_capturing())
+        return StepArgs(g, self.N, 0, 0.0, 0.0, 0.0, 0.0)
 
     def _scheduled_after(self) -> bool:
-        applied = self._phase == 0
-        self._phase = (self._phase + 1) % self.N
-        self.last_applied = applied
-        return applied
+        self.last_applied = self._cursor.advance()
+        return self.last_applied
 
     def _init_ema(self, cfg: EmaConfig, weights: Callable[[int], torch.Tensor]) -> None:
         """Keep an exponential moving average of ``weights(i)`` (the fp32 weights the apply updates).  TF initialises
@@ -751,7 +782,7 @@ class PackedTrainOp(_DeviceTrainOp):
         self._add_weight(weight, stream)
         sched = self._sched_state is not None
         args = self._scheduled_step_args() if sched else None
-        g = self._phase if sched else self.global_step
+        g = args.global_step if sched else self.global_step
         applied = _lib.is_apply_step(g, self.N)
         if sched and not applied:
             # the gradients are already in accum: the launch only advances the device schedule (one CTA)

@@ -332,13 +332,21 @@ GACCUM_API int gaccum_plan_set_window_weight(gaccum_plan* plan, gaccum_window_we
  *     GACCUM_LAMB uses them, then multiplies each by fp32(beta) once (TF1 AdamOptimizer._finish).  Under loss scaling it
  *     is the loss-scaling block (gaccum_loss_scale_state.beta{1,2}_power), as without a device schedule; this block's
  *     beta fields are then 0 and unused.
- *   - The host still chooses the branch, from gaccum_step_args.global_step and accum_n as before.  Only that step's
- *     position in its window matters, g mod N: a window is always the same N launches (N - 1 accumulates, the first
- *     without reading the accumulators, then an apply), so a graph captured over whole windows replays correctly with
- *     any g.  Each launch checks that g selects its branch ((int32)g % N == 0 exactly for an apply).  A launch that
- *     finds otherwise -- e.g. a replayed graph whose capture did not start at a window start, or did not end at a window
- *     end -- changes nothing and sets `refused`; from then on every launch on the plan is a no-op, until
- *     gaccum_schedule_init rewrites the block.  gaccum_step_args.lr and .beta{1,2}_power are ignored.
+ *   - The host still chooses the kernel, from gaccum_step_args.global_step and accum_n as before: the branch, and for an
+ *     accumulate whether it is the window's first (which does not read the accumulators).  Eager launches should pass
+ *     the step they run at.  Each launch checks g against its kernel: (int32)g % N == 0 exactly for an apply, and a
+ *     first accumulate only where (int32)(g - 1) % N == 0.  A launch that finds otherwise changes nothing and sets
+ *     `refused`; from then on every launch on the plan is a no-op, until gaccum_schedule_init rewrites the block.
+ *     gaccum_step_args.lr and .beta{1,2}_power are ignored.
+ *   - A graph captured over whole windows replays correctly at any g whose windows are N launches each (N - 1
+ *     accumulates, the first without reading the accumulators, then an apply).  That holds for every g except across
+ *     the int32 wrap: (int32)g jumps from 2^31 - 1 to -2^31 at g = 2^31 + k 2^32, and unless N is a power of two the
+ *     window that straddles the jump is longer than N (N = 3: applies at 2^31 - 2, then 2^31 + 2).  A replay that
+ *     reaches that window is refused at its first launch whose kernel g does not select, after the launches before it
+ *     ran.  The caller then reads global_step, rewrites the block with gaccum_schedule_init at that step, runs the
+ *     straddling window's remaining micro-steps eagerly (each with its own step), and replays again from the next
+ *     window start.  A replay whose capture did not start at a window start, or did not end at a window end, is
+ *     refused the same way.
  *   - gaccum_step_packed must use force_branch = -1; on an accumulate step its grad_slab may be NULL (the gradients
  *     are already in accum): the launch then only advances the schedule.
  * gaccum_plan_set_device_schedule is host-only: validates `cfg` (end_lr must be 0 and power 1) and keeps `block`

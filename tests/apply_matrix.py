@@ -121,17 +121,17 @@ def oracle_hparams(variant: str, mode: str) -> onp.HParams:
 
 
 def reference_op(variant: str, mode: str, params, names, N: int, adapt: Optional[Sequence[bool]] = None,
-                 ls_cfg=LS_CFG):
+                 ls_cfg=LS_CFG, sched=SCHED, global_step: int = 0):
     """The oracle of one dispatch key: ReferenceTrainOp, LossScaledReferenceTrainOp or LambReferenceTrainOp."""
     hp = oracle_hparams(variant, mode)
     params = [np.array(p, dtype=F32, copy=True) for p in params]
     ls = mode.startswith("ls_")
     lskw = dict(initial_scale=ls_cfg[0], multiplier=ls_cfg[1], growth_interval=ls_cfg[2]) if ls else {}
     if variant == "lamb":
-        return LambReferenceTrainOp(params, names, hp, N, adapt=adapt, **lskw, **SCHED)
+        return LambReferenceTrainOp(params, names, hp, N, adapt=adapt, **lskw, **sched, global_step=global_step)
     if ls:
-        return LossScaledReferenceTrainOp(params, names, hp, N, **lskw, **SCHED)
-    return onp.ReferenceTrainOp(params, names, hp, N, **SCHED)
+        return LossScaledReferenceTrainOp(params, names, hp, N, **lskw, **sched, global_step=global_step)
+    return onp.ReferenceTrainOp(params, names, hp, N, **sched, global_step=global_step)
 
 
 def rel_err(x, ref) -> float:
@@ -197,13 +197,22 @@ class LockStep:
     ||p|| / ||u|| with both norms rounded to fp32 once from their exact sums (either side of a tie for a sum that
     lies within 1e-12 of one).  ``init`` maps tensor indices to their initial values; ``tensor_norms`` turns the
     train op's per-tensor norms on.
+
+    ``sched`` is the learning-rate schedule (``init_lr``, ``num_train_steps``, ``num_warmup_steps``; default ``SCHED``)
+    and ``global_step`` the step both start at.  ``device_schedule``: the train op keeps global_step, the lr and the
+    beta powers on the device, and every micro-step goes through the op's own entry point -- ``op.step()`` packed
+    (gradients added into ``p.grad``, with or without ``has_g``), ``op.run`` with a table, where a case without
+    gradients adds them into the accumulators and runs ``run([None] * T)``.  ``check`` then also compares the device
+    counter, the lr in the stats of every micro-step, and the beta powers in their one home (the schedule block, or the
+    loss-scaling block under loss scaling, the schedule block's then 0).
     """
 
     def __init__(self, man, variant: str, mode: str, layout: str = "table", dtype: str = "fp32", has_g: bool = True,
                  ema: Optional[Tuple[float, bool]] = None, N: int = 3, seed: int = 0, views: Optional[Dict[int, int]] = None,
                  nograd: Sequence[int] = (), zero: Sequence[int] = (), adapt_exclude: Optional[Sequence[str]] = None,
                  injected: bool = False, init: Optional[Dict[int, np.ndarray]] = None, tensor_norms: bool = False,
-                 ls_cfg=LS_CFG):
+                 ls_cfg=LS_CFG, sched: Optional[Dict[str, float]] = None, global_step: int = 0,
+                 device_schedule: bool = False):
         import torch
         import gaccum_b200 as g
         from gaccum_b200.train_op import GaccumTrainOp, PackedTrainOp
@@ -212,6 +221,9 @@ class LockStep:
         self.dtype = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16}[dtype]
         self.views, self.nograd = dict(views or {}), set(nograd)
         self.injected = injected
+        self.ls_cfg, self.sched, self.g0 = ls_cfg, dict(SCHED if sched is None else sched), int(global_step)
+        self.device_schedule = device_schedule
+        self.g_host = self.g0                # the step of the next micro-step, as the oracle counts it
         self.rng = np.random.default_rng(seed)
         names = [n for n, _ in man]
         params = []
@@ -225,8 +237,12 @@ class LockStep:
         self.ls = mode.startswith("ls_")
         lsc = g.LossScaleConfig(*ls_cfg) if self.ls else None
         emac = g.EmaConfig(*ema) if ema is not None else None
-        lr_fn = lambda s: g.learning_rate(SCHED["init_lr"], SCHED["num_train_steps"], SCHED["num_warmup_steps"], s)
-        kw = dict(loss_scale=lsc, ema=emac, exclude_from_layer_adaptation=adapt_exclude)
+        sc = self.sched
+        lr_fn = lambda s: g.learning_rate(sc["init_lr"], sc["num_train_steps"], sc["num_warmup_steps"], s)
+        kw = dict(loss_scale=lsc, ema=emac, exclude_from_layer_adaptation=adapt_exclude, global_step=self.g0)
+        if device_schedule:
+            kw["device_schedule"] = g._lib.ScheduleConfig(**sc)
+            lr_fn = None
         if tensor_norms:
             kw["tensor_norms"] = True
         if layout == "packed":
@@ -237,7 +253,8 @@ class LockStep:
             self.op = GaccumTrainOp([self._device(i, p) for i, p in enumerate(params)], names, hp, N, lr_fn, **kw)
         self.cap = 0 if layout == "packed" else (256 if len(man) <= 256 else 1920)
         adapt = self.op.adapt if variant == "lamb" else None
-        self.ref = reference_op(variant, mode, [p.float().numpy() for p in params], names, N, adapt=adapt, ls_cfg=ls_cfg)
+        self.ref = reference_op(variant, mode, [p.float().numpy() for p in params], names, N, adapt=adapt, ls_cfg=ls_cfg,
+                                sched=self.sched, global_step=self.g0)
         self.tracker = Ema(self._weights(), *ema) if ema is not None else None
         self.clipped = False                 # some window so far had a clip scale other than 1
 
@@ -261,8 +278,9 @@ class LockStep:
         return out
 
     # -- one micro-step ---------------------------------------------------------------------------------------------
-    def step(self, grads) -> bool:
-        torch, op = self.torch, self.op
+    def inputs(self, grads):
+        """This micro-step's gradients as the oracle sees them (host, the upcast) and as the op gets them (dev)."""
+        torch = self.torch
         S = F32(self.ref.scale) if self.ls else F32(1.0)
         host, dev = [], []
         for i, x in enumerate(grads):
@@ -273,10 +291,37 @@ class LockStep:
                 t = torch.from_numpy(x * S).to(self.dtype)                 # gradients of loss * S, in the model's dtype
             host.append(t.float().numpy())                                   # ... what the oracle sees: their upcast
             dev.append(self._device(i, t))
-        g = op.global_step
+        return host, dev
+
+    def step(self, grads, launch=None) -> bool:
+        """One micro-step of the op and its oracle, then ``check``.  ``launch(dev)``, if given, runs the op's micro-step
+        in place of its own entry point (e.g. by replaying a graph captured over one micro-step); a device-scheduled op
+        only."""
+        torch, op = self.torch, self.op
+        host, dev = self.inputs(grads)
+        g = self.g_host if self.device_schedule else op.global_step
         applied = self.g.is_apply_step(g, self.N)
         info = None if self.injected else self.ref.run(host)
-        if self.layout == "packed":
+        if launch is not None:
+            assert self.device_schedule
+            launch(dev)
+        elif self.device_schedule:
+            with torch.no_grad():
+                if self.layout == "packed":
+                    for p, t in zip(op.params, dev):
+                        if t is not None:
+                            p.grad.add_(t)
+                    ran = op.step()
+                elif self.has_g:
+                    ran = op.run(dev)
+                else:
+                    for i, t in enumerate(dev):                # what the accumulate kernel adds: the widened gradient
+                        if t is not None:
+                            op.accum_view(i).add_(t.float())
+                    ran = op.run([None] * len(dev))
+            op.schedule_state()                                # raises if the device refused the launch
+            assert ran == applied
+        elif self.layout == "packed":
             if self.has_g:
                 self.gslab.zero_()
                 for i, t in enumerate(dev):
@@ -300,6 +345,7 @@ class LockStep:
             if applied:
                 op.apply_only(None)
             op.global_step = g + 1
+        self.g_host = g + 1
         if self.injected:
             if applied:
                 st = op.stats()
@@ -397,10 +443,23 @@ class LockStep:
             s = op.loss_scale_state()
             assert (F32(s["scale"]), s["good_windows"], s["skipped_windows"], s["last_skipped"]) == \
                 (ref.scale, ref.good_windows, ref.skipped_windows, ref.last_skipped)
+        if self.device_schedule:
+            block = op._sched_state.cpu()
+            assert int(block[0]) == int(op.global_step_tensor) == ref.global_step == self.g_host
+            assert int(block.view(torch.int32)[11]) == 0, "refused"
+            st = op.stats()
+            assert F32(st["lr"]).tobytes() == F32(self.g.learning_rate(
+                self.sched["init_lr"], self.sched["num_train_steps"], self.sched["num_warmup_steps"], ref.global_step - 1)).tobytes()
+            assert st["applied"] == info.applied
+            sched_b = block.view(torch.float32)[9:11].numpy()
+            if self.ls:
+                assert not sched_b.any(), "the schedule block holds beta powers under loss scaling"
         if self.variant in ("adam", "lamb"):
             if self.ls:
                 words = op._ls_state.cpu().numpy()
                 b1, b2 = words[4], words[5]
+            elif self.device_schedule:
+                b1, b2 = sched_b
             else:
                 b1, b2 = F32(op.beta1_power), F32(op.beta2_power)
             assert (b1, b2) == (F32(ref.beta1_power), F32(ref.beta2_power))

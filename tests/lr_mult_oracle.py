@@ -108,12 +108,14 @@ class LrMultReferenceTrainOp(onp.ReferenceTrainOp):
 
 
 def reference_op(variant: str, mode: str, params, names, N: int, lr_mult: Optional[Sequence[float]] = None,
-                 adapt: Optional[Sequence[bool]] = None, ls_cfg=LS_CFG) -> LrMultReferenceTrainOp:
+                 adapt: Optional[Sequence[bool]] = None, ls_cfg=LS_CFG, sched=SCHED,
+                 global_step: int = 0) -> LrMultReferenceTrainOp:
     """``apply_matrix.reference_op`` with a learning-rate table: the oracle of one dispatch key."""
     hp = oracle_hparams(variant, mode)
     params = [np.array(p, dtype=F32, copy=True) for p in params]
     lskw = dict(initial_scale=ls_cfg[0], multiplier=ls_cfg[1], growth_interval=ls_cfg[2]) if mode.startswith("ls_") else {}
-    return LrMultReferenceTrainOp(params, names, hp, N, lr_mult=lr_mult, adapt=adapt, **lskw, **SCHED)
+    return LrMultReferenceTrainOp(params, names, hp, N, lr_mult=lr_mult, adapt=adapt, **lskw, **sched,
+                                  global_step=global_step)
 
 
 class LrMultLockStep(LockStep):
@@ -127,4 +129,4 @@ class LrMultLockStep(LockStep):
         self.op.plan.set_lr_multipliers(self.lr_mult)
         adapt = self.op.adapt if variant == "lamb" else None
         self.ref = reference_op(variant, mode, self.ref.params, [n for n, _ in man], self.N, lr_mult=self.lr_mult,
-                                adapt=adapt)
+                                adapt=adapt, ls_cfg=self.ls_cfg, sched=self.sched, global_step=self.g0)

@@ -142,3 +142,93 @@ def test_header_documents_the_block():
     hdr = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include", "gaccum.h")).read()
     assert "gaccum_plan_set_device_schedule" in hdr and "gaccum_schedule_init" in hdr
     assert g.version() == 200
+
+
+# ---- the front end's kernel choice across the int32 wrap (train_op.ScheduleCursor) -------------------------------------
+def _c_first_accumulate(step, n):
+    """gaccum_abi.cu first_of_window, in C's arithmetic: (int32)g does not apply and (int32)((int32)g - 1) does."""
+    def c_apply(x):
+        x32 = int(np.int64(x).astype(np.int32))
+        return x32 - int(x32 / n) * n == 0               # C's truncating %
+    g32 = int(np.int64(step).astype(np.int32))
+    return not c_apply(g32) and c_apply(g32 - 1)
+
+
+def _oracle_applies(g0, n, steps):
+    """The reference's predicate (oracle_np.ReferenceTrainOp.run) over ``steps`` micro-steps from g0."""
+    return [int(np.int32(np.int64(g))) % n == 0 for g in range(g0, g0 + steps)]
+
+
+@pytest.mark.parametrize("n", [1, 2, 3, 4, 5, 7])
+@pytest.mark.parametrize("g0", [0, 2**31 - 20, 2**32 - 20, 3 * 2**31 - 20])
+def test_eager_launches_choose_their_kernel_from_the_int32_step(n, g0):
+    from gaccum_b200.train_op import ScheduleCursor
+    cur = ScheduleCursor(n, lambda: pytest.fail("an eager op never reads the device counter"))
+    cur.reset(g0)
+    applies = _oracle_applies(g0, n, 40)
+    for k in range(40):
+        g = cur.launch(False)
+        assert g == g0 + k                                 # StepArgs.global_step: the step the launch runs at
+        apply, first = lib.is_apply_step(g, n), lib.is_first_accumulate(g, n)
+        assert apply == applies[k]
+        assert first == _c_first_accumulate(g, n)
+        # a first accumulate follows an apply: the device's check, (int32)(g - 1) % N == 0
+        if first:
+            assert k == 0 or applies[k - 1]
+        assert cur.advance() == apply
+
+
+@pytest.mark.parametrize("n, applies_at", [
+    (3, [2**31 - 5, 2**31 - 2, 2**31 + 2, 2**31 + 5]),     # the straddling window is 4 launches
+    (5, [2**31 - 8, 2**31 - 3, 2**31 + 3, 2**31 + 8]),     # ... 6 launches
+    (4, [2**31 - 8, 2**31 - 4, 2**31, 2**31 + 4]),         # a power of two: every window is N
+])
+def test_the_window_that_straddles_2_to_the_31(n, applies_at):
+    from gaccum_b200.train_op import ScheduleCursor
+    g0 = applies_at[0]
+    cur = ScheduleCursor(n, lambda: None)
+    cur.reset(g0)
+    seen, firsts = [], []
+    for _ in range(applies_at[-1] - g0 + 1):
+        g = cur.launch(False)
+        if lib.is_first_accumulate(g, n):
+            firsts.append(g)
+        if cur.advance():
+            seen.append(g)
+    assert seen == applies_at
+    assert firsts == [a + 1 for a in applies_at[:-1]]
+
+
+def test_first_eager_launch_after_a_capture_reads_the_device_counter_once():
+    from gaccum_b200.train_op import ScheduleCursor
+    reads = []
+    device = {"g": None}
+
+    def read():
+        reads.append(device["g"])
+        return device["g"]
+
+    cur = ScheduleCursor(3, read)
+    cur.reset(2**31 - 5)                                   # an apply step: a window start
+    for _ in range(3):                                     # the captured window: nothing runs, nothing is read
+        cur.launch(True)
+        cur.advance()
+    assert reads == []
+    device["g"] = 2**31 + 1                                # two replays (the second refused at 2^31 + 1), then
+    assert cur.launch(False) == 2**31 + 1                  # ... the first eager launch reads the counter
+    assert not lib.is_apply_step(2**31 + 1, 3)
+    cur.advance()
+    assert cur.launch(False) == 2**31 + 2 and lib.is_apply_step(2**31 + 2, 3)
+    cur.advance()
+    assert reads == [2**31 + 1]                            # once
+
+
+def test_capture_must_start_at_an_apply_step():
+    from gaccum_b200.train_op import ScheduleCursor
+    cur = ScheduleCursor(3, lambda: None)
+    cur.reset(2**31 + 1)                                   # g mod 3 == 0, but int32(g) does not apply
+    with pytest.raises(ValueError, match="must start at a window start"):
+        cur.launch(True)
+    assert cur.launch(False) == 2**31 + 1                  # the refused capture changed nothing
+    cur.reset(2**31 + 2)
+    assert cur.launch(True) == 2**31 + 2

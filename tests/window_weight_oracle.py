@@ -98,12 +98,14 @@ class WindowWeightReferenceTrainOp(LrMultReferenceTrainOp):
 
 
 def reference_op(variant: str, mode: str, params, names, N: int, lr_mult: Optional[Sequence[float]] = None,
-                 adapt: Optional[Sequence[bool]] = None, ls_cfg=LS_CFG) -> WindowWeightReferenceTrainOp:
+                 adapt: Optional[Sequence[bool]] = None, ls_cfg=LS_CFG, sched=SCHED,
+                 global_step: int = 0) -> WindowWeightReferenceTrainOp:
     """``lr_mult_oracle.reference_op`` with the window weight: the oracle of one dispatch key."""
     hp = oracle_hparams(variant, mode)
     params = [np.array(p, dtype=F32, copy=True) for p in params]
     lskw = dict(initial_scale=ls_cfg[0], multiplier=ls_cfg[1], growth_interval=ls_cfg[2]) if mode.startswith("ls_") else {}
-    return WindowWeightReferenceTrainOp(params, names, hp, N, lr_mult=lr_mult, adapt=adapt, **lskw, **SCHED)
+    return WindowWeightReferenceTrainOp(params, names, hp, N, lr_mult=lr_mult, adapt=adapt, **lskw, **sched,
+                                      global_step=global_step)
 
 
 class WindowWeightLockStep(LrMultLockStep):
@@ -120,7 +122,7 @@ class WindowWeightLockStep(LrMultLockStep):
         self.op.plan.set_window_weight(self.ww.data_ptr())
         adapt = self.op.adapt if variant == "lamb" else None
         self.ref = reference_op(variant, mode, self.ref.params, [n for n, _ in man], self.N, lr_mult=self.lr_mult,
-                                adapt=adapt)
+                                adapt=adapt, ls_cfg=self.ls_cfg, sched=self.sched, global_step=self.g0)
 
     def wstep(self, grads, w) -> bool:
         self.ref.add_weight(w)
