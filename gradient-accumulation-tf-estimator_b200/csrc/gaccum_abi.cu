@@ -64,6 +64,7 @@ struct gaccum_plan {
   uint32_t* d_dp_sync = nullptr;           // data-parallel kernel: block-completion counters and tile tickets (zero between launches)
   unsigned long long* d_barrier = nullptr; // clip-apply kernel: monotonic arrival counter of the consumers' grid barrier
   LaunchCounters* d_counters = nullptr;    // ... two sets of per-launch counters (tickets, pool length, norm accumulator)
+  unsigned int* d_done = nullptr;          // apply_kernel, scheduled accumulate_kernel: CTAs of the launch that are through (zero between launches)
 #ifdef GACCUM_EXPERIMENTS
   unsigned long long* d_debug = nullptr;   // per-CTA timestamps (tools/cta_timeline.py; experiments build only)
 #endif
@@ -88,7 +89,6 @@ struct gaccum_plan {
   gaccum_ema_config ema_cfg{};
   float* ema_slab = nullptr;
   gaccum_ema_state* ema_state = nullptr;
-  unsigned int* d_ema_done = nullptr;      // apply_kernel: CTAs of the launch that are through (zero between launches)
   // per-tensor learning-rate multipliers (gaccum_plan_set_lr_multipliers): 1.0 unless set, the device copy exists on every
   // device plan because every apply kernel reads it
   bool lr_mult_set = false;
@@ -147,6 +147,8 @@ static Scalars make_scalars(const gaccum_hparams& hp, const gaccum_step_args* a)
     s.inv_nf = (n > 0 && (n & (n - 1)) == 0 && n <= (1 << 24)) ? 1.0f / (float)n : 0.0f;
   }
   s.lr = a ? a->lr : 0.0f;
+  s.b1p = a ? a->beta1_power : 0.0f;
+  s.b2p = a ? a->beta2_power : 0.0f;
   s.b1 = (float)hp.beta1;
   s.b2 = (float)hp.beta2;
   s.eps = (float)hp.epsilon;
@@ -159,14 +161,6 @@ static Scalars make_scalars(const gaccum_hparams& hp, const gaccum_step_args* a)
     volatile float o1 = 1.0f - s.b1, o2 = 1.0f - s.b2;   // ApplyAdam: T(1) - beta1()
     s.omb1 = o1;
     s.omb2 = o2;
-    if (a) {
-      volatile float t1 = 1.0f - a->beta2_power;
-      volatile float t2 = sqrtf(t1);
-      volatile float t3 = a->lr * t2;
-      volatile float t4 = 1.0f - a->beta1_power;
-      volatile float t5 = t3 / t4;
-      s.alpha = t5;
-    }
   }
   return s;
 }
@@ -271,6 +265,7 @@ static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, f
   prm.v = v;
   prm.barrier = pl->d_barrier;
   prm.counters = pl->d_counters;
+  prm.done = pl->d_done;
 #ifdef GACCUM_EXPERIMENTS
   prm.debug = pl->d_debug;
 #endif
@@ -287,27 +282,13 @@ static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, f
   prm.lamb.ratios = pl->d_ratios;
   prm.lamb.adapt = pl->d_adapt;
   prm.lamb.num_tensors = pl->T;
-  prm.lamb.beta1_power = a ? a->beta1_power : 0.0f;
-  prm.lamb.beta2_power = a ? a->beta2_power : 0.0f;
   prm.ema.slab = pl->ema_slab;
   prm.ema.state = reinterpret_cast<EmaState*>(pl->ema_state);
-  prm.ema.done = pl->d_ema_done;
   prm.ema.decay = (float)pl->ema_cfg.decay;
   prm.ema.num_updates = pl->ema_cfg.num_updates;
   prm.lrm.mult = pl->d_lr_mult;
-  prm.lrm.bc2 = 1.0f;
-  prm.lrm.bc1 = 1.0f;
-  if (a && pl->hp.variant == GACCUM_ADAM) {
-    // make_scalars' t2 and t4: the alpha of a tile is (lr_t * bc2) / bc1
-    volatile float t1 = 1.0f - a->beta2_power;
-    volatile float t2 = sqrtf(t1);
-    volatile float t4 = 1.0f - a->beta1_power;
-    prm.lrm.bc2 = t2;
-    prm.lrm.bc1 = t4;
-  }
   prm.ww.state = reinterpret_cast<WindowWeightState*>(pl->ww_state);
   prm.sched.state = reinterpret_cast<ScheduleState*>(pl->sched_state);
-  prm.sched.done = pl->d_ema_done;
   prm.sched.accum_n = a ? a->accum_n : 1;
   prm.norms = pl->norms;
 }
@@ -381,9 +362,39 @@ static int check_args(const gaccum_step_args* a) {
   return GACCUM_OK;
 }
 
+// The plan settings an entry point may lack (refuse), in the order refuse checks them
+enum PlanSetting : unsigned {
+  kPlanLossScale = 1u << 0,
+  kPlanLamb = 1u << 1,
+  kPlanHalf = 1u << 2,
+  kPlanEma = 1u << 3,
+  kPlanLrMult = 1u << 4,
+  kPlanWindowWeight = 1u << 5,
+  kPlanSchedule = 1u << 6,
+  kPlanNorms = 1u << 7,
+  kPlanAll = (1u << 8) - 1u,
+};
+// Fails on the first of the settings `lacks` names that the plan has: `what` does not support it
+static int refuse(const gaccum_plan* pl, const unsigned lacks, const char* what) {
+  if (!pl) return GACCUM_OK;
+  const struct { unsigned setting; bool on; const char* name; } settings[] = {
+      {kPlanLossScale, pl->ls_on, "loss scaling"},
+      {kPlanLamb, pl->hp.variant == GACCUM_LAMB, "GACCUM_LAMB"},
+      {kPlanHalf, pl->master != nullptr, "16-bit parameters (gaccum_plan_set_param_dtype)"},
+      {kPlanEma, pl->ema_on, "a moving average (gaccum_plan_set_ema)"},
+      {kPlanLrMult, pl->lr_mult_set, "learning-rate multipliers (gaccum_plan_set_lr_multipliers)"},
+      {kPlanWindowWeight, pl->ww_state != nullptr, "a window weight (gaccum_plan_set_window_weight)"},
+      {kPlanSchedule, pl->sched_state != nullptr, "a device schedule (gaccum_plan_set_device_schedule)"},
+      {kPlanNorms, pl->norms.out != nullptr, "per-tensor norms (gaccum_plan_set_tensor_norms)"},
+  };
+  for (const auto& st : settings)
+    if ((lacks & st.setting) && st.on) return fail(GACCUM_EINVAL, "%s does not support %s", what, st.name);
+  return GACCUM_OK;
+}
+
 static void free_plan_device(gaccum_plan* pl) {
   cudaFree(pl->d_tiles); cudaFree(pl->d_partials); cudaFree(pl->d_stats); cudaFree(pl->d_dp_sync); cudaFree(pl->d_barrier); cudaFree(pl->d_counters);
-  cudaFree(pl->d_adapt); cudaFree(pl->d_lamb_acc); cudaFree(pl->d_ratios); cudaFree(pl->d_ema_done); cudaFree(pl->d_lr_mult);
+  cudaFree(pl->d_adapt); cudaFree(pl->d_lamb_acc); cudaFree(pl->d_ratios); cudaFree(pl->d_done); cudaFree(pl->d_lr_mult);
   cudaFree(pl->d_norms);
 #ifdef GACCUM_EXPERIMENTS
   cudaFree(pl->d_debug);
@@ -509,8 +520,8 @@ int gaccum_plan_create(gaccum_plan** out, int32_t T, const int64_t* numels, cons
 #endif
     if (e == cudaSuccess) e = cudaMalloc(&pl->d_stats, sizeof(gaccum_stats));
     if (e == cudaSuccess) e = cudaMemset(pl->d_stats, 0, sizeof(gaccum_stats));
-    if (e == cudaSuccess) e = cudaMalloc(&pl->d_ema_done, sizeof(unsigned int));
-    if (e == cudaSuccess) e = cudaMemset(pl->d_ema_done, 0, sizeof(unsigned int));
+    if (e == cudaSuccess) e = cudaMalloc(&pl->d_done, sizeof(unsigned int));
+    if (e == cudaSuccess) e = cudaMemset(pl->d_done, 0, sizeof(unsigned int));
     if (e == cudaSuccess) e = cudaMalloc(&pl->d_lr_mult, (size_t)std::max(1, T) * sizeof(float));
     if (e == cudaSuccess && T > 0)
       e = cudaMemcpy(pl->d_lr_mult, pl->lr_mult.data(), (size_t)T * sizeof(float), cudaMemcpyHostToDevice);
@@ -610,10 +621,6 @@ int gaccum_plan_set_param_dtype(gaccum_plan* pl, int32_t dtype, float* master_sl
   return GACCUM_OK;
 }
 
-static int refuse_lamb(const gaccum_plan* pl, const char* what) {
-  return pl && pl->hp.variant == GACCUM_LAMB ? fail(GACCUM_EINVAL, "%s does not support GACCUM_LAMB", what) : GACCUM_OK;
-}
-
 int gaccum_plan_set_layer_adaptation(gaccum_plan* pl, const uint8_t* adapt) {
   if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
   if (pl->hp.variant != GACCUM_LAMB) return fail(GACCUM_EINVAL, "layer adaptation is a GACCUM_LAMB setting (plan variant %d)", pl->hp.variant);
@@ -668,10 +675,6 @@ int gaccum_ema_init(gaccum_plan* pl, gaccum_ema_state* device_state, int64_t num
   return GACCUM_OK;
 }
 
-static int refuse_ema(const gaccum_plan* pl, const char* what) {
-  return pl && pl->ema_on ? fail(GACCUM_EINVAL, "%s does not support a moving average (gaccum_plan_set_ema)", what) : GACCUM_OK;
-}
-
 int gaccum_plan_set_lr_multipliers(gaccum_plan* pl, const float* mult) {
   if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
   if (!mult && pl->T > 0) return fail(GACCUM_EINVAL, "mult is NULL");
@@ -688,12 +691,6 @@ int gaccum_plan_set_lr_multipliers(gaccum_plan* pl, const float* mult) {
   return GACCUM_OK;
 }
 
-static int refuse_lr_mult(const gaccum_plan* pl, const char* what) {
-  return pl && pl->lr_mult_set
-             ? fail(GACCUM_EINVAL, "%s does not support learning-rate multipliers (gaccum_plan_set_lr_multipliers)", what)
-             : GACCUM_OK;
-}
-
 int gaccum_plan_set_window_weight(gaccum_plan* pl, gaccum_window_weight_state* state) {
   if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
   if (!state || !aligned16_host(state)) return fail(GACCUM_EINVAL, "state must be a 16-byte aligned device pointer");
@@ -701,17 +698,6 @@ int gaccum_plan_set_window_weight(gaccum_plan* pl, gaccum_window_weight_state* s
   static_assert(sizeof(gaccum_window_weight_state) == sizeof(WindowWeightState), "header and kernel disagree");
   pl->ww_state = state;
   return GACCUM_OK;
-}
-
-static int refuse_window_weight(const gaccum_plan* pl, const char* what) {
-  return pl && pl->ww_state
-             ? fail(GACCUM_EINVAL, "%s does not support a window weight (gaccum_plan_set_window_weight)", what)
-             : GACCUM_OK;
-}
-
-static int refuse_half(const gaccum_plan* pl, const char* what) {
-  return pl && pl->master ? fail(GACCUM_EINVAL, "%s does not support 16-bit parameters (gaccum_plan_set_param_dtype)", what)
-                          : GACCUM_OK;
 }
 
 int gaccum_loss_scale_init(gaccum_plan* pl, gaccum_loss_scale_state* device_state, gaccum_stream_t stream) {
@@ -824,12 +810,6 @@ int gaccum_plan_set_tensor_norms(gaccum_plan* pl, float* device_out) {
   return GACCUM_OK;
 }
 
-static int refuse_norms(const gaccum_plan* pl, const char* what) {
-  return pl && pl->norms.out
-             ? fail(GACCUM_EINVAL, "%s does not support per-tensor norms (gaccum_plan_set_tensor_norms)", what)
-             : GACCUM_OK;
-}
-
 static int accumulate_impl(gaccum_plan* pl, const float* const* grads, float* accum,
                            const gaccum_step_args* a, gaccum_stream_t stream) {
   if (int rc = check_compute(pl, accum, nullptr, nullptr, false)) return rc;
@@ -840,16 +820,10 @@ static int accumulate_impl(gaccum_plan* pl, const float* const* grads, float* ac
                             : do_accumulate_tab<kCapLarge>(pl, grads, accum, a, st);
 }
 
-static int refuse_schedule(const gaccum_plan* pl, const char* what) {
-  return pl && pl->sched_state
-             ? fail(GACCUM_EINVAL, "%s does not support a device schedule (gaccum_plan_set_device_schedule)", what)
-             : GACCUM_OK;
-}
-
 int gaccum_accumulate(gaccum_plan* pl, const float* const* grads, float* accum, gaccum_stream_t stream) {
   // without step arguments the launch cannot check global_step against its branch: a device-scheduled plan steps with
   // gaccum_step
-  if (int rc = refuse_schedule(pl, "gaccum_accumulate")) return rc;
+  if (int rc = refuse(pl, kPlanSchedule, "gaccum_accumulate")) return rc;
   return accumulate_impl(pl, grads, accum, nullptr, stream);
 }
 
@@ -858,7 +832,7 @@ static int apply_impl(gaccum_plan* pl, const float* const* grads, float* const* 
 
 int gaccum_apply(gaccum_plan* pl, const float* const* grads, float* const* params, float* accum,
                  float* m, float* v, const gaccum_step_args* a, gaccum_stream_t stream) {
-  if (int rc = refuse_schedule(pl, "gaccum_apply")) return rc;
+  if (int rc = refuse(pl, kPlanSchedule, "gaccum_apply")) return rc;
   return apply_impl(pl, grads, params, accum, m, v, a, stream);
 }
 
@@ -884,7 +858,7 @@ int gaccum_step(gaccum_plan* pl, const float* const* grads, float* const* params
 int gaccum_step_packed(gaccum_plan* pl, const float* grad_slab, float* param_slab, float* accum,
                        float* m, float* v, const gaccum_step_args* a, int32_t force_branch,
                        gaccum_stream_t stream) {
-  if (int rc = refuse_half(pl, "gaccum_step_packed")) return rc;
+  if (int rc = refuse(pl, kPlanHalf, "gaccum_step_packed")) return rc;
   if (int rc = check_args(a)) return rc;
   if (pl && pl->sched_state && force_branch >= 0)
     return fail(GACCUM_EINVAL, "a device-scheduled plan takes its branch from global_step: force_branch must be -1 (got %d)", force_branch);
@@ -1009,14 +983,7 @@ static int do_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float*
 
 int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* const* grads, float* m, float* v,
                     const gaccum_step_args* a, uint32_t epoch, gaccum_stream_t stream) {
-  if (pl && pl->ls_on) return fail(GACCUM_EINVAL, "the fused data-parallel apply does not support loss scaling");
-  if (int rc = refuse_lamb(pl, "the fused data-parallel apply")) return rc;
-  if (int rc = refuse_half(pl, "the fused data-parallel apply")) return rc;
-  if (int rc = refuse_ema(pl, "the fused data-parallel apply")) return rc;
-  if (int rc = refuse_lr_mult(pl, "the fused data-parallel apply")) return rc;
-  if (int rc = refuse_window_weight(pl, "the fused data-parallel apply")) return rc;
-  if (int rc = refuse_schedule(pl, "the fused data-parallel apply")) return rc;
-  if (int rc = refuse_norms(pl, "the fused data-parallel apply")) return rc;
+  if (int rc = refuse(pl, kPlanAll, "the fused data-parallel apply")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (comm->world < 2 || comm->world > GACCUM_MAX_RANKS || comm->rank < 0 || comm->rank >= comm->world)
     return fail(GACCUM_EINVAL, "world must be 2..%d and 0 <= rank < world", GACCUM_MAX_RANKS);
@@ -1039,14 +1006,7 @@ int gaccum_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* co
 
 int gaccum_step_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float* const* grads, float* m, float* v,
                    const gaccum_step_args* a, uint32_t epoch, gaccum_stream_t stream) {
-  if (pl && pl->ls_on) return fail(GACCUM_EINVAL, "the fused data-parallel step does not support loss scaling");
-  if (int rc = refuse_lamb(pl, "the fused data-parallel step")) return rc;
-  if (int rc = refuse_half(pl, "the fused data-parallel step")) return rc;
-  if (int rc = refuse_ema(pl, "the fused data-parallel step")) return rc;
-  if (int rc = refuse_lr_mult(pl, "the fused data-parallel step")) return rc;
-  if (int rc = refuse_window_weight(pl, "the fused data-parallel step")) return rc;
-  if (int rc = refuse_schedule(pl, "the fused data-parallel step")) return rc;
-  if (int rc = refuse_norms(pl, "the fused data-parallel step")) return rc;
+  if (int rc = refuse(pl, kPlanAll, "the fused data-parallel step")) return rc;
   if (!comm) return fail(GACCUM_EINVAL, "comm is NULL");
   if (int rc = check_args(a)) return rc;
   if (!grads) return fail(GACCUM_EINVAL, "grads is NULL");
@@ -1126,14 +1086,7 @@ int gaccum_host_session_create(gaccum_host_session** out, gaccum_plan* pl) {
   *out = nullptr;
   if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
   // host-resident models train in fp32 (no fp16 autocast on the CPU): nothing to loss-scale
-  if (pl->ls_on) return fail(GACCUM_EINVAL, "the host-buffer session does not support loss scaling");
-  if (int rc = refuse_half(pl, "the host-buffer session")) return rc;
-  if (int rc = refuse_lamb(pl, "the host-buffer session")) return rc;
-  if (int rc = refuse_ema(pl, "the host-buffer session")) return rc;
-  if (int rc = refuse_lr_mult(pl, "the host-buffer session")) return rc;
-  if (int rc = refuse_window_weight(pl, "the host-buffer session")) return rc;
-  if (int rc = refuse_schedule(pl, "the host-buffer session")) return rc;
-  if (int rc = refuse_norms(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse(pl, kPlanAll, "the host-buffer session")) return rc;
   if (pl->device < 0) return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): libgaccum has no CPU fallback, a CUDA device is required");
   DeviceGuard guard(pl->device);
   gaccum_host_session* s = new (std::nothrow) gaccum_host_session();
@@ -1241,14 +1194,7 @@ int gaccum_step_host(gaccum_host_session* s, const float* const* host_grads, flo
   if (!s || !host_grads) return fail(GACCUM_EINVAL, "bad arguments to gaccum_step_host");
   if (int rc = check_args(a)) return rc;
   gaccum_plan* pl = s->plan;
-  if (pl->ls_on) return fail(GACCUM_EINVAL, "the host-buffer session does not support loss scaling");
-  if (int rc = refuse_half(pl, "the host-buffer session")) return rc;
-  if (int rc = refuse_lamb(pl, "the host-buffer session")) return rc;
-  if (int rc = refuse_ema(pl, "the host-buffer session")) return rc;
-  if (int rc = refuse_lr_mult(pl, "the host-buffer session")) return rc;
-  if (int rc = refuse_window_weight(pl, "the host-buffer session")) return rc;
-  if (int rc = refuse_schedule(pl, "the host-buffer session")) return rc;
-  if (int rc = refuse_norms(pl, "the host-buffer session")) return rc;
+  if (int rc = refuse(pl, kPlanAll, "the host-buffer session")) return rc;
   DeviceGuard guard(pl->device);
   const int b = (int)(s->calls & 1);
   ++s->calls;

@@ -257,9 +257,9 @@ __device__ __forceinline__ float dp_reduce_tile(const TileDesc d, const DpParams
   return acc;
 }
 
-// ---- phase C: one owned tile.  update from the reduced a', broadcast p' to every rank ----
+// ---- phase C: one owned tile.  update from the reduced a' with `rate` (tile_rate), broadcast p' to every rank ----
 template <int VARIANT, int CAP>
-__device__ __forceinline__ void dp_update_tile(const TileDesc d, const DpParams<CAP>& prm, const float s) {
+__device__ __forceinline__ void dp_update_tile(const TileDesc d, const DpParams<CAP>& prm, const float s, const float rate) {
   const size_t soff = (size_t)d.soff32 * kSlabAlign;
   float* __restrict__ a = prm.accum + soff;
   float* __restrict__ m = prm.m + soff;
@@ -278,7 +278,7 @@ __device__ __forceinline__ void dp_update_tile(const TileDesc d, const DpParams<
             [&](int u, uint32_t i) { va[u] = __ldcg(a4 + i); vp[u] = __ldcs(p4 + i); vm[u] = __ldcs(m4 + i); vv[u] = __ldcs(v4 + i); },
             [] {},
             [&](int u, uint32_t i) {
-              update_vec<VARIANT>(va[u], scaled, s, vp[u], vm[u], vv[u], decay, sc);
+              update_vec<VARIANT>(va[u], scaled, s, vp[u], vm[u], vv[u], decay, sc, rate, sc);
               __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
               __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));
 #pragma unroll
@@ -287,7 +287,7 @@ __device__ __forceinline__ void dp_update_tile(const TileDesc d, const DpParams<
             },
             [&](uint32_t i) {
               float px = p[i], mx = m[i], vx = v[i];
-              update_elem<VARIANT>(__ldcg(a + i), scaled, s, px, mx, vx, decay, sc);
+              update_elem<VARIANT>(__ldcg(a + i), scaled, s, px, mx, vx, decay, sc, rate, sc);
               m[i] = mx; v[i] = vx; a[i] = 0.f;
               for (int w = 0; w < W; ++w) prm.param[w][soff + i] = px;
             });
@@ -419,6 +419,8 @@ dp_apply_kernel(const __grid_constant__ DpParams<CAP> prm) {
   }
   __syncthreads();
   const float s = s_bcast[0];
+  // no per-tensor multipliers: the step's lr, or GACCUM_ADAM's alpha from the beta powers
+  const float rate = tile_rate<VARIANT>(prm.sc.lr, 1.0f, __fsqrt_rn(__fsub_rn(1.0f, prm.sc.b2p)), __fsub_rn(1.0f, prm.sc.b1p));
 
   // ---- phase C: sharded update + all-gather by pushes ----------------------------------------------------
   {
@@ -429,7 +431,7 @@ dp_apply_kernel(const __grid_constant__ DpParams<CAP> prm) {
       tl.prefetch();
       TileDesc dn{};
       if (lo + tl.nxt < hi) dn = prm.tiles[lo + tl.nxt];
-      dp_update_tile<VARIANT>(d, prm, s);
+      dp_update_tile<VARIANT>(d, prm, s, rate);
       tl.advance();
       d = dn;
     }

@@ -77,7 +77,7 @@ struct Scalars {
   float eps;     //                                           optimization.py:157
   float wd;      //                                           optimization.py:167
   float clip;    //                                           optimization.py:84
-  float alpha;   // B only: lr*sqrt(1-b2^t)/(1-b1^t)          TF1 ApplyAdam
+  float b1p, b2p;  // GACCUM_ADAM, GACCUM_LAMB: TF1's beta powers of this step (gaccum_step_args; 0 without)
 };
 
 // gaccum_loss_scale_state (gaccum.h): caller-owned device memory, written only by the loss-scaled apply launch
@@ -118,8 +118,6 @@ struct LambParams {
   float* ratios;           // num_tensors: r of the last applied window (gaccum_read_trust_ratios)
   const uint8_t* adapt;    // num_tensors: 1 = layer adaptation (gaccum_plan_set_layer_adaptation)
   int32_t num_tensors;
-  float beta1_power;       // TF1's beta powers of this step (loss-scaled launches use the device block's)
-  float beta2_power;
 };
 
 // gaccum_ema_state (gaccum.h): caller-owned device memory, written by gaccum_ema_init and afterwards only by the apply
@@ -135,18 +133,14 @@ static_assert(sizeof(EmaState) == 16, "gaccum_ema_state is 16 bytes");
 struct EmaParams {
   float* slab;             // the averages, a slab in the plan's layout (16-byte aligned)
   EmaState* state;
-  unsigned int* done;      // apply_kernel: CTAs of the launch that are through (0 between launches)
   float decay;             // fp32(decay)
   int32_t num_updates;     // 1: d = min(decay, (1 + n) / (10 + n))
 };
 
 // Per-tensor learning-rate multipliers (gaccum_plan_set_lr_multipliers).  Every plan has the table (1.0 unless set), so
-// no kernel is specialised on it: each apply kernel reads mult[t] once per tile and uses the tile's lr_t = lr * mult[t]
-// -- GACCUM_ADAM: alpha_t = (lr_t * bc2) / bc1, make_scalars' op order -- where Scalars' lr / alpha would go.
+// no kernel is specialised on it: each apply kernel reads mult[t] once per tile and uses the tile's rate (tile_rate).
 struct LrMultParams {
   const float* mult;       // num_tensors
-  float bc2;               // GACCUM_ADAM: sqrtf(1 - beta2_power) of this step (loss-scaled launches use the device block's)
-  float bc1;               // GACCUM_ADAM: 1 - beta1_power
 };
 
 // gaccum_window_weight_state (gaccum.h): caller-owned device memory.  The producer adds each micro-batch's weight into
@@ -177,11 +171,10 @@ struct ScheduleState {
 };
 static_assert(sizeof(ScheduleState) == 48, "gaccum_schedule_state is 48 bytes");
 
-// The device schedule (gaccum_plan_set_device_schedule).  state == NULL: the host's lr and beta powers (Scalars,
-// LrMultParams, LambParams).  A launch-uniform branch, not a template flag: no kernel is specialised on it.
+// The device schedule (gaccum_plan_set_device_schedule).  state == NULL: the host's lr and beta powers (Scalars).  A
+// launch-uniform branch, not a template flag: no kernel is specialised on it.
 struct ScheduleParams {
   ScheduleState* state;
-  unsigned int* done;      // CTAs of the launch that are through (EmaParams::done: launches on a plan are serialised)
   int32_t accum_n;         // N: the launch checks that global_step selects its branch
 };
 
@@ -221,6 +214,7 @@ struct KernelParams {
   float* stats;       // gaccum_stats
   unsigned long long* barrier;  // apply_clip_kernel: monotonic arrival counter of the consumers' grid barrier
   struct LaunchCounters* counters;  // apply_clip_kernel: two sets of per-launch counters (tickets, pool length, norm accumulator)
+  unsigned int* done;   // apply_kernel, scheduled accumulate_kernel: CTAs of the launch that are through (0 between launches)
 #ifdef GACCUM_EXPERIMENTS
   unsigned long long* debug;  // 16 words per CTA: 4 timestamps (ns) + wait-cycle counters (tools/cta_timeline.py)
 #endif
@@ -237,15 +231,6 @@ struct KernelParams {
 };
 static_assert(sizeof(KernelParams<1920>) <= 32764, "kernel parameters must fit the 32 KB limit");
 
-// What a launch of a device-scheduled plan derives from the block as it finds it (thread 0 of every CTA, before any CTA
-// can write it): the step g, its learning rate, the beta powers, and whether the launch may run at all.
-struct SchedLaunch {
-  long long g;
-  float lr;
-  float bc2, bc1;          // GACCUM_ADAM: sqrt(1 - beta2_power), 1 - beta1_power (LrMultParams' terms)
-  float b1p, b2p;
-  int ok;                  // g selects this launch's branch and no earlier launch was refused
-};
 // optimization.py:29-54 exactly as gaccum_learning_rate evaluates it on the host: polynomial decay (end 0, power 1) of
 // min(g, T) over T, then, with a warm-up, (1 - is_warmup) * lr + is_warmup * (init_lr * (int32(g) / int32(W))).  One
 // correctly rounded fp32 op per TF op; int64 -> fp32 and int32 -> fp32 conversions round to nearest.
@@ -264,30 +249,28 @@ __device__ __forceinline__ float schedule_lr(const float init_lr, const long lon
   }
   return lr;
 }
-// from_zero: the launch is a first accumulate, which does not read the accumulators; it may run only where the previous
-// step applied and left them at +0 ((int32)(g - 1) % N == 0), else it would overwrite that step's gradients
-__device__ __forceinline__ void sched_load(const ScheduleParams& sp, const bool apply, SchedLaunch& sl,
-                                           const bool from_zero = false) {
+// The learning rate of a device-scheduled launch (a LaunchStep) at the block's step g, the beta powers as the block
+// holds them, and whether the launch may run: g selects its branch (apply), no earlier launch was refused, and a first
+// accumulate (from_zero), which does not read the accumulators, follows a step that applied and left them at +0
+// ((int32)(g - 1) % N == 0) -- else it would overwrite that step's gradients
+template <typename Step>
+__device__ __forceinline__ void sched_load(const ScheduleParams& sp, const bool apply, const bool from_zero, Step& sl) {
   const ScheduleState* st = sp.state;
   const long long g = __ldcg(&st->global_step);
-  sl.g = g;
   sl.lr = schedule_lr(__ldcg(&st->init_lr), __ldcg(&st->num_train_steps), __ldcg(&st->num_warmup_steps), g);
   sl.b1p = __ldcg(&st->beta1_power);
   sl.b2p = __ldcg(&st->beta2_power);
-  sl.bc2 = __fsqrt_rn(__fsub_rn(1.0f, sl.b2p));
-  sl.bc1 = __fsub_rn(1.0f, sl.b1p);
   sl.ok = __ldcg(&st->refused) == 0 && ((((int)g % sp.accum_n) == 0) == apply)    // gaccum_is_apply_step
           && (!from_zero || ((int)(g - 1) % sp.accum_n) == 0);
 }
-// One thread, once no CTA of the launch will read the block again: the next step, and (betas) TF1's beta powers
-// advanced with one fp32 multiply each, as after an applied window
-__device__ __forceinline__ void sched_finish(const ScheduleParams& sp, const SchedLaunch& sl, const bool betas, const float b1,
-                                             const float b2) {
+// The next step, and (betas) TF1's beta powers advanced with one fp32 multiply each, as after an applied window.  Only
+// this commit writes the block, so it still holds what the launch found.
+__device__ __forceinline__ void sched_finish(const ScheduleParams& sp, const bool betas, const float b1, const float b2) {
   ScheduleState* st = sp.state;
-  st->global_step = sl.g + 1;
+  st->global_step = __ldcg(&st->global_step) + 1;
   if (betas) {
-    st->beta1_power = __fmul_rn(sl.b1p, b1);
-    st->beta2_power = __fmul_rn(sl.b2p, b2);
+    st->beta1_power = __fmul_rn(__ldcg(&st->beta1_power), b1);
+    st->beta2_power = __fmul_rn(__ldcg(&st->beta2_power), b2);
   }
 }
 // A launch whose branch global_step does not select (a captured graph whose start is not a window start, or a window
@@ -464,8 +447,7 @@ __device__ __forceinline__ Divisor weight_divisor(float W) {
   const uint32_t bits = __float_as_uint(W), e = (bits >> 23) & 0xffu;
   return Divisor{W, ((bits & 0x007fffffu) == 0u && e != 0u && e != 0xffu) ? __fdiv_rn(1.0f, W) : 0.f};
 }
-// The divisor of one apply launch: W as the state holds it when the launch starts (weighted plans), else N.  Read by
-// one thread of each CTA before any CTA can reach window_finish.
+// The divisor of one apply launch: W as the state holds it when the launch starts (weighted plans), else N
 template <typename KP>
 __device__ __forceinline__ Divisor launch_divisor(const KP& prm) {
   return prm.ww.state ? weight_divisor(__ldcg(&prm.ww.state->weight)) : Divisor{prm.sc.nf, prm.sc.inv_nf};
@@ -476,8 +458,7 @@ __device__ __forceinline__ void window_finish(WindowWeightState* st, float W) {
   st->weight = 0.f;
 }
 
-// rate: the learning rate (VARIANT 0) or alpha (VARIANT 1) the update uses -- Scalars' own, or the tile's lr_t / alpha_t
-// (LrMultParams)
+// rate: the tile's learning rate lr_t (VARIANT 0) or alpha_t (VARIANT 1) the update uses (tile_rate)
 template <int VARIANT>
 __device__ __forceinline__ void adam_elem(float c, float& p, float& m, float& v, bool decay,
                                           const Scalars& sc, const float& rate) {
@@ -499,12 +480,9 @@ __device__ __forceinline__ void adam_elem(float c, float& p, float& m, float& v,
     v = v2;
   }
 }
-template <int VARIANT>
-__device__ __forceinline__ const float& sc_rate(const Scalars& sc) { return VARIANT == 0 ? sc.lr : sc.alpha; }
-
 // The tile's rate for tensor multiplier `mult`: lr_t = lr * mult, one correctly rounded multiply; GACCUM_ADAM:
-// alpha_t = (lr_t * sqrt(1 - b2^t)) / (1 - b1^t), with bc2 and bc1 those two bias-correction terms.  mult == 1 gives
-// Scalars' lr / alpha bit for bit.
+// alpha_t = (lr_t * sqrt(1 - b2^t)) / (1 - b1^t), with bc2 and bc1 those two bias-correction terms -- TF1 ApplyAdam's
+// alpha, one rounding per op, when mult == 1.
 template <int VARIANT>
 __device__ __forceinline__ float tile_rate(const float lr, const float mult, const float bc2, const float bc1) {
   const float lr_t = __fmul_rn(lr, mult);
@@ -516,18 +494,13 @@ __device__ __forceinline__ float tensor_mult(const LrMultParams& lrm, const Tile
 }
 
 // optimization.py:83-85: c = a/D (dv: N, or the window weight W), times the clip scale s if `scaled` (never a multiply
-// by 1: it could change a NaN's payload), then one Adam step of p, m, v with `rate` (default: Scalars' lr / alpha)
+// by 1: it could change a NaN's payload), then one Adam step of p, m, v with `rate` (tile_rate)
 template <int VARIANT, typename D>
 __device__ __forceinline__ void update_elem(float a, bool scaled, float s, float& p, float& m, float& v, bool decay,
                                             const Scalars& sc, const float& rate, const D& dv) {
   float c = normalize(a, dv.nf, dv.inv_nf);
   if (scaled) c = __fmul_rn(c, s);
   adam_elem<VARIANT>(c, p, m, v, decay, sc, rate);
-}
-template <int VARIANT>
-__device__ __forceinline__ void update_elem(float a, bool scaled, float s, float& p, float& m, float& v, bool decay,
-                                            const Scalars& sc) {
-  update_elem<VARIANT>(a, scaled, s, p, m, v, decay, sc, sc_rate<VARIANT>(sc), sc);
 }
 template <int VARIANT, typename D>
 __device__ __forceinline__ void update_vec(const float4 a, bool scaled, float s, float4& p, float4& m, float4& v, bool decay,
@@ -536,11 +509,6 @@ __device__ __forceinline__ void update_vec(const float4 a, bool scaled, float s,
   update_elem<VARIANT>(a.y, scaled, s, p.y, m.y, v.y, decay, sc, rate, dv);
   update_elem<VARIANT>(a.z, scaled, s, p.z, m.z, v.z, decay, sc, rate, dv);
   update_elem<VARIANT>(a.w, scaled, s, p.w, m.w, v.w, decay, sc, rate, dv);
-}
-template <int VARIANT>
-__device__ __forceinline__ void update_vec(const float4 a, bool scaled, float s, float4& p, float4& m, float4& v, bool decay,
-                                           const Scalars& sc) {
-  update_vec<VARIANT>(a, scaled, s, p, m, v, decay, sc, sc_rate<VARIANT>(sc), sc);
 }
 
 __device__ __forceinline__ float4 add_rn(const float4 a, const float4 b) {
@@ -741,30 +709,141 @@ __device__ __forceinline__ void accumulate_tile(const TileDesc d, const KernelPa
             [&](uint32_t i) { a[i] = __fadd_rn(FROM_ZERO ? 0.f : a[i], g.elem(i)); });
 }
 
+// ---------------------------------------------------------------------------------------------
+// One launch's step: what it reads from the device state blocks when it starts (launch_begin) and what it writes back
+// when it ends (launch_commit).
+// ---------------------------------------------------------------------------------------------
+// loss scaling: the state as this launch finds it
+__device__ __forceinline__ void ls_load(const LossScaleState* st, LossScaleState& s) {
+  s.scale = __ldcg(&st->scale);
+  s.good_windows = __ldcg(&st->good_windows);
+  s.skipped_windows = __ldcg(&st->skipped_windows);
+  s.beta1_power = __ldcg(&st->beta1_power);
+  s.beta2_power = __ldcg(&st->beta2_power);
+}
+// TF 2 DynamicLossScale, counted in windows (gaccum.h, gaccum_loss_scale_config); BETAS: the optimizer keeps TF1's beta
+// powers, advanced on applied windows only
+template <bool BETAS>
+__device__ __forceinline__ void ls_finish(const LossScaleParams& ls, const LossScaleState& s_ls, const bool skip,
+                                          const float b1, const float b2) {
+  LossScaleState* out = ls.state;
+  const float S = s_ls.scale;
+  if (skip) {
+    const float down = __fdiv_rn(S, ls.multiplier);   // exact: both are powers of two
+    out->scale = down < 1.0f ? 1.0f : down;
+    out->good_windows = 0;
+    out->skipped_windows = s_ls.skipped_windows + 1u;
+    out->last_skipped = 1;
+  } else {
+    const int32_t good = s_ls.good_windows + 1;
+    if (good >= ls.growth_interval) {
+      const float up = __fmul_rn(S, ls.multiplier);
+      if (fabsf(up) <= 3.402823466e38f) out->scale = up;
+      out->good_windows = 0;
+    } else {
+      out->good_windows = good;
+    }
+    out->last_skipped = 0;
+    if constexpr (BETAS) {                            // TF1 AdamOptimizer._finish, applied windows only
+      out->beta1_power = __fmul_rn(s_ls.beta1_power, b1);
+      out->beta2_power = __fmul_rn(s_ls.beta2_power, b2);
+    }
+  }
+}
+
+// The VARIANT of launch_begin and launch_commit: the optimizer of an apply launch (gaccum.h: 0 GACCUM_ADAM_WEIGHT_DECAY,
+// 1 GACCUM_ADAM, 2 GACCUM_LAMB), or kAccumulate
+constexpr int kLamb = 2;
+constexpr int kAccumulate = -1;
+// GACCUM_ADAM and GACCUM_LAMB keep TF1's beta powers: every applied window advances them
+__host__ __device__ constexpr bool keeps_beta_powers(int variant) { return variant == 1 || variant == kLamb; }
+
+// The part of a LaunchStep that only EMA kernels have: an empty base otherwise, so no kernel's shared memory grows
+template <bool EMA> struct StepEma {};
+template <> struct StepEma<true> { EmaLaunch ema; };
+// The step as one launch finds it.  A loss-scaled launch also finds the loss-scaling state, which it keeps in a shared
+// object of its own: held in the same object, the packed Adam kLsClip clip-apply spills 12 more bytes per thread.
+template <bool EMA = false>
+struct LaunchStep : StepEma<EMA> {
+  float lr;
+  float b1p, b2p;          // GACCUM_ADAM, GACCUM_LAMB: TF1's beta powers
+  float bc2, bc1;          // GACCUM_ADAM: sqrt(1 - b2p) and 1 - b1p, the bias corrections of alpha_t (tile_rate)
+  Divisor dv;              // apply launches: N, or the window weight W
+  int ok;                  // 0: the device schedule refused the launch (sched_load)
+};
+static_assert(sizeof(LaunchStep<>) == 32, "the parts a kernel does not have take no space");
+
+// Thread 0 of every CTA, before its CTA can reach a grid barrier or launch_commit -- so before any CTA of the launch can
+// write what it reads, and every CTA finds the same step.  lr and the beta powers are the host's (Scalars), else the
+// device schedule's; a loss-scaled launch takes the beta powers of the loss-scaling block, which advances them on
+// applied windows only.  An accumulate launch (kAccumulate) reads the schedule alone; from_zero: it is a first accumulate.
+template <int VARIANT, int MODE = kNoClip, bool EMA = false, typename KP>
+__device__ __forceinline__ void launch_begin(const KP& prm, LaunchStep<EMA>& st, LossScaleState* ls = nullptr,
+                                             const bool from_zero = false) {
+  st.lr = prm.sc.lr;
+  st.b1p = prm.sc.b1p;
+  st.b2p = prm.sc.b2p;
+  st.ok = 1;
+  if (prm.sched.state) sched_load(prm.sched, VARIANT != kAccumulate, from_zero, st);
+  if constexpr (VARIANT != kAccumulate) {
+    if constexpr (loss_scaled(MODE)) {
+      ls_load(prm.ls.state, *ls);
+      st.b1p = ls->beta1_power;
+      st.b2p = ls->beta2_power;
+    }
+    if constexpr (EMA) ema_load(prm.ema, st.ema);
+    st.dv = launch_divisor(prm);
+    if constexpr (VARIANT == 1) {
+      st.bc2 = __fsqrt_rn(__fsub_rn(1.0f, st.b2p));
+      st.bc1 = __fsub_rn(1.0f, st.b1p);
+    } else {
+      st.bc2 = 1.0f;   // no alpha: tile_rate<0> does not read them
+      st.bc1 = 1.0f;
+    }
+  }
+}
+// The one thread that commits a launch, once no CTA of it reads the state blocks any more: gaccum_stats (gn and s: the
+// global norm and the clip scale, 0 and 1 without clipping), the loss-scaling state, the average (applied windows only),
+// the window weight (applied and skipped windows alike) and the schedule's next step.  The schedule advances the beta
+// powers only where the launch took them from it: an optimizer that keeps them, on a launch that is not loss-scaled.
+template <int VARIANT, int MODE = kNoClip, bool EMA = false, typename KP>
+__device__ __forceinline__ void launch_commit(const KP& prm, const LaunchStep<EMA>& st, const LossScaleState* ls,
+                                              const bool skip, const float gn, const float s) {
+  constexpr bool apply = VARIANT != kAccumulate;
+  prm.stats[0] = apply ? 1.f : 0.f; prm.stats[1] = st.lr; prm.stats[2] = gn; prm.stats[3] = s;
+  if constexpr (loss_scaled(MODE)) ls_finish<keeps_beta_powers(VARIANT)>(prm.ls, *ls, skip, prm.sc.b1, prm.sc.b2);
+  if constexpr (EMA) { if (!skip) ema_finish(prm.ema, st.ema); }
+  if (apply && prm.ww.state) window_finish(prm.ww.state, st.dv.nf);
+  if (prm.sched.state) sched_finish(prm.sched, keeps_beta_powers(VARIANT) && !loss_scaled(MODE), prm.sc.b1, prm.sc.b2);
+}
+// Thread 0 of every CTA of a one-tile-per-CTA launch, after its tile: true in the CTA that commits.  `counted` (the launch
+// commits device state): the last CTA through, by a counter of finished CTAs -- every other CTA has read the state by
+// then -- which it resets for the next launch.  Otherwise block 0, and nothing is counted.
+__device__ __forceinline__ bool commits_launch(unsigned int* done, const bool counted) {
+  if (!counted) return blockIdx.x == 0;
+  __threadfence();
+  if (atomicAdd(done, 1u) != gridDim.x - 1u) return false;
+  *done = 0u;
+  return true;
+}
+
+// Device schedule: every CTA checks the step before its tile, and the last one through commits the launch.  Without one
+// the launch commits nothing but the stats, which no CTA reads: block 0 writes them before its tile, counting nothing.
 template <int CAP, bool FROM_ZERO, bool H = false>
 __global__ void __launch_bounds__(kThreads)
 accumulate_kernel(const __grid_constant__ KernelParams<CAP> prm) {
-  if (prm.sched.state) {
-    // device schedule: every CTA checks the step before its tile; the last one through advances it
-    __shared__ SchedLaunch s_sl;
-    if (threadIdx.x == 0) sched_load(prm.sched, false, s_sl, FROM_ZERO);
+  __shared__ LaunchStep<> s_step;
+  const bool sched = prm.sched.state != nullptr;   // launch-uniform
+  if (sched) {
+    if (threadIdx.x == 0) launch_begin<kAccumulate>(prm, s_step, nullptr, FROM_ZERO);
     __syncthreads();
-    if (!s_sl.ok) { sched_refuse(prm.sched); return; }
-    if ((int)blockIdx.x < prm.num_tiles) accumulate_tile<FROM_ZERO, H>(prm.tiles[blockIdx.x], prm);
-    if (threadIdx.x == 0) {
-      if (blockIdx.x == 0) { prm.stats[0] = 0.f; prm.stats[1] = s_sl.lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f; }
-      __threadfence();
-      if (atomicAdd(prm.sched.done, 1u) == gridDim.x - 1u) {
-        sched_finish(prm.sched, s_sl, false, 0.f, 0.f);
-        *prm.sched.done = 0u;
-      }
-    }
-    return;
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    prm.stats[0] = 0.f; prm.stats[1] = prm.sc.lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f;
+    if (!s_step.ok) { sched_refuse(prm.sched); return; }
+  } else if (blockIdx.x == 0 && threadIdx.x == 0) {
+    launch_begin<kAccumulate>(prm, s_step);
+    launch_commit<kAccumulate>(prm, s_step, nullptr, false, 0.f, 1.f);
   }
   if ((int)blockIdx.x < prm.num_tiles) accumulate_tile<FROM_ZERO, H>(prm.tiles[blockIdx.x], prm);
+  if (sched && threadIdx.x == 0 && commits_launch(prm.done, true)) launch_commit<kAccumulate>(prm, s_step, nullptr, false, 0.f, 1.f);
 }
 
 // gaccum_loss_scale_init: one thread writes the initial loss-scaling state (a kernel, so the call stays asynchronous and
@@ -790,8 +869,7 @@ __global__ void ema_init_kernel(EmaState* st, long long num_updates) {
 // H: p is the master slab (always 16-byte aligned); the model copy is stored after it.
 // EMA: the average e (slab `ema`, always 16-byte aligned) is read with p and stored after it: e - (e - p) * c.
 // dv: the launch's divisor (N, or the window weight W).
-// lr, bc2, bc1: the step's learning rate and GACCUM_ADAM's bias-correction terms (Scalars / LrMultParams, or the device
-// schedule's).
+// lr, bc2, bc1: the step's learning rate and GACCUM_ADAM's bias-correction terms (LaunchStep).
 // norms (launch-uniform, NormParams): the thread's fp32 partials of c^2 (c before any clip scale), p^2 (p before the
 // update) and (p - p')^2 go into `np_`.
 struct NormPart {
@@ -855,40 +933,23 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
             });
 }
 
-// EMA and window weight: every CTA reads n and W (thread 0, before its tile); the CTA that finishes last -- a counter of
-// finished CTAs, so every other CTA of the launch has read n and W by then -- writes n + 1 and d, last_weight = W and
-// W = +0, and resets the counter for the next launch.  One counter (EmaParams::done) serves both.
+// EMA, window weight and device schedule: every CTA reads the state before its tile (launch_begin); the CTA that
+// finishes last commits the launch (commits_launch).
 template <int VARIANT, int CAP, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads)
 apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
-  const EmaParams& ep = prm.ema;
-  WindowWeightState* const ww = prm.ww.state;
-  __shared__ Divisor s_dv;
-  EmaLaunch* s_ema = nullptr;
-  if constexpr (EMA) {
-    __shared__ EmaLaunch s_ema_launch;
-    s_ema = &s_ema_launch;
-  }
-  __shared__ SchedLaunch s_sl;
-  const bool sched = prm.sched.state != nullptr;   // launch-uniform
-  const bool counted = EMA || ww != nullptr || sched;
-  if (counted) {
-    if (threadIdx.x == 0) {
-      if constexpr (EMA) ema_load(ep, *s_ema);
-      s_dv = launch_divisor(prm);
-      if (sched) sched_load(prm.sched, true, s_sl);
-    }
-    __syncthreads();
-    if (sched && !s_sl.ok) { sched_refuse(prm.sched); return; }
-  }
-  const Divisor dv = ww ? s_dv : Divisor{prm.sc.nf, prm.sc.inv_nf};
-  const float lr = sched ? s_sl.lr : prm.sc.lr;
-  const float bc2 = sched ? s_sl.bc2 : prm.lrm.bc2, bc1 = sched ? s_sl.bc1 : prm.lrm.bc1;
+  __shared__ LaunchStep<EMA> s_step;
+  const bool counted = EMA || prm.ww.state != nullptr || prm.sched.state != nullptr;   // launch-uniform
+  if (threadIdx.x == 0) launch_begin<VARIANT, kNoClip, EMA>(prm, s_step);
+  __syncthreads();
+  if (!s_step.ok) { sched_refuse(prm.sched); return; }
+  const Divisor dv = s_step.dv;
+  const float lr = s_step.lr, bc2 = s_step.bc2, bc1 = s_step.bc1;
   const bool norms = prm.norms.out != nullptr;     // launch-uniform
   if ((int)blockIdx.x < prm.num_tiles) {
     const TileDesc d = prm.tiles[blockIdx.x];
     NormPart part;
-    if constexpr (EMA) update_tile<VARIANT, H, CAP, true>(d, prm, dv, lr, bc2, bc1, norms, part, ep.slab, s_ema->c);
+    if constexpr (EMA) update_tile<VARIANT, H, CAP, true>(d, prm, dv, lr, bc2, bc1, norms, part, prm.ema.slab, s_step.ema.c);
     else update_tile<VARIANT, H>(d, prm, dv, lr, bc2, bc1, norms, part);
     if (norms) {
       const int warp = (int)threadIdx.x >> 5;
@@ -898,18 +959,7 @@ apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
       norm_arrive_tile(prm.norms, d, (int)blockIdx.x);
     }
   }
-  if (counted && threadIdx.x == 0) {
-    __threadfence();
-    if (atomicAdd(ep.done, 1u) == gridDim.x - 1u) {
-      if constexpr (EMA) ema_finish(ep, *s_ema);
-      if (ww) window_finish(ww, s_dv.nf);
-      if (sched) sched_finish(prm.sched, s_sl, VARIANT == 1, prm.sc.b1, prm.sc.b2);
-      *ep.done = 0u;
-    }
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    prm.stats[0] = 1.f; prm.stats[1] = lr; prm.stats[2] = 0.f; prm.stats[3] = 1.f;
-  }
+  if (threadIdx.x == 0 && commits_launch(prm.done, counted)) launch_commit<VARIANT, kNoClip, EMA>(prm, s_step, nullptr, false, 0.f, 1.f);
 }
 
 // =============================================================================================
@@ -1144,14 +1194,6 @@ __device__ __forceinline__ void grid_barrier(unsigned long long* barrier) {
   const unsigned long long target = (old / gridDim.x + 1ull) * gridDim.x;
   while (ld_acquire_gpu_u64(barrier) < target) { __nanosleep(20); }
 }
-// loss scaling: the state as this launch finds it (thread 0, before its CTA arrives at the first grid barrier)
-__device__ __forceinline__ void ls_load(const LossScaleState* st, LossScaleState& s) {
-  s.scale = __ldcg(&st->scale);
-  s.good_windows = __ldcg(&st->good_windows);
-  s.skipped_windows = __ldcg(&st->skipped_windows);
-  s.beta1_power = __ldcg(&st->beta1_power);
-  s.beta2_power = __ldcg(&st->beta2_power);
-}
 // thread 0 after the barrier, from the launch-wide counters (`bins`: their accumulator, copied where the thread reads
 // it): the clip scale s and the global norm gn (1 and 0 without clipping) and, loss-scaled, whether the window is
 // skipped -- an element of a' or, with clipping, gn is not finite.  Every CTA computes the same values.
@@ -1169,35 +1211,6 @@ __device__ __forceinline__ void window_decision(const LaunchCounters* ctr, const
     s = clip_scale(g_norm, clip);
     gn = g_norm;
     if constexpr (loss_scaled(MODE)) skip = (nonfinite & kElemNonfinite) != 0 || !(fabsf(g_norm) <= 3.402823466e38f);
-  }
-}
-// block 0's thread 0 at the very end of a loss-scaled launch: TF 2 DynamicLossScale, counted in windows (gaccum.h,
-// gaccum_loss_scale_config); BETAS: the optimizer keeps TF1's beta powers, advanced on applied windows only
-template <bool BETAS>
-__device__ __forceinline__ void ls_finish(const LossScaleParams& ls, const LossScaleState& s_ls, const bool skip,
-                                          const float b1, const float b2) {
-  LossScaleState* out = ls.state;
-  const float S = s_ls.scale;
-  if (skip) {
-    const float down = __fdiv_rn(S, ls.multiplier);   // exact: both are powers of two
-    out->scale = down < 1.0f ? 1.0f : down;
-    out->good_windows = 0;
-    out->skipped_windows = s_ls.skipped_windows + 1u;
-    out->last_skipped = 1;
-  } else {
-    const int32_t good = s_ls.good_windows + 1;
-    if (good >= ls.growth_interval) {
-      const float up = __fmul_rn(S, ls.multiplier);
-      if (fabsf(up) <= 3.402823466e38f) out->scale = up;
-      out->good_windows = 0;
-    } else {
-      out->good_windows = good;
-    }
-    out->last_skipped = 0;
-    if constexpr (BETAS) {                            // TF1 AdamOptimizer._finish, applied windows only
-      out->beta1_power = __fmul_rn(s_ls.beta1_power, b1);
-      out->beta2_power = __fmul_rn(s_ls.beta2_power, b2);
-    }
   }
 }
 
@@ -1337,27 +1350,24 @@ __device__ __forceinline__ void norm_tile2(const TileDesc& d, const uint32_t nve
 
 // Dynamic shared memory of apply_clip_kernel (kClipSmemBytes): 3 groups x kRingVecs float4 of ring, then
 // 3 groups x kStashVecs float4 of stash.
-// Registers: 864 threads in one CTA cap the kernel at 72 per thread.  The AdamWeightDecay instantiations (VARIANT 0)
-// fit without spilling; the plain-Adam ones with clipping (VARIANT 1, used only when tf_adam is combined with
-// clip_norm > 0) spill 8-20 bytes per thread to local memory (ptxas -v).  What that costs has not been measured.
+// Registers: 864 threads in one CTA cap the kernel at 72 per thread.  ptxas -v (CUDA 12.9): only the AdamWeightDecay
+// kClip instantiations without an EMA fit without spilling.  Every other one spills: AdamWeightDecay 4-24 bytes of
+// stores per thread loss-scaled, 44-64 with an EMA; plain Adam (VARIANT 1) 4-44 without an EMA, 52-72 with one.  What
+// that costs has not been measured.
 //
-// Loss scaling (kLsClip, kLsNoClip; gaccum_plan_set_loss_scale).  Thread 0 of every CTA reads S, the counters and the beta
-// powers from prm.ls.state during set-up, i.e. before its CTA arrives at the grid barrier; pass 1 ORs kElemNonfinite
-// into the launch's counters when an element of a' is not finite.  After the barrier every CTA takes the same decision
-// from the same launch-wide flags: skip iff an element was non-finite or, with clipping, gn is.  A skipped window
-// stores a = 0 and leaves p, m and v alone.  Block 0's thread 0 writes the new state at the very end -- after the
-// barrier, so no CTA can see the new S or beta powers in this launch.
+// Device state (loss scaling, EMA, window weight, device schedule): thread 0 of every CTA reads it during set-up
+// (launch_begin), before its CTA arrives at the grid barrier; block 0's thread 0 commits the launch at the very end
+// (launch_commit) -- after the barrier, so no CTA can see a new value in this launch.
+//
+// Loss scaling (kLsClip, kLsNoClip; gaccum_plan_set_loss_scale): pass 1 ORs kElemNonfinite into the launch's counters
+// when an element of a' is not finite.  After the barrier every CTA takes the same decision from the same launch-wide
+// flags: skip iff an element was non-finite or, with clipping, gn is.  A skipped window stores a = 0 and leaves p, m and
+// v alone.
 //
 // 16-bit models (H): pass 1 moves the 16-bit G tile into the G half of the [G | a] slot (bulk_vecs), pass 2 moves the
 // master weights, and every store of p is followed by the model copy.  Ring and stash are the same.
 //
-// EMA: ClipLayout<true> -- pass 2's producer moves e by bulk copy as the fifth stream of the slot.  Thread 0 of every
-// CTA reads n during set-up, before its CTA arrives at the grid barrier; block 0's thread 0 writes n + 1 and d at the
-// very end, on an applied window only, as it writes the loss-scaling state.
-//
-// Window weight (gaccum_plan_set_window_weight): thread 0 of every CTA reads W during set-up into s_dv (N on other
-// plans), which both passes' consumers read tile by tile; block 0's thread 0 writes last_weight = W and W = +0 at the
-// very end, on applied and skipped windows alike.
+// EMA: ClipLayout<true> -- pass 2's producer moves e by bulk copy as the fifth stream of the slot.
 template <int VARIANT, int CAP, int MODE, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kClipThreads, 1)
 apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
@@ -1365,19 +1375,12 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   constexpr int kRingVecs = L::kRingVecs, kP2SlotVecs = L::kP2SlotVecs, kP2Slots = L::kP2Slots, kRingBytes = L::kRingBytes;
   constexpr int kStashTiles = L::kStashTiles, kStashVecs = L::kStashVecs;
   const EmaParams* const ema = &prm.ema;   // read through a pointer: without it nvcc adds instructions to one EMA instantiation
-  EmaLaunch* s_ema = nullptr;            // EMA: n, d and c as this launch found them
-  if constexpr (EMA) {
-    __shared__ EmaLaunch s_ema_launch;
-    s_ema = &s_ema_launch;
-  }
   extern __shared__ __align__(128) unsigned char smem_dyn[];
   __shared__ unsigned long long s_bins[kConsumerThreads / 32][kAccBins];   // one exact accumulator per consumer warp (13 KB)
   __shared__ unsigned int s_nonfinite;
   __shared__ float s_bcast[2];
+  __shared__ LaunchStep<EMA> s_step;
   __shared__ LossScaleState s_ls;        // loss-scaled: the state as this launch found it
-  __shared__ float s_bc[2];              // loss-scaled GACCUM_ADAM: bc2, bc1 (LrMultParams) from the device's beta powers
-  __shared__ Divisor s_dv;               // the launch's divisor: N, or W as this launch found it
-  __shared__ SchedLaunch s_sl;           // device schedule: the step as this launch found it
   __shared__ int s_skip;
   __shared__ uint32_t s_set;
   __shared__ __align__(8) uint64_t s_full1[kGroups][kP1Slots], s_empty1[kGroups][kP1Slots];
@@ -1426,22 +1429,12 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    if constexpr (loss_scaled(MODE)) {
-      ls_load(prm.ls.state, s_ls);
-      if constexpr (VARIANT == 1) {
-        // make_scalars' terms: alpha_t = (lr_t * sqrt(1 - b2^t)) / (1 - b1^t), one rounding per op (tile_rate)
-        s_bc[0] = __fsqrt_rn(__fsub_rn(1.0f, s_ls.beta2_power));
-        s_bc[1] = __fsub_rn(1.0f, s_ls.beta1_power);
-      }
-    }
-    if constexpr (EMA) ema_load(*ema, *s_ema);
-    s_dv = launch_divisor(prm);
-    if (prm.sched.state) sched_load(prm.sched, true, s_sl);
+    launch_begin<VARIANT, MODE, EMA>(prm, s_step, &s_ls);
   }
   for (int i = threadIdx.x; i < (kConsumerThreads / 32) * kAccBins; i += kClipThreads) (&s_bins[0][0])[i] = 0ull;
   __syncthreads();
   // device schedule: every CTA read the same step, so all of them leave here or none does (before any barrier)
-  if (prm.sched.state && !s_sl.ok) { sched_refuse(prm.sched); return; }
+  if (!s_step.ok) { sched_refuse(prm.sched); return; }
   LaunchCounters* const ctr = prm.counters + s_set;
   clear_other_counters(prm.counters, s_set);
 
@@ -1551,11 +1544,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
       RingPos rp;
       int jb = 0;
       bool past_barrier = false;
-      // the bias corrections of the tiles' alpha_t (GACCUM_ADAM): the step's, or under loss scaling the device block's,
-      // which thread 0 wrote before the set-up barrier
-      float bc2 = prm.lrm.bc2, bc1 = prm.lrm.bc1, lr = prm.sc.lr;
-      if (prm.sched.state) { lr = s_sl.lr; bc2 = s_sl.bc2; bc1 = s_sl.bc1; }    // the device schedule's step
-      if constexpr (loss_scaled(MODE) && VARIANT == 1) { bc2 = s_bc[0]; bc1 = s_bc[1]; }
+      const float lr = s_step.lr, bc2 = s_step.bc2, bc1 = s_step.bc1;
       const unsigned long long pool_n = (unsigned long long)max(0, nt - pool_lo);
       while (true) {
         int tile;
@@ -1647,7 +1636,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         float4* const st = park ? stash + (size_t)n_seen * (kTile / 4) : nullptr;
         bool bad = false;
         const float part = norm_tile<MODE, H>(meta.d, prm, ring + (size_t)rp.slot * kP1SlotVecs, &s_empty1[grp][rp.slot], st,
-                                                pol_last, inv_s, bad, s_dv, norms);
+                                                pol_last, inv_s, bad, s_step.dv, norms);
         if constexpr (loss_scaled(MODE)) { if (bad) my_nonfinite |= kElemNonfinite; }
         if (MODE != kLsNoClip || norms) {
           // warp total in fp64, fixed butterfly order; lane 0 adds it EXACTLY into its warp's accumulator and, with
@@ -1708,10 +1697,10 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         const float4* const st = meta.stash_slot != kNoStash ? stash + (size_t)meta.stash_slot * (kTile / 4) : nullptr;
         if constexpr (EMA) {
           update_tile2<VARIANT, MODE, H, CAP, true>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot],
-                                                    st, meta.rate, inv_s, skip, s_dv, norms, ema->slab, s_ema->c);
+                                                    st, meta.rate, inv_s, skip, s_step.dv, norms, ema->slab, s_step.ema.c);
         } else {
           update_tile2<VARIANT, MODE, H>(meta.d, prm, s, ring + (size_t)rp.slot * kP2SlotVecs, &s_empty2[grp][rp.slot], st, meta.rate,
-                                      inv_s, skip, s_dv, norms);
+                                      inv_s, skip, s_step.dv, norms);
         }
         if (norms) {
           float nw = 0.f, nu = 0.f;
@@ -1723,14 +1712,7 @@ apply_clip_kernel(const __grid_constant__ KernelParams<CAP> prm) {
         rp.advance(kP2Slots);
       }
     }
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-      prm.stats[0] = 1.f; prm.stats[1] = prm.sched.state ? s_sl.lr : prm.sc.lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s;
-      if constexpr (loss_scaled(MODE)) ls_finish<VARIANT == 1>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
-      if constexpr (EMA) { if (!skip) ema_finish(*ema, *s_ema); }
-      if (prm.ww.state) window_finish(prm.ww.state, s_dv.nf);
-      // loss-scaled: the beta powers live in the loss-scaling block, which ls_finish advanced
-      if (prm.sched.state) sched_finish(prm.sched, s_sl, !loss_scaled(MODE) && VARIANT == 1, prm.sc.b1, prm.sc.b2);
-    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) launch_commit<VARIANT, MODE, EMA>(prm, s_step, &s_ls, skip, s_bcast[1], s);
     if (norms) {
       // every tile's partials are stored once all consumers are through pass 2: a second grid barrier, then every
       // consumer warp of the grid sums chunks

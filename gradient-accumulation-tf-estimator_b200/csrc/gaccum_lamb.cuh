@@ -200,9 +200,8 @@ __device__ __forceinline__ void lamb_write_tile(const TileDesc& d, const KernelP
             });
 }
 
-// EMA: thread 0 of every CTA reads n during set-up; block 0's thread 0 writes n + 1 and d at the very end, past the
-// grid barriers, on an applied window only.  Window weight: thread 0 of every CTA reads W during set-up (s_dv); block
-// 0's thread 0 writes last_weight = W and W = +0 at the very end, on applied and skipped windows alike.
+// Device state (loss scaling, EMA, window weight, device schedule): thread 0 of every CTA reads it during set-up
+// (launch_begin); block 0's thread 0 commits the launch at the very end, past the grid barriers (launch_commit).
 template <int CAP, int MODE, bool H = false, bool EMA = false>
 __global__ void __launch_bounds__(kThreads, kLambBlocksPerSm)
 lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
@@ -211,17 +210,11 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   const unsigned long long kBarriers = (kPhase1 ? 3 : 2) + (norms ? 1 : 0);
   constexpr int kWarps = kThreads / 32;
   const LambParams& lb = prm.lamb;
-  EmaLaunch* s_ema = nullptr;            // EMA: n, d and c as this launch found them
-  if constexpr (EMA) {
-    __shared__ EmaLaunch s_ema_launch;
-    s_ema = &s_ema_launch;
-  }
   __shared__ unsigned long long s_bins[kWarps][2][kAccBins];   // one pair of exact accumulators per warp (8.5 KB)
   __shared__ unsigned int s_nonfinite[2];
-  __shared__ LossScaleState s_ls;
   __shared__ float s_bcast[2];
-  __shared__ Divisor s_dv;               // the launch's divisor: N, or W as this launch found it
-  __shared__ SchedLaunch s_sl;           // device schedule: the step as this launch found it
+  __shared__ LaunchStep<EMA> s_step;
+  __shared__ LossScaleState s_ls;        // loss-scaled: the state as this launch found it
   __shared__ int s_skip;
   __shared__ uint32_t s_set;
 
@@ -238,18 +231,15 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     s_bcast[0] = 1.f;
     s_bcast[1] = 0.f;
     s_skip = 0;
-    if constexpr (loss_scaled(MODE)) ls_load(prm.ls.state, s_ls);
-    if constexpr (EMA) ema_load(prm.ema, *s_ema);
-    s_dv = launch_divisor(prm);
-    if (prm.sched.state) sched_load(prm.sched, true, s_sl);
+    launch_begin<kLamb, MODE, EMA>(prm, s_step, &s_ls);
   }
   for (int i = threadIdx.x; i < kWarps * 2 * kAccBins; i += kThreads) (&s_bins[0][0][0])[i] = 0ull;
   __syncthreads();
   // device schedule: every CTA read the same step, so all of them leave here or none does (before any barrier)
-  if (prm.sched.state && !s_sl.ok) { sched_refuse(prm.sched); return; }
+  if (!s_step.ok) { sched_refuse(prm.sched); return; }
   const uint32_t set = s_set;
   // the launch's divisor, held in registers: read from shared memory at every use it slowed the unweighted apply 1.6-2.2 %
-  const Divisor dv = s_dv;
+  const Divisor dv = s_step.dv;
   LaunchCounters* const ctr = prm.counters + set;
   LambTensorAcc* const tacc = lb.acc + (size_t)set * lb.num_tensors;
   clear_other_counters(prm.counters, set);
@@ -258,15 +248,11 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     const size_t words = (size_t)lb.num_tensors * (sizeof(LambTensorAcc) / 8);
     for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < words; i += (size_t)gridDim.x * kThreads) other[i] = 0ull;
   }
+  // the step's lr and beta powers, held in registers from set-up on: read from shared memory where phases 2 and 3 use
+  // them, the 16-bit kLsNoClip instantiations spill more
+  const float lr = s_step.lr, b1p = s_step.b1p, b2p = s_step.b2p;
   float inv_s = 1.0f;
-  float b1p = lb.beta1_power, b2p = lb.beta2_power;
-  const float lr = prm.sched.state ? s_sl.lr : prm.sc.lr;
-  if (prm.sched.state) { b1p = s_sl.b1p; b2p = s_sl.b2p; }
-  if constexpr (loss_scaled(MODE)) {
-    inv_s = __fdiv_rn(1.0f, s_ls.scale);   // exact: S is a power of two
-    b1p = s_ls.beta1_power;
-    b2p = s_ls.beta2_power;
-  }
+  if constexpr (loss_scaled(MODE)) inv_s = __fdiv_rn(1.0f, s_ls.scale);   // exact: S is a power of two
 
   // ---- phase 1: a' and the global norm ----
   if constexpr (kPhase1) {
@@ -386,7 +372,7 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     const float rlr = skip ? 0.f : __fmul_rn(__ldcg(&lb.ratios[d.tensor_flags & 0x7fffffffu]),
                                              tile_rate<0>(lr, tensor_mult(prm.lrm, d), 0.f, 1.f));
     float nw = 0.f, nu = 0.f;
-    if constexpr (EMA) lamb_write_tile<H, CAP, true>(d, prm, rlr, !skip, norms, nw, nu, prm.ema.slab, s_ema->c);
+    if constexpr (EMA) lamb_write_tile<H, CAP, true>(d, prm, rlr, !skip, norms, nw, nu, prm.ema.slab, s_step.ema.c);
     else lamb_write_tile<H>(d, prm, rlr, !skip, norms, nw, nu);
     if (norms) {
       norm_store(prm.norms, t, 1, warp, nw);
@@ -394,14 +380,7 @@ lamb_apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
     }
   }
 
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    prm.stats[0] = 1.f; prm.stats[1] = lr; prm.stats[2] = s_bcast[1]; prm.stats[3] = s_bcast[0];
-    if constexpr (loss_scaled(MODE)) ls_finish<true>(prm.ls, s_ls, skip, prm.sc.b1, prm.sc.b2);
-    if constexpr (EMA) { if (!skip) ema_finish(prm.ema, *s_ema); }
-    if (prm.ww.state) window_finish(prm.ww.state, s_dv.nf);
-    // loss-scaled: the beta powers live in the loss-scaling block, which ls_finish advanced
-    if (prm.sched.state) sched_finish(prm.sched, s_sl, !loss_scaled(MODE), prm.sc.b1, prm.sc.b2);
-  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) launch_commit<kLamb, MODE, EMA>(prm, s_step, &s_ls, skip, s_bcast[1], s_bcast[0]);
   if (norms) {
     // every tile's partials are stored once every CTA is through phase 3: one more grid barrier, then every warp of
     // the grid sums chunks
