@@ -116,19 +116,20 @@ static int build_layout(gaccum_plan* pl) {
     const int64_t n = pl->numel[t];
     if (n < 0) return fail(GACCUM_EINVAL, "numels[%d] = %lld is negative", t, (long long)n);
     if (n >= (int64_t)1 << 32) return fail(GACCUM_EINVAL, "tensor %d has %lld elements; limit is 2^32-1", t, (long long)n);
+    // the padded slab ends at or before 2^37, so every tile's slab offset / kSlabAlign fits TileDesc::soff32
+    const int64_t padded_n = (n + kSlabAlign - 1) / kSlabAlign * kSlabAlign;
+    if (off + padded_n > (int64_t)1 << 37) return fail(GACCUM_EINVAL, "slab too large (> 2^37 elements)");
     pl->offset[t] = off;
     for (int64_t to = 0; to < n; to += kTile) {
       TileDesc d;
       d.tensor_flags = (uint32_t)t | (pl->decay[t] ? 0x80000000u : 0u);
       d.len = (uint32_t)std::min<int64_t>(kTile, n - to);
       d.toff = (uint32_t)to;
-      const int64_t s32 = (off + to) / kSlabAlign;
-      if (s32 >= (int64_t)1 << 32) return fail(GACCUM_EINVAL, "slab too large (> 2^37 elements)");
-      d.soff32 = (uint32_t)s32;
+      d.soff32 = (uint32_t)((off + to) / kSlabAlign);
       pl->tiles.push_back(d);
     }
     P += n;
-    off += (n + kSlabAlign - 1) / kSlabAlign * kSlabAlign;
+    off += padded_n;
   }
   if (pl->tiles.size() >= (size_t)1 << 31) return fail(GACCUM_EINVAL, "too many tiles");
   pl->P = P;
@@ -898,9 +899,10 @@ static void shard_bounds(const gaccum_plan* pl, int world, int* bounds /* world 
   }
   while (r <= world) bounds[r++] = nt;
 }
-// slab offset (in units of 32 elements) at which tile t starts; t == num_tiles -> end of the slab
-static uint32_t tile_soff32(const gaccum_plan* pl, int t) {
-  return t < (int)pl->tiles.size() ? pl->tiles[t].soff32 : (uint32_t)(pl->padded / kSlabAlign);
+// slab offset (in units of 32 elements) at which tile t starts; t == num_tiles -> end of the slab, which is 2^32 for a
+// slab of exactly 2^37 elements: int64, not TileDesc's uint32
+static int64_t tile_soff32(const gaccum_plan* pl, int t) {
+  return t < (int)pl->tiles.size() ? (int64_t)pl->tiles[t].soff32 : pl->padded / kSlabAlign;
 }
 // elements of one source region of a staging area = the widest shard's slab span
 static int64_t stage_span(const gaccum_plan* pl, int world) {
@@ -951,7 +953,8 @@ static int do_apply_dp(gaccum_plan* pl, const gaccum_dp_comm* comm, const float*
   prm->num_tiles = (int32_t)pl->tiles.size();
   int bounds[GACCUM_MAX_RANKS + 1];
   shard_bounds(pl, W, bounds);
-  for (int r = 0; r <= W; ++r) { prm->bounds[r] = bounds[r]; prm->shard_base32[r] = tile_soff32(pl, bounds[r]); }
+  // the kernel reads the base of a rank that owns tiles only: a tile start, which fits 32 bits
+  for (int r = 0; r <= W; ++r) { prm->bounds[r] = bounds[r]; prm->shard_base32[r] = (uint32_t)tile_soff32(pl, bounds[r]); }
   prm->stage_span = stage_span(pl, W);
   prm->accum = comm->accum;
   prm->m = m;

@@ -199,7 +199,11 @@ GACCUM_API int gaccum_decay_mask(int32_t num_tensors, const char* const* names,
 /* ---- plan ----------------------------------------------------------------------------- */
 /* Describes the T trainable tensors (tf.trainable_variables() order, optimization.py:70) and
  * lays out the packed fp32 slabs that replace the per-variable `accum_grads` (optimization.py:78)
- * and `adam_m` / `adam_v` (optimization.py:137-148).  device = -1: layout-only plan. */
+ * and `adam_m` / `adam_v` (optimization.py:137-148).  device = -1: layout-only plan.
+ * Limits of the layout, each refused with GACCUM_EINVAL: a tensor holds at most 2^32 - 1 elements (a tile's offset
+ * inside its tensor is 32-bit); the padded slab (gaccum_padded_size) holds at most 2^37 elements, 512 GB in fp32 (a
+ * tile's slab offset is 32-bit in units of 32 elements); a plan has fewer than 2^31 tiles.  Element counts, offsets and
+ * byte counts are int64 everywhere, and every kernel forms its addresses in 64 bits. */
 GACCUM_API int gaccum_plan_create(gaccum_plan** out, int32_t num_tensors, const int64_t* numels,
                                   const uint8_t* decay, const gaccum_hparams* hp, int32_t device);
 GACCUM_API int gaccum_plan_destroy(gaccum_plan* plan);
