@@ -187,6 +187,7 @@ def _load():
         "gaccum_plan_set_device_schedule": (C.c_int, [vp, C.POINTER(ScheduleConfig), vp]),
         "gaccum_schedule_init": (C.c_int, [vp, vp, i64, C.c_float, C.c_float, vp]),
         "gaccum_plan_set_tensor_norms": (C.c_int, [vp, vp]),
+        "gaccum_plan_set_lr_table": (C.c_int, [vp, vp, i64]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -406,6 +407,12 @@ class Plan:
                       stream: int = 0) -> None:
         _check(_load().gaccum_schedule_init(self._h, block or None, int(global_step), float(beta1_power),
                                             float(beta2_power), stream))
+
+    def set_lr_table(self, ptr: int, length: int) -> None:
+        """Take every launch's learning rate from ``length`` fp32 values of device memory at ``ptr`` (4-byte aligned):
+        lr = table[min(global_step, length - 1)] in place of the device schedule's formula (before the first compute
+        call; the plan must be device-scheduled by then).  The table is read at launch time."""
+        _check(_load().gaccum_plan_set_lr_table(self._h, ptr or None, int(length)))
 
     def set_tensor_norms(self, device_out: int) -> None:
         """Write per-tensor gradient, weight and update norms on every apply (before the first compute call):

@@ -100,6 +100,8 @@ struct gaccum_plan {
   // the device schedule (gaccum_plan_set_device_schedule); set only while `computed` is false
   gaccum_schedule_config sched_cfg{};
   gaccum_schedule_state* sched_state = nullptr;
+  // a learning-rate table of the device schedule (gaccum_plan_set_lr_table); set only while `computed` is false
+  LrTableParams lr_table{};
   // per-tensor norms of the apply step (gaccum_plan_set_tensor_norms); set only while `computed` is false.  d_norms holds
   // the partials, the chunk tables and the counters of NormParams in one allocation
   NormParams norms{};
@@ -250,6 +252,9 @@ static int check_compute(gaccum_plan* pl, const float* accum, const float* m, co
   pl->computed = true;   // from here on gaccum_plan_set_loss_scale is refused
   if (pl->device < 0)
     return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): libgaccum has no CPU fallback, a CUDA device is required");
+  if (pl->lr_table.table && !pl->sched_state)
+    return fail(GACCUM_EINVAL, "a learning-rate table (gaccum_plan_set_lr_table) needs a device schedule "
+                               "(gaccum_plan_set_device_schedule), which this plan lacks");
   if (!accum || !aligned16_host(accum)) return fail(GACCUM_EINVAL, "accum must be a 16-byte aligned device pointer");
   if (need_mv && (!m || !v || !aligned16_host(m) || !aligned16_host(v)))
     return fail(GACCUM_EINVAL, "m and v must be 16-byte aligned device pointers");
@@ -292,6 +297,7 @@ static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, f
   prm.sched.state = reinterpret_cast<ScheduleState*>(pl->sched_state);
   prm.sched.accum_n = a ? a->accum_n : 1;
   prm.norms = pl->norms;
+  prm.lrt = pl->lr_table;
 }
 
 template <int CAP>
@@ -372,8 +378,9 @@ enum PlanSetting : unsigned {
   kPlanLrMult = 1u << 4,
   kPlanWindowWeight = 1u << 5,
   kPlanSchedule = 1u << 6,
-  kPlanNorms = 1u << 7,
-  kPlanAll = (1u << 8) - 1u,
+  kPlanLrTable = 1u << 7,
+  kPlanNorms = 1u << 8,
+  kPlanAll = (1u << 9) - 1u,
 };
 // Fails on the first of the settings `lacks` names that the plan has: `what` does not support it
 static int refuse(const gaccum_plan* pl, const unsigned lacks, const char* what) {
@@ -386,6 +393,7 @@ static int refuse(const gaccum_plan* pl, const unsigned lacks, const char* what)
       {kPlanLrMult, pl->lr_mult_set, "learning-rate multipliers (gaccum_plan_set_lr_multipliers)"},
       {kPlanWindowWeight, pl->ww_state != nullptr, "a window weight (gaccum_plan_set_window_weight)"},
       {kPlanSchedule, pl->sched_state != nullptr, "a device schedule (gaccum_plan_set_device_schedule)"},
+      {kPlanLrTable, pl->lr_table.table != nullptr, "a learning-rate table (gaccum_plan_set_lr_table)"},
       {kPlanNorms, pl->norms.out != nullptr, "per-tensor norms (gaccum_plan_set_tensor_norms)"},
   };
   for (const auto& st : settings)
@@ -758,6 +766,18 @@ int gaccum_schedule_init(gaccum_plan* pl, gaccum_schedule_state* block, int64_t 
   return GACCUM_OK;
 }
 
+int gaccum_plan_set_lr_table(gaccum_plan* pl, const float* device_table, int64_t length) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (!device_table) return fail(GACCUM_EINVAL, "device_table is NULL");
+  if (length < 1) return fail(GACCUM_EINVAL, "length must be >= 1 (got %lld)", (long long)length);
+  if (((uintptr_t)device_table & 3u) != 0) return fail(GACCUM_EINVAL, "device_table must be a 4-byte aligned device pointer");
+  if (pl->device < 0) return fail(GACCUM_EINVAL, "layout-only plan (device=-1): a learning-rate table needs a device plan");
+  if (pl->computed) return fail(GACCUM_EINVAL, "the learning-rate table can only be set before the plan's first compute call");
+  pl->lr_table.table = device_table;
+  pl->lr_table.length = length;
+  return GACCUM_OK;
+}
+
 int gaccum_plan_set_tensor_norms(gaccum_plan* pl, float* device_out) {
   if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
   if (!device_out || !aligned16_host(device_out)) return fail(GACCUM_EINVAL, "device_out must be a 16-byte aligned device pointer");
@@ -824,7 +844,7 @@ static int accumulate_impl(gaccum_plan* pl, const float* const* grads, float* ac
 int gaccum_accumulate(gaccum_plan* pl, const float* const* grads, float* accum, gaccum_stream_t stream) {
   // without step arguments the launch cannot check global_step against its branch: a device-scheduled plan steps with
   // gaccum_step
-  if (int rc = refuse(pl, kPlanSchedule, "gaccum_accumulate")) return rc;
+  if (int rc = refuse(pl, kPlanSchedule | kPlanLrTable, "gaccum_accumulate")) return rc;
   return accumulate_impl(pl, grads, accum, nullptr, stream);
 }
 
@@ -833,7 +853,7 @@ static int apply_impl(gaccum_plan* pl, const float* const* grads, float* const* 
 
 int gaccum_apply(gaccum_plan* pl, const float* const* grads, float* const* params, float* accum,
                  float* m, float* v, const gaccum_step_args* a, gaccum_stream_t stream) {
-  if (int rc = refuse(pl, kPlanSchedule, "gaccum_apply")) return rc;
+  if (int rc = refuse(pl, kPlanSchedule | kPlanLrTable, "gaccum_apply")) return rc;
   return apply_impl(pl, grads, params, accum, m, v, a, stream);
 }
 

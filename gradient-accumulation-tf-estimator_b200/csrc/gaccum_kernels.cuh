@@ -202,6 +202,13 @@ struct NormParams {
   int32_t num_chunks;
 };
 
+// A learning-rate table of a device-scheduled plan (gaccum_plan_set_lr_table): caller-owned device memory, read at
+// launch time.  table == NULL: schedule_lr.  A launch-uniform branch in sched_load, not a template flag.
+struct LrTableParams {
+  const float* table;
+  int64_t length;          // >= 1
+};
+
 // Every kernel's parameter block.  Each feature's parameters follow those of the features before it, so adding them
 // moved no member an existing kernel reads.
 template <int CAP>
@@ -228,6 +235,7 @@ struct KernelParams {
   WindowWeightParams ww;  // apply kernels only
   ScheduleParams sched;   // every kernel
   NormParams norms;       // apply kernels only
+  LrTableParams lrt;      // device-scheduled launches only
 };
 static_assert(sizeof(KernelParams<1920>) <= 32764, "kernel parameters must fit the 32 KB limit");
 
@@ -249,15 +257,20 @@ __device__ __forceinline__ float schedule_lr(const float init_lr, const long lon
   }
   return lr;
 }
-// The learning rate of a device-scheduled launch (a LaunchStep) at the block's step g, the beta powers as the block
-// holds them, and whether the launch may run: g selects its branch (apply), no earlier launch was refused, and a first
-// accumulate (from_zero), which does not read the accumulators, follows a step that applied and left them at +0
-// ((int32)(g - 1) % N == 0) -- else it would overwrite that step's gradients
+// The learning rate of a device-scheduled launch (a LaunchStep) at the block's step g -- table[min(g, length - 1)] with
+// a learning-rate table (g >= 0: gaccum_schedule_init keeps it so; a 64-bit index, untouched by the int32 wrap), else
+// schedule_lr -- the beta powers as the block holds them, and whether the launch may run: g selects its branch (apply),
+// no earlier launch was refused, and a first accumulate (from_zero), which does not read the accumulators, follows a
+// step that applied and left them at +0 ((int32)(g - 1) % N == 0) -- else it would overwrite that step's gradients
 template <typename Step>
-__device__ __forceinline__ void sched_load(const ScheduleParams& sp, const bool apply, const bool from_zero, Step& sl) {
+__device__ __forceinline__ void sched_load(const ScheduleParams& sp, const LrTableParams& lt, const bool apply,
+                                           const bool from_zero, Step& sl) {
   const ScheduleState* st = sp.state;
   const long long g = __ldcg(&st->global_step);
-  sl.lr = schedule_lr(__ldcg(&st->init_lr), __ldcg(&st->num_train_steps), __ldcg(&st->num_warmup_steps), g);
+  if (lt.table)                                    // launch-uniform
+    sl.lr = __ldcg(&lt.table[g < lt.length ? g : lt.length - 1]);
+  else
+    sl.lr = schedule_lr(__ldcg(&st->init_lr), __ldcg(&st->num_train_steps), __ldcg(&st->num_warmup_steps), g);
   sl.b1p = __ldcg(&st->beta1_power);
   sl.b2p = __ldcg(&st->beta2_power);
   sl.ok = __ldcg(&st->refused) == 0 && ((((int)g % sp.accum_n) == 0) == apply)    // gaccum_is_apply_step
@@ -784,7 +797,7 @@ __device__ __forceinline__ void launch_begin(const KP& prm, LaunchStep<EMA>& st,
   st.b1p = prm.sc.b1p;
   st.b2p = prm.sc.b2p;
   st.ok = 1;
-  if (prm.sched.state) sched_load(prm.sched, VARIANT != kAccumulate, from_zero, st);
+  if (prm.sched.state) sched_load(prm.sched, prm.lrt, VARIANT != kAccumulate, from_zero, st);
   if constexpr (VARIANT != kAccumulate) {
     if constexpr (loss_scaled(MODE)) {
       ls_load(prm.ls.state, *ls);

@@ -24,7 +24,7 @@ from typing import Callable, Dict, Iterable, List, Optional, Sequence, Tuple, Un
 
 import torch
 
-from . import _lib, graph
+from . import _lib, graph, schedules
 from ._lib import ADAM, ADAM_WEIGHT_DECAY, LAMB, EmaConfig, HParams, LossScaleConfig
 from .train_op import GaccumTrainOp
 
@@ -49,6 +49,11 @@ window_weight = False
 # Report per-tensor gradient, weight and update norms from every apply step (``train_op.tensor_norms()``).  Off by
 # default; create_optimizer reads it.
 tensor_norms = False
+# NVIDIA BERT's polynomial decay of the learning rate after warm-up (``polynomial_decay(power=poly_power,
+# end_learning_rate=end_learning_rate)``; its LAMB recipe uses poly_power = 0.5).  The defaults are the reference's
+# linear decay to 0; create_optimizer reads them.
+poly_power = 1.0
+end_learning_rate = 0.0
 
 LossLike = Union[torch.Tensor, Callable[[], torch.Tensor]]
 LrLike = Union[float, Callable[[int], float]]
@@ -391,7 +396,9 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
     (``layerwise_lr_multipliers``), the number of encoder layers taken from the trainable variables' names.
     With the module attribute ``window_weight`` set, ``loss`` returns (summed loss, weight) and each window is divided by
     its total weight instead of N.  With the module attribute ``tensor_norms`` set, every apply step reports per-tensor
-    gradient, weight and update norms (``train_op.tensor_norms()``).
+    gradient, weight and update norms (``train_op.tensor_norms()``).  The module attributes ``poly_power`` and
+    ``end_learning_rate`` set the polynomial decay after warm-up (``schedules.polynomial_decay``); at their defaults (1.0,
+    0.0) the schedule is the reference's, bit for bit.
     """
     if use_tpu:
         # optimization.py:67-68 wraps the optimizer in tf.contrib.tpu.CrossShardOptimizer: TPU-only.
@@ -405,7 +412,9 @@ def create_optimizer(loss, init_lr, num_train_steps, num_warmup_steps, use_tpu):
                                         _num_encoder_layers([v.name for v in graph.trainable_variables()]))
     cls = LAMBOptimizer if optimizer_type == "lamb" else AdamWeightDecayOptimizer
     optimizer = cls(
-        learning_rate=bert_learning_rate(init_lr, num_train_steps, num_warmup_steps),
+        learning_rate=schedules.with_bert_warmup(
+            schedules.polynomial_decay(init_lr, num_train_steps, end_learning_rate, poly_power), init_lr,
+            num_warmup_steps),
         weight_decay_rate=0.01, beta_1=0.9, beta_2=0.999, epsilon=1e-6,
         exclude_from_weight_decay=["LayerNorm", "layer_norm", "bias"])
     optimizer.lr_multipliers = mult

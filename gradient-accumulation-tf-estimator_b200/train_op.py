@@ -11,7 +11,7 @@ in csrc/.
 from __future__ import annotations
 
 import contextlib
-from typing import Callable, Dict, Optional, Sequence
+from typing import Callable, Dict, Optional, Sequence, Union
 
 import numpy as np
 import torch
@@ -97,6 +97,46 @@ class ScheduleLr:
         return _lib.learning_rate(self.cfg.init_lr, self.cfg.num_train_steps, self.cfg.num_warmup_steps, step)
 
 
+class LrTable:
+    """A device schedule whose learning rates come from a table: the launch at step g uses lr = values[min(g, L - 1)]
+    (gaccum_plan_set_lr_table), so a replayed CUDA graph follows any schedule the host can evaluate -- e.g. one of
+    ``schedules`` (``LrTable((schedules.cosine_decay(1e-4, 10000), 10000))``).  ``values`` is a 1-D array-like of
+    learning rates, or ``(lr_fn, num_steps)``: ``lr_fn.table(num_steps)`` where it has one, else ``lr_fn(g)`` for g in
+    [0, num_steps).  Each value is rounded to fp32 once; ValueError unless there is at least one, and every one is finite,
+    >= 0 and fits fp32.  The table is configuration, not state: checkpoints do not store it, a resumed run passes it
+    again."""
+
+    def __init__(self, values):
+        if isinstance(values, tuple) and len(values) == 2 and callable(values[0]):
+            fn, n = values
+            n = int(n)
+            if n < 1:
+                raise ValueError(f"a learning-rate table needs num_steps >= 1 (got {n})")
+            values = fn.table(n) if hasattr(fn, "table") else [fn(g) for g in range(n)]
+        vals = np.asarray(values, dtype=np.float64)
+        if vals.ndim != 1 or vals.size == 0:
+            raise ValueError(f"a learning-rate table is a non-empty 1-D array (got shape {vals.shape})")
+        with np.errstate(over="ignore"):
+            v32 = vals.astype(np.float32)
+        bad = ~(np.isfinite(vals) & (vals >= 0.0) & np.isfinite(v32))
+        if bad.any():
+            i = int(np.flatnonzero(bad)[0])
+            raise ValueError(f"learning rate {i} of the table is {vals[i]!r}: it must be finite and >= 0, and fit fp32")
+        v32.flags.writeable = False
+        self.values = v32
+
+
+class TableLr:
+    """The learning rate of a table-scheduled train op as a host function: ``float(table[min(g, L - 1)])`` read from the
+    op's device table (synchronous), so an entry rewritten on the device is what it reports."""
+
+    def __init__(self, table: torch.Tensor):
+        self.table = table
+
+    def __call__(self, step: int) -> float:
+        return float(self.table[min(int(step), self.table.numel() - 1)])
+
+
 # the state_dict key of a weighted train op's running window weight W (an fp32 scalar)
 WINDOW_WEIGHT_KEY = "gradient_accumulation/window_weight"
 
@@ -154,10 +194,11 @@ class _DeviceTrainOp(_TrainOpCore):
     def __init__(self, params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step,
                  loss_scale: Optional[LossScaleConfig] = None, exclude_from_layer_adaptation=None,
                  lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False,
-                 device_schedule: Optional[ScheduleConfig] = None, tensor_norms: bool = False):
+                 device_schedule: Union[ScheduleConfig, LrTable, None] = None, tensor_norms: bool = False):
         self.ema: Optional[torch.Tensor] = None          # the moving average of the weights, when one is kept
         self._ema_state: Optional[torch.Tensor] = None
         self._sched_state: Optional[torch.Tensor] = None  # the device schedule's block, when one is kept
+        self.lr_table: Optional[torch.Tensor] = None       # the device copy of an LrTable schedule (writable)
         if not params:
             raise ValueError("no trainable variables")
         # checked before the plan exists, so a bad table fails without touching the device
@@ -193,12 +234,20 @@ class _DeviceTrainOp(_TrainOpCore):
         if device_schedule is not None:
             # gaccum_schedule_state: 6 x 8 bytes.  From here on global_step, the lr and (without loss scaling) the beta
             # powers live on the device; the host tracks the step only to pick each launch's kernel (ScheduleCursor)
-            if lr_fn is not None and not isinstance(lr_fn, ScheduleLr):
+            table = isinstance(device_schedule, LrTable)
+            if lr_fn is not None and (table or not isinstance(lr_fn, ScheduleLr)):
                 raise ValueError("a device-scheduled train op computes its learning rate on the device: pass "
-                                 "lr_fn=None (or device_schedule_lr(cfg))")
-            self.lr_fn = ScheduleLr(device_schedule)
+                                 "lr_fn=None" + ("" if table else " (or device_schedule_lr(cfg))"))
+            # a table schedule still sets a valid config, whose init_lr and step counts the table then ignores
+            cfg = ScheduleConfig(0.0, 0, 0) if table else device_schedule
             self._sched_state = torch.zeros(6, dtype=torch.int64, device=self.device)
-            self.plan.set_device_schedule(device_schedule, self._sched_state.data_ptr())
+            self.plan.set_device_schedule(cfg, self._sched_state.data_ptr())
+            if table:
+                self.lr_table = torch.from_numpy(device_schedule.values.copy()).to(self.device)
+                self.plan.set_lr_table(self.lr_table.data_ptr(), self.lr_table.numel())
+                self.lr_fn = TableLr(self.lr_table)
+            else:
+                self.lr_fn = ScheduleLr(cfg)
             self._cursor = ScheduleCursor(self.N, lambda: self._read_schedule()["global_step"])
             self._write_schedule(self._step, self.beta1_power, self.beta2_power)
         self._norms: Optional[torch.Tensor] = None
@@ -466,7 +515,7 @@ class GaccumTrainOp(_DeviceTrainOp):
                  loss_scale: Optional[LossScaleConfig] = None,
                  exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None,
                  lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False,
-                 device_schedule: Optional[ScheduleConfig] = None, tensor_norms: bool = False):
+                 device_schedule: Union[ScheduleConfig, LrTable, None] = None, tensor_norms: bool = False):
         dtypes = {p.dtype for p in params}
         if len(dtypes) > 1 and dtypes & set(_HALF_DTYPES):
             raise ValueError(f"parameters of mixed dtypes ({', '.join(sorted(str(d) for d in dtypes))}): "
@@ -756,7 +805,7 @@ class PackedTrainOp(_DeviceTrainOp):
                  global_step: int = 0, loss_scale: Optional[LossScaleConfig] = None,
                  exclude_from_layer_adaptation: Optional[Sequence[str]] = None, ema: Optional[EmaConfig] = None,
                  lr_multipliers: Optional[Sequence[float]] = None, window_weight: bool = False,
-                 device_schedule: Optional[ScheduleConfig] = None, tensor_norms: bool = False):
+                 device_schedule: Union[ScheduleConfig, LrTable, None] = None, tensor_norms: bool = False):
         # autograd accumulates a 16-bit parameter's gradient in its own dtype: it cannot add into an fp32 slab
         _refuse_half(params, "PackedTrainOp")
         super().__init__(params, names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step, loss_scale,

@@ -383,6 +383,30 @@ GACCUM_API int gaccum_plan_set_device_schedule(gaccum_plan* plan, const gaccum_s
 GACCUM_API int gaccum_schedule_init(gaccum_plan* plan, gaccum_schedule_state* block, int64_t global_step,
                                     float beta1_power, float beta2_power, gaccum_stream_t stream);
 
+/* A learning-rate table for the device schedule, so a replayed CUDA graph follows any schedule the host can evaluate
+ * (polynomial decay with any power and end value, cosine, exponential, piecewise-constant, each with or without BERT's
+ * warm-up): the host evaluates it once per step, the device looks it up.
+ *   - Every launch of a table plan (gaccum_step, gaccum_step_packed, accumulates included) uses
+ *         lr = device_table[min(g, length - 1)]
+ *     in place of gaccum_learning_rate(init_lr, num_train_steps, num_warmup_steps, g); g is the block's int64
+ *     global_step (>= 0), so the index does not wrap with the int32 branch predicate.  That lr goes everywhere the
+ *     formula's goes: lr_t = fp32(lr * mult[t]), GACCUM_ADAM's alpha, GACCUM_LAMB's r*lr_t and gaccum_stats.lr.
+ *   - Nothing else changes: the branch predicate, `refused`, the beta powers, loss scaling, the moving average, the
+ *     window weight, the per-tensor norms and 16-bit models behave as on any device-scheduled plan.  A table holding
+ *     gaccum_learning_rate(g) at every g computes exactly what the formula computes.
+ *   - The table is read at launch time, stream-ordered: a caller may rewrite entries between launches or graph replays
+ *     and the next launch that reads an entry uses its new value.  Non-finite or negative entries are the caller's
+ *     error: IEEE results propagate, as with a NaN gradient.
+ * The plan must be device-scheduled (gaccum_plan_set_device_schedule, whose cfg is still validated; the table then
+ * ignores its init_lr, num_train_steps and num_warmup_steps).  The setter is host-only: `device_table` is caller-owned
+ * device memory of `length` >= 1 floats, 4-byte aligned, not dereferenced here and read by every launch after it.
+ * Allowed only before the plan's first compute call; combines with the other setters in any order; a first compute call
+ * on a plan that has a table but no device schedule fails with GACCUM_EINVAL.  GACCUM_EINVAL for a NULL plan or table,
+ * length < 1, a misaligned table, a layout-only plan, and after the first compute call.  gaccum_accumulate,
+ * gaccum_apply, gaccum_step_dp, gaccum_apply_dp, gaccum_host_session_create and gaccum_step_host refuse a table plan
+ * with GACCUM_EINVAL.  gaccum_algorithmic_bytes is unchanged (one 4-byte load per CTA). */
+GACCUM_API int gaccum_plan_set_lr_table(gaccum_plan* plan, const float* device_table, int64_t length);
+
 /* Per-tensor norms of the apply step, for watching a run layer by layer (TF1's add_gradients_summaries /
  * optimize_loss(summaries=["gradient_norm"])) without extra passes over the slabs.  Off unless set.  Every apply launch
  * of gaccum_step, gaccum_apply (grads == NULL included) and gaccum_step_packed writes, for every tensor t, row t of
