@@ -188,6 +188,8 @@ def _load():
         "gaccum_schedule_init": (C.c_int, [vp, vp, i64, C.c_float, C.c_float, vp]),
         "gaccum_plan_set_tensor_norms": (C.c_int, [vp, vp]),
         "gaccum_plan_set_lr_table": (C.c_int, [vp, vp, i64]),
+        "gaccum_plan_set_deferred_reset": (C.c_int, [vp, i32]),
+        "gaccum_accum_materialize": (C.c_int, [vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -352,6 +354,15 @@ class Plan:
 
     def read_stats(self, host_ptr: int, stream: int = 0) -> None:
         _check(_load().gaccum_read_stats(self._h, host_ptr, stream))
+
+    def set_deferred_reset(self, on: bool) -> None:
+        """Applies leave the accumulators logically zero instead of storing zeros (gaccum_plan_set_deferred_reset);
+        whatever reads or writes the slab outside a window's first accumulate calls ``accum_materialize`` first."""
+        _check(_load().gaccum_plan_set_deferred_reset(self._h, 1 if on else 0))
+
+    def accum_materialize(self, accum: int, stream: int = 0) -> None:
+        """Store the zeros a deferred-reset apply left logical, if it did (asynchronous on ``stream``)."""
+        _check(_load().gaccum_accum_materialize(self._h, accum, stream))
 
     def set_loss_scale(self, cfg: LossScaleConfig, device_state: int) -> None:
         """Turn dynamic loss scaling on (before the first compute call); ``device_state`` points to 32 bytes of

@@ -106,6 +106,10 @@ struct gaccum_plan {
   // the partials, the chunk tables and the counters of NormParams in one allocation
   NormParams norms{};
   void* d_norms = nullptr;
+  // deferred reset of the accumulators (gaccum_plan_set_deferred_reset): d_reset holds the word accum_zero (unsigned int
+  // 0) and, at floats 4 .. 7, the stats block gaccum_accum_materialize's launch writes instead of gaccum_stats
+  bool deferred = false;
+  unsigned int* d_reset = nullptr;
   std::mutex mu;
   std::map<const void*, int> grid_cache;   // cooperative kernel -> CTAs that fit on one SM (fit)
 };
@@ -298,6 +302,7 @@ static void fill_common(gaccum_plan* pl, KernelParams<CAP>& prm, float* accum, f
   prm.sched.accum_n = a ? a->accum_n : 1;
   prm.norms = pl->norms;
   prm.lrt = pl->lr_table;
+  prm.dr.accum_zero = pl->deferred ? pl->d_reset : nullptr;
 }
 
 template <int CAP>
@@ -380,7 +385,8 @@ enum PlanSetting : unsigned {
   kPlanSchedule = 1u << 6,
   kPlanLrTable = 1u << 7,
   kPlanNorms = 1u << 8,
-  kPlanAll = (1u << 9) - 1u,
+  kPlanDeferredReset = 1u << 9,
+  kPlanAll = (1u << 10) - 1u,
 };
 // Fails on the first of the settings `lacks` names that the plan has: `what` does not support it
 static int refuse(const gaccum_plan* pl, const unsigned lacks, const char* what) {
@@ -395,6 +401,7 @@ static int refuse(const gaccum_plan* pl, const unsigned lacks, const char* what)
       {kPlanSchedule, pl->sched_state != nullptr, "a device schedule (gaccum_plan_set_device_schedule)"},
       {kPlanLrTable, pl->lr_table.table != nullptr, "a learning-rate table (gaccum_plan_set_lr_table)"},
       {kPlanNorms, pl->norms.out != nullptr, "per-tensor norms (gaccum_plan_set_tensor_norms)"},
+      {kPlanDeferredReset, pl->deferred, "a deferred reset of the accumulators (gaccum_plan_set_deferred_reset)"},
   };
   for (const auto& st : settings)
     if ((lacks & st.setting) && st.on) return fail(GACCUM_EINVAL, "%s does not support %s", what, st.name);
@@ -404,7 +411,7 @@ static int refuse(const gaccum_plan* pl, const unsigned lacks, const char* what)
 static void free_plan_device(gaccum_plan* pl) {
   cudaFree(pl->d_tiles); cudaFree(pl->d_partials); cudaFree(pl->d_stats); cudaFree(pl->d_dp_sync); cudaFree(pl->d_barrier); cudaFree(pl->d_counters);
   cudaFree(pl->d_adapt); cudaFree(pl->d_lamb_acc); cudaFree(pl->d_ratios); cudaFree(pl->d_done); cudaFree(pl->d_lr_mult);
-  cudaFree(pl->d_norms);
+  cudaFree(pl->d_norms); cudaFree(pl->d_reset);
 #ifdef GACCUM_EXPERIMENTS
   cudaFree(pl->d_debug);
 #endif
@@ -531,6 +538,8 @@ int gaccum_plan_create(gaccum_plan** out, int32_t T, const int64_t* numels, cons
     if (e == cudaSuccess) e = cudaMemset(pl->d_stats, 0, sizeof(gaccum_stats));
     if (e == cudaSuccess) e = cudaMalloc(&pl->d_done, sizeof(unsigned int));
     if (e == cudaSuccess) e = cudaMemset(pl->d_done, 0, sizeof(unsigned int));
+    if (e == cudaSuccess) e = cudaMalloc(&pl->d_reset, 8 * sizeof(unsigned int));
+    if (e == cudaSuccess) e = cudaMemset(pl->d_reset, 0, 8 * sizeof(unsigned int));
     if (e == cudaSuccess) e = cudaMalloc(&pl->d_lr_mult, (size_t)std::max(1, T) * sizeof(float));
     if (e == cudaSuccess && T > 0)
       e = cudaMemcpy(pl->d_lr_mult, pl->lr_mult.data(), (size_t)T * sizeof(float), cudaMemcpyHostToDevice);
@@ -876,6 +885,41 @@ int gaccum_step(gaccum_plan* pl, const float* const* grads, float* const* params
   return accumulate_impl(pl, grads, accum, a, stream);
 }
 
+int gaccum_plan_set_deferred_reset(gaccum_plan* pl, int32_t on) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (pl->device < 0) return fail(GACCUM_EINVAL, "a layout-only plan (device=-1) has no accumulators to reset");
+  if (on != 0 && on != 1) return fail(GACCUM_EINVAL, "on must be 0 or 1 (got %d)", on);
+  pl->deferred = on != 0;
+  return GACCUM_OK;
+}
+
+// The first-accumulate kernel with no gradients, no schedule and the plan's own stats block: it stores +0 over every
+// tensor while the word is 1, then clears it (accumulate_kernel), and touches no other device state
+extern "C++" {
+template <int CAP>
+static int do_materialize(gaccum_plan* pl, float* accum, cudaStream_t st) {
+  KernelParams<CAP>* prm = new (std::nothrow) KernelParams<CAP>();
+  if (!prm) return fail(GACCUM_ENOMEM, "out of host memory");
+  fill_common(pl, *prm, accum, nullptr, nullptr, nullptr);
+  prm->sched.state = nullptr;
+  prm->stats = reinterpret_cast<float*>(pl->d_reset + 4);
+  const int rc = pl->master ? launch_accumulate<CAP, true>(pl, *prm, true, st) : launch_accumulate<CAP, false>(pl, *prm, true, st);
+  delete prm;
+  return rc;
+}
+}  // extern "C++"
+
+int gaccum_accum_materialize(gaccum_plan* pl, float* accum, gaccum_stream_t stream) {
+  if (!pl) return fail(GACCUM_EINVAL, "plan is NULL");
+  if (pl->device < 0)
+    return fail(GACCUM_ENODEVICE, "layout-only plan (device=-1): libgaccum has no CPU fallback, a CUDA device is required");
+  if (!accum || !aligned16_host(accum)) return fail(GACCUM_EINVAL, "accum must be a 16-byte aligned device pointer");
+  if (!pl->deferred) return GACCUM_OK;      // every apply of this plan stores the zeros itself
+  DeviceGuard guard(pl->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  return pl->T <= kCapSmall ? do_materialize<kCapSmall>(pl, accum, st) : do_materialize<kCapLarge>(pl, accum, st);
+}
+
 int gaccum_step_packed(gaccum_plan* pl, const float* grad_slab, float* param_slab, float* accum,
                        float* m, float* v, const gaccum_step_args* a, int32_t force_branch,
                        gaccum_stream_t stream) {
@@ -890,6 +934,7 @@ int gaccum_step_packed(gaccum_plan* pl, const float* grad_slab, float* param_sla
   cudaStream_t st = (cudaStream_t)stream;
   KernelParams<0> prm{};
   fill_common(pl, prm, accum, m, v, a);
+  prm.dr.accum_zero = nullptr;   // a packed slab (autograd adds into it) always holds real zeros: no deferred reset
   prm.tab.g = grad_slab;
   prm.tab.p = param_slab;
   if (!apply) {

@@ -209,6 +209,15 @@ struct LrTableParams {
   int64_t length;          // >= 1
 };
 
+// Deferred reset of the accumulators (gaccum_plan_set_deferred_reset).  accum_zero == NULL: every apply stores a = +0, as
+// the reference does.  Otherwise no apply stores into the accumulator slab: its commit sets the plan's word *accum_zero to
+// 1, which makes the accumulators logically +0 and the slab's contents unspecified.  The first accumulate of a window
+// (which does not read a) then stores +0 + G where there is a gradient and, while the word is 1, +0 where there is none;
+// the last of its CTAs clears the word.  A launch-uniform branch, not a template flag: no kernel is specialised on it.
+struct DeferredResetParams {
+  unsigned int* accum_zero;
+};
+
 // Every kernel's parameter block.  Each feature's parameters follow those of the features before it, so adding them
 // moved no member an existing kernel reads.
 template <int CAP>
@@ -236,6 +245,7 @@ struct KernelParams {
   ScheduleParams sched;   // every kernel
   NormParams norms;       // apply kernels only
   LrTableParams lrt;      // device-scheduled launches only
+  DeferredResetParams dr; // apply kernels and the first accumulate of a window only
 };
 static_assert(sizeof(KernelParams<1920>) <= 32764, "kernel parameters must fit the 32 KB limit");
 
@@ -352,6 +362,11 @@ __device__ __forceinline__ float4 ld_policy(const float4* p, uint64_t pol) {
 __device__ __forceinline__ void st_policy(float4* p, const float4 v, uint64_t pol) {
   asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1,%2,%3,%4}, %5;"
                :: "l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
+}
+// Drop the 128-byte L2 line at p (128-byte aligned) without writing it back: its contents become unspecified.  For dead
+// accumulator lines of a deferred-reset apply (DeferredResetParams), which would otherwise be written back dirty.
+__device__ __forceinline__ void discard_line(const void* p) {
+  asm volatile("discard.global.L2 [%0], 128;" :: "l"(p) : "memory");
 }
 
 template <int CAP>
@@ -704,13 +719,21 @@ __device__ __forceinline__ void walk_tile(const uint32_t len, const uint32_t nve
 // FROM_ZERO: the first accumulate of a window.  The apply that ended the previous window left every accumulator at
 // +0.0 (optimization.py:78,86-87), so a is not loaded and a = +0 + G is stored (8 instead of 12 B/elem).  The add is
 // kept: it turns a gradient of -0.0 into +0.0, as assign_add onto a zero does, and a NaN comes out as a += G gives it.
+// zero (FROM_ZERO, deferred reset only): the slab holds no zeros (DeferredResetParams), so a tile without a gradient
+// stores them.
 // ---------------------------------------------------------------------------------------------
 template <bool FROM_ZERO, bool H, int CAP>
-__device__ __forceinline__ void accumulate_tile(const TileDesc d, const KernelParams<CAP>& prm) {
+__device__ __forceinline__ void accumulate_tile(const TileDesc d, const KernelParams<CAP>& prm, const bool zero) {
   const Grad<H> g(prm, d);
-  if (g.g == nullptr) return;   // optimization.py:132 -- tensors without a gradient are skipped
   float* __restrict__ a = prm.accum + (size_t)d.soff32 * kSlabAlign;
   float4* a4 = reinterpret_cast<float4*>(a);
+  if (g.g == nullptr) {         // optimization.py:132 -- tensors without a gradient are skipped
+    if (FROM_ZERO && zero) {    // the slab is 16-byte aligned at every tile
+      walk_tile(d.len, d.len >> 2, threadIdx.x, [](int, uint32_t) {}, [] {},
+                [&](int, uint32_t i) { a4[i] = make_float4(0.f, 0.f, 0.f, 0.f); }, [&](uint32_t i) { a[i] = 0.f; });
+    }
+    return;
+  }
   float4 vg[kUnroll], va[kUnroll];
   walk_tile(d.len, g.vec_ok() ? d.len >> 2 : 0u, threadIdx.x,
             [&](int u, uint32_t i) {
@@ -817,7 +840,7 @@ __device__ __forceinline__ void launch_begin(const KP& prm, LaunchStep<EMA>& st,
 }
 // The one thread that commits a launch, once no CTA of it reads the state blocks any more: gaccum_stats (gn and s: the
 // global norm and the clip scale, 0 and 1 without clipping), the loss-scaling state, the average (applied windows only),
-// the window weight (applied and skipped windows alike) and the schedule's next step.  The schedule advances the beta
+// the window weight and the deferred reset's word (applied and skipped windows alike) and the schedule's next step.  The schedule advances the beta
 // powers only where the launch took them from it: an optimizer that keeps them, on a launch that is not loss-scaled.
 template <int VARIANT, int MODE = kNoClip, bool EMA = false, typename KP>
 __device__ __forceinline__ void launch_commit(const KP& prm, const LaunchStep<EMA>& st, const LossScaleState* ls,
@@ -827,6 +850,7 @@ __device__ __forceinline__ void launch_commit(const KP& prm, const LaunchStep<EM
   if constexpr (loss_scaled(MODE)) ls_finish<keeps_beta_powers(VARIANT)>(prm.ls, *ls, skip, prm.sc.b1, prm.sc.b2);
   if constexpr (EMA) { if (!skip) ema_finish(prm.ema, st.ema); }
   if (apply && prm.ww.state) window_finish(prm.ww.state, st.dv.nf);
+  if (apply && prm.dr.accum_zero) *prm.dr.accum_zero = 1u;   // deferred reset: the accumulators are +0 from here on
   if (prm.sched.state) sched_finish(prm.sched, keeps_beta_powers(VARIANT) && !loss_scaled(MODE), prm.sc.b1, prm.sc.b2);
 }
 // Thread 0 of every CTA of a one-tile-per-CTA launch, after its tile: true in the CTA that commits.  `counted` (the launch
@@ -842,21 +866,34 @@ __device__ __forceinline__ bool commits_launch(unsigned int* done, const bool co
 
 // Device schedule: every CTA checks the step before its tile, and the last one through commits the launch.  Without one
 // the launch commits nothing but the stats, which no CTA reads: block 0 writes them before its tile, counting nothing.
+// Deferred reset (FROM_ZERO only): every CTA reads the word before its tile.  All of them find the same value, since only
+// this launch's last CTA through changes it: if it is 1, every CTA is counted and that last one clears it.
+// gaccum_accum_materialize launches this kernel with no gradients and no schedule: a zero fill while the word is 1.
 template <int CAP, bool FROM_ZERO, bool H = false>
 __global__ void __launch_bounds__(kThreads)
 accumulate_kernel(const __grid_constant__ KernelParams<CAP> prm) {
   __shared__ LaunchStep<> s_step;
-  const bool sched = prm.sched.state != nullptr;   // launch-uniform
-  if (sched) {
-    if (threadIdx.x == 0) launch_begin<kAccumulate>(prm, s_step, nullptr, FROM_ZERO);
+  __shared__ unsigned int s_zero;
+  const bool sched = prm.sched.state != nullptr;                     // launch-uniform
+  const bool deferred = FROM_ZERO && prm.dr.accum_zero != nullptr;   // launch-uniform
+  if (sched || deferred) {
+    if (threadIdx.x == 0) {
+      if (sched) launch_begin<kAccumulate>(prm, s_step, nullptr, FROM_ZERO);
+      if (deferred) s_zero = __ldcg(prm.dr.accum_zero);
+    }
     __syncthreads();
-    if (!s_step.ok) { sched_refuse(prm.sched); return; }
-  } else if (blockIdx.x == 0 && threadIdx.x == 0) {
+    if (sched && !s_step.ok) { sched_refuse(prm.sched); return; }
+  }
+  if (!sched && blockIdx.x == 0 && threadIdx.x == 0) {
     launch_begin<kAccumulate>(prm, s_step);
     launch_commit<kAccumulate>(prm, s_step, nullptr, false, 0.f, 1.f);
   }
-  if ((int)blockIdx.x < prm.num_tiles) accumulate_tile<FROM_ZERO, H>(prm.tiles[blockIdx.x], prm);
-  if (sched && threadIdx.x == 0 && commits_launch(prm.done, true)) launch_commit<kAccumulate>(prm, s_step, nullptr, false, 0.f, 1.f);
+  const bool zero = deferred && s_zero != 0u;
+  if ((int)blockIdx.x < prm.num_tiles) accumulate_tile<FROM_ZERO, H>(prm.tiles[blockIdx.x], prm, zero);
+  if ((sched || zero) && threadIdx.x == 0 && commits_launch(prm.done, true)) {
+    if (sched) launch_commit<kAccumulate>(prm, s_step, nullptr, false, 0.f, 1.f);
+    if (zero) *prm.dr.accum_zero = 0u;
+  }
 }
 
 // gaccum_loss_scale_init: one thread writes the initial loss-scaling state (a kernel, so the call stays asynchronous and
@@ -903,6 +940,7 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
   bool bf16 = false;
   if constexpr (H) { q = model_ptr(prm, d); bf16 = prm.half.bf16 != 0; }
   const bool decay = (d.tensor_flags >> 31) != 0;
+  const bool deferred = prm.dr.accum_zero != nullptr;   // launch-uniform: a = +0 is not stored (DeferredResetParams)
   const Scalars& sc = prm.sc;
   const float rate = tile_rate<VARIANT>(lr, tensor_mult(prm.lrm, d), bc2, bc1);
   float4* a4 = reinterpret_cast<float4*>(a);
@@ -929,7 +967,7 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
                                     pb.w, vp[u].w);
               }
               __stcs(p4 + i, vp[u]); __stcs(m4 + i, vm[u]); __stcs(v4 + i, vv[u]);
-              __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
+              if (!deferred) __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
               if constexpr (H) store_model4(q, i, vp[u], bf16);
               if constexpr (EMA) __stcs(e4 + i, ema_vec(ve[u], vp[u], ema_c));
             },
@@ -940,7 +978,8 @@ __device__ __forceinline__ void update_tile(const TileDesc d, const KernelParams
               if (norms) { np_.g = add_sq(np_.g, ax, dv); np_.w = sq_acc(np_.w, px); }
               update_elem<VARIANT>(ax, false, 0.f, px, mx, vx, decay, sc, rate, dv);
               if (norms) np_.u = diff_sq_acc(np_.u, pb, px);
-              p[i] = px; m[i] = mx; v[i] = vx; a[i] = 0.f;
+              p[i] = px; m[i] = mx; v[i] = vx;
+              if (!deferred) a[i] = 0.f;
               if constexpr (H) q[i] = (uint16_t)f2h(px, bf16);
               if constexpr (EMA) e[i] = ema_elem(e[i], px, ema_c);
             });
@@ -1004,7 +1043,7 @@ apply_kernel(const __grid_constant__ KernelParams<CAP> prm) {
 //          ring as soon as pass 1 is drained -- HBM stays busy while the CTAs wait for each other.
 // pass 2   ring slot = [p | m | v | a'] (32 KB).  First the group's own stashed tiles, then tickets over
 //          all other tiles, youngest first (a' still in L2): clip, AdamWeightDecay/Adam,
-//          STG p, m, v, a = 0.
+//          STG p, m, v, a = 0 (deferred reset: no a = 0, and a pool tile's a' lines are discarded from L2).
 // Tiles that bulk copies cannot move (gradient / parameter pointer not 16-byte aligned, or shorter than one
 // float4) go through the same full/empty protocol with nothing copied and are loaded by the consumers with
 // scalar LDGs; producer and consumers evaluate the same predicates (bulk_vecs / bulk_vecs2).
@@ -1269,6 +1308,7 @@ __device__ __forceinline__ float norm_tile(const TileDesc& d, const KernelParams
 // `rate` is the tile's lr_t / alpha_t (SlotMeta::rate; loss-scaled Adam: from the device's beta powers).
 // Loss-scaled: a skipped window (`skip`) stores a = 0 and nothing else.  H: p is the master slab, and the model copy is
 // stored after it (not on a skipped window).
+// Deferred reset (DeferredResetParams): a = 0 is not stored, and a pool tile's a' lines are discarded from L2.
 // EMA: the slot is [p | m | v | a' | e], and e - (e - p) * c is stored after p (not on a skipped window).
 // norms (launch-uniform): the slot is kept for norm_tile2 instead of being released after the loads, and the tile's
 // elements in it are made those norm_tile2 reads -- p before the update in the slot's p quarter (where the vector path
@@ -1291,13 +1331,21 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
   if constexpr (H) { q = model_ptr(prm, d); bf16 = prm.half.bf16 != 0; }
   const bool decay = (d.tensor_flags >> 31) != 0;
   const bool write = !loss_scaled(MODE) || !skip;
+  const bool deferred = prm.dr.accum_zero != nullptr;   // launch-uniform: a = +0 is not stored (DeferredResetParams)
   float4* a4 = reinterpret_cast<float4*>(a);
   float4* m4 = reinterpret_cast<float4*>(m);
   float4* v4 = reinterpret_cast<float4*>(v);
   float4* p4 = reinterpret_cast<float4*>(p);
   float4* e4 = reinterpret_cast<float4*>(e);
   float4 va[kUnroll], vp[kUnroll], vm[kUnroll], vv[kUnroll], ve[kUnroll];
-  walk_tile(d.len, bulk_vecs2(d, p), threadIdx.x & (kThreads - 1),
+  const uint32_t nvec = bulk_vecs2(d, p);
+  if (deferred && stash == nullptr) {
+    // a' of a pool tile has landed in the slot: its whole lines in global memory are dead (a tail line still holds
+    // elements the scalar path reads below), and dropping them saves the write-back of those still in L2
+    const uint32_t line = threadIdx.x & (kThreads - 1);
+    if (line < nvec / 8u) discard_line(a + 32u * line);
+  }
+  walk_tile(d.len, nvec, threadIdx.x & (kThreads - 1),
             [&](int u, uint32_t i) {
               vp[u] = slot[i]; vm[u] = slot[kTile / 4 + i]; vv[u] = slot[2 * (kTile / 4) + i];
               va[u] = stash != nullptr ? stash[i] : slot[3 * (kTile / 4) + i];
@@ -1312,7 +1360,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
                 if constexpr (EMA) __stcs(e4 + i, ema_vec(ve[u], vp[u], ema_c));
                 if (norms) slot[kTile / 4 + i] = vp[u];
               }
-              __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
+              if (!deferred) __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
             },
             [&](uint32_t i) {
               float* const sf = reinterpret_cast<float*>(slot);
@@ -1327,7 +1375,7 @@ __device__ __forceinline__ void update_tile2(const TileDesc& d, const KernelPara
               } else if (norms) {
                 sf[i] = p[i];
               }
-              a[i] = 0.f;
+              if (!deferred) a[i] = 0.f;
             });
 }
 // norms, after update_tile2: the tile's partials of p^2 (p before the update) and, unless the window is skipped,
@@ -1363,10 +1411,10 @@ __device__ __forceinline__ void norm_tile2(const TileDesc& d, const uint32_t nve
 
 // Dynamic shared memory of apply_clip_kernel (kClipSmemBytes): 3 groups x kRingVecs float4 of ring, then
 // 3 groups x kStashVecs float4 of stash.
-// Registers: 864 threads in one CTA cap the kernel at 72 per thread.  ptxas -v (CUDA 12.9): only the AdamWeightDecay
-// kClip instantiations without an EMA fit without spilling.  Every other one spills: AdamWeightDecay 4-24 bytes of
-// stores per thread loss-scaled, 44-64 with an EMA; plain Adam (VARIANT 1) 4-44 without an EMA, 52-72 with one.  What
-// that costs has not been measured.
+// Registers: 864 threads in one CTA cap the kernel at 72 per thread.  ptxas -v (CUDA 12.9): only the fp32 AdamWeightDecay
+// kClip instantiations without an EMA fit without spilling (the 16-bit ones store 8 bytes per thread since the deferred
+// reset).  Every other one spills: AdamWeightDecay 4-24 bytes of stores per thread loss-scaled, 44-68 with an EMA; plain
+// Adam (VARIANT 1) 8-44 without an EMA, 52-80 with one.  What that costs has not been measured.
 //
 // Device state (loss scaling, EMA, window weight, device schedule): thread 0 of every CTA reads it during set-up
 // (launch_begin), before its CTA arrives at the grid barrier; block 0's thread 0 commits the launch at the very end

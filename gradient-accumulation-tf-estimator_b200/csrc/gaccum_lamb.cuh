@@ -137,6 +137,7 @@ __device__ __forceinline__ void lamb_update_tile(const TileDesc& d, const Kernel
 }
 
 // ---- phase 3: p = p - (r*lr)*u and a = +0 (a = +0 only on a skipped window) ----
+// Deferred reset (DeferredResetParams): a = +0 is not stored, and the u lines read are discarded from L2.
 // EMA: e is read with p and u, and e - (e - p) * c stored after p.
 // norms (launch-uniform): the thread's fp32 partials of p^2 (p before the update; on a skipped window p is read for it)
 // and (p - p')^2 go into nw and nu.
@@ -151,11 +152,13 @@ __device__ __forceinline__ void lamb_write_tile(const TileDesc& d, const KernelP
   uint16_t* q = nullptr;
   bool bf16 = false;
   if constexpr (H) { q = model_ptr(prm, d); bf16 = prm.half.bf16 != 0; }
+  const bool deferred = prm.dr.accum_zero != nullptr;   // launch-uniform: a = +0 is not stored (DeferredResetParams)
   float4* a4 = reinterpret_cast<float4*>(a);
   float4* p4 = reinterpret_cast<float4*>(p);
   float4* e4 = reinterpret_cast<float4*>(e);
   float4 vu[kUnroll], vp[kUnroll], ve[kUnroll];
-  walk_tile(d.len, H || aligned16(p) ? d.len >> 2 : 0u, threadIdx.x,
+  const uint32_t nvec = H || aligned16(p) ? d.len >> 2 : 0u;
+  walk_tile(d.len, nvec, threadIdx.x,
             [&](int u, uint32_t i) {
               if (write) {
                 vu[u] = __ldcs(a4 + i); vp[u] = __ldcs(p4 + i);
@@ -183,7 +186,7 @@ __device__ __forceinline__ void lamb_write_tile(const TileDesc& d, const KernelP
               } else if (norms) {
                 nw = sq_acc(nw, vp[u]);
               }
-              __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
+              if (!deferred) __stcs(a4 + i, make_float4(0.f, 0.f, 0.f, 0.f));   // optimization.py:86-87
             },
             [&](uint32_t i) {
               if (write) {
@@ -196,8 +199,19 @@ __device__ __forceinline__ void lamb_write_tile(const TileDesc& d, const KernelP
               } else if (norms) {
                 nw = sq_acc(nw, p[i]);
               }
-              a[i] = 0.f;
+              if (!deferred) a[i] = 0.f;
             });
+  if (deferred) {
+    // the u lines are dead once read: a line is vectors 8l .. 8l + 7, which 8 lanes of one warp have loaded and used by
+    // now; whole vector lines only (a tail line holds elements other threads read)
+    __syncwarp();
+    const uint32_t tid = threadIdx.x;
+#pragma unroll
+    for (int u = 0; u < kUnroll; ++u) {
+      const uint32_t i = u * kThreads + tid;
+      if ((tid & 7u) == 0u && i + 8u <= nvec) discard_line(a4 + i);
+    }
+  }
 }
 
 // Device state (loss scaling, EMA, window weight, device schedule): thread 0 of every CTA reads it during set-up

@@ -42,6 +42,10 @@ class DataParallelTrainOp:
         self.group = process_group if process_group is not None and process_group is not True else None
         self.world = dist.get_world_size(self.group) if dist.is_initialized() else 1
         self.allreduces = 0
+        if self.world > 1 and hasattr(engine, "_set_deferred_reset"):
+            # the all-reduce and the checkpoint paths read, swap and zero the slab between launches: every apply
+            # stores its zeros
+            engine._set_deferred_reset(False)
 
     def _weighted(self) -> bool:
         return getattr(self.engine, "window_weight", None) is not None
@@ -161,6 +165,7 @@ class FusedDataParallelTrainOp:
         self._handles = [symm.rendezvous(t, gname) for t in (self.param_slab, self.stage, self.ctrl)]
         hp_, hs_, hc_ = self._handles
         self.engine = GaccumTrainOp(list(params), names, hp, accum_n, lr_fn, exclude_from_weight_decay, global_step)
+        self.engine._set_deferred_reset(False)     # the fused exchange + apply kernel stores the zeros itself
         self.plan = self.engine.plan
         self.comm = _lib.DpComm()
         self.comm.rank, self.comm.world = self.rank, self.world

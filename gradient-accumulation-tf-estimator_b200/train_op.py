@@ -281,8 +281,14 @@ class _DeviceTrainOp(_TrainOpCore):
 
     @global_step.setter
     def global_step(self, g: int) -> None:
-        self._step = int(g)
-        if getattr(self, "_sched_state", None) is not None:
+        g = int(g)
+        sched = getattr(self, "_sched_state", None) is not None
+        # deferred reset: the accumulators may be logically zero only while the next launch is a window's first
+        # accumulate, which does not read them; a launch at any other new step would
+        if getattr(self, "_deferred", False) and (sched or g != self._step) and not _lib.is_first_accumulate(g, self.N):
+            self._materialize()
+        self._step = g
+        if sched:
             st = self._read_schedule()      # keeps the beta powers; a refused schedule starts afresh
             self._write_schedule(self._step, st["beta1_power"], st["beta2_power"])
 
@@ -396,6 +402,12 @@ class _DeviceTrainOp(_TrainOpCore):
 
     def _zeros_slab(self) -> torch.Tensor:
         return torch.zeros(max(self.plan.padded_size, 32), dtype=torch.float32, device=self.device)
+
+    def _materialize(self) -> None:
+        """A deferred-reset op (GaccumTrainOp): store the zeros its last apply left logical, if it did, on the current
+        stream (gaccum_accum_materialize; no sync)."""
+        if getattr(self, "_deferred", False):
+            self.plan.accum_materialize(self._accum_ptr, self._stream())
 
     def _stream(self, stream: Optional[int] = None) -> int:
         return torch.cuda.current_stream(self.device).cuda_stream if stream is None else stream
@@ -551,6 +563,31 @@ class GaccumTrainOp(_DeviceTrainOp):
         self._grad_ptrs = None
         self.last_lr = 0.0
         self.last_applied = False
+        # N >= 2: the apply leaves the accumulators logically zero instead of storing zeros (4 B/param less HBM traffic
+        # per window); the window's first accumulate, which does not read them, stores +0 + G.  With N = 1 every step
+        # applies and reads them.
+        self._deferred = False
+        if self.N >= 2:
+            self._set_deferred_reset(True)
+
+    @property
+    def accum(self) -> torch.Tensor:
+        """The accumulator slab (optimization.py:78), in the plan's layout.  After an apply of a deferred-reset op it is
+        first zeroed on the current stream (no sync), so every reader and writer sees the zeros the reference's apply
+        stores."""
+        self._materialize()
+        return self._accum
+
+    @accum.setter
+    def accum(self, t: torch.Tensor) -> None:
+        self._accum = t
+
+    def _set_deferred_reset(self, on: bool) -> None:
+        """Front ends whose collectives read or write the slab between launches keep the apply's zero store."""
+        if not on:
+            self._materialize()
+        self.plan.set_deferred_reset(on)
+        self._deferred = bool(on)
 
     def _grad_table(self, grads: Sequence[Optional[torch.Tensor]]):
         key = tuple(0 if g is None else g.data_ptr() for g in grads)
@@ -608,12 +645,14 @@ class GaccumTrainOp(_DeviceTrainOp):
         return self._after(g, _lib.is_apply_step(g, self.N), lr)
 
     def accumulate_only(self, grads: Sequence[Optional[torch.Tensor]]) -> None:
-        """The false branch alone (used by the data-parallel driver); does not touch global_step."""
+        """The false branch alone (used by the data-parallel driver); does not touch global_step.  Reads the
+        accumulators: ``self.accum`` materializes a deferred reset first."""
         self._refuse_schedule("accumulate_only")
         self.plan.accumulate(self._grad_table(grads), self.accum.data_ptr(), self._stream())
 
     def apply_only(self, grads: Optional[Sequence[Optional[torch.Tensor]]] = None) -> None:
-        """The true branch alone; ``grads=None`` applies the accumulators as they are."""
+        """The true branch alone; ``grads=None`` applies the accumulators as they are (``self.accum`` materializes a
+        deferred reset first)."""
         self._refuse_schedule("apply_only")
         lr = _f32(self.lr_fn(self.global_step))
         self._refresh_param_table()
@@ -622,13 +661,17 @@ class GaccumTrainOp(_DeviceTrainOp):
                         self._step_args(self.global_step, lr), self._stream())
         self.last_lr, self.last_applied = lr, True
         self._advance_beta_powers()
+        if not _lib.is_first_accumulate(self._step, self.N):
+            self._materialize()      # global_step is unchanged: its launch may read the accumulators
 
     def _after(self, g: int, applied: bool, lr: float) -> bool:
         """Bookkeeping once micro-step ``g`` is launched."""
         self.last_lr, self.last_applied = lr, applied
         if applied:
             self._advance_beta_powers()
-        self.global_step = g + 1                                # optimization.py:102-103
+        # optimization.py:102-103.  Not through the setter: after an apply, step g + 1 is a window's first accumulate
+        # (N >= 2), which does not read the accumulators, so a deferred reset stays deferred
+        self._step = g + 1
         return applied
 
     __call__ = run

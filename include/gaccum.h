@@ -456,6 +456,26 @@ GACCUM_API int gaccum_plan_set_tensor_norms(gaccum_plan* plan, float* device_out
 GACCUM_API int gaccum_step(gaccum_plan* plan, const float* const* grads, float* const* params,
                            float* accum, float* m, float* v, const gaccum_step_args* args,
                            gaccum_stream_t stream);
+/* Deferred reset of the accumulators, as zero_grad(set_to_none=True) defers a gradient's reset: off unless set.  The
+ * apply branch then stores nothing into `accum` (32 instead of 36 B x P, with clipping also no write-back of a' lines
+ * still in L2) and leaves the accumulators LOGICALLY +0.0 on applied and loss-scale-skipped windows alike, for every
+ * optimizer: a plan-owned device word records it and the slab's contents are unspecified until the next write.  The
+ * first micro-step of a window (the precondition above) stores +0.0 + G where there is a gradient and, while the word
+ * is set, +0.0 where there is none, then clears the word; its results are bit for bit those of a plan without the mode.
+ * Every other launch that READS accum -- gaccum_accumulate, gaccum_apply, a gaccum_step that is not a window's first
+ * accumulate, and any read or write of the slab by the caller -- must follow gaccum_accum_materialize on the same stream
+ * when an apply may have run since the last first accumulate (e.g. after global_step was reassigned).
+ *   gaccum_plan_set_deferred_reset: on = 1 or 0; host-only, at any time.  Turning the mode off does not write the slab:
+ *   materialize first.  GACCUM_EINVAL for a NULL or layout-only plan, or on not 0 or 1.  gaccum_step_dp,
+ *   gaccum_apply_dp, gaccum_host_session_create and gaccum_step_host refuse such a plan with GACCUM_EINVAL.
+ *   gaccum_step_packed ignores the mode (its caller adds into the slab between launches, so the slab holds real zeros):
+ *   its applies store them and it neither reads nor writes the word -- a slab it shares with launches of the mode is
+ *   materialized first.  gaccum_algorithmic_bytes is unchanged.
+ *   gaccum_accum_materialize: asynchronous on `stream` and graph-capturable; stores +0.0 into every tensor element of
+ *   `accum` if the word is set (4 B x P) and clears it, else changes nothing; it reads and writes no other device state
+ *   (not gaccum_stats, the device schedule or any other block).  GACCUM_OK without a launch on a plan without the mode. */
+GACCUM_API int gaccum_plan_set_deferred_reset(gaccum_plan* plan, int32_t on);
+GACCUM_API int gaccum_accum_materialize(gaccum_plan* plan, float* accum, gaccum_stream_t stream);
 /* The two branches on their own (the data-parallel driver accumulates locally, all-reduces the
  * slab, then applies with grads == NULL).  gaccum_apply ignores args->global_step.
  * gaccum_accumulate has no step arguments and always reads accum: accum += G for any accum.
