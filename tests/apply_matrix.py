@@ -167,6 +167,23 @@ def check_global_norm(gn: np.float32, c: Sequence[np.ndarray]) -> None:
     assert np.isfinite(gn) and err <= eno.clip_norm_bound(e, n), (float(gn), math.sqrt(e), err, eno.clip_norm_bound(e, n))
 
 
+RESETS = ("materialized", "deferred", "stored")
+# What a deferred-reset test writes into the raw accumulators right after an apply, as fp32 bit patterns; None is
+# 1 + window.  A quiet NaN with a payload and -inf propagate into p, m, v and the norms if read; -0.0 survives only in
+# a tensor without a gradient that the first accumulate left unwritten; 3e38 overflows the loss-scaling test; the
+# smallest denormal and 1 + window change a sum they are added into once.
+POISON = (0x7FC0BEEF, 0xFF800000, 0x80000000, int(np.array(3.0e38, F32).view(np.uint32)), 0x00000001, None)
+PAD_BITS = 0x7FC0DEAD                 # the slab's padding: a NaN no kernel may read or write
+
+
+def poison_bits(tensor: int, window: int) -> int:
+    """The poison of tensor ``tensor`` after the apply that ends window ``window``, as a signed int32."""
+    v = POISON[(tensor + window) % len(POISON)]
+    if v is None:
+        v = int(np.array(1 + window, F32).view(np.uint32))
+    return int(np.array(v, np.uint32).view(np.int32))
+
+
 def trust_ratio_candidates(p: np.ndarray, u: np.ndarray) -> List[np.float32]:
     """LAMB's r = ||p|| / ||u|| with each norm rounded to fp32 once from its exact sum of squares: one value, or, for
     a sum within LAMB_TIE_REL of a rounding boundary, the values either side of it gives."""
@@ -205,6 +222,17 @@ class LockStep:
     gradients adds them into the accumulators and runs ``run([None] * T)``.  ``check`` then also compares the device
     counter, the lr in the stats of every micro-step, and the beta powers in their one home (the schedule block, or the
     loss-scaling block under loss scaling, the schedule block's then 0).
+
+    ``reset`` (table layout, N >= 2): how the accumulators get back to zero after an apply (RESETS).
+    "materialized" reads them through ``op.accum``, which stores a deferred reset's zeros after every micro-step.
+    "deferred" is the path a training loop takes: nothing calls ``gaccum_accum_materialize`` (a counter on the plan
+    checks it at every ``check``); the raw slab is compared only where it is defined, after a micro-step that did not
+    apply; right after an apply every tensor's raw accumulators are poisoned (POISON, rotated by tensor and window), so
+    a kernel that reads them, or leaves a tensor without a gradient unwritten, fails.  "stored" turns the mode off: the
+    raw slab holds +0.0 right after every apply.  Both write NaN into the slab's padding at construction; ``finish``
+    checks that nothing touched it and reads ``op.accum`` once.  A case without gradients runs its accumulates through
+    ``op.run`` and, at an apply, adds the gradients into the raw slab (mid-window, so defined) before ``run([None] *
+    T)``.  ``first_over_poison`` counts first accumulates that found a poisoned slab and a tensor without a gradient.
     """
 
     def __init__(self, man, variant: str, mode: str, layout: str = "table", dtype: str = "fp32", has_g: bool = True,
@@ -212,7 +240,7 @@ class LockStep:
                  nograd: Sequence[int] = (), zero: Sequence[int] = (), adapt_exclude: Optional[Sequence[str]] = None,
                  injected: bool = False, init: Optional[Dict[int, np.ndarray]] = None, tensor_norms: bool = False,
                  ls_cfg=LS_CFG, sched: Optional[Dict[str, float]] = None, global_step: int = 0,
-                 device_schedule: bool = False):
+                 device_schedule: bool = False, reset: str = "materialized"):
         import torch
         import gaccum_b200 as g
         from gaccum_b200.train_op import GaccumTrainOp, PackedTrainOp
@@ -257,6 +285,28 @@ class LockStep:
                                 sched=self.sched, global_step=self.g0)
         self.tracker = Ema(self._weights(), *ema) if ema is not None else None
         self.clipped = False                 # some window so far had a clip scale other than 1
+        assert reset in RESETS and (reset == "materialized" or (layout == "table" and N >= 2)), (reset, layout, N)
+        self.reset = reset
+        self.windows = 0                     # applies so far: the poison's rotation
+        self.poisoned = False                # the raw slab holds poison (the window's first accumulate is next)
+        self.first_over_poison = 0
+        self.materializes = 0                # calls of gaccum_accum_materialize ...
+        self.expected_materializes = 0       # ... and how many of them a test made on purpose
+        if reset != "materialized":
+            if reset == "stored":
+                self.op._set_deferred_reset(False)
+            assert self.op._deferred == (reset == "deferred")
+            plan, real = self.op.plan, self.op.plan.accum_materialize
+
+            def counted(*a):
+                self.materializes += 1
+                return real(*a)
+            plan.accum_materialize = counted
+            covered = np.zeros(self.op._accum.numel(), bool)
+            for o, (_, s) in zip(self.op.plan.offsets, man):
+                covered[o:o + int(np.prod(s))] = True
+            self.pad_idx = torch.from_numpy(np.flatnonzero(~covered)).cuda()
+            self.op._accum.view(torch.int32)[self.pad_idx] = np.array(PAD_BITS, np.uint32).view(np.int32).item()
 
     # -- inputs -----------------------------------------------------------------------------------------------------
     def _device(self, i: int, t):
@@ -312,12 +362,12 @@ class LockStep:
                         if t is not None:
                             p.grad.add_(t)
                     ran = op.step()
-                elif self.has_g:
+                elif self.has_g or (self.reset != "materialized" and not applied):
                     ran = op.run(dev)
                 else:
                     for i, t in enumerate(dev):                # what the accumulate kernel adds: the widened gradient
                         if t is not None:
-                            op.accum_view(i).add_(t.float())
+                            self.accum_view(i).add_(t.float())
                     ran = op.run([None] * len(dev))
             op.schedule_state()                                # raises if the device refused the launch
             assert ran == applied
@@ -338,8 +388,12 @@ class LockStep:
                     if t is not None:
                         p.grad.add_(t)
                 assert op.step() == applied
-        elif self.has_g:
+        elif self.has_g or (self.reset != "materialized" and not applied):
             assert op.run(dev) == applied
+        elif self.reset != "materialized":
+            # the apply's gradients go in through the accumulate kernel on the raw slab, which is defined mid-window
+            op.plan.accumulate(op._grad_table(dev), op._accum_ptr, op._stream())
+            assert op.run([None] * len(dev))
         else:
             op.accumulate_only(dev)
             if applied:
@@ -353,8 +407,69 @@ class LockStep:
                 self.ref.reduced = onp.Reduced(F32(st["global_norm"]), ratios)
             info = self.ref.run(host)
         assert info.applied == applied
+        if self.poisoned and any(x is None and n > 0 for x, n in zip(grads, self._sizes())):
+            self.first_over_poison += 1
+        self.poisoned = False
         self.check(info)
+        if applied:
+            self.windows += 1
+            if self.reset == "deferred":
+                self.poison()
         return applied
+
+    # -- the accumulators without materializing a deferred reset ------------------------------------------------------
+    def _sizes(self) -> List[int]:
+        return [int(np.prod(s)) for _, s in self.man]
+
+    def raw_accum(self):
+        """The accumulator slab as the kernels left it: ``op.accum`` unless a test of the deferred reset runs."""
+        return self.op.accum if self.reset == "materialized" else self.op._accum
+
+    def accum_view(self, i: int):
+        return self.op._view(self.raw_accum(), i)
+
+    def poison(self) -> None:
+        """Right after an apply of a deferred-reset op: POISON into every tensor's raw accumulators, on the op's
+        stream.  The slab is logically +0 until the window's first accumulate, which must not read it."""
+        torch = self.torch
+        with torch.no_grad():
+            for i in range(len(self.man)):
+                self.accum_view(i).view(torch.int32).fill_(poison_bits(i, self.windows))
+        self.poisoned = True
+
+    def set_reset(self, reset: str) -> None:
+        """Turn the op's deferred reset on ("deferred") or off ("stored") between micro-steps.  Turning it off
+        materializes first."""
+        assert reset in ("deferred", "stored") and self.reset != "materialized"
+        if self.op._deferred and reset == "stored":
+            self.expected_materializes += 1
+            self.poisoned = False
+        self.op._set_deferred_reset(reset == "deferred")
+        self.reset = reset
+
+    def read_accum(self) -> None:
+        """The op's own read of the accumulators (``op.accum``, which materializes a deferred reset) against the
+        oracle: every tensor element bit for bit, +0.0 right after an apply."""
+        self.expected_materializes += self.op._deferred
+        got = self._slab(self.op.accum)
+        assert self.materializes == self.expected_materializes
+        for i, a in enumerate(got):
+            assert _bits_equal(a, self.ref.accum[i]), f"accumulator of {self.man[i][0]} read through op.accum"
+        self.poisoned = False
+
+    def finish(self) -> None:
+        """The end of a case: no unplanned materialize ran, the padding is untouched, and one ``op.accum`` read
+        matches the oracle."""
+        if self.reset == "materialized":
+            return
+        assert self.materializes == self.expected_materializes
+        self.check_padding()
+        self.read_accum()
+        self.check_padding()
+
+    def check_padding(self) -> None:
+        pad = self.op._accum.view(self.torch.int32)[self.pad_idx].cpu().numpy()
+        assert (pad == np.array(PAD_BITS, np.uint32).view(np.int32)).all(), "a kernel wrote the slab's padding"
 
     def run(self, steps: int, inf_at: Optional[Tuple[int, int, int]] = None, sigma: float = 0.1) -> None:
         """``steps`` micro-steps; ``inf_at = (step, tensor, element)`` puts one inf into that gradient."""
@@ -386,8 +501,10 @@ class LockStep:
         torch, op, ref = self.torch, self.op, self.ref
         torch.cuda.synchronize()
         names = [n for n, _ in self.man]
-        for i, a in enumerate(self._slab(op.accum)):
-            assert _bits_equal(a, ref.accum[i]), f"accumulator of {names[i]}"
+        assert self.materializes == self.expected_materializes, "the accumulators were materialized"
+        if not (self.reset == "deferred" and info.applied):    # right after a deferred reset the slab is unspecified
+            for i, a in enumerate(self._slab(self.raw_accum())):
+                assert _bits_equal(a, ref.accum[i]), f"accumulator of {names[i]}"
         if info.applied and not self.skipped() and (self.mode in ("clip", "ls_clip")) and info.clip_scale != F32(1.0):
             self.clipped = True
         exact = self.injected or (self.variant != "lamb" and not self.clipped)

@@ -9,12 +9,17 @@ Each case trains a small model with tails, a multi-tile tensor, one element, a t
 zero-element tensor (CAP 1920: plus 300 tiny tensors) at N = 3 for ten micro-steps -- four applied windows.  Loss-scaled
 cases put one inf into a gradient in the middle of the third window, which is skipped; S grows once before that.  The
 train op and the oracle are compared after every micro-step (``LockStep.check``).
+
+The 288 table-layout keys also run with the deferred reset as a training loop runs it (``reset="deferred"``: no
+materialize, the raw accumulators poisoned after every apply, so every first accumulate finds a poisoned slab and a
+tensor without a gradient); those with gradients also run with the mode off (``reset="stored"``: the applies store
++0.0).
 """
 import zlib
 
 import pytest
 
-from apply_matrix import Case, LockStep, matrix_cases
+from apply_matrix import RESETS, Case, LockStep, matrix_cases
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -32,12 +37,20 @@ def _man(layout):
     return MAN + TINY if layout.startswith("t1920") else MAN
 
 
-@pytest.mark.parametrize("case", matrix_cases(), ids=lambda c: c.id)
-def test_apply_instantiation_matches_the_oracle(case: Case):
+def reset_cases():
+    """Every dispatch key with the accumulators read after every micro-step ("materialized"); every table-layout key
+    (the packed entry point ignores the mode) with the deferred reset as training runs it; and, with the mode off,
+    those with gradients (without, the applies launch the same kernels)."""
+    return [pytest.param(c, r, id=c.id if r == "materialized" else f"{c.id}-{r}") for r in RESETS for c in matrix_cases()
+            if r == "materialized" or (c.layout != "packed" and (r == "deferred" or c.has_g))]
+
+
+@pytest.mark.parametrize("case, reset", reset_cases())
+def test_apply_instantiation_matches_the_oracle(case: Case, reset):
     layout = "packed" if case.layout == "packed" else "table"
     dtype = case.layout.split("_")[-1] if layout == "table" else "fp32"
     run = LockStep(_man(case.layout), case.variant, case.mode, layout, dtype, case.has_g, EMA if case.ema else None,
-                   N=3, seed=zlib.crc32(case.id.encode()), nograd=NOGRAD)
+                   N=3, seed=zlib.crc32(case.id.encode()), nograd=NOGRAD, reset=reset)
     assert run.cap == {"packed": 0, "table": 256 if case.layout.startswith("t256") else 1920}[layout]
     ls = case.mode.startswith("ls_")
     run.run(STEPS, inf_at=INF_AT if ls else None)
@@ -46,6 +59,13 @@ def test_apply_instantiation_matches_the_oracle(case: Case):
         assert st["skipped_windows"] == 1 and not st["last_skipped"] and st["scale"] == 16.0   # grew to 32, halved once
     if case.ema:
         assert run.op.ema_state()["num_updates"] == (3 if ls else 4)
+    if reset == "deferred":
+        assert run.first_over_poison == 3          # after the applies at steps 0, 3 and 6
+    run.finish()
+
+
+def test_reset_case_count():
+    assert len(reset_cases()) == 336 + 288 + 144
 
 
 @pytest.mark.parametrize("num_updates", [False, True])

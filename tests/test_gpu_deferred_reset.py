@@ -6,9 +6,15 @@ Every case runs a deferred-reset op and a twin with the mode off side by side on
 for bit at every micro-step: parameters (and master weights), m, v, the stats block and the device state blocks, and
 -- at the steps a case reads them -- the accumulators through ``accum`` and ``accum_view``.  Reading the accumulators
 materializes a deferred reset, so the main loops read them only where no apply came since the last first accumulate,
-leaving the first accumulate to store the zeros of tensors without a gradient itself."""
+leaving the first accumulate to store the zeros of tensors without a gradient itself.
+
+Each case runs twice: once as above, and once with the deferred op's raw slab poisoned right after every apply
+(``Pair(poison=True)``; never the twin's), so that a launch or a read that should have materialized first, or a first
+accumulate that reads the slab, differs from the twin."""
 import numpy as np
 import pytest
+
+from apply_matrix import poison_bits
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -38,10 +44,10 @@ def _stats_bits(op):
 class Pair:
     """A deferred-reset GaccumTrainOp and its twin without the mode, built from the same parameters."""
 
-    def __init__(self, N, hp=None, dtype=torch.float32, seed=0, **kw):
+    def __init__(self, N, hp=None, dtype=torch.float32, seed=0, poison=False, **kw):
         from gaccum_b200 import _lib
         from gaccum_b200.train_op import GaccumTrainOp
-        self.N, self.dtype = N, dtype
+        self.N, self.dtype, self.poison, self.windows = N, dtype, poison, 0
         gen = torch.Generator(device="cuda").manual_seed(seed)
         init = [(torch.randn(s, device="cuda", generator=gen) * 0.02).to(dtype) for _, s in MAN]
         hp = hp if hp is not None else _lib.HParams.bert()
@@ -72,7 +78,18 @@ class Pair:
         a, b = self.op.run(g), self.twin.run(g)
         assert a == b
         self.i += 1
+        if a:
+            self.after_apply()
         return a
+
+    def after_apply(self):
+        """``poison``: the deferred op's raw accumulators, logically +0 until the window's first accumulate, get a
+        value per tensor that no correct launch reads (``apply_matrix.POISON``)."""
+        self.windows += 1
+        if self.poison and _next_is_first(self):
+            with torch.no_grad():
+                for i in range(len(MAN)):
+                    self.op._view(self.op._accum, i).view(torch.int32).fill_(poison_bits(i, self.windows))
 
     def check(self, what, accum=False):
         op, tw = self.op, self.twin
@@ -105,11 +122,15 @@ def _next_is_first(pair):
     return _lib.is_first_accumulate(pair.op._step if pair.op._sched_state is None else pair.op._cursor.step, pair.N)
 
 
+POISON = (False, True)
+
+
 @pytest.mark.parametrize("N", [2, 3, 4, 8])
 def test_clip_apply_matches_the_zero_storing_twin(N):
-    p = Pair(N, seed=N)
-    assert p.run_windows(3) == 3
-    p.check("end", accum=True)
+    for poison in POISON:
+        p = Pair(N, seed=N, poison=poison)
+        assert p.run_windows(3) == 3
+        p.check("end", accum=True)
 
 
 @pytest.mark.parametrize("read", [False, True])
@@ -119,22 +140,25 @@ def test_single_pass_apply_and_reads_right_after_an_apply(read):
     from gaccum_b200 import _lib
     hp = _lib.HParams.bert()
     hp.clip_norm = 0.0
-    p = Pair(3, hp=hp, seed=11)
-    p.run_windows(3, read_every_step=read)
+    for poison in POISON:
+        p = Pair(3, hp=hp, seed=11, poison=poison)
+        p.run_windows(3, read_every_step=read)
 
 
 def test_tf_adam_and_lamb():
     from gaccum_b200 import _lib
-    Pair(4, hp=_lib.HParams.tf_adam(), seed=5).run_windows(2)
-    Pair(3, hp=_lib.HParams.lamb(), seed=6).run_windows(3)
     hp = _lib.HParams.lamb()
     hp.clip_norm = 0.0
-    Pair(2, hp=hp, seed=7).run_windows(3)
+    for poison in POISON:
+        Pair(4, hp=_lib.HParams.tf_adam(), seed=5, poison=poison).run_windows(2)
+        Pair(3, hp=_lib.HParams.lamb(), seed=6, poison=poison).run_windows(3)
+        Pair(2, hp=hp, seed=7, poison=poison).run_windows(3)
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16])
 def test_16_bit_models(dtype):
-    Pair(3, dtype=dtype, seed=8).run_windows(3)
+    for poison in POISON:
+        Pair(3, dtype=dtype, seed=8, poison=poison).run_windows(3)
 
 
 @pytest.mark.parametrize("clip", [1.0, 0.0])
@@ -143,104 +167,117 @@ def test_loss_scale_skips(clip):
     from gaccum_b200 import _lib
     hp = _lib.HParams.bert()
     hp.clip_norm = clip
-    p = Pair(3, hp=hp, seed=9, loss_scale=_lib.LossScaleConfig(2.0 ** 8, 2.0, 2))
-    p.run_windows(1)
-    p.step(); p.step(inf_at=0); p.step()                 # the whole window is skipped
-    assert p.op.loss_scale_state()["last_skipped"]
-    p.check("skipped window")
-    p.run_windows(2)
-    assert p.op.loss_scale_state() == p.twin.loss_scale_state()
+    for poison in POISON:
+        p = Pair(3, hp=hp, seed=9, loss_scale=_lib.LossScaleConfig(2.0 ** 8, 2.0, 2), poison=poison)
+        p.run_windows(1)
+        p.step(); p.step(inf_at=0); p.step()             # the whole window is skipped
+        assert p.op.loss_scale_state()["last_skipped"]
+        p.check("skipped window")
+        p.run_windows(2)
+        assert p.op.loss_scale_state() == p.twin.loss_scale_state()
 
 
 def test_ema_and_lamb_with_ema():
     from gaccum_b200 import _lib
-    Pair(3, seed=12, ema=_lib.EmaConfig(0.99, True)).run_windows(3)
-    Pair(2, hp=_lib.HParams.lamb(), seed=13, ema=_lib.EmaConfig(0.9)).run_windows(2)
+    for poison in POISON:
+        Pair(3, seed=12, ema=_lib.EmaConfig(0.99, True), poison=poison).run_windows(3)
+        Pair(2, hp=_lib.HParams.lamb(), seed=13, ema=_lib.EmaConfig(0.9), poison=poison).run_windows(2)
 
 
 def test_device_schedule_with_refused_launches():
     from gaccum_b200 import _lib
     cfg = _lib.ScheduleConfig(1e-3, 1000, 5)
-    p = Pair(3, seed=14, device_schedule=cfg)
-    p.run_windows(2)
-    # right after an apply, an apply launched out of place (device at 7); then, mid-window, a first accumulate launched
-    # one step late (device at 11)
-    for extra, wrong in ((0, 9), (1, 10)):
-        for _ in range(extra):
-            p.step()
-        g = p.op._cursor.step
-        for op in (p.op, p.twin):
-            args = _lib.StepArgs(wrong, 3, 0, 0.0, 0.0, 0.0, 0.0)
-            op.plan.step(op._grad_table(p.grads()), op._param_ptrs, op._accum_ptr, op._m_ptr, op._v_ptr, args, op._stream())
-        torch.cuda.synchronize()
-        assert p.op._read_schedule()["refused"] and p.twin._read_schedule()["refused"]
-        p.check(f"refused launch at {wrong}, device at {g}", accum=True)
-        for op in (p.op, p.twin):
-            op.global_step = g                           # the documented recovery
-        p.run_windows(1)
-    p.check("end", accum=True)
+    for poison in POISON:
+        p = Pair(3, seed=14, device_schedule=cfg, poison=poison)
+        p.run_windows(2)
+        # right after an apply, an apply launched out of place (device at 7); then, mid-window, a first accumulate
+        # launched one step late (device at 11)
+        for extra, wrong in ((0, 9), (1, 10)):
+            for _ in range(extra):
+                p.step()
+            g = p.op._cursor.step
+            for op in (p.op, p.twin):
+                args = _lib.StepArgs(wrong, 3, 0, 0.0, 0.0, 0.0, 0.0)
+                op.plan.step(op._grad_table(p.grads()), op._param_ptrs, op._accum_ptr, op._m_ptr, op._v_ptr, args,
+                             op._stream())
+            torch.cuda.synchronize()
+            assert p.op._read_schedule()["refused"] and p.twin._read_schedule()["refused"]
+            p.check(f"refused launch at {wrong}, device at {g}", accum=True)
+            for op in (p.op, p.twin):
+                op.global_step = g                       # the documented recovery
+            p.run_windows(1)
+        p.check("end", accum=True)
 
 
 def test_branches_alone_and_global_step_reassignment():
-    p = Pair(3, seed=15)
-    p.run_windows(1)                                     # an apply just ran: the accumulators are logically zero
-    g = p.grads()
-    for op in (p.op, p.twin):
-        op.accumulate_only(g)
-    p.check("accumulate_only after an apply", accum=True)
-    p.run_windows(1)
-    g = p.grads()
-    for op in (p.op, p.twin):
-        op.apply_only(g)                                 # right after an apply
-    p.check("apply_only after an apply")
-    p.run_windows(1)
-    for op in (p.op, p.twin):
-        op.apply_only(None)
-    p.run_windows(1)
-    assert p.op.global_step == 13                        # right after the apply at 12
-    # mid-window (reads the accumulators); unchanged, an apply; an apply after an apply; unchanged, a first accumulate
-    for g_new in (14, 15, 18, 19):
+    for poison in POISON:
+        p = Pair(3, seed=15, poison=poison)
+        p.run_windows(1)                                 # an apply just ran: the accumulators are logically zero
+        g = p.grads()
         for op in (p.op, p.twin):
-            op.global_step = g_new
-        p.step()
-        p.check(f"global_step = {g_new}", accum=not _next_is_first(p))
-    p.run_windows(2)
+            op.accumulate_only(g)
+        p.check("accumulate_only after an apply", accum=True)
+        p.run_windows(1)
+        g = p.grads()
+        for op in (p.op, p.twin):
+            op.apply_only(g)                             # right after an apply
+        p.after_apply()
+        p.check("apply_only after an apply")
+        p.run_windows(1)
+        for op in (p.op, p.twin):
+            op.apply_only(None)
+        p.after_apply()
+        p.run_windows(1)
+        assert p.op.global_step == 13                    # right after the apply at 12
+        # mid-window (reads the accumulators); unchanged, an apply; an apply after an apply; unchanged, a first
+        # accumulate
+        for g_new in (14, 15, 18, 19):
+            for op in (p.op, p.twin):
+                op.global_step = g_new
+            p.step()
+            p.check(f"global_step = {g_new}", accum=not _next_is_first(p))
+        p.run_windows(2)
 
 
 @pytest.mark.parametrize("where", ["mid_window", "after_apply"])
 def test_checkpoint_round_trip(where):
-    p = Pair(4, seed=16)
-    p.run_windows(1)
-    if where == "mid_window":
-        p.step(); p.step()
-    sd_a, sd_b = p.op.state_dict(), p.twin.state_dict()
-    for k in sd_b:
-        _same(sd_a[k], sd_b[k], f"state_dict {k}")
-    # both restored into fresh ops whose slabs hold other values; the deferred one restores at a step right after one
-    # of its own applies
-    fresh = Pair(4, seed=17)
-    fresh.run_windows(1)
-    fresh.op.load_state_dict(sd_a)
-    fresh.twin.load_state_dict(sd_b)
-    fresh.gen, fresh.i = p.gen, p.i
-    fresh.check("restored", accum=True)
-    fresh.run_windows(2)
-    assert fresh.op.global_step == fresh.twin.global_step
+    for poison in POISON:
+        p = Pair(4, seed=16, poison=poison)
+        p.run_windows(1)
+        if where == "mid_window":
+            p.step(); p.step()
+        sd_a, sd_b = p.op.state_dict(), p.twin.state_dict()
+        for k in sd_b:
+            _same(sd_a[k], sd_b[k], f"state_dict {k}")
+        # both restored into fresh ops whose slabs hold other values; the deferred one restores at a step right after
+        # one of its own applies
+        fresh = Pair(4, seed=17, poison=poison)
+        fresh.run_windows(1)
+        fresh.op.load_state_dict(sd_a)
+        fresh.twin.load_state_dict(sd_b)
+        fresh.gen, fresh.i, fresh.windows = p.gen, p.i, p.windows
+        fresh.check("restored", accum=True)
+        fresh.run_windows(2)
+        assert fresh.op.global_step == fresh.twin.global_step
 
 
 def test_data_parallel_driver_on_one_rank():
     from gaccum_b200.distributed import DataParallelTrainOp
-    p = Pair(3, seed=18)
-    dp, dt = DataParallelTrainOp(p.op, None), DataParallelTrainOp(p.twin, None)
-    assert p.op._deferred                                # one rank: the driver delegates to the engine
-    for _ in range(7):
-        g = p.grads()
-        assert dp.run(g) == dt.run(g)
-        p.i += 1
-        p.check(f"dp step {p.i}", accum=not _next_is_first(p))
-    sa, sb = dp.state_dict(), dt.state_dict()
-    for k in sb:
-        _same(sa[k], sb[k], f"dp state_dict {k}")
+    for poison in POISON:
+        p = Pair(3, seed=18, poison=poison)
+        dp, dt = DataParallelTrainOp(p.op, None), DataParallelTrainOp(p.twin, None)
+        assert p.op._deferred                            # one rank: the driver delegates to the engine
+        for _ in range(7):
+            g = p.grads()
+            a = dp.run(g)
+            assert a == dt.run(g)
+            p.i += 1
+            if a:
+                p.after_apply()
+            p.check(f"dp step {p.i}", accum=not _next_is_first(p))
+        sa, sb = dp.state_dict(), dt.state_dict()
+        for k in sb:
+            _same(sa[k], sb[k], f"dp state_dict {k}")
 
 
 def test_a_plan_without_the_mode_stores_zeros_and_one_with_it_does_not():
@@ -266,7 +303,7 @@ def test_a_plan_without_the_mode_stores_zeros_and_one_with_it_does_not():
 def test_the_packed_entry_point_keeps_storing_zeros_on_a_deferred_plan():
     """gaccum_step_packed ignores the mode: its own slab (here beside the op's) gets the zeros from its applies."""
     from gaccum_b200 import _lib
-    p = Pair(2, seed=20)
+    p = Pair(2, seed=20, poison=True)
     plan, n = p.op.plan, p.op.plan.padded_size
     slabs = [torch.zeros(n, device="cuda") for _ in range(4)]
     gslab = torch.randn(n, device="cuda", generator=p.gen) * 0.05

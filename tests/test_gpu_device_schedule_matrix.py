@@ -21,7 +21,7 @@ import zlib
 import numpy as np
 import pytest
 
-from apply_matrix import LAYOUTS, MODES, VARIANTS, Case, _bits_equal, matrix_cases
+from apply_matrix import LAYOUTS, MODES, VARIANTS, Case, _bits_equal, matrix_cases, poison_bits
 from tensor_norms_oracle import assert_close, expected_norms
 from window_weight_oracle import WindowWeightLockStep
 
@@ -53,13 +53,13 @@ class Scheduled(WindowWeightLockStep):
     norms are checked against ``tensor_norms_oracle`` from the accumulators, gradients, W, S and weights around it."""
 
     def __init__(self, case: Case, seed: int, injected: bool = True, sched=SCHED, global_step: int = 0, n: int = N,
-                 device_schedule: bool = True, man=None):
+                 device_schedule: bool = True, man=None, reset: str = "materialized"):
         layout, dtype, m = _setup(case)
         man = m if man is None else man
         super().__init__(man, case.variant, case.mode, layout, dtype, case.has_g, EMA if case.ema else None, N=n,
                          seed=seed, nograd=NOGRAD if man is not None and len(man) > 5 else (), injected=injected,
                          lr_mult=[CYCLE[i % len(CYCLE)] for i in range(len(man))], tensor_norms=True, sched=sched,
-                         global_step=global_step, device_schedule=device_schedule)
+                         global_step=global_step, device_schedule=device_schedule, reset=reset)
         self.step_no = 0
 
     def step(self, grads, launch=None) -> bool:
@@ -67,7 +67,8 @@ class Scheduled(WindowWeightLockStep):
         if applied:
             host, _ = self.inputs(grads)
             S = F32(self.ref.scale) if self.ls else None
-            before = ([x.copy() for x in self._slab(self.op.accum)], [x.copy() for x in self._weights()], F32(self.ref.weight))
+            before = ([x.copy() for x in self._slab(self.raw_accum())], [x.copy() for x in self._weights()],
+                      F32(self.ref.weight))
         out = super().step(grads, launch)
         if applied:
             acc, w0, W = before
@@ -90,10 +91,15 @@ class Scheduled(WindowWeightLockStep):
 
 
 def _buffers(run):
-    """Every device buffer of the op's state, and the blocks it keeps, as host tensors."""
+    """Every device buffer of the op's state, and the blocks it keeps, as host tensors.  A test of the deferred reset
+    reads the raw accumulators, and only mid-window: right after an apply they are unspecified."""
+    from gaccum_b200 import _lib
     op = run.op
     torch.cuda.synchronize()
-    out = {"accum": op.accum, "m": op.m, "v": op.v, "sched": op._sched_state, "ww": run.ww,
+    accum = run.raw_accum()
+    if run.reset == "deferred" and _lib.is_first_accumulate(run.g_host, run.N):
+        accum = None
+    out = {"accum": accum, "m": op.m, "v": op.v, "sched": op._sched_state, "ww": run.ww,
            "norms": op.tensor_norms_tensor, "stats": torch.tensor(list(op.stats().values()), dtype=torch.float32)}
     out["weights"] = op.param_slab if run.layout == "packed" else (op.master if op.master is not None else None)
     for i, p in enumerate(op.params):
@@ -138,20 +144,31 @@ def test_case_count():
     assert len(matrix_cases()) == 336
 
 
-@pytest.mark.parametrize("case", matrix_cases(), ids=lambda c: c.id)
-def test_every_dispatch_key_matches_the_oracle(case: Case):
-    run = Scheduled(case, zlib.crc32(case.id.encode()) ^ 0x5C)
+# the table layouts again with the deferred reset as training runs it (the packed entry point ignores the mode)
+DISPATCH_KEYS = [pytest.param(c, "materialized", id=c.id) for c in matrix_cases()] + \
+    [pytest.param(c, "deferred", id=f"{c.id}-deferred") for c in matrix_cases() if c.layout != "packed"]
+
+
+@pytest.mark.parametrize("case, reset", DISPATCH_KEYS)
+def test_every_dispatch_key_matches_the_oracle(case: Case, reset):
+    run = Scheduled(case, zlib.crc32(case.id.encode()) ^ 0x5C, reset=reset)
     applies = sum(run.micro() for _ in range(STEPS))
     assert applies == 5
     if run.ls:
         assert run.op.loss_scale_state()["skipped_windows"] == 1
+    if reset == "deferred":
+        assert run.first_over_poison == 4                # after the applies at steps 0, 3, 6 and 9
+    run.finish()
 
 
 # ---- b. one window as a CUDA graph -------------------------------------------------------------------------------------
-def _capture(run, launches, weights=False):
+def _capture(run, launches, weights=False, poison=None):
     """Capture ``launches`` micro-steps of ``run.op`` over static gradient buffers; returns (graph, static buffers).
     ``weights``: each micro-step's weight add is captured too, from a static device scalar (the last entry of its
-    buffers), as a producer's would be; else the weights are added eagerly before each replay (``Scheduled.wstep``)."""
+    buffers), as a producer's would be; else the weights are added eagerly before each replay (``Scheduled.wstep``).
+    ``poison`` (a deferred-reset run): a T-entry int32 device tensor, copied into each tensor's raw accumulators right
+    after a captured apply, so every replay's first accumulate finds the values it held at that replay."""
+    from gaccum_b200 import _lib
     op = run.op
     _, dev = run.inputs(run.grads(0.1))
     static = [[None if t is None else torch.zeros_like(t) for t in dev] for _ in range(launches)]
@@ -172,6 +189,9 @@ def _capture(run, launches, weights=False):
                 op.step()
             else:
                 op.run(static[j][:len(op.params)])
+            if poison is not None and _lib.is_apply_step(run.g_host + j, run.N):
+                for i in range(len(op.params)):
+                    run.accum_view(i).view(torch.int32).copy_(poison[i])
     torch.cuda.synchronize()
     return graph, static
 
@@ -185,22 +205,31 @@ def _fill(static, dev, weight=None):
 
 
 GRAPH_KEYS = [(v, m, l, e) for v in VARIANTS for m in MODES for l in LAYOUTS for e in (False, True)]
+GRAPH_PARAMS = [pytest.param(*k, r, id=f"{k[0]}-{k[1]}-{k[2]}-{'ema' if k[3] else 'noema'}"
+                             + ("" if r == "materialized" else f"-{r}"))
+                for r in ("materialized", "deferred") for k in GRAPH_KEYS if r == "materialized" or k[2] != "packed"]
 
 
-@pytest.mark.parametrize("variant, mode, layout, ema", GRAPH_KEYS,
-                         ids=[f"{v}-{m}-{l}-{'ema' if e else 'noema'}" for v, m, l, e in GRAPH_KEYS])
-def test_one_window_replayed_matches_the_eager_run(variant, mode, layout, ema):
+@pytest.mark.parametrize("variant, mode, layout, ema, reset", GRAPH_PARAMS)
+def test_one_window_replayed_matches_the_eager_run(variant, mode, layout, ema, reset):
+    """``reset="deferred"``: the captured window starts with its apply, after which the graph copies a poison into the
+    raw accumulators; between replays that poison is set to values other than the eager twin's, so a first accumulate
+    that read it could not match the twin by reading the same garbage."""
     case = Case(variant, mode, True, layout, ema)
     seed = zlib.crc32(case.id.encode()) ^ 0x6A
-    eager, graphed = Scheduled(case, seed), Scheduled(case, seed)
+    eager, graphed = Scheduled(case, seed, reset=reset), Scheduled(case, seed, reset=reset)
     for _ in range(N):                                   # an eager window: every kernel loads before the capture
         eager.micro()
         graphed.micro()
     _assert_same(_buffers(eager), _buffers(graphed), "eager window")
-    graph, static = _capture(graphed, N, weights=True)
+    deferred = reset == "deferred"
+    poison = torch.zeros(len(graphed.man), dtype=torch.int32, device="cuda") if deferred else None
+    graph, static = _capture(graphed, N, weights=True, poison=poison)
     assert graphed.op.global_step == N                   # nothing ran during the capture
     windows = (STEPS + 2) // N - 1
     for w in range(windows):
+        if deferred:                                     # the eager twin's apply below poisons with window + 1
+            poison.copy_(torch.tensor([poison_bits(i, eager.windows + 1 + 3) for i in range(len(graphed.man))]))
         for j in range(N):
             s = eager.step_no
             S = F32(eager.ref.scale) if eager.ls else F32(1.0)
@@ -214,6 +243,11 @@ def test_one_window_replayed_matches_the_eager_run(variant, mode, layout, ema):
         graph.replay()
         _assert_same(_buffers(eager), _buffers(graphed), f"replay {w}")
     assert graphed.op.global_step == eager.g_host == N * (windows + 1)
+    if deferred:
+        assert eager.first_over_poison == windows + 1
+        assert graphed.materializes == 0
+        graphed.check_padding()
+        eager.finish()
 
 
 # ---- c. refusal and recovery -------------------------------------------------------------------------------------------
@@ -309,14 +343,20 @@ WRAP_KEYS = [("adamw", "noclip"), ("adamw", "clip"), ("lamb", "ls_clip")]
 WRAP_MAN = MAN[:5]
 
 
-@pytest.mark.parametrize("base", [2**31, 2**32], ids=["at_2_31", "at_2_32"])
-@pytest.mark.parametrize("n", [3, 4, 5])
-@pytest.mark.parametrize("variant, mode", WRAP_KEYS, ids=[f"{v}-{m}" for v, m in WRAP_KEYS])
-def test_the_int32_wrap(variant, mode, n, base):
+WRAP_PARAMS = [pytest.param(v, m, n, base, r, id=f"{v}-{m}-{n}-{bid}" + ("" if r == "materialized" else f"-{r}"))
+               for r in ("materialized", "deferred") for v, m in WRAP_KEYS for n in (3, 4, 5)
+               for base, bid in ((2**31, "at_2_31"), (2**32, "at_2_32"))]
+
+
+@pytest.mark.parametrize("variant, mode, n, base, reset", WRAP_PARAMS)
+def test_the_int32_wrap(variant, mode, n, base, reset):
+    """``reset="deferred"``: the window that straddles 2^31 is longer than N, and its first accumulate finds a poisoned
+    slab all the same."""
     case = Case(variant, mode, True, "t256_fp32", False)
     g0 = base - 2 * n
-    runs = [Scheduled(case, 17 + n, sched=WRAP_SCHED, global_step=g0, n=n, device_schedule=d, man=WRAP_MAN)
-            for d in (False, True)]
+    man = WRAP_MAN if reset == "materialized" else WRAP_MAN + [MAN[NOGRAD[0]]]     # + a tensor without a gradient
+    runs = [Scheduled(case, 17 + n, sched=WRAP_SCHED, global_step=g0, n=n, device_schedule=d, man=man,
+                      reset=reset) for d in (False, True)]
     applied = []
     for _ in range(4 * n):
         a = [r.micro() for r in runs]                 # each op against its own oracle, accumulators included
@@ -331,6 +371,10 @@ def test_the_int32_wrap(variant, mode, n, base):
     starts = [g0 + k for k, a in enumerate(applied) if a]
     gaps = set(np.diff(starts))
     assert gaps == ({n} if base == 2**32 or n == 4 else {n, n + 1})
+    for r in runs:
+        if reset == "deferred":
+            assert r.first_over_poison == sum(applied[:-1])
+        r.finish()
 
 
 def _assert_same_ops(runs):

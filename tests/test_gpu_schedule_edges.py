@@ -9,7 +9,13 @@ Shapes are derived from the GPU's SM count (``Schedule``), never hard-coded:
 * LAMB CTA ranges, with tensor boundaries on and one tile off CTA boundaries, a tensor across three or more CTAs,
   neighbours with alternating adaptation flags and the three cases of r = 1 (no adaptation, ||p|| = 0, ||u|| = 0);
 * three launches on one plan, which alternate between the two counter sets, are bit-identical.
+
+The pool-tile and LAMB cases run twice: reading the accumulators after every micro-step, and with the deferred reset
+as training runs it (``LockStep(reset="deferred")``), where the clip-apply discards its pool tiles' a' lines and LAMB
+its u lines from L2, and every first accumulate finds a poisoned slab.
 """
+import itertools
+
 import numpy as np
 import pytest
 
@@ -70,10 +76,20 @@ def _awkward(dtype):
     return man, views, {"nograd/kernel"}
 
 
-def _lockstep(man, views, nograd, variant, mode, dtype, has_g, ema, seed, N=2):
+RESETS = ("materialized", "deferred")
+
+
+def _lockstep(man, views, nograd, variant, mode, dtype, has_g, ema, seed, reset, N=2):
     names = [n for n, _ in man]
     return LockStep(man, variant, mode, dtype=dtype, has_g=has_g, ema=(0.9, True) if ema else None, N=N, seed=seed,
-                    views={names.index(n): o for n, o in views.items()}, nograd=[names.index(n) for n in nograd])
+                    views={names.index(n): o for n, o in views.items()}, nograd=[names.index(n) for n in nograd],
+                    reset=reset)
+
+
+def _finish(run):
+    if run.reset == "deferred":
+        assert run.first_over_poison > 0
+    run.finish()
 
 
 @pytest.mark.parametrize("dtype", ["fp32", "bf16"])
@@ -86,12 +102,14 @@ def test_awkward_tiles_in_the_pool(sched, has_g, ema, ls, dtype):
     aw, views, nograd = _awkward(dtype)
     man = [("lead/kernel", (lead * T,))] + aw
     assert sched.pool_lo(lead + 1, ema) == lead
-    run = _lockstep(man, views, nograd, "adamw", "ls_clip" if ls else "clip", dtype, has_g, ema, seed=3)
-    if ls:
-        run.run(5, inf_at=(1, 8, 3))                                # an inf in a 13-element pool tile
-        assert run.op.loss_scale_state()["skipped_windows"] == 1
-    else:
-        run.run(3)
+    for reset in RESETS:
+        run = _lockstep(man, views, nograd, "adamw", "ls_clip" if ls else "clip", dtype, has_g, ema, 3, reset)
+        if ls:
+            run.run(5, inf_at=(1, 8, 3))                            # an inf in a 13-element pool tile
+            assert run.op.loss_scale_state()["skipped_windows"] == 1
+        else:
+            run.run(3)
+        _finish(run)
 
 
 def _mirror(G, ema, dtype):
@@ -124,12 +142,14 @@ def test_unstashable_tiles_between_stashed_ones(sched, has_g, ema, dtype):
     G = sched.clip_groups(3 * sched.sms)
     man, views, nograd = _mirror(G, ema, dtype)
     ls = not has_g
-    run = _lockstep(man, views, nograd, "adamw", "ls_clip" if ls else "clip", dtype, has_g, ema, seed=4)
-    if ls:
-        run.run(5, inf_at=(1, 2, 5))                                # an inf in own tile j = 1 of group 1
-        assert run.op.loss_scale_state()["skipped_windows"] == 1
-    else:
-        run.run(3)
+    for reset in RESETS:
+        run = _lockstep(man, views, nograd, "adamw", "ls_clip" if ls else "clip", dtype, has_g, ema, 4, reset)
+        if ls:
+            run.run(5, inf_at=(1, 2, 5))                            # an inf in own tile j = 1 of group 1
+            assert run.op.loss_scale_state()["skipped_windows"] == 1
+        else:
+            run.run(3)
+        _finish(run)
 
 
 def _lamb_manifest(s: Schedule, nt: int):
@@ -163,9 +183,9 @@ def test_lamb_cta_ranges(sched, which):
     assert sum(-(-n // T) for _, (n,) in man) == nt
     names = [n for n, _ in man]
     zw, zu, empty = names.index("zero_w/kernel"), names.index("zero_u/bias"), names.index("empty/kernel")
-    for dtype, mode in (("fp32", "clip"), ("bf16", "ls_clip")):
+    for (dtype, mode), reset in itertools.product((("fp32", "clip"), ("bf16", "ls_clip")), RESETS):
         run = LockStep(man, "lamb", mode, dtype=dtype, N=2, seed=5 + which, zero=[zw], nograd=[zu],
-                       adapt_exclude=("noadapt",))
+                       adapt_exclude=("noadapt",), reset=reset)
         adapt = run.op.adapt
         assert adapt[zw] and adapt[zu] and adapt[empty]
         assert any(adapt[i] != adapt[i + 1] for i in range(4, len(man) - 1))
@@ -183,6 +203,7 @@ def test_lamb_cta_ranges(sched, which):
                         assert r[i] != np.float32(1.0), names[i]
                 window += 1
         assert window == 2
+        _finish(run)
 
 
 @pytest.mark.parametrize("variant", ["adamw", "lamb"])
