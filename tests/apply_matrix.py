@@ -6,8 +6,8 @@ with its composed oracle.
   this mapping covers exactly the apply kernels in the built library; ``tests/test_gpu_apply_matrix.py`` runs every case.
 * ``Schedule``: the tile and CTA bookkeeping of the clip-apply and the LAMB kernels, for tests that place tiles on their
   boundaries (``tests/test_gpu_schedule_edges.py``).
-* ``reference_op``: the expected values, composed from the existing oracles (``oracle_np.ReferenceTrainOp``,
-  ``LossScaledReferenceTrainOp``, ``LambReferenceTrainOp``); a 16-bit model is the fp32 oracle fed the upcast gradients.
+* ``reference_op``: the expected values of one dispatch key, ``composed_oracle.ComposedReferenceTrainOp``; a 16-bit
+  model is the fp32 oracle fed the upcast gradients.
 * ``LockStep``: one train op on the GPU and its oracle, stepped together and compared after every micro-step.
 
 Importable without torch (the inventory test runs without a GPU).  Test infrastructure only.
@@ -23,9 +23,8 @@ import numpy as np
 
 import exact_norm_oracle as eno
 import oracle_np as onp
+from composed_oracle import ComposedReferenceTrainOp, trust_ratio
 from ema_oracle import Ema
-from lamb_oracle import LambReferenceTrainOp, trust_ratio
-from loss_scale_oracle import LossScaledReferenceTrainOp
 
 F32 = np.float32
 
@@ -121,17 +120,14 @@ def oracle_hparams(variant: str, mode: str) -> onp.HParams:
 
 
 def reference_op(variant: str, mode: str, params, names, N: int, adapt: Optional[Sequence[bool]] = None,
-                 ls_cfg=LS_CFG, sched=SCHED, global_step: int = 0):
-    """The oracle of one dispatch key: ReferenceTrainOp, LossScaledReferenceTrainOp or LambReferenceTrainOp."""
+                 lr_mult: Optional[Sequence[float]] = None, window_weight: bool = False, ls_cfg=LS_CFG, sched=SCHED,
+                 global_step: int = 0) -> ComposedReferenceTrainOp:
+    """The oracle of one dispatch key, with learning-rate multipliers ``lr_mult`` and the window weight if given."""
     hp = oracle_hparams(variant, mode)
     params = [np.array(p, dtype=F32, copy=True) for p in params]
-    ls = mode.startswith("ls_")
-    lskw = dict(initial_scale=ls_cfg[0], multiplier=ls_cfg[1], growth_interval=ls_cfg[2]) if ls else {}
-    if variant == "lamb":
-        return LambReferenceTrainOp(params, names, hp, N, adapt=adapt, **lskw, **sched, global_step=global_step)
-    if ls:
-        return LossScaledReferenceTrainOp(params, names, hp, N, **lskw, **sched, global_step=global_step)
-    return onp.ReferenceTrainOp(params, names, hp, N, **sched, global_step=global_step)
+    lskw = dict(initial_scale=ls_cfg[0], multiplier=ls_cfg[1], growth_interval=ls_cfg[2]) if mode.startswith("ls_") else {}
+    return ComposedReferenceTrainOp(params, names, hp, N, adapt=adapt, lr_mult=lr_mult, window_weight=window_weight,
+                                    **lskw, **sched, global_step=global_step)
 
 
 def rel_err(x, ref) -> float:
@@ -233,6 +229,12 @@ class LockStep:
     checks that nothing touched it and reads ``op.accum`` once.  A case without gradients runs its accumulates through
     ``op.run`` and, at an apply, adds the gradients into the raw slab (mid-window, so defined) before ``run([None] *
     T)``.  ``first_over_poison`` counts first accumulates that found a poisoned slab and a tensor without a gradient.
+
+    ``lr_mult``: the plan gets the learning-rate table before its first compute call (``Plan.set_lr_multipliers``, what
+    the train ops' ``lr_multipliers`` argument does).  ``window_weight``: the plan divides each window by W
+    (``Plan.set_window_weight`` on a zeroed 16-byte block ``ww``, what the train ops' ``window_weight=True`` does);
+    ``wstep(grads, w)`` adds w into the device W (an fp32 add on the stream) and into the oracle's, then steps both, and
+    ``check`` also compares W and last_weight exactly.
     """
 
     def __init__(self, man, variant: str, mode: str, layout: str = "table", dtype: str = "fp32", has_g: bool = True,
@@ -240,7 +242,8 @@ class LockStep:
                  nograd: Sequence[int] = (), zero: Sequence[int] = (), adapt_exclude: Optional[Sequence[str]] = None,
                  injected: bool = False, init: Optional[Dict[int, np.ndarray]] = None, tensor_norms: bool = False,
                  ls_cfg=LS_CFG, sched: Optional[Dict[str, float]] = None, global_step: int = 0,
-                 device_schedule: bool = False, reset: str = "materialized"):
+                 device_schedule: bool = False, reset: str = "materialized", lr_mult: Optional[Sequence[float]] = None,
+                 window_weight: bool = False):
         import torch
         import gaccum_b200 as g
         from gaccum_b200.train_op import GaccumTrainOp, PackedTrainOp
@@ -281,8 +284,10 @@ class LockStep:
             self.op = GaccumTrainOp([self._device(i, p) for i, p in enumerate(params)], names, hp, N, lr_fn, **kw)
         self.cap = 0 if layout == "packed" else (256 if len(man) <= 256 else 1920)
         adapt = self.op.adapt if variant == "lamb" else None
-        self.ref = reference_op(variant, mode, [p.float().numpy() for p in params], names, N, adapt=adapt, ls_cfg=ls_cfg,
-                                sched=self.sched, global_step=self.g0)
+        lr_mult = None if lr_mult is None else np.asarray(lr_mult, F32)
+        self.ref = reference_op(variant, mode, [p.float().numpy() for p in params], names, N, adapt=adapt,
+                                lr_mult=lr_mult, window_weight=window_weight, ls_cfg=ls_cfg, sched=self.sched,
+                                global_step=self.g0)
         self.tracker = Ema(self._weights(), *ema) if ema is not None else None
         self.clipped = False                 # some window so far had a clip scale other than 1
         assert reset in RESETS and (reset == "materialized" or (layout == "table" and N >= 2)), (reset, layout, N)
@@ -307,6 +312,12 @@ class LockStep:
                 covered[o:o + int(np.prod(s))] = True
             self.pad_idx = torch.from_numpy(np.flatnonzero(~covered)).cuda()
             self.op._accum.view(torch.int32)[self.pad_idx] = np.array(PAD_BITS, np.uint32).view(np.int32).item()
+        if lr_mult is not None:
+            self.op.plan.set_lr_multipliers(lr_mult)
+        self.ww = None
+        if window_weight:
+            self.ww = torch.zeros(4, dtype=torch.float32, device="cuda")
+            self.op.plan.set_window_weight(self.ww.data_ptr())
 
     # -- inputs -----------------------------------------------------------------------------------------------------
     def _device(self, i: int, t):
@@ -342,6 +353,13 @@ class LockStep:
             host.append(t.float().numpy())                                   # ... what the oracle sees: their upcast
             dev.append(self._device(i, t))
         return host, dev
+
+    def wstep(self, grads, w, launch=None) -> bool:
+        """``step`` with the micro-batch's weight w added into the device W and the oracle's first."""
+        self.ref.add_weight(w)
+        with self.torch.no_grad():
+            self.ww[0].add_(float(w))
+        return self.step(grads, launch)
 
     def step(self, grads, launch=None) -> bool:
         """One micro-step of the op and its oracle, then ``check``.  ``launch(dev)``, if given, runs the op's micro-step
@@ -495,7 +513,7 @@ class LockStep:
         return out
 
     def skipped(self) -> bool:
-        return bool(getattr(self.ref, "last_skipped", False))
+        return bool(self.ref.last_skipped)
 
     def check(self, info) -> None:
         torch, op, ref = self.torch, self.op, self.ref
@@ -587,3 +605,7 @@ class LockStep:
                 assert _bits_equal(e, self.tracker.avg[i]), f"average of {names[i]}"
             es = op.ema_state()
             assert es["num_updates"] == self.tracker.num_updates and F32(es["decay"]) == self.tracker.decay
+        if self.ww is not None:
+            got = self.ww[:2].cpu().numpy()
+            assert got[0].tobytes() == F32(ref.weight).tobytes(), (got[0], ref.weight)
+            assert got[1].tobytes() == F32(ref.last_weight).tobytes(), (got[1], ref.last_weight)

@@ -7,8 +7,8 @@ op per TF op -- one numpy ufunc with ``dtype=float32`` each:
     e = e - (e - p) * c
 
 once per APPLIED window, after the update, on every tensor.  ``EmaReferenceTrainOp`` layers it on any reference train op
-of this repository (``oracle_np.ReferenceTrainOp``, ``LossScaledReferenceTrainOp``, ``LambReferenceTrainOp``, the C
-oracle): it averages the reference's parameters whenever a step applied and loss scaling did not skip its window.
+of this repository (``oracle_np.ReferenceTrainOp``, ``composed_oracle.ComposedReferenceTrainOp``, the C oracle): it
+averages the reference's parameters whenever a step applied and loss scaling did not skip its window.
 """
 from typing import List, Sequence, Tuple
 

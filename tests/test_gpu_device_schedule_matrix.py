@@ -21,9 +21,8 @@ import zlib
 import numpy as np
 import pytest
 
-from apply_matrix import LAYOUTS, MODES, VARIANTS, Case, _bits_equal, matrix_cases, poison_bits
+from apply_matrix import LAYOUTS, MODES, VARIANTS, Case, LockStep, _bits_equal, matrix_cases, poison_bits
 from tensor_norms_oracle import assert_close, expected_norms
-from window_weight_oracle import WindowWeightLockStep
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -48,8 +47,8 @@ def _setup(case: Case):
     return layout, dtype, (MAN + TINY if case.layout.startswith("t1920") else MAN)
 
 
-class Scheduled(WindowWeightLockStep):
-    """A device-scheduled ``WindowWeightLockStep`` with learning-rate multipliers and per-tensor norms; every apply's
+class Scheduled(LockStep):
+    """A device-scheduled ``LockStep`` with learning-rate multipliers, window weights and per-tensor norms; every apply's
     norms are checked against ``tensor_norms_oracle`` from the accumulators, gradients, W, S and weights around it."""
 
     def __init__(self, case: Case, seed: int, injected: bool = True, sched=SCHED, global_step: int = 0, n: int = N,
@@ -58,8 +57,8 @@ class Scheduled(WindowWeightLockStep):
         man = m if man is None else man
         super().__init__(man, case.variant, case.mode, layout, dtype, case.has_g, EMA if case.ema else None, N=n,
                          seed=seed, nograd=NOGRAD if man is not None and len(man) > 5 else (), injected=injected,
-                         lr_mult=[CYCLE[i % len(CYCLE)] for i in range(len(man))], tensor_norms=True, sched=sched,
-                         global_step=global_step, device_schedule=device_schedule, reset=reset)
+                         lr_mult=[CYCLE[i % len(CYCLE)] for i in range(len(man))], window_weight=True, tensor_norms=True,
+                         sched=sched, global_step=global_step, device_schedule=device_schedule, reset=reset)
         self.step_no = 0
 
     def step(self, grads, launch=None) -> bool:
@@ -82,12 +81,6 @@ class Scheduled(WindowWeightLockStep):
         self.step_no += 1
         inf = INF_AT[1:] if self.ls and s == INF_AT[0] else None
         return self.wstep(self.grads(0.1, inf), WEIGHTS[s % len(WEIGHTS)], launch)
-
-    def wstep(self, grads, w, launch=None) -> bool:
-        self.ref.add_weight(w)
-        with torch.no_grad():
-            self.ww[0].add_(float(w))
-        return self.step(grads, launch)
 
 
 def _buffers(run):

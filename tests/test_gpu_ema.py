@@ -15,8 +15,8 @@ import pytest
 import oracle_c
 import oracle_np as onp
 from common import make_params, rel_err
+from composed_oracle import ComposedReferenceTrainOp
 from ema_oracle import Ema, EmaReferenceTrainOp, ema_coefficients
-from lamb_oracle import LambReferenceTrainOp
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -145,7 +145,8 @@ def test_ema_follows_the_oracle_trajectory(variant, num_updates):
     params = _params(MAN, 2)
     names = [n for n, _ in MAN]
     if variant == "lamb":
-        ref = LambReferenceTrainOp([x.copy() for x in params], names, onp.HParams(variant=2, clip_norm=clip), N, **SCHED)
+        ref = ComposedReferenceTrainOp([x.copy() for x in params], names, onp.HParams(variant=2, clip_norm=clip), N,
+                                       **SCHED)
     else:
         hpo = onp.HParams.bert() if variant == "adamw" else onp.HParams.tf_adam()
         ref = onp.ReferenceTrainOp([x.copy() for x in params], names, hpo, N, **SCHED)

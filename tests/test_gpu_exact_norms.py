@@ -5,7 +5,7 @@ a. Every dispatch key that clips or runs LAMB (224 cases), in ``LockStep``'s inj
    kernel's global norm and trust ratios, so p, m, v, the master weights, the model copy, the EMA and the clip scale
    are compared bit for bit in every window, clipped ones included; gn is held to the exact sum of the window's c
    within the derived bound, and r to the ratio of the correctly rounded norms.  On the apply matrix's model, and
-   with mixed window weights and learning-rate multipliers (``WindowWeightLockStep``).
+   with mixed window weights and learning-rate multipliers.
 b. Known answers: c (and the first window's p) in {+-1, +-2, +-3} * 2^-j, so every partial sum in every order is exact:
    gn and the per-tensor gradient and weight norms must equal the norms of the exact sums bit for bit, and every
    element counts (one dropped or counted twice changes the integer sum, and sqrtf tells the two apart).  Unaligned
@@ -24,7 +24,6 @@ import pytest
 import exact_norm_oracle as eno
 import oracle_np as onp
 from apply_matrix import Case, LockStep, Schedule, matrix_cases
-from window_weight_oracle import WindowWeightLockStep
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -72,9 +71,9 @@ def test_clipped_and_lamb_windows_are_bit_exact(case: Case):
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c.id)
 def test_weighted_windows_with_lr_multipliers_are_bit_exact(case: Case):
     layout, dtype, man = _setup(case)
-    run = WindowWeightLockStep(man, case.variant, case.mode, layout, dtype, case.has_g, EMA if case.ema else None, N=3,
-                               seed=zlib.crc32(case.id.encode()) ^ 3, nograd=NOGRAD, injected=True,
-                               lr_mult=[CYCLE[i % len(CYCLE)] for i in range(len(man))])
+    run = LockStep(man, case.variant, case.mode, layout, dtype, case.has_g, EMA if case.ema else None, N=3,
+                   seed=zlib.crc32(case.id.encode()) ^ 3, nograd=NOGRAD, injected=True,
+                   lr_mult=[CYCLE[i % len(CYCLE)] for i in range(len(man))], window_weight=True)
     ls = case.mode.startswith("ls_")
     for s in range(STEPS):
         run.wstep(run.grads(0.1, INF_AT[1:] if ls and s == INF_AT[0] else None), WEIGHTS[s % len(WEIGHTS)])

@@ -1,6 +1,6 @@
 """The LAMB apply step on the GPU (include/gaccum.h, GACCUM_LAMB; csrc/gaccum_lamb.cuh).
 
-* Trajectories against the numpy oracle (tests/lamb_oracle.py): p within 1e-5; m / v as the AdamWeightDecay parity
+* Trajectories against the numpy oracle (tests/composed_oracle.py): p within 1e-5; m / v as the AdamWeightDecay parity
   tests hold them (bit-exact without clipping); the accumulators +0; the trust ratios within 1e-6.
 * Determinism: p and the ratios are bit-identical over repeated launches and CUDA-graph replays.
 * Layout: one 30522 x 1024 tensor, 1920 tiny tensors, unaligned views, the packed entry point, full-size BERT-Small.
@@ -12,7 +12,7 @@ import pytest
 
 import oracle_np as onp
 from common import make_params, rel_err
-from lamb_oracle import LambReferenceTrainOp
+from composed_oracle import ComposedReferenceTrainOp
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -60,8 +60,8 @@ def _op(man, params, hp, N, dtype=torch.float32, **kw):
 
 
 def _ref(man, params, hp, N, **kw):
-    return LambReferenceTrainOp([p.copy() for p in params], [n for n, _ in man], hp, N,
-                                adapt_exclude=kw.pop("adapt_exclude", ADAPT_EXCLUDE), **SCHED, **kw)
+    return ComposedReferenceTrainOp([p.copy() for p in params], [n for n, _ in man], hp, N,
+                                    adapt_exclude=kw.pop("adapt_exclude", ADAPT_EXCLUDE), **SCHED, **kw)
 
 
 def _grads(man, rng, sigma=0.1, nograd=NOGRAD):
@@ -267,7 +267,7 @@ def test_fullsize_bert_small_window():
     grads = [[rng.normal(0, 1e-3, s).astype(np.float32) for _, s in man] for _ in range(4)]
     hp, hpo = _hp(1.0)
     op = _op(man, params, hp, 4, adapt_exclude=None, global_step=1)
-    ref = LambReferenceTrainOp([p.copy() for p in params], [n for n, _ in man], hpo, 4, global_step=1, **SCHED)
+    ref = ComposedReferenceTrainOp([p.copy() for p in params], [n for n, _ in man], hpo, 4, global_step=1, **SCHED)
     for gr in grads:
         op.run(_cuda(gr)); ref.run(gr)
     torch.cuda.synchronize()
@@ -381,8 +381,8 @@ def test_create_optimizer_with_optimizer_type_lamb(monkeypatch):
     tv = [graph.add_variable(n, torch.from_numpy(p.copy()).cuda()) for (n, _), p in zip(man, params)]
     train_op = opt.create_optimizer(None, 1e-3, 50, 3, False)
     assert isinstance(train_op.optimizer, opt.LAMBOptimizer)
-    ref = LambReferenceTrainOp([p.copy() for p in params], [n for n, _ in man], onp.HParams(variant=2), 2,
-                               init_lr=1e-3, num_train_steps=50, num_warmup_steps=3)
+    ref = ComposedReferenceTrainOp([p.copy() for p in params], [n for n, _ in man], onp.HParams(variant=2), 2,
+                                   init_lr=1e-3, num_train_steps=50, num_warmup_steps=3)
     assert train_op.engine.adapt == ref.adapt == [True, False, False]
     rng = np.random.default_rng(22)
     for _ in range(9):

@@ -35,8 +35,8 @@ import pytest
 import exact_norm_oracle as eno
 import oracle_np as onp
 from apply_matrix import LAMB_TIE_REL, LS_CFG, SCHED, oracle_hparams, reference_op
+from composed_oracle import trust_ratio
 from ema_oracle import Ema
-from lamb_oracle import trust_ratio
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu

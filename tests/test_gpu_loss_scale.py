@@ -4,7 +4,7 @@
   scaling fed g: p, m, v, the accumulators, gn and the clip scale, growth events included.
 * A window in which a gradient overflows -- at its first micro-step, a middle one or the apply step; in a stashed or a
   pool tile of the clip kernel, a vector body, a scalar tail or an unaligned view -- leaves p, m and v unchanged bit for
-  bit, zeroes the accumulators and backs S off; later windows match the numpy oracle (tests/loss_scale_oracle.py).
+  bit, zeroes the accumulators and backs S off; later windows match the numpy oracle (tests/composed_oracle.py).
 """
 import os
 import socket
@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 
 import oracle_np as onp
-from loss_scale_oracle import LossScaledReferenceTrainOp
+from composed_oracle import ComposedReferenceTrainOp
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -172,7 +172,7 @@ def test_overflowed_window_is_skipped(kind, when, where):
     params = _params(BIG, 3)
     cfg = dict(initial_scale=2.0 ** 10, multiplier=2.0, growth_interval=1000)
     op = _gaccum_op(BIG, params, hp, N, g.LossScaleConfig(cfg["initial_scale"], cfg["multiplier"], cfg["growth_interval"]))
-    ref = LossScaledReferenceTrainOp([p.copy() for p in params], [n for n, _ in BIG], hp_o, N, constant_lr=LR, **cfg)
+    ref = ComposedReferenceTrainOp([p.copy() for p in params], [n for n, _ in BIG], hp_o, N, constant_lr=LR, **cfg)
     ubuf = torch.zeros(1100, device="cuda")
     rng = np.random.default_rng(4)
     t_i, e_i = WHERE[where]
@@ -215,8 +215,8 @@ def test_squared_sum_overflow_skips_only_with_clipping(variant_b):
         hp, hp_o = _hp(variant_b, clip)
         params = _params(MAN, 5)
         op = _gaccum_op(MAN, params, hp, 1, g.LossScaleConfig(1.0, 2.0, 100))
-        ref = LossScaledReferenceTrainOp([p.copy() for p in params], [n for n, _ in MAN], hp_o, 1, constant_lr=LR,
-                                         initial_scale=1.0, multiplier=2.0, growth_interval=100)
+        ref = ComposedReferenceTrainOp([p.copy() for p in params], [n for n, _ in MAN], hp_o, 1, constant_lr=LR,
+                                       initial_scale=1.0, multiplier=2.0, growth_interval=100)
         rng = np.random.default_rng(6)
         for step in range(2):                    # (with clipping off, v = inf afterwards: later steps would make NaNs)
             grads = [rng.normal(0, 0.1, s).astype(np.float32) for _, s in MAN]
@@ -249,7 +249,7 @@ def test_random_trajectories_with_overflows_match_the_oracle(seed):
     cfg = dict(initial_scale=2.0 ** int(rng.integers(0, 20)), multiplier=2.0 ** int(rng.integers(1, 3)),
                growth_interval=int(rng.integers(1, 4)))
     op = _gaccum_op(MAN, params, hp, N, g.LossScaleConfig(cfg["initial_scale"], cfg["multiplier"], cfg["growth_interval"]))
-    ref = LossScaledReferenceTrainOp([p.copy() for p in params], [n for n, _ in MAN], hp_o, N, constant_lr=LR, **cfg)
+    ref = ComposedReferenceTrainOp([p.copy() for p in params], [n for n, _ in MAN], hp_o, N, constant_lr=LR, **cfg)
     for step in range(8 * N + 2):
         # small gradients: gn < 1, so the clip scale is exactly 1 on both sides and every value compares bit for bit
         grads = [(rng.normal(0, 1e-5, s) * np.float32(ref.scale)).astype(np.float32) for _, s in MAN]

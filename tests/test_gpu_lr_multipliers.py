@@ -1,7 +1,7 @@
 """Per-tensor learning-rate multipliers on the GPU (include/gaccum.h, gaccum_plan_set_lr_multipliers).
 
 * Every dispatch key (tests/apply_matrix.py: 336 cases, all 120 apply instantiations) with a table holding 0, 1, a value
-  below 1 and one above 1, against the composed oracle (tests/lr_mult_oracle.py) after every micro-step; loss-scaled
+  below 1 and one above 1, against the composed oracle (tests/composed_oracle.py) after every micro-step; loss-scaled
   cases go through one overflowed window.
 * Oracle-free identities, bit for bit, for every variant x mode: a table of ones is a plan without the call; a uniform m
   is the run whose lr_fn returns fp32(lr * m) (stats.lr aside); a multiplier of 0 freezes that tensor's weights (and a
@@ -16,9 +16,9 @@ import numpy as np
 import pytest
 
 import oracle_np as onp
-from apply_matrix import Case, matrix_cases
+from apply_matrix import Case, LockStep, matrix_cases
 from common import make_params, rel_err
-from lr_mult_oracle import LrMultLockStep, LrMultReferenceTrainOp
+from composed_oracle import ComposedReferenceTrainOp
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -44,8 +44,8 @@ def test_apply_instantiation_with_a_table_matches_the_oracle(case: Case):
     layout = "packed" if case.layout == "packed" else "table"
     dtype = case.layout.split("_")[-1] if layout == "table" else "fp32"
     man = MAN + TINY if case.layout.startswith("t1920") else MAN
-    run = LrMultLockStep(man, case.variant, case.mode, layout, dtype, case.has_g, EMA if case.ema else None, N=3,
-                         seed=zlib.crc32(case.id.encode()), nograd=NOGRAD, lr_mult=_table(len(man)))
+    run = LockStep(man, case.variant, case.mode, layout, dtype, case.has_g, EMA if case.ema else None, N=3,
+                   seed=zlib.crc32(case.id.encode()), nograd=NOGRAD, lr_mult=_table(len(man)))
     ls = case.mode.startswith("ls_")
     run.run(STEPS, inf_at=INF_AT if ls else None)
     if ls:
@@ -281,8 +281,8 @@ def test_create_optimizer_with_layerwise_lr_decay(monkeypatch):
     expect = [0.8 ** 5 if "/embeddings/" in n else
               next((0.8 ** (4 - i) for i in range(3) if f"encoder/layer_{i}/" in n), 1.0) for n in names]
     assert np.array_equal(train_op.engine.lr_multipliers, np.array(expect, F32))
-    ref = LrMultReferenceTrainOp([p.copy() for p in params], names, onp.HParams.bert(), 2, lr_mult=expect,
-                                 init_lr=1e-3, num_train_steps=50, num_warmup_steps=3)
+    ref = ComposedReferenceTrainOp([p.copy() for p in params], names, onp.HParams.bert(), 2, lr_mult=expect,
+                                   init_lr=1e-3, num_train_steps=50, num_warmup_steps=3)
     rng = np.random.default_rng(14)
     for _ in range(9):
         gr = [rng.normal(0, 0.1, s).astype(F32) for _, s in man]
@@ -304,9 +304,9 @@ def test_apply_gradients_takes_the_table():
     o = opt.AdamWeightDecayOptimizer(1e-2, weight_decay_rate=0.01,
                                      exclude_from_weight_decay=["LayerNorm", "layer_norm", "bias"])
     o.lr_multipliers = table
-    ref = LrMultReferenceTrainOp([p.copy() for p in params], [n for n, _ in man],
-                                 onp.HParams(weight_decay_rate=0.01, clip_norm=0.0), 1, lr_mult=[0.25, 0.5, 1.0],
-                                 constant_lr=1e-2)
+    ref = ComposedReferenceTrainOp([p.copy() for p in params], [n for n, _ in man],
+                                   onp.HParams(weight_decay_rate=0.01, clip_norm=0.0), 1, lr_mult=[0.25, 0.5, 1.0],
+                                   constant_lr=1e-2)
     rng = np.random.default_rng(16)
     for _ in range(3):
         gr = [rng.normal(0, 0.1, s).astype(F32) for _, s in man]

@@ -3,7 +3,7 @@
 * Every dispatch key (tests/apply_matrix.py: 336 cases, all 120 apply instantiations): a weight of 1 per micro-step is
   the unweighted run bit for bit (p, m, v, accumulators, stats, EMA, trust ratios, loss-scaling block), and mixed
   integer weights whose totals are not powers of two, with learning-rate multipliers on, match the composed oracle
-  (tests/window_weight_oracle.py) after every micro-step.
+  (tests/composed_oracle.py) after every micro-step.
 * A uniform power-of-two weight k with gradients scaled by k is the unweighted run, bit for bit.
 * The property the feature exists for: one weighted window over micro-batches with different numbers of valid tokens is
   one step on the concatenated batch with a per-token-mean loss; the unweighted window is not.
@@ -15,9 +15,7 @@ import zlib
 import numpy as np
 import pytest
 
-from apply_matrix import Case, matrix_cases
-from lr_mult_oracle import LrMultLockStep
-from window_weight_oracle import WindowWeightLockStep
+from apply_matrix import Case, LockStep, matrix_cases
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -72,10 +70,10 @@ def _assert_same_state(a, b):
 def test_weights_of_one_are_the_unweighted_run(case: Case):
     layout, dtype, man = _setup(case)
     seed = zlib.crc32(case.id.encode())
-    kw = dict(N=N, seed=seed, nograd=NOGRAD)
+    kw = dict(N=N, seed=seed, nograd=NOGRAD, lr_mult=np.ones(len(man), F32))
     ema = EMA if case.ema else None
-    a = WindowWeightLockStep(man, case.variant, case.mode, layout, dtype, case.has_g, ema, **kw)
-    b = LrMultLockStep(man, case.variant, case.mode, layout, dtype, case.has_g, ema, lr_mult=np.ones(len(man), F32), **kw)
+    a = LockStep(man, case.variant, case.mode, layout, dtype, case.has_g, ema, window_weight=True, **kw)
+    b = LockStep(man, case.variant, case.mode, layout, dtype, case.has_g, ema, **kw)
     ls = case.mode.startswith("ls_")
     for s in range(STEPS):
         gr = a.grads(0.1, INF_AT[1:] if ls and s == INF_AT[0] else None)
@@ -91,9 +89,9 @@ def test_weights_of_one_are_the_unweighted_run(case: Case):
 @pytest.mark.parametrize("case", matrix_cases(), ids=lambda c: c.id)
 def test_mixed_weights_match_the_oracle(case: Case):
     layout, dtype, man = _setup(case)
-    run = WindowWeightLockStep(man, case.variant, case.mode, layout, dtype, case.has_g, EMA if case.ema else None, N=N,
-                               seed=zlib.crc32(case.id.encode()) ^ 1, nograd=NOGRAD,
-                               lr_mult=[CYCLE[i % len(CYCLE)] for i in range(len(man))])
+    run = LockStep(man, case.variant, case.mode, layout, dtype, case.has_g, EMA if case.ema else None, N=N,
+                   seed=zlib.crc32(case.id.encode()) ^ 1, nograd=NOGRAD,
+                   lr_mult=[CYCLE[i % len(CYCLE)] for i in range(len(man))], window_weight=True)
     ls = case.mode.startswith("ls_")
     for s in range(STEPS):
         run.wstep(run.grads(0.1, INF_AT[1:] if ls and s == INF_AT[0] else None), WEIGHTS[s % len(WEIGHTS)])
@@ -354,7 +352,8 @@ POW2_STEPS = [(4.0, 0.1), (32.0, 0.1), (32.0, 0.1), (2.0 ** -127, 1e-30), (2.0 *
                                                    ("adamw", "clip", "packed"), ("adam", "ls_clip", "table"),
                                                    ("lamb", "clip", "table")])
 def test_power_of_two_window_totals_match_the_oracle(variant, mode, layout):
-    run = WindowWeightLockStep(MAN, variant, mode, layout, "fp32", True, None, N=2, seed=77, nograd=NOGRAD)
+    run = LockStep(MAN, variant, mode, layout, "fp32", True, None, N=2, seed=77, nograd=NOGRAD,
+                   lr_mult=np.ones(len(MAN), F32), window_weight=True)
     lasts = []
     for w, sigma in POW2_STEPS:
         run.wstep(run.grads(sigma), w)                     # W and last_weight compared bit for bit after every step
@@ -369,9 +368,8 @@ def test_bert_small_full_size_with_mixed_weights_matches_the_oracle(variant):
     their real sizes) with clipping, mixed weights whose window totals are not powers of two, against the oracle
     after every apply."""
     import oracle_np as onp
-    from apply_matrix import SCHED, oracle_hparams, rel_err
+    from apply_matrix import SCHED, oracle_hparams, reference_op, rel_err
     from gaccum_b200.train_op import GaccumTrainOp
-    from window_weight_oracle import reference_op
     g = _g()
     man = onp.MANIFESTS["bert_small"]()
     names = [n for n, _ in man]
@@ -382,7 +380,8 @@ def test_bert_small_full_size_with_mixed_weights_matches_the_oracle(variant):
     lr_fn = lambda s: g.learning_rate(SCHED["init_lr"], SCHED["num_train_steps"], SCHED["num_warmup_steps"], s)
     n = 4
     op = GaccumTrainOp([torch.from_numpy(p.copy()).cuda() for p in params], names, hp, n, lr_fn, window_weight=True)
-    ref = reference_op(variant, "clip", params, names, n, adapt=op.adapt if variant == "lamb" else None)
+    ref = reference_op(variant, "clip", params, names, n, adapt=op.adapt if variant == "lamb" else None,
+                       window_weight=True)
     weights = (37.0, 5.0, 1000.0, 3.0, 11.0, 64.0, 7.0, 250.0, 19.0)
     for s, w in enumerate(weights):
         grads = [(rng.standard_normal(sh, dtype=np.float32) * F32(1e-3)) for _, sh in man]

@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 
 import oracle_np as onp
-from lamb_oracle import LambReferenceTrainOp, lamb_update, norm
+from composed_oracle import ComposedReferenceTrainOp, lamb_update, norm
 
 F32 = np.float32
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -94,8 +94,8 @@ def test_oracle_agrees_with_fp64_closed_form(seed):
     names = [n for n, _ in man]
     params = [rng.normal(0, 0.05, s).astype(F32) for _, s in man]
     grads = [[rng.normal(0, 0.1, s).astype(F32) for _, s in man] for _ in range(3 * N + 1)]
-    ref = LambReferenceTrainOp([x.copy() for x in params], names, _hp(weight_decay_rate=wd, clip_norm=clip), N,
-                               constant_lr=1e-3, adapt_exclude=["LayerNorm"])
+    ref = ComposedReferenceTrainOp([x.copy() for x in params], names, _hp(weight_decay_rate=wd, clip_norm=clip), N,
+                                   constant_lr=1e-3, adapt_exclude=["LayerNorm"])
     for g in grads:
         ref.run(g)
     exp = _closed_form_run(params, names, grads, N, float(F32(1e-3)), 0.9, 0.999, 1e-6, wd, clip, ref.decay, ref.adapt)

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 import oracle_np as onp
-from loss_scale_oracle import LossScaledReferenceTrainOp, update_scale
+from composed_oracle import ComposedReferenceTrainOp, update_scale
 
 MAN = [("a/kernel", (37, 5)), ("a/bias", (5,)), ("LayerNorm/gamma", (9,)), ("emb", (300,))]
 F32 = np.float32
@@ -29,7 +29,7 @@ def _hp(variant_b, clip):
 
 
 def _ls_op(hp, N, **kw):
-    return LossScaledReferenceTrainOp(_params(1), [n for n, _ in MAN], hp, N, constant_lr=1e-3, **kw)
+    return ComposedReferenceTrainOp(_params(1), [n for n, _ in MAN], hp, N, constant_lr=1e-3, **kw)
 
 
 @pytest.mark.parametrize("bad", [np.inf, -np.inf, np.nan, "finite"])

@@ -1,7 +1,7 @@
 """Per-tensor learning-rate multipliers without a GPU: the C setter's checks on layout-only plans, its combination with
 the other setters, the refusals of the entry points that do not support it (C and Python), the byte counts, ELECTRA's
-layer-wise table and the optimizers' key matching, and the oracle's identities (all ones = no table; a uniform m = the
-schedule times m)."""
+layer-wise table and the optimizers' key matching, and the oracle's identities (every option at identity = the reference
+oracles; all ones = no table; a uniform m = the schedule times m)."""
 import ctypes as C
 import itertools
 import math
@@ -9,11 +9,10 @@ import math
 import numpy as np
 import pytest
 
+import oracle_c
 import oracle_np as onp
-from apply_matrix import LS_CFG, SCHED, oracle_hparams
-from lamb_oracle import LambReferenceTrainOp
-from loss_scale_oracle import LossScaledReferenceTrainOp
-from lr_mult_oracle import LrMultReferenceTrainOp
+from apply_matrix import SCHED, oracle_hparams, reference_op
+from composed_oracle import ComposedReferenceTrainOp
 
 F32 = np.float32
 
@@ -193,39 +192,19 @@ VARIANTS = ("adamw", "adam", "lamb")
 MODES = ("noclip", "clip", "ls_noclip", "ls_clip")
 
 
-def _existing(variant, mode, params, names, N):
-    """The oracle of one dispatch key as apply_matrix.reference_op composes it."""
-    hp = oracle_hparams(variant, mode)
-    params = [p.copy() for p in params]
-    ls = dict(initial_scale=LS_CFG[0], multiplier=LS_CFG[1], growth_interval=LS_CFG[2]) if mode.startswith("ls_") else {}
-    if variant == "lamb":
-        return LambReferenceTrainOp(params, names, hp, N, **ls, **SCHED)
-    if ls:
-        return LossScaledReferenceTrainOp(params, names, hp, N, **ls, **SCHED)
-    return onp.ReferenceTrainOp(params, names, hp, N, **SCHED)
-
-
-def _new(variant, mode, params, names, N, lr_mult):
-    hp = oracle_hparams(variant, mode)
-    ls = dict(initial_scale=LS_CFG[0], multiplier=LS_CFG[1], growth_interval=LS_CFG[2]) if mode.startswith("ls_") else {}
-    return LrMultReferenceTrainOp([p.copy() for p in params], names, hp, N, lr_mult=lr_mult, **ls, **SCHED)
-
-
 def _same_state(a, b):
-    """a: LrMultReferenceTrainOp; b: the oracle it is compared with."""
+    """a: the oracle with a table; b: the oracle it is compared with."""
     for what in ("params", "m", "v", "accum"):
         for x, y in zip(getattr(a, what), getattr(b, what)):
             assert np.array_equal(x.view(np.uint32), y.view(np.uint32)), what
     assert (F32(a.beta1_power), F32(a.beta2_power)) == (F32(b.beta1_power), F32(b.beta2_power))
-    if a.ls:
-        assert (a.scale, a.good_windows, a.skipped_windows, a.last_skipped) == \
-            (b.scale, b.good_windows, b.skipped_windows, b.last_skipped)
-    if hasattr(b, "ratios"):
-        assert np.array_equal(np.array(a.ratios, F32), np.array(b.ratios, F32))
+    assert (a.scale, a.good_windows, a.skipped_windows, a.last_skipped) == \
+        (b.scale, b.good_windows, b.skipped_windows, b.last_skipped)
+    assert np.array_equal(np.array(a.ratios, F32), np.array(b.ratios, F32))
 
 
 def _drive(a, b, N, seed, steps=10, m=1.0):
-    """a: the new oracle, b: one fed fp32(lr * m) (m = 1: the schedule itself)."""
+    """a: the oracle with a table, b: one fed fp32(lr * m) (m = 1: the schedule itself)."""
     rng = np.random.default_rng(seed)
     for s in range(steps):
         grads = [rng.normal(0, 0.1, sh).astype(F32) for _, sh in MAN]
@@ -239,14 +218,57 @@ def _drive(a, b, N, seed, steps=10, m=1.0):
         _same_state(a, b)
 
 
+IDENTITY_KEYS = [(v, m) for v in ("adamw", "adam") for m in ("noclip", "clip")]
+
+
+@pytest.mark.parametrize("g0", [0, 2**31 - 2], ids=["from_0", "from_2_31_minus_2"])
+@pytest.mark.parametrize("variant, mode", IDENTITY_KEYS)
+def test_oracle_at_identity_is_the_reference_oracle(variant, mode, g0):
+    """Every option of the composed oracle at its identity -- a table of ones, a window weight that totals N in every
+    window, loss scaling whose S stays 1 -- computes what oracle_np's and the C oracle's restatements of the reference
+    compute, bit for bit, after every micro-step: with a tensor that never gets a gradient, one that misses some, a
+    one-element tensor, and from two steps before global_step's int32 wrap (where a window is longer than N)."""
+    N = 3
+    rng = np.random.default_rng(6)
+    params = [rng.normal(0, 0.05, s).astype(F32) for _, s in MAN]
+    names = [n for n, _ in MAN]
+    hp = oracle_hparams(variant, mode)
+    a = ComposedReferenceTrainOp([p.copy() for p in params], names, hp, N, lr_mult=[1.0] * len(MAN),
+                                 window_weight=True, initial_scale=1.0, growth_interval=2**30, **SCHED, global_step=g0)
+    refs = [cls([p.copy() for p in params], names, hp, N, **SCHED, global_step=g0)
+            for cls in (onp.ReferenceTrainOp, oracle_c.COracleTrainOp)]
+    in_window = 0                                           # micro-steps of the open window so far
+    for s in range(3 * N + 2):
+        grads = [rng.normal(0, 0.1, sh).astype(F32) for _, sh in MAN]
+        grads[1] = None
+        if s % 3 == 2:
+            grads[4] = None
+        in_window += 1
+        applies = int(np.int64(g0 + s).astype(np.int32)) % N == 0
+        ia = a.run([None if x is None else x.copy() for x in grads], weight=N - in_window + 1 if applies else 1.0)
+        if applies:
+            in_window = 0
+            assert a.last_weight == N and a.weight == 0
+        for b in refs:
+            ib = b.run(grads)
+            assert (ia.global_step, ia.applied) == (ib.global_step, ib.applied) and ia.applied == applies
+            for k in ("lr", "global_norm", "clip_scale"):
+                assert F32(getattr(ia, k)).tobytes() == F32(getattr(ib, k)).tobytes(), (type(b).__name__, k)
+            for what in ("params", "m", "v", "accum"):
+                for i, (x, y) in enumerate(zip(getattr(a, what), getattr(b, what))):
+                    assert x.tobytes() == y.tobytes(), (type(b).__name__, what, names[i])
+            assert (F32(a.beta1_power), F32(a.beta2_power)) == (F32(b.beta1_power), F32(b.beta2_power))
+    assert a.scale == 1.0 and a.skipped_windows == 0
+
+
 @pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("variant", VARIANTS)
 def test_oracle_with_ones_is_the_oracle_without(variant, mode):
     rng = np.random.default_rng(3)
     params = [rng.normal(0, 0.05, s).astype(F32) for _, s in MAN]
     names = [n for n, _ in MAN]
-    for lr_mult in (None, [1.0] * len(MAN)):
-        _drive(_new(variant, mode, params, names, 3, lr_mult), _existing(variant, mode, params, names, 3), 3, 5)
+    _drive(reference_op(variant, mode, params, names, 3, lr_mult=[1.0] * len(MAN)),
+           reference_op(variant, mode, params, names, 3), 3, 5)
 
 
 @pytest.mark.parametrize("m", [0.0, 0.3, 2.5])
@@ -256,10 +278,10 @@ def test_uniform_multiplier_is_the_schedule_times_m(variant, mode, m):
     rng = np.random.default_rng(4)
     params = [rng.normal(0, 0.05, s).astype(F32) for _, s in MAN]
     names = [n for n, _ in MAN]
-    ref = _existing(variant, mode, params, names, 3)
+    ref = reference_op(variant, mode, params, names, 3)
     base = ref.lr
     ref.lr = lambda g: np.multiply(F32(base(g)), F32(m), dtype=F32)      # an lr_fn returning fp32(lr * m)
-    _drive(_new(variant, mode, params, names, 3, [m] * len(MAN)), ref, 3, 6, m=m)
+    _drive(reference_op(variant, mode, params, names, 3, lr_mult=[m] * len(MAN)), ref, 3, 6, m=m)
 
 
 def test_oracle_multiplier_zero_freezes_the_weights_only():
@@ -267,7 +289,7 @@ def test_oracle_multiplier_zero_freezes_the_weights_only():
     params = [rng.normal(0, 0.05, s).astype(F32) for _, s in MAN]
     names = [n for n, _ in MAN]
     for variant in VARIANTS:
-        op = _new(variant, "clip", params, names, 2, [0.0, 1.0, 1.0, 0.5, 2.0])
+        op = reference_op(variant, "clip", params, names, 2, lr_mult=[0.0, 1.0, 1.0, 0.5, 2.0])
         for _ in range(4):
             op.run([rng.normal(0, 0.1, s).astype(F32) for _, s in MAN])
         assert np.array_equal(op.params[0], params[0]) and not np.array_equal(op.params[4], params[4])

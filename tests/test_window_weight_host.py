@@ -9,9 +9,7 @@ import numpy as np
 import pytest
 
 import oracle_np as onp
-from apply_matrix import LS_CFG, SCHED, oracle_hparams
-from lr_mult_oracle import LrMultReferenceTrainOp
-from window_weight_oracle import reference_op
+from apply_matrix import reference_op
 
 F32 = np.float32
 BLOCK = 0x50000       # a 16-byte aligned address: the setter is host-only and never dereferences it
@@ -140,12 +138,6 @@ MODES = ["noclip", "clip", "ls_noclip", "ls_clip"]
 VARIANTS = ["adamw", "adam", "lamb"]
 
 
-def _unweighted(variant, mode, params, N):
-    hp = oracle_hparams(variant, mode)
-    lskw = dict(initial_scale=LS_CFG[0], multiplier=LS_CFG[1], growth_interval=LS_CFG[2]) if mode.startswith("ls_") else {}
-    return LrMultReferenceTrainOp([p.copy() for p in params], [n for n, _ in MAN], hp, N, **lskw, **SCHED)
-
-
 def _same(a, b, k=1.0):
     for xs, ys in ((a.params, b.params), (a.m, b.m), (a.v, b.v)):
         for x, y in zip(xs, ys):
@@ -164,8 +156,8 @@ def test_oracle_with_w_equal_k_n_and_k_scaled_gradients_is_unweighted(variant, m
     N = 3
     rng = np.random.default_rng(0)
     params = [rng.normal(0, 0.05, s).astype(F32) for _, s in MAN]
-    w = reference_op(variant, mode, params, [n for n, _ in MAN], N)
-    u = _unweighted(variant, mode, params, N)
+    w = reference_op(variant, mode, params, [n for n, _ in MAN], N, window_weight=True)
+    u = reference_op(variant, mode, params, [n for n, _ in MAN], N)
     for s in range(10):
         grads = [rng.normal(0, 0.1, sh).astype(F32) for _, sh in MAN]
         if mode.startswith("ls_") and s == 4:
@@ -184,7 +176,7 @@ def test_oracle_with_w_equal_k_n_and_k_scaled_gradients_is_unweighted(variant, m
 def test_oracle_divides_by_the_weight():
     rng = np.random.default_rng(1)
     params = [rng.normal(0, 0.05, s).astype(F32) for _, s in MAN]
-    w = reference_op("adamw", "noclip", params, [n for n, _ in MAN], 2)
+    w = reference_op("adamw", "noclip", params, [n for n, _ in MAN], 2, window_weight=True)
     w.global_step = 1
     g1 = [rng.normal(0, 0.1, sh).astype(F32) for _, sh in MAN]
     g2 = [rng.normal(0, 0.1, sh).astype(F32) for _, sh in MAN]
@@ -198,13 +190,21 @@ def test_oracle_divides_by_the_weight():
     assert w.last_weight == 40.0 and w.weight == 0.0
 
 
+def test_unweighted_oracle_refuses_a_weight():
+    params = [np.zeros(s, F32) for _, s in MAN]
+    u = reference_op("adamw", "noclip", params, [n for n, _ in MAN], 2)
+    with pytest.raises(ValueError, match="window weight"):
+        u.run([None] * len(MAN), weight=1.0)
+    assert u.global_step == 0
+
+
 # ---- the data-parallel driver at world 2 over gloo ------------------------------------------------------------------
 DP_MAN = [("l0/kernel", (33, 7)), ("l0/bias", (7,)), ("LayerNorm/gamma", (7,)), ("emb", (301,))]
 DP_N, DP_STEPS, DP_WORLD, DP_CUT = 3, 8, 2, 5
 
 
 class WeightedOracleEngine:
-    """Test-only adapter: ``WindowWeightReferenceTrainOp`` behind the engine interface ``DataParallelTrainOp`` drives
+    """Test-only adapter: a weighted ``ComposedReferenceTrainOp`` behind the engine interface ``DataParallelTrainOp`` drives
     (GaccumTrainOp's), its accumulators aliased to one flat slab and its running W in a 0-dim fp32 tensor,
     ``window_weight``, as a weighted GaccumTrainOp exposes it."""
 
@@ -284,7 +284,7 @@ def _dp_grads(rank, step):
 def _dp_ref(fill=None):
     rng = np.random.default_rng(5)
     params = [rng.normal(0, 0.02, s).astype(F32) if fill is None else np.full(s, fill, F32) for _, s in DP_MAN]
-    return reference_op("adamw", "clip", params, [n for n, _ in DP_MAN], DP_N)
+    return reference_op("adamw", "clip", params, [n for n, _ in DP_MAN], DP_N, window_weight=True)
 
 
 def _dp_worker(rank, port, outdir):
